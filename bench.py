@@ -2,21 +2,23 @@
 """bench.py — edges/s for forward+backward of the layer of one BASELINE.json config, with the HBM roofline of its dominant
 kernel, the reference's CPU path timed beside it, parity against the oracle and an end-to-end number on host buffers.
 
-    python bench.py [--config 1..5] [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--config 1..5] [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
-Default (what the driver runs): config 2 = BASELINE configs[1], the config the metric is quoted on — one GCNConv 128->128
+Default: config 2 = BASELINE configs[1], the config the metric is quoted on — one GCNConv 128->128
 (add_self_loops, relu, bias) forward + backward on RMAT N = 10 M, E = 100 M, fp32.
-    1: 2-layer GCN 1433->16->7 on a Cora-shaped graph          3: GATConv 8 heads x 64 on RMAT N = 5 M, E = 50 M
-    4: SAGEConv mean 128->128 on 1024 batched ER graphs         5: GCNConv 256->256 on RMAT N = 100 M, E = 1 B, 8 GPUs
+    1: 2-layer GCN 1433->16->7 on a Cora-shaped graph          3: GATConv 8 heads x 64 on RMAT N = 2 M, E = 50 M
+    4: SAGEConv mean 128->128 on 1024 batched ER graphs         5: GCNConv 256->256 on RMAT N = 25 M, E = 1 B, 8 GPUs
 
 `value`   : graph edges per second, every input resident in HBM (CUDA events around the K timed steps, max over ranks).
 `e2e`     : the same step through the C ABI's host-buffer entry (config 2: gnnb_gcn_conv_step_host) or the public layer
             call on pinned host arrays (other configs): inputs H2D and results D2H inside the timed region.
 `roofline`: the dominant kernel timed alone with CUDA events on its launch stream; achieved = algorithmic bytes per launch
-            (SURVEY.md §8d gather model) / duration against MEASURED_PEAKS.json; `traffic` = DRAM bytes per launch read from
-            the committed ncu capture of the same kernel (profiles/), never a literal.
+            (SURVEY.md §8d gather model) / duration against MEASURED_PEAKS.json, else the H100 SXM data sheet's 3.35 TB/s.
 `cpu_baseline`, `parity_rel_err`: the oracle's restatement of the reference's CPU algorithm on a bounded sample of the
             same workload, timed on the host cores; the GPU runs the same sample and the two results are compared.
+`--dump-outputs DIR`: after the timed steps, what the timed path computed in its last step (layer output, input and
+            parameter gradients) as DIR/<name>.npy in float32; node-indexed arrays above 16 MB are cut to a fixed seeded
+            sample of rows (DIR/sample_rows.npy).  Inputs are seeded, so two builds can be compared output for output.
 `--impl reference`: the reference's CPU path (oracle port; Julia cannot run here) at the FULL size of the config when the
             host has the memory (config 2: ~60 GB), else the bounded sample (says which).
 """
@@ -36,10 +38,10 @@ SEED = 17
 CFG = {
     1: dict(name="configs[0]: 2-layer GCNConv 1433->16->7, Cora-shaped graph", nodes=2708, edges=10556, dim=1433),
     2: dict(name="configs[1]: GCNConv 128->128, RMAT", nodes=10_000_000, edges=100_000_000, dim=128),
-    3: dict(name="configs[2]: GATConv 8 heads x 64 (concat), RMAT", nodes=5_000_000, edges=50_000_000, dim=512),
+    3: dict(name="configs[2]: GATConv 8 heads x 64 (concat), RMAT", nodes=2_000_000, edges=50_000_000, dim=512),
     4: dict(name="configs[3]: SAGEConv mean 128->128, 1024 batched ER graphs (1000 nodes, 5000 edges each)",
             nodes=1_024_000, edges=5_120_000, dim=128),
-    5: dict(name="configs[4]: GCNConv 256->256, RMAT, node-partitioned over 8 GPUs", nodes=100_000_000,
+    5: dict(name="configs[4]: GCNConv 256->256, RMAT, node-partitioned over 8 GPUs", nodes=25_000_000,
             edges=1_000_000_000, dim=256),
 }
 CPU_SAMPLE = {2: (1_000_000, 10_000_000), 3: (100_000, 1_000_000), 4: (64, None), 5: (1_000_000, 10_000_000)}
@@ -61,6 +63,8 @@ def parse():
     ap.add_argument("--no-parity", action="store_true", help="skip the full-size parity check of the partitioned path (debug)")
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer leg (debug)")
     ap.add_argument("--ref-sample", action="store_true", help="--impl reference on the bounded sample instead of the full size")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32, <= 64 MB in all)")
     a = ap.parse_args()
     c = CFG[a.config]
     a.nodes = a.nodes or c["nodes"]
@@ -77,29 +81,11 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(name, kernel=None):
-    """dram__bytes_read.sum + dram__bytes_write.sum (bytes) of one launch in a committed profiles/*_ncu_raw.csv: the first
-    launch whose kernel name contains `kernel` (launch 1 if None); None if the file or the kernel is missing"""
-    import csv
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "Tbyte": 1e12}
-    try:
-        tot, col = 0.0, 2
-        with open(os.path.join(ROOT, "profiles", name)) as f:
-            for row in csv.reader(f):
-                if row and row[0] == "Kernel Name" and kernel is not None:
-                    col = next(i for i, v in enumerate(row) if i >= 2 and kernel in v)
-                if row and row[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    tot += float(row[col]) * unit[row[1]]
-        return tot or None
-    except Exception:
-        return None
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measurement"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -397,8 +383,43 @@ def capture_step(torch, step, dev):
 
 
 def make_flush(torch, dev):
-    buf = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)      # 256 MB > the 126 MB L2
+    buf = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)      # 256 MB > the 50 MB L2
     return lambda: buf.zero_()
+
+
+DUMP_ARRAY_BYTES = 16 << 20        # larger node-indexed outputs are sampled by rows
+DUMP_TOTAL_BYTES = 64 << 20
+
+
+def dump_outputs(args, torch, arrays):
+    """--dump-outputs: `arrays()` (name -> tensor, node-indexed ones as rows (N, ...)) as DIR/<name>.npy, float32.  Arrays
+    above DUMP_ARRAY_BYTES keep a fixed seeded sample of their rows, the same rows for every array of that length (sized
+    by the widest of them), listed in DIR/sample_rows.npy.  Nothing is written if the files would exceed DUMP_TOTAL_BYTES."""
+    if not args.dump_outputs:
+        return
+    import numpy as np
+    arrays = {name: t.detach() for name, t in arrays().items()}
+    widest = {}
+    for t in arrays.values():
+        if t.dim() >= 2 and t.numel() * 4 > DUMP_ARRAY_BYTES:
+            widest[t.shape[0]] = max(widest.get(t.shape[0], 0), t.numel() // t.shape[0])
+    if len(widest) > 1:
+        raise ValueError(f"--dump-outputs: sampled arrays must share one row count, got {sorted(widest)}")
+    picks = {n: np.sort(np.random.default_rng(SEED).choice(n, size=min(n, max(1, DUMP_ARRAY_BYTES // (4 * w))), replace=False))
+             for n, w in widest.items()}
+    out = {}
+    for name, t in arrays.items():
+        if t.shape and t.shape[0] in picks and t.dim() >= 2:
+            t = t[torch.as_tensor(picks[t.shape[0]], device=t.device)]
+        out[name] = t.float().cpu().numpy()
+    for idx in picks.values():
+        out["sample_rows"] = idx.astype(np.float64)
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_TOTAL_BYTES:
+        raise ValueError(f"--dump-outputs: {total} bytes exceed the {DUMP_TOTAL_BYTES}-byte cap")
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a)
 
 
 def base_line(args, value, ms, n_gpus, workload, extra_cfg, clocks, e2e, launches, roof, cpu, parity, dtype="f32"):
@@ -430,9 +451,11 @@ def run_config2(args, torch, gnn, dev):
     t_plan = time.perf_counter() - t0
 
     gen = torch.Generator(device=dev).manual_seed(0)
+    torch.manual_seed(0)
     layer = gnn.GCNConv(D, D, torch.relu, device=dev)
     x = gnn.unrows(torch.randn(n, D, device=dev, generator=gen)).requires_grad_(True)
     dy = gnn.unrows(torch.randn(n, D, device=dev, generator=gen))
+    last = {}
 
     def step():
         x.grad = None
@@ -440,6 +463,8 @@ def run_config2(args, torch, gnn, dev):
         layer.bias.grad = None
         y = layer(g, x)
         y.backward(dy)
+        if args.dump_outputs:                          # detached: a kept autograd graph would pin the gradient
+            last["y"] = y.detach()                     # accumulators to this stream and break the CUDA-graph capture
         return y
 
     for _ in range(args.warmup):
@@ -449,6 +474,9 @@ def run_config2(args, torch, gnn, dev):
     ms, clocks = timed_region(torch, step, args.steps, dev, dev.index or 0)
     launches = gnn.launch_count() - l0
     value = E / (ms * 1e-3)
+    dump_outputs(args, torch, lambda: {"y": gnn.rows(last["y"]), "dx": gnn.rows(x.grad), "dW": layer.weight.grad,
+                                       "db": layer.bias.grad})
+    last.clear()
 
     # ---- the dominant kernel alone: fused GCN propagate (both directions), CUDA events on the launch stream
     xr = gnn.rows(x.detach())
@@ -464,12 +492,7 @@ def run_config2(args, torch, gnn, dev):
     kms = 0.5 * (kt[0] + kt[1])
     peak, peak_src = measured_peaks()
     achieved = alg_bytes / (kms * 1e-3) / 1e9
-    default_wl = (n, E, D) == (CFG[2]["nodes"], CFG[2]["edges"], CFG[2]["dim"])
-    traffic = ncu_traffic("r2_seg_lean_v0_ncu_raw.csv") if default_wl else None
     roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": traffic, "traffic_GBps": (traffic / (kms * 1e-3) / 1e9) if traffic else None,
-            "traffic_frac_of_peak": (traffic / (kms * 1e-3) / 1e9 / peak) if traffic else None,
-            "traffic_source": "profiles/r2_seg_lean_v0_ncu_raw.csv (ncu --set full, same kernel, same workload)",
             "kernel": "gnnb::seg_lean_kernel<1,1,false,0,SUM> (fused GCN propagate, D=128, per-edge scale stream)",
             "kernel_ms": {"forward": kt[0], "transposed": kt[1]}, "algorithmic_bytes_per_launch": alg_bytes,
             "compulsory_bytes_per_launch": compulsory, "peak_source": peak_src, "share_of_step": 2 * kms / ms}
@@ -531,7 +554,7 @@ def run_config2(args, torch, gnn, dev):
     workload = (f"GCNConv {D}->{D} (add_self_loops, relu, bias) fwd+bwd on RMAT N={n} E={E} seed {SEED} (BASELINE configs[1]); "
                 f"edges counted = graph edges E (the {n} self loops are extra work)")
     return base_line(args, value, ms, 1, workload,
-                     {"l2": "inputs (5.1 GB features) are far larger than the 126 MB L2; no flush needed",
+                     {"l2": "inputs (5.1 GB features) are far larger than the 50 MB L2; no flush needed",
                       "plan_build_ms": t_plan * 1e3, "graph_gen_ms": t_gen * 1e3, "chunk_edges": 128},
                      clocks, e2e, launches, roof, cpu, parity)
 
@@ -559,11 +582,15 @@ def run_config1(args, torch, gnn, dev):
     dy_h = torch.randn(n, 7, generator=gen)
     dy = gnn.unrows(dy_h.to(dev))
 
+    last = {}
+
     def step():
         for p in params:
             p.grad = None
         y = l2(g, l1(g, x))
         y.backward(dy)
+        if args.dump_outputs:                          # detached: a kept autograd graph would pin the gradient
+            last["y"] = y.detach()                     # accumulators to this stream and break the CUDA-graph capture
         return y
 
     for _ in range(max(args.warmup, 3)):
@@ -573,16 +600,22 @@ def run_config1(args, torch, gnn, dev):
     l0 = gnn.launch_count()
     ms_eager, clocks = timed_region(torch, step, args.steps, dev, dev.index or 0, flush)
     launches = gnn.launch_count() - l0
+
+    def outputs():
+        return {"y": gnn.rows(last["y"]), "dW1": l1.weight.grad, "db1": l1.bias.grad, "dW2": l2.weight.grad,
+                "db2": l2.bias.grad}
+    dump_outputs(args, torch, outputs)                  # the eager steps' (a failed capture would leave no gradients)
     # the whole step as ONE CUDA graph launch (launch-latency bound otherwise: ~40 kernels of a few microseconds)
     graph_ms = None
     cg, graph_note = capture_step(torch, step, dev)
     if cg is not None:
         graph_ms, _ = timed_region(torch, cg.replay, args.steps, dev, dev.index or 0, flush)
+        dump_outputs(args, torch, outputs)              # the replays' outputs: the timed path
     ms = graph_ms if graph_ms is not None else ms_eager
     peak, peak_src = measured_peaks()
     bytes_step = 4 * (2 * n * 1433 + 4 * n * 16 + 4 * n * 7 + 3 * 1433 * 16) + 2 * 2 * (E + n) * (4 * 16 + 12)
     roof = {"bound": "hbm", "achieved": bytes_step / (ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-            "frac": bytes_step / (ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src,
+            "frac": bytes_step / (ms * 1e-3) / 1e9 / peak, "peak_source": peak_src,
             "kernel": "whole step (no dominant kernel: ~40 launches of 2-10 us each; the 15.5 MB feature matrix is the only "
                       "array above 1 MB)", "algorithmic_bytes_per_launch": bytes_step,
             "launch_bound": {"eager_ms": ms_eager, "cuda_graph_ms": graph_ms, "launches_per_step": launches / args.steps,
@@ -658,12 +691,16 @@ def run_config3(args, torch, gnn, dev):
     x = gnn.unrows(torch.randn(n, D, device=dev, generator=gen)).requires_grad_(True)
     dy = gnn.unrows(torch.randn(n, D, device=dev, generator=gen))
 
+    last = {}
+
     def step():
         x.grad = None
         for p_ in layer.parameters():
             p_.grad = None
         y = layer(g, x)
         y.backward(dy)
+        if args.dump_outputs:                          # detached: a kept autograd graph would pin the gradient
+            last["y"] = y.detach()                     # accumulators to this stream and break the CUDA-graph capture
         return y
 
     for _ in range(args.warmup):
@@ -672,6 +709,9 @@ def run_config3(args, torch, gnn, dev):
     l0 = gnn.launch_count()
     ms, clocks = timed_region(torch, step, args.steps, dev, dev.index or 0)
     launches = gnn.launch_count() - l0
+    dump_outputs(args, torch, lambda: {"y": gnn.rows(last["y"]), "dx": gnn.rows(x.grad),
+                                       **{"d_" + k.replace(".", "_"): v.grad for k, v in layer.named_parameters()}})
+    last.clear()
     # dominant kernels alone
     g2 = gnn.add_self_loops(g)
     p = g2.plan()
@@ -691,7 +731,7 @@ def run_config3(args, torch, gnn, dev):
     alg_b = E2 * (2 * 4 * D + 4 + 8 * H) + 4 * (n + 1) + 2 * 4 * D * n
     peak, peak_src = measured_peaks()
     roof = {"bound": "hbm", "achieved": alg_b / (kb * 1e-3) / 1e9, "peak": peak, "unit": "GB/s", "frac": alg_b / (kb * 1e-3) / 1e9 / peak,
-            "traffic": ncu_traffic("r2_gat_lean_ncu_raw.csv", "gat_bwd_lean_kernel"), "peak_source": peak_src,
+            "peak_source": peak_src,
             "kernel": "gnnb::gat_bwd_lean_kernel<4> (attention backward over the work items of the CSR-by-source plan: dout and Wx rows gathered per edge)",
             "kernel_ms": {"gat_fwd": kf, "gat_bwd_total": kb}, "algorithmic_bytes_per_launch": alg_b,
             "forward": {"achieved": alg_f / (kf * 1e-3) / 1e9, "frac": alg_f / (kf * 1e-3) / 1e9 / peak, "algorithmic_bytes": alg_f},
@@ -746,7 +786,7 @@ def run_config3(args, torch, gnn, dev):
                          f"materialised), fwd+bwd estimated as 2.5 x forward (Zygote's pullback re-traverses every edge tensor)"}
     workload = (f"GATConv {D} -> {Cc} x {H} heads (concat, self loops, relu, slope 0.2) fwd+bwd on RMAT N={n} E={E} seed {SEED} "
                 "(BASELINE configs[2]; N is this project's choice)")
-    return base_line(args, E / (ms * 1e-3), ms, 1, workload, {"l2": "inputs (10 GB features) far larger than L2"},
+    return base_line(args, E / (ms * 1e-3), ms, 1, workload, {"l2": "inputs (4.1 GB features) far larger than L2"},
                      clocks, e2e, launches, roof, cpu, parity)
 
 
@@ -773,12 +813,16 @@ def run_config4(args, torch, gnn, dev):
     x = gnn.unrows(torch.randn(n, D, device=dev, generator=gen)).requires_grad_(True)
     dy = gnn.unrows(torch.randn(n, D, device=dev, generator=gen))
 
+    last = {}
+
     def step():
         x.grad = None
         layer.weight.grad = None
         layer.bias.grad = None
         y = layer(g, x)
         y.backward(dy)
+        if args.dump_outputs:                          # detached: a kept autograd graph would pin the gradient
+            last["y"] = y.detach()                     # accumulators to this stream and break the CUDA-graph capture
         return y
 
     for _ in range(args.warmup):
@@ -788,10 +832,15 @@ def run_config4(args, torch, gnn, dev):
     l0 = gnn.launch_count()
     ms_eager, clocks = timed_region(torch, step, args.steps, dev, dev.index or 0, flush)
     launches = gnn.launch_count() - l0
+
+    def outputs():
+        return {"y": gnn.rows(last["y"]), "dx": gnn.rows(x.grad), "dW": layer.weight.grad, "db": layer.bias.grad}
+    dump_outputs(args, torch, outputs)                  # the eager steps' (a failed capture would leave no gradients)
     cg, graph_note = capture_step(torch, step, dev)      # ~45 launches of 0.02-0.3 ms: CPU launch latency otherwise dominates
     graph_ms = None
     if cg is not None:
         graph_ms, _ = timed_region(torch, cg.replay, args.steps, dev, dev.index or 0, flush)
+        dump_outputs(args, torch, outputs)              # the replays' outputs: the timed path
     ms = graph_ms if graph_ms is not None else ms_eager
     xr = gnn.rows(x.detach()); out = torch.empty_like(xr); p = g.plan()
     gnn._lib.check(lib.gnnb_graph_csr(p.h, 1, None, None, None, None))
@@ -800,7 +849,7 @@ def run_config4(args, torch, gnn, dev):
     alg = E * (4 * D + 4) + 4 * (n + 1) + 4 * D * n
     peak, peak_src = measured_peaks()
     roof = {"bound": "hbm", "achieved": alg / (kms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s", "frac": alg / (kms * 1e-3) / 1e9 / peak,
-            "traffic": ncu_traffic("r2_seg_lean_mean_c4_ncu_raw.csv"), "peak_source": peak_src,
+            "peak_source": peak_src,
             "kernel": "gnnb::seg_lean_kernel<1,0,false,0,MEAN> (fused mean propagate, D=128) after an L2 flush",
             "kernel_ms": kms, "algorithmic_bytes_per_launch": alg, "compulsory_bytes_per_launch": 2 * 4 * D * n + 4 * E + 4 * (n + 1),
             "share_of_step": 2 * kms / ms,
@@ -902,7 +951,7 @@ def run_reference(args):
     sample = (f"the full config: RMAT N={n} E={E} D={D}" if full else
               f"bounded sample RMAT N={n} E={E} D={D} of RMAT N={n_full} E={E_full} (host has {avail_gb:.0f} GB free, full size "
               f"needs {need_gb:.0f} GB)" if cfg == 2 else
-              f"bounded sample RMAT N={n} E={E} D={D}; config {cfg} itself (102 GB of features) is not run on the CPU")
+              f"bounded sample RMAT N={n} E={E} D={D}; config {cfg} itself (26 GB of features, 1 B edges) is not run on the CPU")
     line = {
         "impl": "reference", "metric": "edges/sec fwd+bwd GCNConv 128-dim on 100M-edge graph", "value": val, "unit": "edges/s",
         "n_gpus": args.gpus, "steps": len(timed), "warmup": nwarm, "ms_per_step": dt * 1e3,
@@ -934,6 +983,8 @@ def run_ours(args):
         dist.init_process_group("nccl", device_id=dev)
         if args.config not in (2, 5):
             raise SystemExit("configs 1, 3, 4 are single-GPU workloads")
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs covers the single-GPU runs")
         from gnnb200 import partition
         if args.config == 5 and "GNNB_HALO_BUFFERS" not in os.environ:
             os.environ["GNNB_HALO_BUFFERS"] = "1"    # 1 KB rows: one halo buffer per shard (forward and backward alternate)

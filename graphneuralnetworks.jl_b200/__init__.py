@@ -1,4 +1,4 @@
-"""graphneuralnetworks.jl_b200 — B200-native (sm_100a) message-passing engine behind GNNlib.jl's
+"""graphneuralnetworks.jl_b200 — H100-native (sm_90a) message-passing engine behind GNNlib.jl's
 `propagate` / `apply_edges` / `aggregate_neighbors` API (see DESIGN.md, INTEGRATION.md).
 
 Import name: ``gnnb200`` (the directory name contains a dot, so the repo-root shim ``gnnb200.py`` loads this

@@ -87,7 +87,7 @@ static int plan_weights(gnnb_graph* g, const Csr& c, int msg, const float* w, si
 extern "C" {
 
 const char* gnnb_last_error(void) { return t_err; }
-const char* gnnb_version(void) { return "gnnb200 0.1 sm_100a"; }
+const char* gnnb_version(void) { return "gnnb200 0.1 sm_90a"; }
 int gnnb_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }

@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers for libgnnb200 (sm_100a only).
+// common.cuh — shared host/device helpers for libgnnb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,6 +44,9 @@ extern std::atomic<int64_t> g_launches;
     } while (0)
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// SMs of the H100 SXM: the block-count caps of the grid-stride and two-stage reduction kernels are multiples of it
+constexpr int kNumSMs = 132;
 
 // ---- one direction of a plan: CSR over `nrows` reduction rows ---------------------------------
 struct Csr {

@@ -1,11 +1,11 @@
 // dense.cu — the per-layer dense contraction of the conv layers:  σ.(W * x .+ b)  and its pullback
 // (GNNlib/src/layers/conv.jl:39,69-71 for gcn_conv; :281 for sage_conv).
 //
-// This is the only true dense contraction on the hot path.  The reference sends it to BLAS/cuBLAS sgemm; so do we — it
-// is a plain library GEMM — but through cuBLASLt from the CUDA 12.9 toolkit with
-//   * compute type CUBLAS_COMPUTE_32F_EMULATED_16BFX9: fp32 inputs/outputs, each operand split into three bf16 terms,
-//     nine bf16 tensor-core (tcgen05) products accumulated in fp32 — fp32-level accuracy at tensor-core speed
-//     (falls back to CUBLAS_COMPUTE_32F, the SIMT sgemm, if the emulated type is unavailable);
+// This is the only true dense contraction on the hot path.  The shapes the layers use most go to the hand-written
+// 3xTF32 wgmma kernels of dense_tc.cu; every other shape is a plain library GEMM, as in the reference (BLAS/cuBLAS
+// sgemm), through cuBLASLt from the CUDA 12.9 toolkit with
+//   * compute type CUBLAS_COMPUTE_32F_EMULATED_16BFX9 where the library offers it (fp32 in/out, each operand split into
+//     three bf16 terms), else CUBLAS_COMPUTE_32F, the fp32 sgemm;
 //   * the bias and relu fused into the GEMM epilogue (CUBLASLT_EPILOGUE_[RELU_]BIAS);
 // and hand-written kernels for the elementwise pullback pieces (relu mask × upstream gradient + bias gradient in one
 // pass).  cuBLASLt 12.9 is dlopen'ed by absolute path so that it does not collide with the older cuBLAS a host
@@ -209,7 +209,7 @@ int gnnb_linear(const float* x, const float* W, const float* bias, int relu, int
     if (N < 0 || Din <= 0 || Dout <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
     if (N == 0) return GNNB_OK;
     if (!x || !W || !y) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
-    {   // hand-written tcgen05 3xTF32 kernel for K, Nout <= 128 (dense_tc.cu); cuBLASLt for every other shape
+    {   // hand-written wgmma 3xTF32 kernels (dense_tc.cu) for the shapes they cover; cuBLASLt for every other shape
         const int rc = linear_tf32x3(x, W, bias, relu, N, Din, Dout, y, (cudaStream_t)stream);
         if (rc != GNNB_EUNSUPPORTED) return rc;
     }
@@ -218,7 +218,7 @@ int gnnb_linear(const float* x, const float* W, const float* bias, int relu, int
 }
 
 // σ.(W * vcat(x1, x2) .+ b) without the vcat: the two column blocks of W hit x1 and x2 in two accumulating passes of the
-// tcgen05 kernel (the second adds the first's result before the activation).  sage_conv, conv.jl:281.
+// wgmma kernel (the second adds the first's result before the activation).  sage_conv, conv.jl:281.
 int gnnb_linear2(const float* x1, const float* x2, const float* W, const float* bias, int relu, int64_t N, int64_t Din1,
                  int64_t Din2, int64_t Dout, float* y, void* stream) {
     if (N < 0 || Din1 <= 0 || Din2 <= 0 || Dout <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
@@ -280,7 +280,7 @@ int gnnb_linear2_bwd(const float* dy, const float* y, const float* x1, const flo
 // the relu mask x upstream gradient and the deterministic two-stage bias gradient, one pass over dy (and y)
 static int act_bwd_launch(const float* dy, const float* y, int relu, int64_t N, int64_t D, float* dpre, float* db, cudaStream_t st) {
     // about 8 CTAs per SM worth of blocks: long row runs per block keep the deterministic final pass short
-    int64_t rpb = ceil_div(N, 148 * 8);
+    int64_t rpb = ceil_div(N, kNumSMs * 8);
     const int rows_per_block = (int)(rpb < 64 ? 64 : rpb);
     const int nblocks = (int)ceil_div(N, rows_per_block);
     float* partial = nullptr;
@@ -305,7 +305,7 @@ int gnnb_bias_act(const float* x, const float* bias, int relu, int64_t N, int64_
         GNNB_FAIL(GNNB_EUNSUPPORTED, "bias_act: D must be a multiple of 4 and pointers 16 B aligned");
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t nvec = N * (D / 4);
-    const unsigned grid = (unsigned)(ceil_div(nvec, 256) < 148 * 16 ? ceil_div(nvec, 256) : 148 * 16);
+    const unsigned grid = (unsigned)(ceil_div(nvec, 256) < kNumSMs * 16 ? ceil_div(nvec, 256) : kNumSMs * 16);
     if (relu) bias_act_kernel<1><<<grid, 256, 0, st>>>(x, bias, nvec, (int)(D / 4), y);
     else bias_act_kernel<0><<<grid, 256, 0, st>>>(x, bias, nvec, (int)(D / 4), y);
     GNNB_LAUNCHED();
@@ -343,7 +343,7 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
     } else if (db && N == 0) {
         GNNB_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * Dout, st));
     }
-    // dX = dPre * W : rows of dPre (K = Dout) against W^T stored K-major => the same tcgen05 kernel on a transposed copy of W
+    // dX = dPre * W : rows of dPre (K = Dout) against W^T stored K-major => the same wgmma kernel on a transposed copy of W
     if (dx && g_tc_enabled && Dout % 32 == 0 && Dout <= 128 && Din % 16 == 0 && Din <= 128 && Din >= 16) {
         static float* wt = nullptr;
         if (!wt) GNNB_CUDA(cudaMalloc(&wt, sizeof(float) * 128 * 128));
@@ -354,7 +354,7 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
         else if (rc != GNNB_EUNSUPPORTED) return rc;
     } else if (dx && g_tc_enabled && (Dout > 128 || Din > 128) && Dout % 32 == 0 && Dout <= 2048 && Din % 128 == 0 && Din <= 1024 &&
                N >= 2048) {
-        // wide shapes: the same product through the wide tcgen05 kernel on a transposed copy of W (<= 8 MB, kept)
+        // wide shapes: the same product through the wide wgmma kernel on a transposed copy of W (<= 8 MB, kept)
         static float* wtw = nullptr; static size_t wtw_elems = 0;
         if (wtw_elems < (size_t)(Dout * Din)) {
             if (wtw) { cudaDeviceSynchronize(); cudaFree(wtw); wtw = nullptr; wtw_elems = 0; }
@@ -372,7 +372,7 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
     // dW row-major (Dout, Din) = col-major (Din x Dout) = X(Din x N) dPre^T(N x Dout)
     if (dW) {
         if (!x) GNNB_FAIL(GNNB_EINVAL, "dW needs x");
-        const int rc = dw_tf32x3(dpre, x, N, Din, Dout, dW, st);      // tcgen05, MN-major operands, split-K
+        const int rc = dw_tf32x3(dpre, x, N, Din, Dout, dW, st);      // wgmma, transposing producers, split-K
         if (rc == GNNB_OK) return GNNB_OK;
         if (rc != GNNB_EUNSUPPORTED) return rc;
         GNNB_TRY(lt::matmul(CUBLAS_OP_N, CUBLAS_OP_T, Din, Dout, N, x, Din, dpre, Dout, dW, Din, nullptr, 0, st));

@@ -1,42 +1,41 @@
-// dense_tc.cu — hand-written tcgen05 kernel for the per-layer dense contraction  Y = act(X * W^T + b)
+// dense_tc.cu — hand-written wgmma kernels for the per-layer dense contraction  Y = act(X * W^T + b)
 // (GNNlib/src/layers/conv.jl:69-71 `l.σ.(weight * x .+ l.bias)`; X is (N rows, K), W is (Nout, K) row-major).
 //
 // fp32 in, fp32 out, fp32-level accuracy on the TF32 tensor cores by the 3xTF32 split:
-//     x = x_big + x_small,  x_big = x with the low 13 mantissa bits cleared (what kind::tf32 reads anyway),
+//     x = x_big + x_small,  x_big = x with the low 13 mantissa bits cleared (what the tf32 MMA reads anyway),
 //     x_small = x - x_big (exact in fp32);   x*w ~= x_big*w_big + x_big*w_small + x_small*w_big
-// (the dropped x_small*w_small term is 2^-22 relative).  Accumulation is fp32 in TMEM.
+// (the dropped x_small*w_small term is 2^-22 relative).  The big*big products accumulate in one register accumulator
+// and the two cross terms (2^-11 smaller) in a second one; the epilogue adds the two.
 //
-// Shape: one persistent CTA per SM.  W (<= 128 x 128) is split once into two K-major 128B-swizzled shared-memory
-// images (w_big, w_small).  Row tiles of 128 rows of X stream through a 2-stage ring, one 32-float K-block per stage:
-//   warps 0-7   loaders : coalesced LDG.128 of the K-block, split in registers, st.shared into the canonical UMMA
-//                         K-major SWIZZLE_128B layout (x_big, x_small), fence.proxy.async, arrive on full[stage]
-//   warp  8     MMA     : one elected thread issues 12 tcgen05.mma.kind::tf32 (M=128, N=Nout, K=8) per K-block into a
-//                         double-buffered TMEM accumulator; tcgen05.commit frees the stage / publishes the tile
-//   warps 9-12  epilogue: tcgen05.ld 32 lanes x 32 columns, + bias, relu, 16 B stores of the finished rows
-// The kernel is HBM-bound by design (2 x 4 x K bytes per row against 6 K^2 flops on 1.1 PF/s of TF32).
+// Shape: one persistent CTA per SM, 384 threads.  W (<= 128 x 128) is split once into two K-major 128B-swizzled
+// shared-memory images (w_big, w_small).  Row tiles of 128 rows of X stream through a 3-stage ring, one 32-float K-block
+// per stage:
+//   warps 0-3    producers : coalesced LDG.128 of the K-block, split in registers, st.shared into the canonical K-major
+//                            SWIZZLE_128B layout (x_big, x_small), fence.proxy.async, arrive on full[stage]
+//   warps 4-11   consumers : two warpgroups, 64 rows of the tile each: 12 wgmma.m64n128k8.tf32 per K-block from shared
+//                            memory into registers, then + bias, relu, stores straight from the accumulator fragment
+// The kernel is HBM-bound by design (2 x 4 x K bytes per row against 6 K^2 flops on the TF32 tensor cores).
 // Every mbarrier wait is bounded: a broken pipeline makes the kernel flag an error and drain instead of hanging.
 #include "common.cuh"
 
 namespace gnnb {
 
 namespace tc {
-constexpr int BM = 128;           // rows per tile (UMMA M)
+constexpr int BM = 128;           // rows per tile (two warpgroups x wgmma M = 64)
 constexpr int BK = 32;            // floats per K-block = one 128 B swizzle row
-constexpr int NSTAGE = 2;            // (3 until the epilogue staging below needed the room; the loaders prefetch one more block in registers)
-constexpr int LOADERS = 256;      // warps 0-7
-constexpr int MMA_WARP = 8;
-constexpr int EPI_WARP0 = 9;      // warps 9-12
-constexpr int THREADS = 13 * 32;
+constexpr int BN = 128;           // wgmma N: W images hold 128 rows, zero beyond Nout
+constexpr int NSTAGE = 3;
+constexpr int PRODUCERS = 128;    // warps 0-3
+constexpr int CONSUMER_WARPS = 8; // warps 4-11 = warpgroups 1 and 2
+constexpr int THREADS = PRODUCERS + CONSUMER_WARPS * 32;
 constexpr int KBLK_BYTES = BM * 128;          // one operand image of a K-block: 128 rows x 128 B = 16 KB
 constexpr int W_BYTES = 4 * KBLK_BYTES;       // up to K = 128: 64 KB per image
 constexpr int SMEM_W_BIG = 0;
 constexpr int SMEM_W_SMALL = W_BYTES;
 constexpr int SMEM_A = 2 * W_BYTES;           // stages: [big 16 KB][small 16 KB]
-constexpr int EPI_LD = 36;            // floats per staged row: 32 + 4 of padding keeps float4 accesses conflict-free
-constexpr int SMEM_EPI = SMEM_A + NSTAGE * 2 * KBLK_BYTES;   // 4 epilogue warps x 32 rows x EPI_LD floats
-constexpr int SMEM_BIAS = SMEM_EPI + 4 * 32 * EPI_LD * 4;
+constexpr int SMEM_BIAS = SMEM_A + NSTAGE * 2 * KBLK_BYTES;
 constexpr int SMEM_BAR = SMEM_BIAS + 512;
-constexpr int SMEM_TOTAL = SMEM_BAR + 128;
+constexpr int SMEM_TOTAL = SMEM_BAR + 64;
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bar_init(uint32_t bar, uint32_t count) {
@@ -61,30 +60,60 @@ __device__ __forceinline__ bool bar_wait(uint32_t bar, uint32_t parity, int* err
     return false;
 }
 __device__ __forceinline__ float tf32_big(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-           ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+// wgmma shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (stride byte offset), leading byte
+// offset unused by this layout.  A step of K = 8 tf32 inside the 128 B swizzle row advances the start address by 32 B.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// D(64 x 128, fp32 registers) (+)= A(64 x 8) * B(128 x 8)^T, both operands tf32 K-major in shared memory.
+// Fragment of D: register 4j + 2h + c of thread (warp w of the warpgroup, lane l) is row 16w + l/4 + 8h, column 8j + 2(l%4) + c.
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+        "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA
+__device__ __forceinline__ void fence_acc(float* d) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// one 32-wide K-block of the 3xTF32 product: cross terms into dc, big*big into dm (dc == dm: one accumulator);
+// the images are K-major SWIZZLE_128B, A starting at this warpgroup's 64 rows
+__device__ __forceinline__ void mma_kblock(float* dm, float* dc, uint32_t a_big, uint32_t a_small, uint32_t b_big,
+                                           uint32_t b_small, bool first) {
+    wgmma_fence();
+    fence_acc(dm);
+    fence_acc(dc);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {                      // 4 x (K = 8 tf32 = 32 B) per K-block, small terms first
+        const uint32_t o = j * 32;
+        const uint32_t acc = (first && j == 0) ? 0u : 1u;
+        wgmma_tf32(dc, gmma_desc(a_small + o), gmma_desc(b_big + o), acc);
+        wgmma_tf32(dc, gmma_desc(a_big + o), gmma_desc(b_small + o), 1u);
+        wgmma_tf32(dm, gmma_desc(a_big + o), gmma_desc(b_big + o), dm == dc ? 1u : acc);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_acc(dm);
+    fence_acc(dc);
 }
 
 struct Params {
@@ -99,6 +128,32 @@ struct Params {
     const float* __restrict__ wimg;  // wide kernel only: W split and swizzled per (quarter, K-block), see tcx::w_image_kernel
 };
 
+// epilogue of one 64 x 128 accumulator pair: columns col_base + [0, 128) of rows row0 + [0, 64), `ncols` of them valid
+__device__ __forceinline__ void store_tile(const Params& p, const float* dm, const float* dc, const float* sbias, int64_t row0,
+                                           int col_base, int ncols) {
+    const int lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3;
+    const int64_t r0 = row0 + w4 * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        if (c >= ncols) continue;
+        const float b0 = sbias[col_base + c], b1 = sbias[col_base + c + 1];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t row = r0 + 8 * h;
+            if (row >= p.M) continue;
+            float2 o = make_float2((dm[4 * j + 2 * h] + dc[4 * j + 2 * h]) + b0, (dm[4 * j + 2 * h + 1] + dc[4 * j + 2 * h + 1]) + b1);
+            const size_t at = (size_t)row * p.Nout + col_base + c;
+            if (p.addend) {
+                const float2 a = *reinterpret_cast<const float2*>(p.addend + at);
+                o.x += a.x; o.y += a.y;
+            }
+            if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+            *reinterpret_cast<float2*>(p.y + at) = o;
+        }
+    }
+}
+
 __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -107,27 +162,20 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params 
     const uint32_t sbase = s_u32(smem);
     const uint32_t bar_full = sbase + SMEM_BAR;                // [NSTAGE]
     const uint32_t bar_empty = bar_full + 8 * NSTAGE;          // [NSTAGE]
-    const uint32_t bar_tfull = bar_empty + 8 * NSTAGE;         // [2]
-    const uint32_t bar_tempty = bar_tfull + 16;                // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SMEM_BAR + 8 * (2 * NSTAGE + 4));
     float* sbias = reinterpret_cast<float*>(smem + SMEM_BIAS);
 
-    // ---- one-time setup: barriers, TMEM, bias, W split into the two swizzled K-major images
+    // ---- one-time setup: barriers, bias, W split into the two swizzled K-major images (rows >= Nout zero)
     if (tid == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { bar_init(bar_full + 8 * s, LOADERS); bar_init(bar_empty + 8 * s, 1); }
-        for (int a = 0; a < 2; ++a) { bar_init(bar_tfull + 8 * a, 1); bar_init(bar_tempty + 8 * a, 128); }
+        for (int s = 0; s < NSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    for (int i = tid; i < 128; i += THREADS) sbias[i] = (p.bias && i < p.Nout) ? p.bias[i] : 0.f;
+    for (int i = tid; i < BN; i += THREADS) sbias[i] = (p.bias && i < p.Nout) ? p.bias[i] : 0.f;
     {
         const int kv = p.K >> 2;                               // float4 per row of W
-        for (int idx = tid; idx < p.Nout * kv; idx += THREADS) {
+        for (int idx = tid; idx < BN * kv; idx += THREADS) {
             const int n = idx / kv, c4 = idx - n * kv, kb = c4 >> 3, c = c4 & 7;
-            const float4 v = __ldg(reinterpret_cast<const float4*>(p.w + (size_t)n * p.ldw) + c4);
+            const float4 v = n < p.Nout ? __ldg(reinterpret_cast<const float4*>(p.w + (size_t)n * p.ldw) + c4)
+                                        : make_float4(0.f, 0.f, 0.f, 0.f);
             const float4 b = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
             const float4 s = make_float4(v.x - b.x, v.y - b.y, v.z - b.z, v.w - b.w);
             const int off = kb * KBLK_BYTES + (n >> 3) * 1024 + (n & 7) * 128 + ((c ^ (n & 7)) << 4);
@@ -135,31 +183,28 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params 
             *reinterpret_cast<float4*>(smem + SMEM_W_SMALL + off) = s;
         }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // W images are read by the tensor core (async proxy)
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    fence_proxy_async();                                       // W images are read by the tensor core (async proxy)
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp < 8) {
-        // ================= loaders =================
-        const int c = tid & 7, r32 = tid >> 3, rr = r32 & 7;
+    if (warp < PRODUCERS / 32) {
+        // ================= producers =================
+        const int c = tid & 7, r16 = tid >> 3, rr = r16 & 7;
         // flattened (tile, K-block) sequence of this CTA; the next item is prefetched into registers while the current
-        // one waits for its shared-memory slot: 8 x 16 B per thread (32 KB per SM) in flight
+        // one waits for its shared-memory slot
         const int64_t my_tiles = (ntiles > (int64_t)blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
         const int64_t total = my_tiles * KB;
         auto fetch = [&](int64_t item, float4* v) {
             const int64_t tile = blockIdx.x + (item / KB) * gridDim.x;
             const int kb = (int)(item % KB);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int64_t row = tile * BM + r32 + 32 * i;
+            for (int i = 0; i < 8; ++i) {
+                const int64_t row = tile * BM + r16 + 16 * i;
                 v[i] = (item < total && row < p.M)
                            ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)row * p.K + kb * BK) + c)
                            : make_float4(0.f, 0.f, 0.f, 0.f);
             }
         };
-        float4 v[4], vn[4];
+        float4 v[8], vn[8];
         fetch(0, v);
         for (int64_t it = 0; it < total; ++it) {
             fetch(it + 1, vn);
@@ -167,128 +212,57 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params 
             if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((it / NSTAGE) & 1) ^ 1), p.err)) break;
             unsigned char* abig = smem + SMEM_A + stage * 2 * KBLK_BYTES;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
+            for (int i = 0; i < 8; ++i) {
                 const float4 b = make_float4(tf32_big(v[i].x), tf32_big(v[i].y), tf32_big(v[i].z), tf32_big(v[i].w));
                 const float4 s = make_float4(v[i].x - b.x, v[i].y - b.y, v[i].z - b.z, v[i].w - b.w);
-                const int off = ((r32 >> 3) + 4 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
+                const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
                 *reinterpret_cast<float4*>(abig + off) = b;
                 *reinterpret_cast<float4*>(abig + KBLK_BYTES + off) = s;
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             bar_arrive(bar_full + 8 * stage);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) v[i] = vn[i];
+            for (int i = 0; i < 8; ++i) v[i] = vn[i];
         }
-    } else if (warp == MMA_WARP) {
-        // ================= MMA issuer =================
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.Nout >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        uint32_t it = 0, tcount = 0;
+    } else {
+        // ================= consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile =================
+        const int wg = (warp - PRODUCERS / 32) >> 2;
+        float dm[64] = {}, dc[64] = {};
+        uint32_t it = 0;
         bool alive = true;
-        for (int64_t tile = blockIdx.x; alive && tile < ntiles; tile += gridDim.x, ++tcount) {
-            const int acc = tcount & 1;
-            if (!bar_wait(bar_tempty + 8 * acc, ((tcount >> 1) & 1) ^ 1, p.err)) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tmem_d = tmem_base + acc * 128;
+        for (int64_t tile = blockIdx.x; alive && tile < ntiles; tile += gridDim.x) {
             for (int kb = 0; kb < KB; ++kb, ++it) {
                 const int stage = it % NSTAGE;
                 if (!bar_wait(bar_full + 8 * stage, (it / NSTAGE) & 1, p.err)) { alive = false; break; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) {
-                    const uint32_t a_big = sbase + SMEM_A + stage * 2 * KBLK_BYTES, a_small = a_big + KBLK_BYTES;
-                    const uint32_t w_big = sbase + SMEM_W_BIG + kb * KBLK_BYTES, w_small = sbase + SMEM_W_SMALL + kb * KBLK_BYTES;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {              // 4 x (K = 8 tf32 = 32 B) per K-block, small terms first
-                        const uint32_t o = j * 32;
-                        umma_tf32(tmem_d, umma_desc(a_small + o), umma_desc(w_big + o), idesc, (kb | j) != 0);
-                        umma_tf32(tmem_d, umma_desc(a_big + o), umma_desc(w_small + o), idesc, 1u);
-                        umma_tf32(tmem_d, umma_desc(a_big + o), umma_desc(w_big + o), idesc, 1u);
-                    }
-                    umma_commit(bar_empty + 8 * stage);        // smem stage reusable once these MMAs have read it
-                    if (kb == KB - 1) umma_commit(bar_tfull + 8 * acc);   // accumulator complete
-                }
-                __syncwarp();
+                const uint32_t a_big = sbase + SMEM_A + stage * 2 * KBLK_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
+                const uint32_t w_big = sbase + SMEM_W_BIG + kb * KBLK_BYTES, w_small = sbase + SMEM_W_SMALL + kb * KBLK_BYTES;
+                mma_kblock(dm, dc, a_big, a_small, w_big, w_small, kb == 0);
+                if (lane == 0) bar_arrive(bar_empty + 8 * stage);   // this warp's reads of the stage are complete
             }
+            if (alive) store_tile(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
         }
-    } else {
-        // ================= epilogue (4 warps; warp w owns TMEM lanes 32*(w%4) .. +31 = rows of the tile) =================
-        const int q = warp & 3;
-        uint32_t tcount = 0;
-        for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-            const int acc = tcount & 1;
-            if (!bar_wait(bar_tfull + 8 * acc, (tcount >> 1) & 1, p.err)) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // A thread holds 32 consecutive columns of ONE row after tcgen05.ld; stored from there, a warp's STG.128 touches
-            // 32 different rows (ncu, round 1: 108 M store wavefronts, L1TEX 80 % busy — the kernel's limiter).  The chunk
-            // is therefore transposed through a padded shared-memory tile and written as whole 128 B row segments.
-            float* stg = reinterpret_cast<float*>(smem + SMEM_EPI) + q * (32 * EPI_LD);
-            const int64_t row0 = tile * BM + q * 32;
-            for (int c0 = 0; c0 < p.Nout; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * 128 + c0, r);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    float4 o;
-                    o.x = __uint_as_float(r[j]) + sbias[c0 + j];
-                    o.y = __uint_as_float(r[j + 1]) + sbias[c0 + j + 1];
-                    o.z = __uint_as_float(r[j + 2]) + sbias[c0 + j + 2];
-                    o.w = __uint_as_float(r[j + 3]) + sbias[c0 + j + 3];
-                    *reinterpret_cast<float4*>(stg + lane * EPI_LD + j) = o;
-                }
-                __syncwarp();
-                const int f = (lane & 7) * 4;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int rr = (lane >> 3) + 4 * i;
-                    float4 o = *reinterpret_cast<const float4*>(stg + rr * EPI_LD + f);
-                    if (row0 + rr < p.M && c0 + f < p.Nout) {
-                        const size_t at = (size_t)(row0 + rr) * p.Nout + c0 + f;
-                        if (p.addend) {
-                            const float4 a = *reinterpret_cast<const float4*>(p.addend + at);
-                            o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-                        }
-                        if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                        *reinterpret_cast<float4*>(p.y + at) = o;
-                    }
-                }
-                __syncwarp();
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            bar_arrive(bar_tempty + 8 * acc);
-        }
-    }
-    // ---- teardown
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
     }
 }
 }  // namespace tc
 
 // =====================================================================================================================
 // dW = dPre^T * X  (the weight pullback of the dense layer):  dW[i][j] = sum_r dPre[r][i] * X[r][j],  r over all N rows.
-// Both operands are "MN-major" in memory (the reduction index r is the slow one), which UMMA reads directly.  For
-// MN-major tf32 the only shared-memory layout is SWIZZLE_128B_BASE32B (cute::UMMA::Layout_MN_SW128_32B_Atom): atoms of
-// 4 k-rows x 128 B (32 consecutive m), the 32 B chunk index of a row XORed with the row index (Swizzle<2,5,2> on the
-// byte address); LBO = stride between atoms along M/N, SBO = stride between 4-k groups (one K = 8 MMA spans two).
-// The loaders are a straight copy + split + swizzle of the global rows.
-// Split-K: every CTA reduces a contiguous range of rows into its own TMEM accumulator and writes a (128 x Din) partial;
-// a second kernel adds the partials in CTA order (deterministic).
+// Both operands are "MN-major" in memory (the reduction index r is the slow one); tf32 wgmma reads K-major shared memory
+// only, so the producers transpose 32 rows of each operand into the same K-major SWIZZLE_128B images the forward kernel
+// uses: A = dPre^T (128 rows i), B = X^T (Din rows j, zero up to 128).  A lane covers 8 rows r x 4 float4 columns, which
+// keeps both the global loads (64 B runs) and the transposing shared-memory stores (2-way) cheap.
+// Split-K: every CTA reduces a contiguous range of rows into its own register accumulators and writes a (128 x Din)
+// partial; a second kernel adds the partials in CTA order (deterministic).
+// The accumulation chain is cut every FLUSH row blocks and each short chain is added into an fp32 register sum with
+// ordinary round-to-nearest adds, so the length of the tensor core's accumulation chain does not grow with N.
 // =====================================================================================================================
 namespace tcw {
 using namespace tc;
-// The TMEM accumulator does not round to nearest: a long accumulation chain drifts by ~2^-25.7 of the running sum per
-// MMA (measured: 5.3e-6 relative after 264 accumulations).  The chain is therefore cut every FLUSH row blocks (128
-// rows = 48 accumulations); the epilogue warps add each short partial into an fp32 shared-memory sum with ordinary
-// round-to-nearest adds while the MMA warp already fills the other TMEM accumulator.
-constexpr int WSTAGE = 2;
+constexpr int WSTAGE = 3;
 constexpr int FLUSH = 4;                      // row blocks (of 32 rows) per accumulation chain
-constexpr int IMG = 32 * 512;                 // one 32-row image of a 128-float-wide operand: 16 KB
-constexpr int STAGE_BYTES = 4 * IMG;          // dPre big/small, X big/small
-constexpr int SMEM_ACC = WSTAGE * STAGE_BYTES;            // fp32 running sum, [col][row] (conflict-free per warp)
-constexpr int SMEM_BARW = SMEM_ACC + 128 * 128 * 4;
-constexpr int SMEM_TOTALW = SMEM_BARW + 128;
+constexpr int STAGE_BYTES = 4 * KBLK_BYTES;   // dPre big/small, X big/small
+constexpr int SMEM_BARW = WSTAGE * STAGE_BYTES;
+constexpr int SMEM_TOTALW = SMEM_BARW + 64;
 
 struct ParamsW {
     const float* __restrict__ dpre;   // [M][128]
@@ -299,14 +273,9 @@ struct ParamsW {
     int* err;
 };
 
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr & 0x3ffffu) >> 4) | ((uint64_t)(512 >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-           ((uint64_t)1 << 46) | ((uint64_t)1 << 61);          // layout type 1 = SWIZZLE_128B_BASE32B
-}
-// byte offset of float4 number f4 of k-row k inside a 32-row image that is `na` 32-float atoms wide
-__device__ __forceinline__ int mn_off(int k, int f4, int na) {
-    const int f = f4 & 7, kr = k & 3;
-    return ((k >> 2) * na + (f4 >> 3)) * 512 + kr * 128 + ((((f >> 1) ^ kr)) << 5) + ((f & 1) << 4);
+// byte offset of element (row n, k) of a K-major SWIZZLE_128B image, k < 32
+__device__ __forceinline__ int kmajor_off(int n, int k) {
+    return (n >> 3) * 1024 + (n & 7) * 128 + ((((k >> 2) ^ (n & 7))) << 4) + (k & 3) * 4;
 }
 
 __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) {
@@ -314,48 +283,45 @@ __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t sbase = s_u32(smem);
     const uint32_t bar_full = sbase + SMEM_BARW, bar_empty = bar_full + 8 * WSTAGE;
-    const uint32_t bar_tfull = bar_empty + 8 * WSTAGE, bar_tempty = bar_tfull + 16;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SMEM_BARW + 8 * (2 * WSTAGE + 4));
-    float* sacc = reinterpret_cast<float*>(smem + SMEM_ACC);
     const int nfB = p.Din >> 2;                   // float4 per row of X
-    const int naB = p.Din >> 5;                   // 32-float atoms along N
     const int64_t r_begin = (int64_t)blockIdx.x * p.rows_per_cta;
     const int64_t r_end = (r_begin + p.rows_per_cta < p.M) ? r_begin + p.rows_per_cta : p.M;
     const int64_t nblk = (r_end > r_begin) ? (r_end - r_begin + 31) / 32 : 0;
-    const int64_t ngroups = (nblk + FLUSH - 1) / FLUSH;
 
     if (tid == 0) {
-        for (int s = 0; s < WSTAGE; ++s) { bar_init(bar_full + 8 * s, LOADERS); bar_init(bar_empty + 8 * s, 1); }
-        for (int a = 0; a < 2; ++a) { bar_init(bar_tfull + 8 * a, 1); bar_init(bar_tempty + 8 * a, 128); }
+        for (int s = 0; s < WSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    // rows j >= Din of the X^T images are never written: zero them once
+    for (int i = tid; i < SMEM_BARW / 16; i += THREADS) reinterpret_cast<float4*>(smem)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    fence_proxy_async();
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp < 8) {
-        // ---- loaders: 32 rows of dPre (128 floats) and of X (Din floats) per stage, straight copy + split + swizzle
+    if (warp < PRODUCERS / 32) {
+        // ---- producers: 32 rows of dPre (128 floats) and of X (Din floats) per stage, transposed + split + swizzled
+        const int rl = lane >> 2, fl = lane & 3;
         auto fetch = [&](int64_t blk, float4* va, float4* vb) {
             const int64_t r0 = r_begin + blk * 32;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int idx = tid + 256 * i;
-                const int ka = idx >> 5, fa = idx & 31;
-                const int64_t ra = r0 + ka;
-                va[i] = (blk < nblk && ra < r_end) ? __ldg(reinterpret_cast<const float4*>(p.dpre + (size_t)ra * 128) + fa)
-                                                    : make_float4(0.f, 0.f, 0.f, 0.f);
-                const int kb = idx / nfB, fb = idx - kb * nfB;
-                const int64_t rb = r0 + kb;
-                vb[i] = (blk < nblk && kb < 32 && rb < r_end) ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)rb * p.Din) + fb)
-                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int q = 0; q < 8; ++q) {
+                const int64_t r = r0 + rl + 8 * (q & 3);
+                const int f = 4 * (warp + 4 * (q >> 2)) + fl;
+                const bool in = blk < nblk && r < r_end;
+                va[q] = in ? __ldg(reinterpret_cast<const float4*>(p.dpre + (size_t)r * 128) + f) : make_float4(0.f, 0.f, 0.f, 0.f);
+                vb[q] = (in && f < nfB) ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)r * p.Din) + f)
+                                        : make_float4(0.f, 0.f, 0.f, 0.f);
             }
         };
-        float4 va[4], vb[4], na[4], nb[4];
+        auto put1 = [&](unsigned char* big, int n, int k, float e) {
+            const int off = kmajor_off(n, k);
+            const float b = tf32_big(e);
+            *reinterpret_cast<float*>(big + off) = b;
+            *reinterpret_cast<float*>(big + KBLK_BYTES + off) = e - b;
+        };
+        auto put = [&](unsigned char* big, int n0, int k, float4 v) {
+            put1(big, n0, k, v.x); put1(big, n0 + 1, k, v.y); put1(big, n0 + 2, k, v.z); put1(big, n0 + 3, k, v.w);
+        };
+        float4 va[8], vb[8], na[8], nb[8];
         fetch(0, va, vb);
         for (int64_t blk = 0; blk < nblk; ++blk) {
             fetch(blk + 1, na, nb);
@@ -363,91 +329,48 @@ __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) 
             if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((blk / WSTAGE) & 1) ^ 1), p.err)) break;
             unsigned char* st = smem + stage * STAGE_BYTES;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int idx = tid + 256 * i;
-                {
-                    const int k = idx >> 5, f = idx & 31;
-                    const int off = mn_off(k, f, 4);
-                    const float4 b = make_float4(tf32_big(va[i].x), tf32_big(va[i].y), tf32_big(va[i].z), tf32_big(va[i].w));
-                    *reinterpret_cast<float4*>(st + off) = b;
-                    *reinterpret_cast<float4*>(st + IMG + off) = make_float4(va[i].x - b.x, va[i].y - b.y, va[i].z - b.z, va[i].w - b.w);
-                }
-                {
-                    const int k = idx / nfB, f = idx - k * nfB;
-                    if (k < 32) {
-                        const int off = mn_off(k, f, naB);
-                        const float4 b = make_float4(tf32_big(vb[i].x), tf32_big(vb[i].y), tf32_big(vb[i].z), tf32_big(vb[i].w));
-                        *reinterpret_cast<float4*>(st + 2 * IMG + off) = b;
-                        *reinterpret_cast<float4*>(st + 3 * IMG + off) = make_float4(vb[i].x - b.x, vb[i].y - b.y, vb[i].z - b.z, vb[i].w - b.w);
-                    }
-                }
+            for (int q = 0; q < 8; ++q) {
+                const int k = rl + 8 * (q & 3);
+                const int f = 4 * (warp + 4 * (q >> 2)) + fl;
+                put(st, 4 * f, k, va[q]);
+                if (f < nfB) put(st + 2 * KBLK_BYTES, 4 * f, k, vb[q]);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             bar_arrive(bar_full + 8 * stage);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) { va[i] = na[i]; vb[i] = nb[i]; }
-        }
-    } else if (warp == MMA_WARP) {
-        // M = 128 (rows of dW), N = Din, both operands MN-major (bits 15, 16)
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) |
-                               ((uint32_t)(p.Din >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        for (int64_t blk = 0; blk < nblk; ++blk) {
-            const int64_t grp = blk / FLUSH;
-            const int acc = (int)(grp & 1);
-            const bool first = (blk % FLUSH) == 0, last = (blk % FLUSH) == FLUSH - 1 || blk == nblk - 1;
-            if (first) {
-                if (!bar_wait(bar_tempty + 8 * acc, (uint32_t)(((grp >> 1) & 1) ^ 1), p.err)) break;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            }
-            const int stage = (int)(blk % WSTAGE);
-            if (!bar_wait(bar_full + 8 * stage, (uint32_t)((blk / WSTAGE) & 1), p.err)) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (lane == 0) {
-                const uint32_t tmem_d = tmem_base + acc * 128;
-                const uint32_t a_big = sbase + stage * STAGE_BYTES, a_small = a_big + IMG, b_big = a_big + 2 * IMG, b_small = a_big + 3 * IMG;
-#pragma unroll
-                for (int kg = 0; kg < 4; ++kg) {               // 4 groups of 8 rows (MMA K = 8 = two 4-row K-atoms)
-                    const uint32_t ao = kg * 2 * 4 * 512, bo = kg * 2 * naB * 512;
-                    umma_tf32(tmem_d, umma_desc_mn(a_small + ao, 4 * 512), umma_desc_mn(b_big + bo, naB * 512), idesc, (first && kg == 0) ? 0u : 1u);
-                    umma_tf32(tmem_d, umma_desc_mn(a_big + ao, 4 * 512), umma_desc_mn(b_small + bo, naB * 512), idesc, 1u);
-                    umma_tf32(tmem_d, umma_desc_mn(a_big + ao, 4 * 512), umma_desc_mn(b_big + bo, naB * 512), idesc, 1u);
-                }
-                umma_commit(bar_empty + 8 * stage);
-                if (last) umma_commit(bar_tfull + 8 * acc);
-            }
-            __syncwarp();
+            for (int q = 0; q < 8; ++q) { va[q] = na[q]; vb[q] = nb[q]; }
         }
     } else {
-        // ---- epilogue: add every short chain into the fp32 shared-memory sum, then write this CTA's partial
-        const int q = warp & 3;
-        const int row = q * 32 + lane;                             // row i of dW = TMEM lane i
-        for (int64_t grp = 0; grp < ngroups; ++grp) {
-            const int acc = (int)(grp & 1);
-            if (!bar_wait(bar_tfull + 8 * acc, (uint32_t)((grp >> 1) & 1), p.err)) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int c0 = 0; c0 < p.Din; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * 128 + c0, r);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        // ---- consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of dW (M = 128), N = Din (padded to 128)
+        const int wg = (warp - PRODUCERS / 32) >> 2;
+        float acc[64] = {}, sum[64];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    float* a = sacc + (c0 + j) * 128 + row;
-                    *a = (grp == 0) ? __uint_as_float(r[j]) : *a + __uint_as_float(r[j]);
-                }
+        for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+        for (int64_t blk = 0; blk < nblk; ++blk) {
+            const int stage = (int)(blk % WSTAGE);
+            if (!bar_wait(bar_full + 8 * stage, (uint32_t)((blk / WSTAGE) & 1), p.err)) break;
+            const uint32_t a_big = sbase + stage * STAGE_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
+            const uint32_t b_big = sbase + stage * STAGE_BYTES + 2 * KBLK_BYTES, b_small = b_big + KBLK_BYTES;
+            mma_kblock(acc, acc, a_big, a_small, b_big, b_small, (blk % FLUSH) == 0);
+            if (lane == 0) bar_arrive(bar_empty + 8 * stage);
+            if ((blk % FLUSH) == FLUSH - 1 || blk == nblk - 1) {
+#pragma unroll
+                for (int i = 0; i < 64; ++i) sum[i] += acc[i];
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            bar_arrive(bar_tempty + 8 * acc);
         }
-        float* prow = p.partial + ((size_t)blockIdx.x * 128 + row) * p.Din;
-        for (int c0 = 0; c0 < p.Din; c0 += 4) {
-            float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (ngroups > 0) o = make_float4(sacc[(c0 + 0) * 128 + row], sacc[(c0 + 1) * 128 + row], sacc[(c0 + 2) * 128 + row], sacc[(c0 + 3) * 128 + row]);
-            *reinterpret_cast<float4*>(prow + c0) = o;
+        const int w4 = warp & 3;
+        const int i0 = wg * 64 + w4 * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            if (c >= p.Din) continue;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float* prow = p.partial + ((size_t)blockIdx.x * 128 + i0 + 8 * h) * p.Din;
+                *reinterpret_cast<float2*>(prow + c) = make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
+            }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == MMA_WARP) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
 }
 
 __global__ void dw_reduce_kernel(const float* __restrict__ partial, int nparts, int n, float* __restrict__ dW) {
@@ -460,31 +383,26 @@ __global__ void dw_reduce_kernel(const float* __restrict__ partial, int nparts, 
 }  // namespace tcw
 
 // =====================================================================================================================
-// Wide shapes (K and/or Nout above 128: GATConv's 512 -> 8 x 64 projection, config 5's 256 -> 256 layer).  W no longer
-// fits beside the ring, so every stage carries one K-block of BOTH operands: 128 rows of X, split big/small by the loader
-// warps, and 128 rows of W (one column quarter of the output), which a small pre-pass has already split and swizzled in
-// global memory so that ONE cp.async.bulk (32 KB, mbarrier complete_tx) drops it into the stage.  Item order per CTA: row
-// tile -> output quarter -> K-block; the X tile is re-read from L2 for every quarter (HBM sees it once), the W image
-// (2 x the size of W, <= 2 MB at 512 x 512) lives in L2.  First version (loaders splitting W as well, one stage of register
-// prefetch): 16.5 ms at 5 M x 512 x 512, tensor pipe 44 % active, no unit saturated: the loaders were the critical path.
-// The big*big products accumulate in one TMEM accumulator and the two cross terms in a second one: the tensor core's
-// accumulator truncates (dw_tf32x3 below measured ~2^-25.7 of the running sum per accumulation), so the chain that carries
-// the full-magnitude sum is kept at K/8 accumulations (64 at K = 512) while the 2K/8 cross-term accumulations act on a sum
-// 2^-11 smaller.  The epilogue adds the two.  Two such pairs (4 x 128 columns = all of TMEM) double-buffer MMA and epilogue.
+// Wide shapes (K and/or Nout above 128: GATConv's 512 -> 8 x 64 projection, 256 -> 256 layers).  W no longer fits beside
+// the ring, so every stage carries one K-block of BOTH operands: 128 rows of X, split big/small by the producer warps, and
+// 128 rows of W (one column quarter of the output), which a small pre-pass has already split and swizzled in global
+// memory so that ONE cp.async.bulk (32 KB, mbarrier complete_tx) drops it into the stage.  Item order per CTA: row tile ->
+// output quarter -> K-block; the X tile is re-read from L2 for every quarter (HBM sees it once), the W image (2 x the size
+// of W, <= 2 MB at 512 x 512) lives in L2.  The big*big products and the cross terms accumulate in separate register
+// accumulators, so the chain that carries the full-magnitude sum is K/8 accumulations long.
 // =====================================================================================================================
 namespace tcx {
 using namespace tc;
 constexpr int XSTAGE = 3;
 constexpr int XSTAGE_BYTES = 4 * KBLK_BYTES;                    // X big, X small, W big, W small: 64 KB
-constexpr int SMEM_EPI_X = XSTAGE * XSTAGE_BYTES;
-constexpr int SMEM_BIAS_X = SMEM_EPI_X + 4 * 32 * EPI_LD * 4;
+constexpr int SMEM_BIAS_X = XSTAGE * XSTAGE_BYTES;
 constexpr int MAX_NOUT = 1024;
 constexpr int SMEM_BAR_X = SMEM_BIAS_X + MAX_NOUT * 4;
-constexpr int SMEM_TOTAL_X = SMEM_BAR_X + 128;
+constexpr int SMEM_TOTAL_X = SMEM_BAR_X + 64;
 
 // W (Nout x K, row stride ldw) -> the shared-memory images the MMA reads, laid out in global memory block by block:
 // block (quarter nq, K-block kb) = [big 16 KB][small 16 KB], each already in the K-major SWIZZLE_128B order.  One
-// cp.async.bulk of 32 KB then fills the W half of a stage: no loader thread touches W.
+// cp.async.bulk of 32 KB then fills the W half of a stage: no producer thread touches W.
 __global__ void w_image_kernel(const float* __restrict__ w, int ldw, int K, int Nout, float* __restrict__ wimg) {
     const int kv = K >> 2, KB = K / BK;
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -518,45 +436,34 @@ __global__ void __launch_bounds__(THREADS, 1) linear_wide_tf32x3_kernel(const Pa
     const uint32_t sbase = s_u32(smem);
     const uint32_t bar_full = sbase + SMEM_BAR_X;              // [XSTAGE]
     const uint32_t bar_empty = bar_full + 8 * XSTAGE;          // [XSTAGE]
-    const uint32_t bar_tfull = bar_empty + 8 * XSTAGE;         // [2]
-    const uint32_t bar_tempty = bar_tfull + 16;                // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SMEM_BAR_X + 8 * (2 * XSTAGE + 4));
     float* sbias = reinterpret_cast<float*>(smem + SMEM_BIAS_X);
 
     if (tid == 0) {
-        // a stage is full when the 256 loader threads have stored X and the bulk copy of the W block has landed
-        for (int s = 0; s < XSTAGE; ++s) { bar_init(bar_full + 8 * s, LOADERS + 1); bar_init(bar_empty + 8 * s, 1); }
-        for (int a = 0; a < 2; ++a) { bar_init(bar_tfull + 8 * a, 1); bar_init(bar_tempty + 8 * a, 128); }
+        // a stage is full when the 128 producer threads have stored X and the bulk copy of the W block has landed
+        for (int s = 0; s < XSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS + 1); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == MMA_WARP) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     for (int i = tid; i < p.Nout; i += THREADS) sbias[i] = p.bias ? p.bias[i] : 0.f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp < 8) {
-        // ================= loaders: X only (4 float4 per thread and stage), two stages ahead in registers =================
-        const int c = tid & 7, r32 = tid >> 3, rr = r32 & 7;
+    if (warp < PRODUCERS / 32) {
+        // ================= producers: X only (8 float4 per thread and stage), two stages ahead in registers =================
+        const int c = tid & 7, r16 = tid >> 3, rr = r16 & 7;
         const int64_t total = my_tiles * NQ * KB;
         // (tile, quarter, K-block) of the next item to fetch, advanced without divisions
         int64_t f_tile = blockIdx.x;
         int f_nq = 0, f_kb = 0;
         auto fetch = [&](int64_t item, float4* va) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int64_t row = f_tile * BM + r32 + 32 * i;
+            for (int i = 0; i < 8; ++i) {
+                const int64_t row = f_tile * BM + r16 + 16 * i;
                 va[i] = (item < total && row < p.M)
                             ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)row * p.K + f_kb * BK) + c)
                             : make_float4(0.f, 0.f, 0.f, 0.f);
             }
             if (++f_kb == KB) { f_kb = 0; if (++f_nq == NQ) { f_nq = 0; f_tile += gridDim.x; } }
         };
-        float4 va[4], na[4], na2[4];
+        float4 va[8], na[8], na2[8];
         fetch(0, va);
         fetch(1, na);
         int w_blk = 0;                                          // (quarter, K-block) of the current item: index of its W block
@@ -574,103 +481,37 @@ __global__ void __launch_bounds__(THREADS, 1) linear_wide_tf32x3_kernel(const Pa
             }
             if (++w_blk == w_blocks) w_blk = 0;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int off = ((r32 >> 3) + 4 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
+            for (int i = 0; i < 8; ++i) {
+                const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
                 const float4 b = make_float4(tf32_big(va[i].x), tf32_big(va[i].y), tf32_big(va[i].z), tf32_big(va[i].w));
                 *reinterpret_cast<float4*>(sa + off) = b;
                 *reinterpret_cast<float4*>(sa + KBLK_BYTES + off) = make_float4(va[i].x - b.x, va[i].y - b.y, va[i].z - b.z, va[i].w - b.w);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             bar_arrive(bar_full + 8 * stage);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) { va[i] = na[i]; na[i] = na2[i]; }
-        }
-    } else if (warp == MMA_WARP) {
-        // ================= MMA issuer: M = 128, N = 128 per instruction =================
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        uint32_t it = 0, ucount = 0;                           // ucount: (tile, quarter) units done by this CTA
-        bool alive = true;
-        const int64_t units = my_tiles * NQ;
-        for (int64_t u = 0; alive && u < units; ++u, ++ucount) {
-            const int acc = ucount & 1;
-            if (!bar_wait(bar_tempty + 8 * acc, ((ucount >> 1) & 1) ^ 1, p.err)) break;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t d_main = tmem_base + acc * 256, d_cross = d_main + 128;
-            for (int kb = 0; kb < KB; ++kb, ++it) {
-                const int stage = it % XSTAGE;
-                if (!bar_wait(bar_full + 8 * stage, (it / XSTAGE) & 1, p.err)) { alive = false; break; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) {
-                    const uint32_t a_big = sbase + stage * XSTAGE_BYTES, a_small = a_big + KBLK_BYTES;
-                    const uint32_t w_big = a_big + 2 * KBLK_BYTES, w_small = a_big + 3 * KBLK_BYTES;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint32_t o = j * 32;
-                        umma_tf32(d_cross, umma_desc(a_small + o), umma_desc(w_big + o), idesc, (kb | j) != 0);
-                        umma_tf32(d_cross, umma_desc(a_big + o), umma_desc(w_small + o), idesc, 1u);
-                        umma_tf32(d_main, umma_desc(a_big + o), umma_desc(w_big + o), idesc, (kb | j) != 0);
-                    }
-                    umma_commit(bar_empty + 8 * stage);
-                    if (kb == KB - 1) umma_commit(bar_tfull + 8 * acc);
-                }
-                __syncwarp();
-            }
+            for (int i = 0; i < 8; ++i) { va[i] = na[i]; na[i] = na2[i]; }
         }
     } else {
-        // ================= epilogue: main + cross + bias (+ addend), activation, whole 128 B row segments =================
-        const int q = warp & 3;
-        uint32_t ucount = 0;
-        float* stg = reinterpret_cast<float*>(smem + SMEM_EPI_X) + q * (32 * EPI_LD);
+        // ================= consumers: M = 64 rows per warpgroup, N = 128 columns of one output quarter =================
+        const int wg = (warp - PRODUCERS / 32) >> 2;
+        float dm[64] = {}, dc[64] = {};
+        uint32_t it = 0;
         for (int64_t t = 0; t < my_tiles; ++t) {
             const int64_t tile = blockIdx.x + t * gridDim.x;
-            const int64_t row0 = tile * BM + q * 32;
-            for (int nq = 0; nq < NQ; ++nq, ++ucount) {
-                const int acc = ucount & 1;
-                if (!bar_wait(bar_tfull + 8 * acc, (ucount >> 1) & 1, p.err)) goto done;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                for (int c0 = 0; c0 < 128; c0 += 32) {
-                    uint32_t r[32], r2[32];
-                    const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + acc * 256 + c0;
-                    tmem_ld32(ta, r);
-                    tmem_ld32(ta + 128, r2);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    const int cg = nq * 128 + c0;                  // first output column of this chunk
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float4 o;
-                        o.x = (__uint_as_float(r[j]) + __uint_as_float(r2[j])) + sbias[cg + j];
-                        o.y = (__uint_as_float(r[j + 1]) + __uint_as_float(r2[j + 1])) + sbias[cg + j + 1];
-                        o.z = (__uint_as_float(r[j + 2]) + __uint_as_float(r2[j + 2])) + sbias[cg + j + 2];
-                        o.w = (__uint_as_float(r[j + 3]) + __uint_as_float(r2[j + 3])) + sbias[cg + j + 3];
-                        *reinterpret_cast<float4*>(stg + lane * EPI_LD + j) = o;
-                    }
-                    __syncwarp();
-                    const int f = (lane & 7) * 4;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int rr = (lane >> 3) + 4 * i;
-                        float4 o = *reinterpret_cast<const float4*>(stg + rr * EPI_LD + f);
-                        if (row0 + rr < p.M) {
-                            const size_t at = (size_t)(row0 + rr) * p.Nout + cg + f;
-                            if (p.addend) {
-                                const float4 a = *reinterpret_cast<const float4*>(p.addend + at);
-                                o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-                            }
-                            if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                            *reinterpret_cast<float4*>(p.y + at) = o;
-                        }
-                    }
-                    __syncwarp();
+            for (int nq = 0; nq < NQ; ++nq) {
+                for (int kb = 0; kb < KB; ++kb, ++it) {
+                    const int stage = it % XSTAGE;
+                    if (!bar_wait(bar_full + 8 * stage, (it / XSTAGE) & 1, p.err)) return;
+                    const uint32_t a_big = sbase + stage * XSTAGE_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
+                    const uint32_t w_big = sbase + stage * XSTAGE_BYTES + 2 * KBLK_BYTES, w_small = w_big + KBLK_BYTES;
+                    mma_kblock(dm, dc, a_big, a_small, w_big, w_small, kb == 0);
+                    if (lane == 0) bar_arrive(bar_empty + 8 * stage);
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                bar_arrive(bar_tempty + 8 * acc);
+                store_tile(p, dm, dc, sbias, tile * BM + wg * 64, nq * 128, 128);
             }
         }
-    done:;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == MMA_WARP) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
 }
 }  // namespace tcx
 

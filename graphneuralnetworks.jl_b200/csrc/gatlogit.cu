@@ -164,7 +164,7 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
     const size_t smem = sizeof(float) * (size_t)LOGIT_WARPS * A;
     if (smem > 200 * 1024) GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms_bwd: 2*H*C too large for the block stage");
     int64_t want = ceil_div(N, LOGIT_WARPS);
-    const int nblocks = (int)(want < 148 * 4 ? want : 148 * 4);
+    const int nblocks = (int)(want < kNumSMs * 4 ? want : kNumSMs * 4);
     static float* part_buf = nullptr; static size_t part_bytes = 0;
     const size_t need = sizeof(float) * (size_t)nblocks * A;
     if (part_bytes < need) { if (part_buf) { cudaDeviceSynchronize(); cudaFree(part_buf); } GNNB_CUDA(cudaMalloc(&part_buf, need)); part_bytes = need; }

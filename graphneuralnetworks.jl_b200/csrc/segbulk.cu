@@ -6,9 +6,8 @@
 // D*4-byte row of its edge from HBM/L2 into the warp's shared-memory ring, completion is tracked by an mbarrier
 // per stage (complete_tx::bytes), and the warp consumes a stage of 32 rows with conflict-free LDS.128 while the
 // next stages are in flight.  Bytes in flight per SM are bounded by shared memory (~190 KB) instead of by the
-// register file — the ncu capture of the register-staged kernel (profiles/r1_seg_reduce_v1.md) showed it was
-// latency/issue bound at 52 % of HBM bandwidth with 54 warp-instructions per edge; here an edge costs one
-// LDS.128 + 8 FP32 ops + a ballot-mask test.
+// register file, which bounds the register-staged kernel; here an edge costs one LDS.128 + 8 FP32 ops + a ballot-mask
+// test.
 //
 // Used for fp32 rows of 128, 256, 384 or 512 floats (the configurations of BASELINE.json); everything else takes
 // the register-staged kernel.  Results are bit-identical to it (same order of additions).
@@ -233,7 +232,7 @@ static int launch_bulk(const BulkParams& p, cudaStream_t st) {
 }
 
 // returns GNNB_EUNSUPPORTED (without setting the error text) when the shape is not covered.
-// (the cp.async / LDGSTS ring variants measured in round 1 — 1.5-4x slower, profiles/r1_seg_variants.md — are gone)
+// (the cp.async / LDGSTS ring variants of round 1 measured slower and are gone)
 int seg_reduce_bulk(const Csr& c, const SegArgs& a, int64_t E, int chunk, float* ws, int fill, int cfg,
                     cudaStream_t st) {
     if (a.D % 128 != 0 || a.D > 512 || a.D == 384) return GNNB_EUNSUPPORTED;

@@ -149,7 +149,7 @@ __device__ __forceinline__ float4 lcomb(float4 a, float4 v, float s1, float s2, 
 // KV float4 per lane: one warp covers a row of KV*128 floats.  SMODE 0: no gathered-node scale, 1: per-edge stream es,
 // 2: gather cs[col].  HALO 0: one source base; 1: nodes >= split live in x2 (the halo rows of a shard).
 // (Staging the most gathered rows in a persisting-L2 window, with or without cache-streaming loads for the rest, was
-// measured 2-50 % slower: profiles/r2_seg_lean.md.)  Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
+// measured slower.)  Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
 // compiler keeps the loop free of divergence handling; shuffles are never executed under a lane-dependent condition.
 template <int KV, int SMODE, bool HAS_W, int HALO, int AGG>
 __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
@@ -255,19 +255,19 @@ __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
 
 // ---- A/B variant 13: the same pass with the rows staged in shared memory by TMA (D = 128, SUM) ---------------------------
 // BASELINE's north_star asks for "TMA staging of node-feature tiles into shared memory".  Round 1 measured one
-// cp.async.bulk per 512 B row: TMA-unit bound (~56 cycles per request per SM), 2.2x slower than register staging.  This
-// is the Blackwell form of the idea: cp.async.bulk.tensor.2d ... tile::gather4 moves FOUR indexed rows (2 KB) per request.
-// Persistent CTAs (one per SM, 8 warps); every warp is its own producer and consumer: lane 0 issues the gather4 of the
+// cp.async.bulk per 512 B row, which the TMA unit's request rate bounds.  This variant stages the rows through a 2-D tensor
+// map instead: one cp.async.bulk.tensor.2d tile load (box = one row) per gathered row, four rows per mbarrier.
+// Persistent CTAs (one per SM, 8 warps); every warp is its own producer and consumer: lane 0 issues the loads of the
 // next four edges into the warp's private ring of 8 stages (16 KB, 32 rows in flight per warp, 256 per SM — no registers
 // held by loads in flight), all lanes wait on the stage's mbarrier (complete_tx) and reduce the four rows with LDS.128.
 // A stage is refilled with the NEXT batch's rows as soon as it has been consumed.  Same items, same arithmetic order:
 // bit-identical to the register-staged kernel.
-// Rows of KV*128 floats: a group of four edges is one request of 4 x 512 B (KV = 1), 4 x 1 KB (KV = 2) or two requests of
-// 4 x 1 KB on one barrier (KV = 4: a TMA box is at most 256 elements wide).  128 KB of ring per CTA in every case.
+// Rows of KV*128 floats: a group of four edges is 4 x 512 B (KV = 1), 4 x 1 KB (KV = 2) or 4 x 2 KB in two column halves
+// (KV = 4: a TMA box is at most 256 elements wide), all on the group's one barrier.  128 KB of ring per CTA in every case.
 template <int KV> struct G4 {
     static constexpr int WARPS = KV == 4 ? 4 : 8;
     static constexpr int STAGES = KV == 1 ? 8 : 4;                // groups in flight per warp
-    static constexpr int REQS = KV == 4 ? 2 : 1;                  // gather4 requests per group
+    static constexpr int REQS = KV == 4 ? 2 : 1;                  // column halves per row
     static constexpr int BOX_COLS = KV * 128 / REQS;
     static constexpr int ROW_BYTES = KV * 512;
     static constexpr int STAGE_BYTES = 4 * ROW_BYTES;
@@ -305,9 +305,13 @@ __global__ void __launch_bounds__(G4<KV>::WARPS * 32, 1) seg_gather4_kernel(cons
             tma::fence_proxy_async();                  // the stage was read through the generic proxy
             tma::mbar_expect_tx(bar0 + 8 * st, C::STAGE_BYTES);
 #pragma unroll
-            for (int rq = 0; rq < C::REQS; ++rq)       // request rq lands its 4 x BOX_COLS block after the previous one
-                tma::gather4(ring_u + st * C::STAGE_BYTES + rq * (4 * C::BOX_COLS * 4), &map, rq * C::BOX_COLS, c0, c1, c2, c3,
-                             bar0 + 8 * st);
+            for (int rq = 0; rq < C::REQS; ++rq) {     // column half rq lands its 4 x BOX_COLS block after the previous one
+                const uint32_t dst = ring_u + st * C::STAGE_BYTES + rq * (4 * C::BOX_COLS * 4);
+                tma::load_row(dst, &map, rq * C::BOX_COLS, c0, bar0 + 8 * st);
+                tma::load_row(dst + C::BOX_COLS * 4, &map, rq * C::BOX_COLS, c1, bar0 + 8 * st);
+                tma::load_row(dst + 2 * C::BOX_COLS * 4, &map, rq * C::BOX_COLS, c2, bar0 + 8 * st);
+                tma::load_row(dst + 3 * C::BOX_COLS * 4, &map, rq * C::BOX_COLS, c3, bar0 + 8 * st);
+            }
         }
     };
 
@@ -647,7 +651,7 @@ int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, bo
     p.sign = (a.aggr == GNNB_MIN) ? -1.f : 1.f;
     if (p.n_items == 0) return GNNB_OK;
     const int use_halo = halo ? 1 : 0;
-    if (g_variant == 13 && agg == AG_SUM && !halo && a.w == nullptr) {      // rows staged by TMA tile::gather4 (A/B variant)
+    if (g_variant == 13 && agg == AG_SUM && !halo && a.w == nullptr) {      // rows staged by TMA tile loads (A/B variant)
         if (a.D == 128) return launch_gather4<1>(p, smode, a.x, c.ncols, st);
         if (a.D == 256) return launch_gather4<2>(p, smode, a.x, c.ncols, st);
         return launch_gather4<4>(p, smode, a.x, c.ncols, st);

@@ -34,9 +34,8 @@ namespace gnnb {
 // 128 / 256 / 512 floats, taking the per-edge scale stream when the caller has one, and seg_reduce_kernel below for every
 // other shape; 10 = the lean kernel gathering cs[col] itself; 12 = seg_reduce_kernel everywhere (the round-1 default);
 // 5 = the same without the 64-register cap; 1 = shared-memory ring filled by cp.async.bulk (segbulk.cu);
-// 13 = the lean pass with the rows staged by TMA tile::gather4 (D = 128 sums; seglean.cu), everything else as 0.
-// Round 1's LDGSTS rings (2..4) and round 2's index-prefetch variants (6..9) were measured slower and removed
-// (profiles/r1_seg_variants.md, profiles/r2_seg_lean.md).
+// 13 = the lean pass with the rows staged by TMA tile loads (D = 128 sums; seglean.cu), everything else as 0.
+// Round 1's LDGSTS rings (2..4) and round 2's index-prefetch variants (6..9) were measured slower and removed.
 int g_variant = 0;
 
 template <int VEC> struct VecT;
@@ -249,8 +248,8 @@ template <int VEC, int TPR, int K, bool ISMAX>
 static int launch_seg(const SegParams& p, cudaStream_t st) {
     const int gpb = 256 / TPR;  // groups per block
     dim3 grid((unsigned)ceil_div(p.nchunks, gpb), (unsigned)ceil_div(p.D, (int64_t)VEC * TPR * K));
-    // One warp per 512 B row (D = 128 fp32): throughput follows the number of resident warps, not the loads per warp
-    // (profiles/r1_seg_variants.md): cap the kernel at 64 registers => 4 CTAs x 8 warps per SM.  Variant 5 keeps the
+    // One warp per 512 B row (D = 128 fp32): throughput follows the number of resident warps, not the loads per warp:
+    // cap the kernel at 64 registers => 4 CTAs x 8 warps per SM.  Variant 5 keeps the
     // uncapped build (77 registers, 24 warps) for A/B runs.
     if (VEC == 4 && TPR == 32 && K == 1 && g_variant != 5) {
         seg_reduce_kernel<4, 32, 1, ISMAX, 8, 4><<<grid, 256, 0, st>>>(p);

@@ -1,6 +1,6 @@
 // tma.cuh — tensor maps (cuTensorMapEncodeTiled through the runtime's driver-entry-point query: no link against libcuda)
 // and the device-side wrappers of the TMA instructions this library issues: mbarrier transaction counting and
-// cp.async.bulk.tensor.2d ... tile::gather4 (four indexed rows of a 2-D tensor per request, sm_100+).
+// cp.async.bulk.tensor.2d ... tile (one box of a 2-D tensor per request).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -54,10 +54,10 @@ __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
                  : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
-// four rows {r0..r3} of the 2-D tensor behind `map`, columns [col, col + box_cols), into 4 consecutive box rows at dst
-__device__ __forceinline__ void gather4(uint32_t dst, const CUtensorMap* map, int col, int r0, int r1, int r2, int r3, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-                 ::"r"(dst), "l"(map), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar) : "memory");
+// columns [col, col + box_cols) of row `row` of the 2-D tensor behind `map` (box_rows = 1) into dst
+__device__ __forceinline__ void load_row(uint32_t dst, const CUtensorMap* map, int col, int row, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"(map), "r"(col), "r"(row), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 

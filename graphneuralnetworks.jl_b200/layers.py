@@ -11,7 +11,7 @@ bias, σ, negative_slope, channel, heads, concat, add_self_loops, dropout``; SAG
 (GraphNeuralNetworks/src/layers/conv.jl:77-104, 309-346, 770-787).
 
 Arrays are Julia-shaped and column-major: x is (Din, N), weight is (Dout, Din), GAT's ``a`` is (2C, H).
-The dense contractions `σ.(W*x .+ b)` go through gnnb_linear / gnnb_linear_bwd (hand-written tcgen05 3xTF32 kernels with
+The dense contractions `σ.(W*x .+ b)` go through gnnb_linear / gnnb_linear_bwd (hand-written wgmma 3xTF32 kernels with
 the bias/relu epilogue; cuBLASLt for shapes they do not cover) when the shape allows, torch's fp32 matmul otherwise.
 
 Further down: the layers SURVEY.md §8f ranks first because they re-parameterise the same kernels — graph_conv, gin_conv,
@@ -457,7 +457,7 @@ class GATConv(torch.nn.Module):
 # ------------------------------------------------------------------------------------------ SAGEConv
 class _Linear2Fn(torch.autograd.Function):
     """σ.(W * vcat(x1, x2) .+ b) for σ ∈ {identity, relu} through gnnb_linear2 / gnnb_linear2_bwd: the two column blocks
-    of W meet x1 and x2 in two accumulating passes of the tcgen05 kernel — no (Din1+Din2, N) vcat temporary."""
+    of W meet x1 and x2 in two accumulating passes of the wgmma kernel — no (Din1+Din2, N) vcat temporary."""
 
     @staticmethod
     def forward(ctx, x1, x2, W, bias, relu_flag):
@@ -503,7 +503,7 @@ def sage_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     D1, D2, Dout = r1.shape[1], r2.shape[1], W.shape[0]
     if (r1.is_cuda and r1.dtype == torch.float32 and W.dtype == torch.float32 and Dout == 128 and D1 % 32 == 0 and D2 % 32 == 0
             and D1 <= 128 and D2 <= 128 and (sig is identity or _is_relu(sig))):
-        # the two column blocks of W in two accumulating tcgen05 passes: no vcat temporary
+        # the two column blocks of W in two accumulating wgmma passes: no vcat temporary
         return unrows(_Linear2Fn.apply(r1.contiguous(), r2.contiguous(), W, None if b is None else b.contiguous(), _is_relu(sig)))
     xm = unrows(torch.cat([r1, r2], dim=1))                   # vcat(xi, m): (2·in, N)
     return _linear(l, W, xm, True)                            # σ.(W * vcat(xi, m) .+ b): one GEMM, bias/σ in the epilogue

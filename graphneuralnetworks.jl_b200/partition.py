@@ -691,7 +691,7 @@ def bench_multi(args, world, rank, dev, seed, ClockSampler, measured_peaks, cpu_
                                    f"(BASELINE configs[{1 if D == 128 else 4}]), node-partitioned over {world} GPUs, halo exchange over NVLink",
                        "parallelism": f"node-partition x{world}, {ownership} ownership, shards built on the device from generated chunks",
                        "halo_exchange": os.environ.get("GNNB_HALO", "push") + (" (one kernel writes rows into peer halo buffers over NVLink, CUDA IPC)" if os.environ.get("GNNB_HALO", "push") == "push" else " (pack kernel + NCCL all_to_all_single)"),
-                       "l2": "per-GPU features and halo buffers are far larger than the 126 MB L2",
+                       "l2": "per-GPU features and halo buffers are far larger than the 50 MB L2",
                        "plan_build_ms": t_plan * 1e3, "plan_build_phases_ms_rank0": {k: round(v, 1) for k, v in dg.timing.items()},
                        "nccl_connection_setup_ms": t_comm * 1e3, "chunk_edges": 128,
                        "per_rank": {"kernel_ms": allst[:, 0].tolist(), "halo_exchange_ms": allst[:, 1].tolist(),
@@ -705,7 +705,8 @@ def bench_multi(args, world, rank, dev, seed, ClockSampler, measured_peaks, cpu_
                          "halo": {"bytes_received_slowest_rank": float(allst[:, 4].max()) * D * 4,
                                   "ms": float(allst[:, 1].max()),
                                   "GBps_per_gpu": float(allst[:, 4].max()) * D * 4 / (float(allst[:, 1].max()) * 1e-3) / 1e9,
-                                  "nvlink_peak_GBps": 770.0}},
+                                  "nvlink_peak_GBps": 450.0,
+                                  "nvlink_peak_source": "H100 SXM data sheet (900 GB/s NVLink, both directions), not a measurement"}},
             "cpu_baseline": cpu, "parity_rel_err": par,
         }
         print(json.dumps(line), flush=True)

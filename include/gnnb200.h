@@ -1,5 +1,5 @@
 /*
- * gnnb200.h — C ABI of libgnnb200.so, the B200-native (sm_100a) message-passing engine that sits
+ * gnnb200.h — C ABI of libgnnb200.so, the H100-native (sm_90a) message-passing engine that sits
  * behind GNNlib.jl's `propagate` / `apply_edges` / `aggregate_neighbors` hot path.
  *
  * Every entry point below replaces one reference interface; the citation after "replaces:" is
@@ -60,7 +60,7 @@ typedef struct gnnb_graph* gnnb_graph_t;
 
 /* thread-local text of the last failure on this thread ("" if none) */
 const char* gnnb_last_error(void);
-/* library version string, e.g. "gnnb200 0.1 sm_100a" */
+/* library version string, e.g. "gnnb200 0.1 sm_90a" */
 const char* gnnb_version(void);
 /* number of CUDA devices visible (0 when there is none; never fails) */
 int gnnb_device_count(void);
@@ -200,11 +200,11 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
 
 /* ------------------------------------------------------- dense layer part
  * replaces: l.σ.(weight * x .+ l.bias) of the conv layers (GNNlib/src/layers/conv.jl:39,69-71; :281) and its pullback.
- * Din, Dout <= 128: hand-written tcgen05 kernels (csrc/dense_tc.cu: 3xTF32 split, TMEM accumulators, bias/relu epilogue
- * written as whole row segments, W resident in shared memory); Din % 32 == 0 <= 2048 and Dout % 128 == 0 <= 1024 with at
- * least 2048 nodes: the wide tcgen05 kernel of the same file (both operands streamed, W through cp.async.bulk; forward and
+ * Din, Dout <= 128: hand-written wgmma kernels (csrc/dense_tc.cu: 3xTF32 split, register accumulators, bias/relu
+ * epilogue, W resident in shared memory); Din % 32 == 0 <= 2048 and Dout % 128 == 0 <= 1024 with at
+ * least 2048 nodes: the wide wgmma kernel of the same file (both operands streamed, W through cp.async.bulk; forward and
  * dx); every other shape: a library GEMM like the reference's, issued through cuBLASLt 12.9
- * with the fp32-emulated compute type (bf16 x9, fp32 accumulate; SIMT sgemm if unavailable), bias (+relu) in the epilogue.  x (Din,N), W (Dout,Din) row-major as the layer stores it, bias NULL or Dout floats, y (Dout,N).
+ * with the fp32-emulated compute type where the library offers it (bf16 x9, fp32 accumulate), else the fp32 sgemm, bias (+relu) in the epilogue.  x (Din,N), W (Dout,Din) row-major as the layer stores it, bias NULL or Dout floats, y (Dout,N).
  * relu: 0 = identity, 1 = relu. */
 int gnnb_linear(const float* x, const float* W, const float* bias, int relu, int64_t N, int64_t Din,
                 int64_t Dout, float* y, void* stream);
@@ -215,7 +215,7 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
                     int64_t Din, int64_t Dout, float* dpre_ws, float* dx, float* dW, float* db, void* stream);
 /* σ.(W * vcat(x1, x2) .+ b) — sage_conv's dense part (GNNlib/src/layers/conv.jl:281) — without the (Din1+Din2, N) vcat
  * temporary: the two column blocks of W (Dout, Din1+Din2, row-major as the layer stores it) meet x1 (Din1,N) and x2 (Din2,N)
- * in two passes of the tcgen05 kernel, the second adding the first's result before bias / activation.  Pullback: dx1, dx2,
+ * in two passes of the wgmma kernel, the second adding the first's result before bias / activation.  Pullback: dx1, dx2,
  * dW (Dout, Din1+Din2), db, each may be NULL.  Shapes: Din1, Din2 multiples of 32 <= 128, Dout = 128 (forward also Dout a
  * multiple of 16 <= 128); GNNB_EUNSUPPORTED otherwise (callers concatenate and use gnnb_linear). */
 int gnnb_linear2(const float* x1, const float* x2, const float* W, const float* bias, int relu, int64_t N, int64_t Din1,
@@ -232,7 +232,7 @@ int gnnb_bias_act_bwd(const float* dy, const float* y, int relu, int64_t N, int6
 /* 1 (default) = try the fp32-emulated tensor-core GEMM; 0 = force the SIMT sgemm.  *_active: -1 not yet used,
  * 0 unavailable / off, 1 in use. */
 int gnnb_dense_set_emulation(int on);
-/* The hand-written tcgen05 kernels (csrc/dense_tc.cu: 3xTF32 split, TMEM accumulators, bias/relu epilogue) serve
+/* The hand-written wgmma kernels (csrc/dense_tc.cu: 3xTF32 split, register accumulators, bias/relu epilogue) serve
  * Din, Dout <= 128 (Din % 32 == 0, Dout % 16 == 0) and the wide shapes named above for gnnb_linear and the dx part of
  * gnnb_linear_bwd (dW: Dout == 128 only); 0 switches them off (cuBLASLt everywhere).  gnnb_dense_tc_error() != 0 means one of its bounded pipeline waits expired. */
 int gnnb_dense_set_tensor_core_kernel(int on);
@@ -393,8 +393,8 @@ int gnnb_set_chunk_edges(int chunk);
  * 0 = default: the lean work-item kernel (csrc/seglean.cu), taking the plan's per-edge scale stream when there is one;
  * 10 = the lean kernel gathering cs[col] per edge;  12 = seg_reduce_kernel (the round-1 default: register-staged
  * LDG.128, 64-register cap);  5 = the same without the register cap;  1 = TMA-staged: one cp.async.bulk (UBLKCP) per
- * row into a shared-memory ring, mbarrier completion;  13 = the lean pass with rows staged by TMA tile::gather4 (four
- * indexed rows per request into a per-warp shared-memory ring; D = 128 sums).  Measurements: profiles/r1_seg_variants.md, profiles/r2_seg_lean.md. */
+ * row into a shared-memory ring, mbarrier completion;  13 = the lean pass with rows staged by TMA 2-D tile loads (one
+ * row per request, four rows per mbarrier, into a per-warp shared-memory ring; D = 128 sums). */
 int gnnb_set_kernel_variant(int v);
 
 #ifdef __cplusplus

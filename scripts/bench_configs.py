@@ -85,8 +85,8 @@ if 4 in which:  # 1024 ER graphs x (1000 nodes, 5000 edges), block-diagonal batc
     del g, x, dy, xr, out
     torch.cuda.empty_cache()
 
-if 3 in which:  # GATConv 8 heads x 64, RMAT N=5M, E=50M (+5M self loops)
-    n, E, H, C = 5_000_000, 50_000_000, 8, 64
+if 3 in which:  # GATConv 8 heads x 64, RMAT N=2M, E=50M (+2M self loops)
+    n, E, H, C = 2_000_000, 50_000_000, 8, 64
     D = H * C
     g = gnn.rmat_graph(n, E, 17, device=dev)
     layer = gnn.GATConv(D, C, torch.relu, heads=H, device=dev)

@@ -1,4 +1,5 @@
-"""small calls of the kernels added late in round 2, meant to run under `compute-sanitizer --tool memcheck`"""
+"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback and the TMA-staged reduce
+(variant 13), meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gnnb200 as gnn
@@ -11,6 +12,19 @@ y = torch.empty(N, Nout, device="cuda")
 gnn._lib.check(lib.gnnb_linear(x.data_ptr(), W.data_ptr(), b.data_ptr(), 1, N, K, Nout, y.data_ptr(), None))
 ref = (x.double() @ W.double().t() + b.double()).clamp(min=0)
 print("wide linear err", float((y.double() - ref).norm() / ref.norm()), "tc_error", lib.gnnb_dense_tc_error())
+# narrow linear kernel (tail tile, Nout < 128) and its pullback: dx through the same kernel, dW through the split-K kernel
+N, K, Nout = 1000 + 13, 96, 128
+x = torch.randn(N, K, device="cuda"); W = torch.randn(Nout, K, device="cuda") / K ** 0.5; b = torch.randn(Nout, device="cuda")
+y = torch.empty(N, Nout, device="cuda")
+gnn._lib.check(lib.gnnb_linear(x.data_ptr(), W.data_ptr(), b.data_ptr(), 1, N, K, Nout, y.data_ptr(), None))
+dy = torch.randn(N, Nout, device="cuda"); ws = torch.empty_like(dy); dx = torch.empty_like(x); dW = torch.empty_like(W)
+dbl = torch.empty(Nout, device="cuda")
+gnn._lib.check(lib.gnnb_linear_bwd(dy.data_ptr(), y.data_ptr(), x.data_ptr(), W.data_ptr(), 1, N, K, Nout, ws.data_ptr(),
+                                   dx.data_ptr(), dW.data_ptr(), dbl.data_ptr(), None))
+dpre = dy.double() * (y > 0)
+print("narrow linear dx err", float((dx.double() - dpre @ W.double()).norm() / (dpre @ W.double()).norm()),
+      "dW err", float((dW.double() - dpre.t() @ x.double()).norm() / (dpre.t() @ x.double()).norm()),
+      "tc_error", lib.gnnb_dense_tc_error())
 # closing line
 D = 36
 z = torch.randn(1001, D, device="cuda"); bb = torch.randn(D, device="cuda"); o = torch.empty_like(z)
@@ -29,5 +43,14 @@ for Dm in (128, 256):
     dy = torch.where(torch.isfinite(ym), torch.randn_like(ym), torch.zeros_like(ym))
     ym.backward(dy)
     print("max pullback D", Dm, float(xm.grad.abs().sum()))
+# rows staged by TMA tile loads (variant 13) against the default kernel: same bits
+xs = gnn.unrows(torch.randn(n, 128, device="cuda"))
+ref = gnn.propagate(gnn.copy_xj, g, "+", xj=xs)
+lib.gnnb_set_kernel_variant(13)
+try:
+    got = gnn.propagate(gnn.copy_xj, g, "+", xj=xs)
+finally:
+    lib.gnnb_set_kernel_variant(0)
+print("variant 13 bit-identical", bool(torch.equal(ref, got)))
 torch.cuda.synchronize()
 print("done")

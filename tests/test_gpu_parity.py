@@ -1,4 +1,4 @@
-"""Parity of the CUDA path (through the Python mirror -> C ABI -> sm_100a kernels) with the CPU oracle.
+"""Parity of the CUDA path (through the Python mirror -> C ABI -> sm_90a kernels) with the CPU oracle.
 
 Bar (BASELINE.json north_star): bit-exact for index arithmetic; fp32 aggregations within 1e-5 relative
 (normwise, the reference's `isapprox` semantics, GNNlib/test/test_module.jl:75-151) of the fp64 oracle — the
@@ -777,13 +777,13 @@ def test_halo_addressing_and_gather_rows(graph, oracle, gnn, variant, D):
 @pytest.mark.parametrize("N,Din,Dout", [(1000, 128, 128), (777, 16, 8), (5000, 64, 256), (33, 1432, 16), (0, 8, 8),
                                         (4096, 64, 128), (130000, 128, 64), (300, 32, 16), (129, 96, 48), (1, 128, 128),
                                         (400000, 128, 128), (70001, 96, 128),
-                                        # the wide tcgen05 kernel (K or Nout above 128, N >= 2048): GATConv 512 -> 8 x 64, config 5
+                                        # the wide wgmma kernel (K or Nout above 128, N >= 2048): GATConv 512 -> 8 x 64, config 5
                                         (40000, 512, 512), (3000, 256, 256), (20001, 512, 128), (2048, 160, 384),
                                         (9000, 1024, 1024)])
 @pytest.mark.parametrize("relu_flag,with_bias", [(1, True), (0, True), (1, False), (0, False)])
 @pytest.mark.parametrize("emulate", [1, 0])
 def test_linear_c_abi(gnn, N, Din, Dout, relu_flag, with_bias, emulate):
-    # emulate=1: hand-written tcgen05 3xTF32 kernel where the shape allows, cuBLASLt fp32-emulated GEMM elsewhere;
+    # emulate=1: hand-written wgmma 3xTF32 kernel where the shape allows, cuBLASLt fp32-emulated GEMM elsewhere;
     # emulate=0: cuBLASLt SIMT sgemm only (tensor-core kernel switched off)
     """gnnb_linear / gnnb_linear_bwd (σ.(W*x .+ b), conv.jl:69-71) against fp64: the fp32-emulated tensor-core GEMM must
     stay inside the 1e-5 bar, like the SIMT sgemm."""
@@ -814,7 +814,7 @@ def test_linear_c_abi(gnn, N, Din, Dout, relu_flag, with_bias, emulate):
         else:
             assert (db == 0).all()
         assert lib.gnnb_dense_emulation_active() in (-1, 0, 1)
-        assert lib.gnnb_dense_tc_error() == 0          # the tcgen05 pipeline never timed out
+        assert lib.gnnb_dense_tc_error() == 0          # the wgmma pipeline never timed out
     finally:
         lib.gnnb_dense_set_emulation(1)
         lib.gnnb_dense_set_tensor_core_kernel(1)
@@ -1006,7 +1006,7 @@ def test_gat_logit_terms_c_abi(gnn, Cc, H, n):
 @pytest.mark.parametrize("N,D1,D2", [(70001, 128, 128), (5000, 96, 32), (129, 128, 64)])
 @pytest.mark.parametrize("relu_flag,with_bias", [(1, True), (0, False)])
 def test_linear2_c_abi(gnn, N, D1, D2, relu_flag, with_bias):
-    """gnnb_linear2 / gnnb_linear2_bwd — σ.(W * vcat(x1, x2) .+ b) as two accumulating tcgen05 passes over the column blocks
+    """gnnb_linear2 / gnnb_linear2_bwd — σ.(W * vcat(x1, x2) .+ b) as two accumulating wgmma passes over the column blocks
     of W (sage_conv, conv.jl:281) — against float64."""
     lib = gnn._lib.lib
     Dout = 128

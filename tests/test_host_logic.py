@@ -141,19 +141,6 @@ def _bench_module():
     return mod
 
 
-def test_bench_reads_roofline_traffic_from_the_committed_ncu_extracts():
-    """roofline.traffic must come from the committed CSV of the CURRENT kernel, selected by name — not a literal"""
-    b = _bench_module()
-    lean = b.ncu_traffic("r2_seg_lean_v0_ncu_raw.csv")
-    assert lean is not None and 35e9 < lean < 45e9                        # config 2: 39.2 GB per launch
-    fwd = b.ncu_traffic("r2_gat_lean_ncu_raw.csv", "gat_fwd_lean_kernel")
-    bwd = b.ncu_traffic("r2_gat_lean_ncu_raw.csv", "gat_bwd_lean_kernel")
-    assert fwd is not None and bwd is not None and bwd > fwd > 50e9       # config 3: 94.7 / 126.4 GB
-    assert b.ncu_traffic("r2_gat_lean_ncu_raw.csv", "no_such_kernel") is None
-    assert b.ncu_traffic("no_such_file.csv") is None
-    assert b.ncu_traffic("r2_seg_lean_mean_c4_ncu_raw.csv") is not None   # config 4's mean kernel
-
-
 def test_bench_argument_surface():
     """the flags the driver and the scripts rely on"""
     import sys
@@ -166,4 +153,38 @@ def test_bench_argument_surface():
         sys.argv = old
     assert (a.gpus, a.steps, a.warmup, a.config) == (8, 4, 3, 5)
     assert a.no_parity and a.no_cpu and a.no_e2e and a.impl != "reference"
-    assert (a.nodes, a.edges, a.dim) == (100_000_000, 1_000_000_000, 256)     # config 5 = BASELINE configs[4]
+    assert (a.nodes, a.edges, a.dim) == (25_000_000, 1_000_000_000, 256)      # config 5 = BASELINE configs[4]
+
+
+def test_bench_dump_outputs_samples_rows_and_caps_size(tmp_path, monkeypatch):
+    """--dump-outputs: float32 files; node-indexed arrays above the per-array size share one fixed seeded row sample
+    (stored as sample_rows.npy and sized by the widest array); small arrays whole; over the total cap nothing is written"""
+    import os
+    from types import SimpleNamespace
+    import numpy as np
+    b = _bench_module()
+    n = 40000
+    y = torch.arange(n * 128, dtype=torch.float64).reshape(n, 128)         # 20.5 MB as float32: sampled
+    dx = -torch.arange(n * 160, dtype=torch.float64).reshape(n, 160)       # wider: sets the sample size
+    dW = torch.rand(128, 128)
+    arrays = lambda: {"y": y, "dx": dx, "dW": dW}
+    b.dump_outputs(SimpleNamespace(dump_outputs=None), torch, lambda: 1 / 0)   # no flag: not even evaluated
+    out = tmp_path / "d"
+    b.dump_outputs(SimpleNamespace(dump_outputs=str(out)), torch, arrays)
+    got = {f[:-4]: np.load(out / f) for f in os.listdir(out)}
+    assert sorted(got) == ["dW", "dx", "sample_rows", "y"]
+    assert all(a.dtype == np.float32 for k, a in got.items() if k != "sample_rows")
+    rows = got["sample_rows"].astype(np.int64)
+    assert got["sample_rows"].dtype == np.float64 and np.all(np.diff(rows) > 0) and rows[-1] < n
+    assert len(rows) == b.DUMP_ARRAY_BYTES // (4 * 160)
+    assert np.array_equal(got["y"], y.numpy()[rows].astype(np.float32))
+    assert np.array_equal(got["dx"], dx.numpy()[rows].astype(np.float32))
+    assert got["dx"].nbytes <= b.DUMP_ARRAY_BYTES and np.array_equal(got["dW"], dW.numpy())
+    assert sum(a.nbytes for a in got.values()) <= b.DUMP_TOTAL_BYTES
+    again = tmp_path / "again"
+    b.dump_outputs(SimpleNamespace(dump_outputs=str(again)), torch, arrays)
+    assert np.array_equal(np.load(again / "sample_rows.npy"), got["sample_rows"])       # seeded: same rows every run
+    monkeypatch.setattr(b, "DUMP_TOTAL_BYTES", 1 << 20)
+    with pytest.raises(ValueError):
+        b.dump_outputs(SimpleNamespace(dump_outputs=str(tmp_path / "over")), torch, arrays)
+    assert not (tmp_path / "over").exists()

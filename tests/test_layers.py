@@ -523,7 +523,7 @@ def test_agnn_conv(gnn, be):
 @pytest.mark.parametrize("sig", ["relu", "identity"])
 def test_sage_conv_split_weight_path(gnn, be, sig):
     """SAGEConv 128 -> 128 on a CUDA device takes gnnb_linear2 (the CPU test double keeps the vcat formula): the two column blocks of W meet x_i and the aggregated neighbours in two
-    accumulating tcgen05 passes instead of a (2·in, N) vcat + one GEMM (conv.jl:281); output, dx, dW, db against float64."""
+    accumulating wgmma passes instead of a (2·in, N) vcat + one GEMM (conv.jl:281); output, dx, dW, db against float64."""
     rng = np.random.default_rng(11)
     dev = be.dev
     g, R, s, t = make_graph(gnn, rng, dev)
