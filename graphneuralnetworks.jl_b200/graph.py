@@ -259,10 +259,37 @@ def add_self_loops(g: GNNGraph) -> GNNGraph:
     return h
 
 
+class _WeightedDegreeFn(torch.autograd.Function):
+    """Weighted degree as NNlib.scatter(+, w, idx) (GNNGraphs/src/query.jl:359-369), with scatter's pullback:
+    dw = Δ[t] for dir=:in, Δ[s] for :out, and the sum of the two for :both."""
+
+    @staticmethod
+    def forward(ctx, w, plan, d, n_nodes):
+        out = torch.empty(n_nodes, dtype=torch.float32, device=plan.device)
+        with torch.cuda.device(plan.device):
+            _lib.check(lib.gnnb_degree(plan.h, d, w.data_ptr(), out.data_ptr(), _stream(plan.device)))
+        ctx.plan, ctx.d, ctx.n_edges = plan, d, w.numel()
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        plan = ctx.plan
+        dout = dout.to(torch.float32).contiguous()
+        which = {_lib.DIR_IN: (_lib.DST,), _lib.DIR_OUT: (_lib.SRC,), _lib.DIR_BOTH: (_lib.DST, _lib.SRC)}[ctx.d]
+        dw = None
+        with torch.cuda.device(plan.device):
+            for k in which:
+                part = torch.empty(ctx.n_edges, dtype=torch.float32, device=dout.device)
+                _lib.check(lib.gnnb_gather(plan.h, k, dout.data_ptr(), 1, part.data_ptr(), _stream(plan.device)))
+                dw = part if dw is None else dw + part
+        return dw, None, None, None
+
+
 def degree(g: GNNGraph, T=None, *, dir: str = "out", edge_weight=True) -> torch.Tensor:
     """degree(g, T; dir, edge_weight) — GNNGraphs/src/query.jl:314-331,355-369 (note the reference default dir=:out).
 
-    edge_weight: True -> the graph's own weights if any, False/None -> counts, tensor -> those weights."""
+    edge_weight: True -> the graph's own weights if any, False/None -> counts, tensor -> those weights.  With weights
+    that require grad the result is differentiable in them (the reference's weighted degree is a scatter(+))."""
     assert dir in ("in", "out", "both")  # query.jl:339
     if isinstance(edge_weight, torch.Tensor):
         w = edge_weight
@@ -271,13 +298,16 @@ def degree(g: GNNGraph, T=None, *, dir: str = "out", edge_weight=True) -> torch.
     else:
         w = None
     p = g.plan()
-    out = torch.empty(g.num_nodes, dtype=torch.float32, device=p.device)
     if w is not None:
         assert w.numel() == g.num_edges
         w = w.to(device=p.device, dtype=torch.float32).contiguous()
     d = {"out": _lib.DIR_OUT, "in": _lib.DIR_IN, "both": _lib.DIR_BOTH}[dir]
-    with torch.cuda.device(p.device):
-        _lib.check(lib.gnnb_degree(p.h, d, _ptr(w), out.data_ptr(), _stream(p.device)))
+    if w is not None and w.requires_grad and torch.is_grad_enabled():
+        out = _WeightedDegreeFn.apply(w, p, d, g.num_nodes)
+    else:
+        out = torch.empty(g.num_nodes, dtype=torch.float32, device=p.device)
+        with torch.cuda.device(p.device):
+            _lib.check(lib.gnnb_degree(p.h, d, _ptr(w), out.data_ptr(), _stream(p.device)))
     if T is None:
         T = torch.float32 if w is not None else g.s.dtype
     return out.to(T)

@@ -51,30 +51,64 @@ def np_rows(x_jl):
     return gnnb200.rows(x_jl.detach()).cpu().numpy()
 
 
+def chunk_graph(rng, n, chunk, menu, n_empty=4):
+    """configuration-model multigraph whose rows meet the edges of the chunk decomposition (segwalk.cuh) on purpose.
+    In- and out-degrees come from `menu` (degrees around chunk/4 and 1-2 chunks).  Node ids 1-6 get the same prefix in
+    both directions, so in both plans rows of C, C+1 and 2C edges start exactly on a chunk boundary, the (2C+1)-edge
+    row ends on one, a long row ends with a one-edge piece and another starts with one.  The other ids draw from the
+    menu, `n_empty` of them get no edge; the out-degrees are another shuffle of the same draws, so the sums match and
+    row starts fall at many offsets mod C and mod 32.  t = repeat(ids, indeg), s = a permutation of repeat(ids, outdeg),
+    the edge list in random order."""
+    C = chunk
+    prefix = [C, C + 1, C - 1, 2 * C, C - 1, 2 * C + 1]
+    rest = np.concatenate([rng.choice(menu, n - len(prefix) - n_empty), np.zeros(n_empty, np.int64)])
+    ids = np.arange(1, n + 1)
+    t = np.repeat(ids, np.concatenate([prefix, rng.permutation(rest)]))
+    s = rng.permutation(np.repeat(ids, np.concatenate([prefix, rng.permutation(rest)])))
+    p = rng.permutation(len(s))
+    return s[p].astype(np.int64), t[p].astype(np.int64)
+
+
 GRAPHS = {
     "small": dict(n=37, E=150),
     "empty_rows": dict(n=200, E=300, empty_frac=0.6),
     "hubs": dict(n=500, E=3000, hubs=3, hub_deg=1000, src_hubs=2),   # rows far longer than the 128-edge chunk, both plans
     "sparse": dict(n=5000, E=40),                          # rows >> edges: row-parallel empty fill path
+    # rows at the edges of the work decomposition, at the default chunk and at the smallest (plan built while it is set)
+    "chunk_edges": dict(n=320, chunk=128, menu=(1, 31, 32, 33, 127, 128, 129, 255, 256, 257)),
+    "chunk32": dict(n=320, chunk=32, menu=(1, 31, 32, 33, 63, 64, 65)),
 }
+SHORT_ROWS = ("small", "empty_rows", "sparse")             # every row fits in one chunk
+
+
+def fixture_plan(gnn, name, s, t, n):
+    """a device graph of (s, t) whose plan has the chunk size of GRAPHS[name]"""
+    try:
+        if "chunk" in GRAPHS[name]:
+            gnn._lib.check(gnn._lib.lib.gnnb_set_chunk_edges(GRAPHS[name]["chunk"]))
+        g = gnn.GNNGraph(s, t, num_nodes=n).to("cuda")
+        g.plan()                   # the plan keeps the chunk it was created with; add_self_loops and by-source inherit it
+    finally:
+        gnn._lib.lib.gnnb_set_chunk_edges(128)
+    return g
+
+
+def build_graph(gnn, name):
+    rng = np.random.default_rng(list(GRAPHS).index(name))
+    kw = dict(GRAPHS[name])
+    s, t = chunk_graph(rng, **kw) if "chunk" in kw else make_graph(rng, **kw)
+    return name, s, t, kw["n"], fixture_plan(gnn, name, s, t, kw["n"])
 
 
 @pytest.fixture(scope="module", params=list(GRAPHS))
 def graph(request, gnn):
-    rng = np.random.default_rng(list(GRAPHS).index(request.param))
-    kw = GRAPHS[request.param]
-    s, t = make_graph(rng, **kw)
-    g = gnn.GNNGraph(s, t, num_nodes=kw["n"]).to("cuda")
-    return request.param, s, t, kw["n"], g
+    return build_graph(gnn, request.param)
 
 
 @pytest.fixture(scope="module", params=[k for k in GRAPHS if k != "sparse"])
 def graph_with_edges(request, gnn):
     """the graphs whose targets mostly have in-edges (GAT always runs with self loops; `sparse` adds nothing there)"""
-    rng = np.random.default_rng(list(GRAPHS).index(request.param))
-    kw = GRAPHS[request.param]
-    s, t = make_graph(rng, **kw)
-    return request.param, s, t, kw["n"], gnn.GNNGraph(s, t, num_nodes=kw["n"]).to("cuda")
+    return build_graph(gnn, request.param)
 
 
 @pytest.fixture(scope="module")
@@ -168,7 +202,7 @@ def _check_propagate_copy_xj(graph, oracle, gnn, D, aggr):
     assert rel(got, ref64) < TOL
     if aggr in ("max", "min"):       # order independent: bit-exact
         assert (got == oracle.propagate_unfused(aggr, s, t, n, x)).all()
-    elif name in ("small", "empty_rows", "sparse"):   # rows <= chunk: same summation order as NNlib's CPU scatter
+    elif name in SHORT_ROWS:          # rows <= chunk: same summation order as NNlib's CPU scatter
         assert (got == oracle.propagate_unfused(aggr, s, t, n, x)).all()
 
 
@@ -200,7 +234,7 @@ def test_propagate_weighted(graph, oracle, gnn, D, aggr, fn):
     got = np_rows(got)
     ref64 = oracle.propagate_unfused(aggr, s, t, n, x.astype(np.float64), w.astype(np.float64))
     assert rel(got, ref64) < TOL
-    if aggr != "mean" and name != "hubs":
+    if aggr in ("max", "min") or (aggr == "+" and name in SHORT_ROWS):     # order independent, or one group per row
         assert (got == oracle.propagate_unfused(aggr, s, t, n, x, w)).all()
 
 
@@ -385,10 +419,20 @@ def test_gcn_closed_form_and_conv_weight(gnn):
     np.testing.assert_allclose(y[0, 1], wn[2] / np.sqrt(d[1] * d[0]) + wn[3] / np.sqrt(d[1] * d[2]), rtol=1e-6)
     y2 = l(g, x, w.cuda(), norm_fn=lambda d: 1 / torch.sqrt(d)).detach().cpu().numpy()
     np.testing.assert_allclose(y, y2, rtol=1e-6)
-    # gradient w.r.t. the edge weights exists and is a vector (conv.jl:47-52)
+    # gradient w.r.t. the edge weights (conv.jl:45-50), against float64 autograd of y = W c .* A_w' (c .* x) + b with
+    # c = 1 ./ sqrt.(the in-degree weighted by the same w): both the messages and the normalisation depend on w
     wv = torch.rand(6, device="cuda", requires_grad=True)
-    l(g, gnn.colmajor(torch.rand(1, 3).cuda()), wv).sum().backward()
+    xv = gnn.colmajor(torch.rand(1, 3).cuda())
+    l(g, xv, wv).sum().backward()
     assert wv.grad.shape == (6,) and wv.grad.dtype == torch.float32
+    w64 = wv.detach().cpu().double().requires_grad_(True)
+    si, ti = torch.tensor(s) - 1, torch.tensor(t) - 1
+    c = 1 / torch.sqrt(torch.zeros(3, dtype=torch.float64).index_add(0, ti, w64))
+    xc = xv.detach().cpu().double()[0] * c
+    agg = torch.zeros(3, dtype=torch.float64).index_add(0, ti, w64 * xc[si]) * c
+    y64 = float(l.weight.detach()) * agg + float(l.bias.detach())
+    (rw,) = torch.autograd.grad(y64.sum(), w64)
+    assert rel(wv.grad.cpu().numpy(), rw.numpy()) < 1e-5
     # conv_weight = 0 => output == 0 == w*x exactly (conv.jl:55-65), on the reference's TEST_GRAPHS
     adj1 = np.array([[0, 1, 0, 1], [1, 0, 1, 0], [0, 1, 0, 1], [1, 0, 1, 0]])
     adj2 = np.array([[0, 0, 0, 1], [0, 0, 0, 0], [0, 0, 0, 1], [1, 0, 1, 0]])
@@ -516,19 +560,65 @@ def _gat_reference_bwd(oracle, s, t, n, Wx, el, er, dout, slope):
     return out, alpha, dWx, del_, der
 
 
-@pytest.mark.parametrize("Cc,H", [(64, 8), (16, 4), (8, 2), (4, 1), (32, 2), (128, 1), (128, 4), (2, 3), (1, 4), (16, 1), (32, 4), (64, 4),
-                                  (16, 8), (4, 32)])
+def _gat_del_f32(s, t, n, Wx, el, er, dout, slope):
+    """del of _gat_reference_bwd evaluated in float32 with sequential sums: the rounding any float32 evaluation of
+    the closed form meets"""
+    f = np.float32
+    z = el[t - 1] + er[s - 1]
+    u = np.where(z > 0, z, f(slope) * z)
+    mx = np.full((n, u.shape[1]), -np.inf, f)
+    np.maximum.at(mx, t - 1, u)
+    ex = np.exp(u - mx[t - 1])
+    S = np.zeros((n, u.shape[1]), f)
+    np.add.at(S, t - 1, ex)
+    alpha = ex / S[t - 1]
+    dalpha = (dout[t - 1] * Wx[s - 1]).sum(-1, dtype=f)
+    T = np.zeros_like(S)
+    np.add.at(T, t - 1, alpha * dalpha)
+    dz = alpha * (dalpha - T[t - 1]) * np.where(z > 0, f(1), f(slope))
+    del_ = np.zeros_like(S)
+    np.add.at(del_, t - 1, dz)
+    return del_
+
+
+GAT_SHAPES = [(64, 8), (16, 4), (8, 2), (4, 1), (32, 2), (128, 1), (128, 4), (2, 3), (1, 4), (16, 1), (32, 4), (64, 4), (16, 8),
+              (4, 32)]
+
+
+@pytest.mark.parametrize("Cc,H", GAT_SHAPES)
 def test_gat_aggregate_c_abi(graph_with_edges, oracle, gnn, Cc, H):
+    """fused GAT forward and pullback against the fp64 closed form, el and er ~ N(0, 1)"""
+    _check_gat_aggregate(graph_with_edges, oracle, gnn, Cc, H, "unit")
+
+
+@pytest.mark.parametrize("logits", ["sharp", "rising"])
+@pytest.mark.parametrize("Cc,H", GAT_SHAPES)
+def test_gat_aggregate_c_abi_sharp_and_rising_logits(graph_with_edges, oracle, gnn, Cc, H, logits):
+    """the same at the logits where an online softmax goes wrong: `sharp` el, er 25x N(0, 1), as trained attention is;
+    `rising` the edges stably sorted by source with el = 0, er[j] = 0.05 j, so the logits of a row increase in COO order
+    and the running max moves at every edge (j is the 1-based node id: no logit sits on the leaky-relu kink)"""
+    _check_gat_aggregate(graph_with_edges, oracle, gnn, Cc, H, logits)
+
+
+def _check_gat_aggregate(graph_with_edges, oracle, gnn, Cc, H, logits):
     name, s, t, n, g = graph_with_edges
     lib = gnn._lib.lib
     rng = np.random.default_rng(Cc * 10 + H)
-    s2, t2 = oracle.add_self_loops(s, t, n)
-    g2 = gnn.add_self_loops(g)
-    E2 = len(s2)
     Wx = rng.standard_normal((n, H, Cc)).astype(np.float32)
     el = rng.standard_normal((n, H)).astype(np.float32)
     er = rng.standard_normal((n, H)).astype(np.float32)
     dout = rng.standard_normal((n, H, Cc)).astype(np.float32)
+    if logits == "sharp":
+        el, er = 25 * el, 25 * er
+    elif logits == "rising":
+        order = np.argsort(s, kind="stable")
+        s, t = s[order], t[order]
+        g = fixture_plan(gnn, name, s, t, n)
+        el = np.zeros((n, H), np.float32)
+        er = np.repeat((0.05 * np.arange(1, n + 1, dtype=np.float32))[:, None], H, axis=1)     # every z > 0
+    s2, t2 = oracle.add_self_loops(s, t, n)
+    g2 = gnn.add_self_loops(g)
+    E2 = len(s2)
     slope = 0.2
     dev = lambda a: torch.as_tensor(a).cuda().contiguous()
     Wx_d, el_d, er_d, do_d = dev(Wx), dev(el), dev(er), dev(dout)
@@ -550,7 +640,18 @@ def test_gat_aggregate_c_abi(graph_with_edges, oracle, gnn, Cc, H):
     scale = np.linalg.norm(dWx_ref) / np.sqrt(dWx_ref.size) * np.sqrt(Cc)      # dz is a difference of O(1) terms
     assert np.abs(del_.cpu().numpy() - del_ref).max() < 2e-4 * max(scale, 1)
     assert np.abs(der.cpu().numpy() - der_ref).max() < 2e-4 * max(scale, 1)
-    assert rel(del_.cpu().numpy(), del_ref) < 2e-4 and rel(der.cpu().numpy(), der_ref) < 2e-4
+    if logits == "unit":
+        assert rel(del_.cpu().numpy(), del_ref) < 2e-4 and rel(der.cpu().numpy(), der_ref) < 2e-4
+    else:
+        assert rel(der.cpu().numpy(), der_ref) < 2e-4
+        # del_i sums dz = α (dα - Σ α dα) over row i.  With every z > 0 (`rising`) a shift of el moves all logits of the
+        # row alike and the softmax cancels it: del vanishes identically, which the max-abs bar above checks.  With
+        # sharp attention α is nearly one-hot, del falls far below the float32 rounding of the O(1) terms it is a
+        # difference of, and even the float32 evaluation of the closed form misses 2e-4 normwise: the bar is 2e-4 or
+        # 4x the error of that evaluation, whichever is larger
+        if logits == "sharp":
+            f32_err = rel(_gat_del_f32(s2, t2, n, Wx, el, er, dout, slope), del_ref)
+            assert rel(del_.cpu().numpy(), del_ref) < max(2e-4, 4 * f32_err)
 
 
 def test_gat_unsupported_shape_is_loud(gnn):
@@ -946,6 +1047,41 @@ def test_at_scale_gat_layer_against_the_oracle(gnn, oracle):
     o, _ = oracle.gat_aggregate(s2, t2, n, Wx, np.ascontiguousarray(a.T))
     ref = np.maximum(o.reshape(n, D) + layer.bias.detach().cpu().numpy(), 0)
     assert rel(np_rows(y), ref) < 1e-5
+    # the pullback (dx, dW, da, db) at a size whose fp64 host autograd stays within a few GB, hub rows longer than the
+    # chunk in both plans, against torch autograd of the layer formula in fp64 (as tests/test_layers.py _gat_reference)
+    n, E = 20_000, 200_000
+    s, t = oracle.rmat(n, E, 17)
+    s2, t2 = oracle.add_self_loops(s, t, n)
+    assert np.bincount(t2 - 1).max() > 128 and np.bincount(s2 - 1).max() > 128
+    g = gnn.GNNGraph(s, t, num_nodes=n).cuda()
+    layer = gnn.GATConv(D, Cc, torch.relu, heads=H, device="cuda")
+    with torch.no_grad():
+        layer.bias.normal_()
+    x = rng.standard_normal((n, D)).astype(np.float32)
+    dy = rng.standard_normal((n, D)).astype(np.float32)
+    xt = jl(x).requires_grad_(True)
+    y = layer(g, xt)
+    y.backward(jl(dy))
+    F64 = torch.float64
+    x64 = torch.as_tensor(x, dtype=F64).requires_grad_(True)
+    W64, a64, b64 = (p.detach().cpu().to(F64).requires_grad_(True) for p in (layer.dense_x.weight, layer.a, layer.bias))
+    si, ti = torch.as_tensor(s2 - 1), torch.as_tensor(t2 - 1)
+    Wx = (x64 @ W64.t()).reshape(n, H, Cc)
+    logit = (Wx * a64[:Cc].t()).sum(-1)[ti] + (Wx * a64[Cc:].t()).sum(-1)[si]         # rows 1..C of a pair with the target
+    z = torch.nn.functional.leaky_relu(logit, 0.2)
+    mx = torch.full((n, H), -float("inf"), dtype=F64).scatter_reduce(0, ti[:, None].expand_as(z), z.detach(), "amax")
+    ez = torch.exp(z - mx[ti])
+    alpha = ez / torch.zeros(n, H, dtype=F64).index_add(0, ti, ez)[ti]
+    pre = torch.zeros(n, H, Cc, dtype=F64).index_add(0, ti, alpha[:, :, None] * Wx[si]).reshape(n, D) + b64
+    yg = np_rows(y)
+    assert rel(yg, np.maximum(pre.detach().numpy(), 0)) < 1e-5
+    assert int(((yg > 0) != (pre.detach().numpy() > 0)).sum()) < 1e-6 * yg.size
+    cot = torch.as_tensor(dy, dtype=F64) * torch.as_tensor(yg > 0)          # relu' on the mask of the output it belongs to
+    gx, gW, ga, gb = torch.autograd.grad((pre * cot).sum(), [x64, W64, a64, b64])
+    del Wx, logit, z, ez, alpha, pre
+    errs = dict(dx=rel(np_rows(xt.grad), gx.numpy()), dW=rel(layer.dense_x.weight.grad.cpu().numpy(), gW.numpy()),
+                da=rel(layer.a.grad.cpu().numpy(), ga.numpy()), db=rel(layer.bias.grad.cpu().numpy(), gb.numpy()))
+    assert all(v < 1e-5 for v in errs.values()), errs
 
 
 def test_at_scale_sage_on_batched_graphs_against_the_oracle(gnn, oracle):

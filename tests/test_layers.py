@@ -104,12 +104,47 @@ def r64(a, requires_grad=False):
     return x.requires_grad_(requires_grad) if requires_grad else x
 
 
-def grads_match(gnn, out, x, ref_out, ref_x, tol=2e-5):
-    """same random cotangent through both graphs; x Julia-shaped (D.., N), ref_x rows (N, ..D)"""
+class Twins:
+    """float64 twins, requiring grad, of every parameter the holders own (named_parameters() of a module, the tensor
+    fields of an NT that require grad).  P(param) is the twin the reference formula uses; P.pairs lists the
+    (parameter, twin) pairs for grads_match."""
+
+    def __init__(self, *holders):
+        self._twin, self.pairs = {}, []
+        for h in holders:
+            ps = ([p for _, p in h.named_parameters()] if isinstance(h, torch.nn.Module) else
+                  [v for v in vars(h).values() if isinstance(v, torch.Tensor) and v.requires_grad])
+            for p in ps:
+                if id(p) not in self._twin:
+                    self._twin[id(p)] = p64(p).requires_grad_(True)
+                    self.pairs.append((p, self._twin[id(p)]))
+
+    def __call__(self, p):
+        return self._twin[id(p)]
+
+
+def grads_match(gnn, out, ref_out, pairs, tol=2e-5):
+    """the same seeded cotangent through both graphs, then the gradient of every (mirror leaf, float64 reference leaf)
+    pair compared.  A Julia-shaped mirror leaf (D.., N) meets its reference in rows (N, ..D); a leaf of the
+    reference's own shape (a parameter, an edge-weight vector) is compared as it is.  A reference leaf None marks a
+    gradient that vanishes identically (a shift the softmax cancels): its norm must stay within tol of the largest
+    reference gradient's."""
     g = torch.randn(ref_out.shape, dtype=F64, generator=torch.Generator().manual_seed(7))
-    (gx,) = torch.autograd.grad((gnn.rows(out).double() * g.to(out.device)).sum(), x, retain_graph=True)
-    (rx,) = torch.autograd.grad((ref_out * g).sum(), ref_x, retain_graph=True)
-    assert rel(gnn.rows(gx), rx) < tol
+    got = torch.autograd.grad((gnn.rows(out).double() * g.to(out.device)).sum(), [m for m, _ in pairs],
+                              retain_graph=True)
+    want = torch.autograd.grad((ref_out * g).sum(), [r for _, r in pairs if r is not None], retain_graph=True)
+    scale = max(float(_c64(b).norm()) for b in want)
+    want = iter(want)
+    for i, (a, (_, r)) in enumerate(zip(got, pairs)):
+        if r is None:
+            assert float(_c64(a).norm()) < tol * scale, f"gradient of input {i} should vanish"
+            continue
+        b = next(want)
+        if a.shape != b.shape:
+            a = gnn.rows(a)
+        assert a.shape == b.shape
+        err = rel(a, b)
+        assert err < tol, f"gradient of input {i} {tuple(b.shape)}: {err:.2e}"
 
 
 # ------------------------------------------------------------------------------------------------ pin the fake
@@ -180,46 +215,60 @@ def setp(rng, param):
         param.copy_(torch.as_tensor(rng.standard_normal(tuple(param.shape)), dtype=torch.float32))
 
 
-@pytest.mark.parametrize("case", ["plain", "no_loops", "edge_weight", "use_edge_weight", "norm_fn", "wide_to_narrow",
-                                  "conv_weight"])
+GRAPH_WEIGHTED = ("use_edge_weight", "weighted_norm_fn")      # graph weights (requiring grad) and use_edge_weight
+
+
+@pytest.mark.parametrize("case", ["plain", "no_loops", "edge_weight", "use_edge_weight", "norm_fn", "weighted_norm_fn",
+                                  "wide_to_narrow", "conv_weight"])
 def test_gcn_conv_branches(gnn, be, case):
+    """every branch of gcn_conv; gradients of x, the NT's weight and bias, and the edge weights the case uses"""
     rng = np.random.default_rng(1)
     dev = be.dev
-    g, R, s, t = make_graph(gnn, rng, dev, weights=(case == "use_edge_weight"))
+    g, R, s, t = make_graph(gnn, rng, dev, weights=(case in GRAPH_WEIGHTED))
     Din, Dout = (12, 5) if case == "wide_to_narrow" else (5, 8)
     x = rng.standard_normal((R.n, Din))
     W = rng.standard_normal((Dout, Din)) / 3
     b = rng.standard_normal(Dout)
-    l = NT(weight=f32(W, dev), bias=f32(b, dev), σ=torch.tanh,
-           add_self_loops=case != "no_loops", use_edge_weight=case == "use_edge_weight")
+    l = NT(weight=f32(W, dev).requires_grad_(case != "conv_weight"), bias=f32(b, dev).requires_grad_(True),
+           σ=torch.tanh, add_self_loops=case != "no_loops", use_edge_weight=case in GRAPH_WEIGHTED)
+    P = Twins(l)
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
+    pairs = [(xt, xr)] + P.pairs
     kw, w_ref, Rl = {}, None, (R.with_loops() if l.add_self_loops else R)
     ones = torch.ones(R.n if l.add_self_loops else 0, dtype=F64)
     if case == "edge_weight":
         ew = rng.uniform(0.5, 1.5, len(s))
-        kw["edge_weight"] = f32(ew, dev)
-        w_ref = torch.cat([p64(kw["edge_weight"]), ones])
-    if case == "use_edge_weight":
-        w_ref = torch.cat([p64(g.w), ones])
-    Wr = r64(W)
+        kw["edge_weight"] = f32(ew, dev).requires_grad_(True)
+        pairs.append((kw["edge_weight"], r64(ew, True)))
+        w_ref = torch.cat([pairs[-1][1], ones])
+    if case in GRAPH_WEIGHTED:                            # GNNGraph keeps the weight tensor it is given
+        g.w.requires_grad_(True)
+        pairs.append((g.w, p64(g.w).requires_grad_(True)))
+        w_ref = torch.cat([pairs[-1][1], ones])
+    Wr = P(l.weight) if case != "conv_weight" else None
     if case == "conv_weight":
         W2 = rng.standard_normal((Dout, Din)) / 3
-        kw["conv_weight"] = f32(W2, dev)
-        Wr = r64(W2)
-    if case == "norm_fn":
+        kw["conv_weight"] = f32(W2, dev).requires_grad_(True)
+        Wr = r64(W2, True)
+        pairs.append((kw["conv_weight"], Wr))
+    if case in ("norm_fn", "weighted_norm_fn"):           # a custom norm on the (weighted) in-degree
         kw["norm_fn"] = lambda d: 1.0 / (1.0 + d)
-        c = 1.0 / (1.0 + Rl.indeg())
-        agg = Rl.propagate(xr * c[:, None]) * c[:, None]
+        c = 1.0 / (1.0 + Rl.indeg(w_ref))
+        agg = Rl.propagate(xr * c[:, None], w=w_ref) * c[:, None]
     else:
         agg = Rl.gcn(xr, w_ref)
-    ref = torch.tanh(agg @ Wr.t() + r64(b))
+    ref = torch.tanh(agg @ Wr.t() + P(l.bias))
     out = gnn.gcn_conv(l, g, xt, **kw)
     assert out.shape == (Dout, R.n)
     assert rel(gnn.rows(out), ref) < 2e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+    n_fwd = None if be.calls is None else len(be.calls)
+    grads_match(gnn, out, ref, pairs, 2e-5 * be.tol)
     if be.calls is not None:
+        fwd, bwd = be.calls[:n_fwd], be.calls[n_fwd:]
         assert saw(be, "gnnb_gcn_propagate") == (case in ("plain", "no_loops", "wide_to_narrow", "conv_weight"))
-        assert not saw(be, "gnnb_gather") and not saw(be, "gnnb_scatter")            # never the (D,E) intermediate
+        assert "gnnb_gather" not in fwd and not saw(be, "gnnb_scatter")              # never the (D,E) intermediate
+        # the only gather is the weighted degree's pullback, one (1, E) row per weighted call
+        assert bwd.count("gnnb_gather") == (1 if case in ("edge_weight",) + GRAPH_WEIGHTED else 0)
 
 
 def test_gcn_conv_argument_errors(gnn, be):
@@ -249,23 +298,26 @@ def test_sage_graph_gin_layers(gnn, be, aggr):
     # SAGEConv: σ(W [x_i ; aggr_j x_j] + b)
     layer = gnn.SAGEConv(Din, Dout, torch.relu, aggr=op, device=dev)
     setp(rng, layer.bias)
+    P = Twins(layer)
     out = layer(g, xt)
-    ref = torch.relu(torch.cat([xr, m], dim=1) @ p64(layer.weight).t() + p64(layer.bias))
+    ref = torch.relu(torch.cat([xr, m], dim=1) @ P(layer.weight).t() + P(layer.bias))
     assert rel(gnn.rows(out), ref) < 2e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs, 2e-5 * be.tol)
     # GraphConv: σ(W1 x_i + W2 aggr_j x_j + b)
     layer = gnn.GraphConv(Din, Dout, torch.tanh, aggr=op, device=dev)
     setp(rng, layer.bias)
+    P = Twins(layer)
     out = layer(g, xt)
-    ref = torch.tanh(xr @ p64(layer.weight1).t() + m @ p64(layer.weight2).t() + p64(layer.bias))
+    ref = torch.tanh(xr @ P(layer.weight1).t() + m @ P(layer.weight2).t() + P(layer.bias))
     assert rel(gnn.rows(out), ref) < 2e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs, 2e-5 * be.tol)
     # GINConv: nn((1 + ϵ) x_i + aggr_j x_j)
     layer = gnn.GINConv(lambda v: v ** 2, 0.3, aggr=op)
+    assert not list(layer.parameters())
     out = layer(g, xt)
     ref = (1.3 * xr + m) ** 2
     assert rel(gnn.rows(out), ref) < 2e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr)], 2e-5 * be.tol)
     if be.calls is not None:
         assert set(be.calls) <= {"gnnb_graph_create", "gnnb_propagate", "gnnb_propagate_bwd"}
 
@@ -289,22 +341,17 @@ def test_gat_conv_fused_and_composed(gnn, be, heads, concat, fused):
     Din, C_ = 5, 4
     layer = gnn.GATConv(Din, C_, heads=heads, concat=concat, device=dev)
     setp(rng, layer.bias)
+    P = Twins(layer)
     x = rng.standard_normal((R.n, Din))
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
     out = layer(g, xt, fused=fused)
     Rl = R.with_loops()
-    bias = p64(layer.bias)
-    ref = _gat_reference(Rl, xr, p64(layer.dense_x.weight), p64(layer.a), C_, heads, 0.2, concat, bias)
+    ref = _gat_reference(Rl, xr, P(layer.dense_x.weight), P(layer.a), C_, heads, 0.2, concat, P(layer.bias))
     assert out.shape == ((C_ * heads if concat else C_), R.n)
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
-    # parameter gradients through the fused pullback (a, W) against autograd of the formula
-    ga, gw = torch.autograd.grad(gnn.rows(out).double().sum(), [layer.a, layer.dense_x.weight])
-    a64 = p64(layer.a).requires_grad_(True)
-    W64 = p64(layer.dense_x.weight).requires_grad_(True)
-    r2 = _gat_reference(Rl, xr.detach(), W64, a64, C_, heads, 0.2, concat, bias)
-    ra, rw = torch.autograd.grad(r2.sum(), [a64, W64])
-    assert rel(ga, ra) < 2e-5 * be.tol and rel(gw, rw) < 2e-5 * be.tol
+    # x and every parameter (W, a, bias) through the fused pullback against autograd of the formula
+    assert {id(m) for m, _ in P.pairs} == {id(layer.a), id(layer.dense_x.weight), id(layer.bias)}
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs, 2e-5 * be.tol)
     if be.calls is not None:
         assert saw(be, "gnnb_gat_aggregate") == fused
         assert saw(be, "gnnb_gather") == (not fused)
@@ -347,16 +394,18 @@ def test_sg_and_tag_conv(gnn, be, weighted):
     Din, Dout, k = 7, 4, 3
     x = rng.standard_normal((R.n, Din))
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
-    ew = f32(rng.uniform(0.5, 1.5, len(s)), dev) if weighted else None
+    ew = f32(rng.uniform(0.5, 1.5, len(s)), dev).requires_grad_(True) if weighted else None
+    ew64 = p64(ew).requires_grad_(True) if weighted else None
     Rl = R.with_loops()
-    w_ref = torch.cat([p64(ew), torch.ones(R.n, dtype=F64)]) if weighted else None
+    w_ref = torch.cat([ew64, torch.ones(R.n, dtype=F64)]) if weighted else None
     hops = [xr]
     for _ in range(k):
         hops.append(Rl.gcn(hops[-1], w_ref))
     for cls, fn in ((gnn.SGConv, gnn.sg_conv), (gnn.TAGConv, gnn.tag_conv)):
         layer = cls(Din, Dout, k, device=dev)
         setp(rng, layer.bias)
-        W, b = p64(layer.weight), p64(layer.bias)
+        P = Twins(layer)
+        W, b = P(layer.weight), P(layer.bias)
         out = layer(g, xt, ew)
         if cls is gnn.SGConv:
             ref = hops[k] @ W.t() + b                                     # W Â^k x + b
@@ -368,7 +417,7 @@ def test_sg_and_tag_conv(gnn, be, weighted):
             ref = ref + b
         assert out.shape == (Dout, R.n)
         assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-        grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+        grads_match(gnn, out, ref, [(xt, xr)] + P.pairs + ([(ew, ew64)] if weighted else []), 2e-5 * be.tol)
         assert rel(gnn.rows(fn(layer, g, xt, ew)), ref) < 3e-6 * be.tol
     if not weighted:   # sgc_conv (conv.jl:407-448) is the same function under its older name
         assert rel(gnn.sgc_conv(layer, g, xt), gnn.sg_conv(layer, g, xt)) < 1e-6
@@ -385,10 +434,11 @@ def test_gated_graph_conv(gnn, be):
     dims, L, Din = 6, 3, 4
     layer = gnn.GatedGraphConv(dims, L, aggr=gnn.mean, device=dev)
     setp(rng, layer.gru.b)
+    P = Twins(layer)
     x = rng.standard_normal((R.n, Din))
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
     out = layer(g, xt)
-    Wi, Wh, b, Wl = (p64(p) for p in (layer.gru.Wi, layer.gru.Wh, layer.gru.b, layer.weight))
+    Wi, Wh, b, Wl = (P(p) for p in (layer.gru.Wi, layer.gru.Wh, layer.gru.b, layer.weight))
     h = torch.cat([xr, torch.zeros(R.n, dims - Din, dtype=F64)], dim=1)
     for i in range(L):
         m = R.propagate(h @ Wl[:, :, i].t(), "mean")
@@ -399,7 +449,7 @@ def test_gated_graph_conv(gnn, be):
         h = (1 - z) * hc + z * h
     assert out.shape == (dims, R.n)
     assert rel(gnn.rows(out), h) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, h, xr, 2e-5 * be.tol)
+    grads_match(gnn, out, h, [(xt, xr)] + P.pairs, 2e-5 * be.tol)
     with pytest.raises(AssertionError, match="less or equal"):
         layer(g, jl(gnn, rng.standard_normal((R.n, dims + 1)), dev))
 
@@ -414,24 +464,31 @@ def test_gatv2_conv(gnn, be, heads, concat, ein):
                           add_self_loops=(ein == 0), device=dev)
     setp(rng, layer.bias)
     setp(rng, layer.dense_i.bias)
+    P = Twins(layer)
     x = rng.standard_normal((R.n, Din))
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
-    e = jl(gnn, rng.standard_normal((len(s), ein)), dev) if ein else None
+    pairs = [(xt, xr)] + P.pairs
+    if ein:
+        ea = rng.standard_normal((len(s), ein))
+        e, er = jl(gnn, ea, dev, True), r64(ea, True)
+        pairs.append((e, er))
+    else:
+        e = None
     out = layer(g, xt, e)
     Rl = R if ein else R.with_loops()
-    Wi = (xr @ p64(layer.dense_i.weight).t() + p64(layer.dense_i.bias)).reshape(R.n, heads, C_)
-    Wj = (xr @ p64(layer.dense_j.weight).t()).reshape(R.n, heads, C_)
+    Wi = (xr @ P(layer.dense_i.weight).t() + P(layer.dense_i.bias)).reshape(R.n, heads, C_)
+    Wj = (xr @ P(layer.dense_j.weight).t()).reshape(R.n, heads, C_)
     z = Wi[Rl.t] + Wj[Rl.s]
     if ein:
-        z = z + (p64(gnn.rows(e)) @ p64(layer.dense_e.weight).t()).reshape(-1, heads, C_)
-    logit = (torch.nn.functional.leaky_relu(z, 0.2) * p64(layer.a).t()).sum(-1)       # (E, H)
+        z = z + (er @ P(layer.dense_e.weight).t()).reshape(-1, heads, C_)
+    logit = (torch.nn.functional.leaky_relu(z, 0.2) * P(layer.a).t()).sum(-1)       # (E, H)
     alpha = Rl.softmax(logit)
     o = Rl.scatter_sum(alpha[:, :, None] * Wj[Rl.s])
     o = o.reshape(R.n, heads * C_) if concat else o.mean(dim=1)
-    ref = torch.tanh(o + p64(layer.bias))
+    ref = torch.tanh(o + P(layer.bias))
     assert out.shape == ((C_ * heads if concat else C_), R.n)
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+    grads_match(gnn, out, ref, pairs, 2e-5 * be.tol)
     if not ein:
         with pytest.raises(AssertionError, match="not specified in the layer constructor"):
             layer(g, xt, jl(gnn, rng.standard_normal((len(s), 2)), dev))
@@ -454,22 +511,38 @@ def test_transformer_conv(gnn, be, cfg):
     for d in (layer.W1, layer.W2, layer.W3, layer.W4, layer.W6):
         if d is not None and d.bias is not None:
             setp(rng, d.bias)
+    P = Twins(layer)
     x = rng.standard_normal((R.n, Din))
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
-    e = jl(gnn, rng.standard_normal((len(s), ein)), dev) if ein else None
+    # gradients that vanish identically: the key bias adds q_i·b to every logit of row i, which the softmax cancels;
+    # a batch norm removes per-channel constants ahead of it (root and value biases before BN1 — every node has an
+    # in-edge and the α of a row sum to 1 — and the last feed-forward bias before BN2)
+    vanish = [layer.W4.bias]
+    if layer.BN1 is not None:
+        vanish += [layer.W1.bias, layer.W2.bias]
+    if layer.BN2 is not None:
+        vanish += [layer.FF[1].bias]
+    vanish = {id(p) for p in vanish if p is not None}
+    pairs = [(xt, xr)] + [(m, None if id(m) in vanish else r) for m, r in P.pairs]
+    if ein:
+        ea = rng.standard_normal((len(s), ein))
+        e, er = jl(gnn, ea, dev, True), r64(ea, True)
+        pairs.append((e, er))
+    else:
+        e = None
     out = layer(g, xt, e)
     Rl = R.with_loops() if cfg.get("add_self_loops") else R
 
     def dense(d, v):
-        y = v @ p64(d.weight).t()
-        return y if d.bias is None else y + p64(d.bias)
+        y = v @ P(d.weight).t()
+        return y if d.bias is None else y + P(d.bias)
 
     q = dense(layer.W3, xr).reshape(R.n, heads, C_)
     k = dense(layer.W4, xr).reshape(R.n, heads, C_)
     v = dense(layer.W2, xr).reshape(R.n, heads, C_)
     ke, ve = k[Rl.s], v[Rl.s]
     if ein:
-        ee = dense(layer.W6, p64(gnn.rows(e))).reshape(-1, heads, C_)
+        ee = dense(layer.W6, er).reshape(-1, heads, C_)
         ke, ve = ke + ee, ve + ee
     alpha = Rl.softmax((q[Rl.t] * ke).sum(-1) / np.sqrt(C_))                 # (E, H)
     h = Rl.scatter_sum(alpha[:, :, None] * ve)
@@ -477,28 +550,28 @@ def test_transformer_conv(gnn, be, cfg):
     if layer.W1 is not None:
         r = dense(layer.W1, xr)
         if layer.W5 is not None:
-            beta = torch.sigmoid(torch.cat([h, r, h - r], dim=1) @ p64(layer.W5.weight).t())
+            beta = torch.sigmoid(torch.cat([h, r, h - r], dim=1) @ P(layer.W5.weight).t())
             h = beta * r + (1 - beta) * h
         else:
             h = h + r
     if cfg.get("skip_connection"):
         h = h + xr
 
-    def bn(v):      # training-mode batch norm over nodes, γ = 1, β = 0
-        return (v - v.mean(0)) / torch.sqrt(v.var(0, unbiased=False) + 1e-5)
+    def bn(B, v):   # training-mode batch norm over nodes (γ = 1, β = 0 as initialised, but differentiated)
+        return (v - v.mean(0)) / torch.sqrt(v.var(0, unbiased=False) + 1e-5) * P(B.bn.weight) + P(B.bn.bias)
 
     if layer.BN1 is not None:
-        h = bn(h)
+        h = bn(layer.BN1, h)
     if layer.FF is not None:
         h1 = h
         h = dense(layer.FF[1], torch.relu(dense(layer.FF[0], h)))
         if cfg.get("skip_connection"):
             h = h + h1
         if layer.BN2 is not None:
-            h = bn(h)
+            h = bn(layer.BN2, h)
     assert out.shape == ((C_ * heads if concat else C_), R.n)
     assert rel(gnn.rows(out), h) < 5e-6 * be.tol
-    grads_match(gnn, out, xt, h, xr, tol=5e-5 * be.tol)
+    grads_match(gnn, out, h, pairs, tol=5e-5 * be.tol)
 
 
 def test_agnn_conv(gnn, be):
@@ -508,13 +581,14 @@ def test_agnn_conv(gnn, be):
     x = rng.standard_normal((R.n, 6))
     xt, xr = jl(gnn, x, dev, True), r64(x, True)
     layer = gnn.AGNNConv(init_beta=1.7, device=dev)
+    P = Twins(layer)
     out = layer(g, xt)
     Rl = R.with_loops()
     xn = xr / xr.norm(dim=1, keepdim=True)
-    alpha = Rl.softmax(1.7 * (xn[Rl.t] * xn[Rl.s]).sum(-1, keepdim=True))
+    alpha = Rl.softmax(P(layer.beta) * (xn[Rl.t] * xn[Rl.s]).sum(-1, keepdim=True))
     ref = Rl.scatter_sum(alpha * xr[Rl.s])
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 2e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs, 2e-5 * be.tol)
     (gb,) = torch.autograd.grad(out.sum(), layer.beta)
     assert torch.isfinite(gb).all()
 

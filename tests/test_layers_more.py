@@ -1,6 +1,7 @@
 """The remaining functional layers (graphneuralnetworks.jl_b200/layers_more.py: cheb, edge, nn, res-gated, cg, megnet,
 gmm, egnn, d conv) against float64 formulas written with dense adjacency matrices / explicit per-edge loops — no code
-shared with the mirror.  Forward and input gradients.  Back ends: the CPU test double and (under -m gpu) CUDA."""
+shared with the mirror.  Forward, and the gradients of the inputs, of every parameter and of the edge weights and
+features each case uses.  Back ends: the CPU test double and (under -m gpu) CUDA."""
 import operator
 
 import numpy as np
@@ -45,24 +46,52 @@ def jl(gnn, a, dev, grad=False):
     return x.requires_grad_(True) if grad else x
 
 
-def grads_match(gnn, out, x, ref_out, ref_x, tol):
+class Twins:
+    """float64 twins, requiring grad, of every parameter of the modules: P(param) is the twin the reference formula
+    uses, P.pairs(*modules) the (parameter, twin) pairs of those modules (all of them by default) for grads_match."""
+
+    def __init__(self, *modules):
+        self._twin, self._all = {}, []
+        for m in modules:
+            for _, p in m.named_parameters():
+                if id(p) not in self._twin:
+                    self._twin[id(p)] = c64(p).requires_grad_(True)
+                    self._all.append(p)
+
+    def __call__(self, p):
+        return self._twin[id(p)]
+
+    def pairs(self, *modules):
+        ps = [p for m in modules for _, p in m.named_parameters()] if modules else self._all
+        return [(p, self._twin[id(p)]) for p in ps]
+
+
+def grads_match(gnn, out, ref_out, pairs, tol):
+    """the same seeded cotangent through both graphs, then the gradient of every (mirror leaf, float64 reference leaf)
+    pair compared; a Julia-shaped mirror leaf (D, N) / (D, E) meets its reference in rows"""
     cot = torch.randn(ref_out.shape, dtype=F64, generator=torch.Generator().manual_seed(3))
-    (gx,) = torch.autograd.grad((gnn.rows(out).double() * cot.to(out.device)).sum(), x, retain_graph=True)
-    (rx,) = torch.autograd.grad((ref_out * cot).sum(), ref_x, retain_graph=True)
-    assert rel(gnn.rows(gx), rx) < tol
+    got = torch.autograd.grad((gnn.rows(out).double() * cot.to(out.device)).sum(), [m for m, _ in pairs],
+                              retain_graph=True)
+    want = torch.autograd.grad((ref_out * cot).sum(), [r for _, r in pairs], retain_graph=True)
+    for i, (a, b) in enumerate(zip(got, want)):
+        if a.shape != b.shape:
+            a = gnn.rows(a)
+        assert a.shape == b.shape
+        err = rel(a, b)
+        assert err < tol, f"gradient of input {i} {tuple(b.shape)}: {err:.2e}"
 
 
-def dense(d, v):
-    y = v @ c64(d.weight).t()
+def dense(d, v, P):
+    y = v @ P(d.weight).t()
     if d.bias is not None:
-        y = y + c64(d.bias)
+        y = y + P(d.bias)
     sig = getattr(d, "sigma", None)
     return sig(y) if sig is not None else y
 
 
-def seq(chain, v):
+def seq(chain, v, P):
     for d in chain:
-        v = dense(d, v)
+        v = dense(d, v, P)
     return v
 
 
@@ -84,22 +113,25 @@ def test_cheb_conv(gnn, be, k, weights):
     n, Din, Dout = g.num_nodes, 4, 3
     layer = gnn.ChebConv(Din, Dout, k, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     x = rng.standard_normal((n, Din))
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
     out = layer(g, xt)
     dinv = torch.diag(1 / A.sum(1).sqrt())
     L = torch.eye(n, dtype=F64) - dinv @ A @ dinv
     Lt = 2 / torch.linalg.eigvalsh((L + L.t()) / 2)[-1] * L - torch.eye(n, dtype=F64)
-    W = c64(layer.weight)
+    W = P(layer.weight)
     Zp, Z = xr, Lt.t() @ xr                                                       # rows form of X * L̃
     Y = Zp @ W[:, :, 0].t() + Z @ W[:, :, 1].t()
     for i in range(2, k):
         Z, Zp = 2 * Lt.t() @ Z - Zp, Z
         Y = Y + Z @ W[:, :, i].t()
-    ref = Y + c64(layer.bias)
+    ref = Y + P(layer.bias)
     assert out.shape == (Dout, n)
     assert rel(gnn.rows(out), ref) < 2e-5 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 1e-4 * be.tol)
+    # x and the parameters; edge weights reach L̃ through an iterative λmax estimate (KrylovKit there, Lanczos here)
+    # whose derivative neither side defines, so their gradient is not compared
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs(), 1e-4 * be.tol)
     with pytest.raises(AssertionError, match="input channel size"):
         layer(g, jl(gnn, rng.standard_normal((n, Din + 1)), be.dev))
 
@@ -111,17 +143,18 @@ def test_edge_conv(gnn, be, aggr):
     n, Din, Dout = g.num_nodes, 4, 5                      # message, torch's amax splits the gradient: not comparable
     nn = gnn.layers._DenseAct(2 * Din, Dout, torch.tanh, device=be.dev)
     randomise_biases(rng, nn)
+    P = Twins(nn)
     layer = gnn.EdgeConv(nn, aggr=max if aggr == "max" else operator.add)
     x = rng.standard_normal((n, Din))
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
     out = layer(g, xt)
-    m = dense(nn, torch.cat([xr[t], xr[s] - xr[t]], dim=1))
+    m = dense(nn, torch.cat([xr[t], xr[s] - xr[t]], dim=1), P)
     if aggr == "+":
         ref = scatter_sum(t, m, n)
     else:
         ref = torch.full((n, Dout), -float("inf"), dtype=F64).scatter_reduce(0, t[:, None].expand_as(m), m, "amax")
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 3e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs(), 3e-5 * be.tol)
 
 
 def test_nn_conv(gnn, be):
@@ -132,15 +165,18 @@ def test_nn_conv(gnn, be):
     randomise_biases(rng, nn)
     layer = gnn.NNConv(Din, Dout, nn, torch.tanh, aggr=gnn.mean, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     x, e = rng.standard_normal((n, Din)), rng.standard_normal((E, De))
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
-    out = layer(g, xt, jl(gnn, e, be.dev))
-    We = dense(nn, c64(e))                                                        # (E, Dout*Din), Julia column o + Dout*i
+    et, er = jl(gnn, e, be.dev, True), c64(e).requires_grad_(True)
+    out = layer(g, xt, et)
+    We = dense(nn, er, P)                                                         # (E, Dout*Din), Julia column o + Dout*i
     m = torch.stack([sum(We[:, o + Dout * i] * xr[s, i] for i in range(Din)) for o in range(Dout)], dim=1)
     cnt = torch.bincount(t, minlength=n).clamp(min=1).double()
-    ref = torch.tanh(xr @ c64(layer.weight).t() + scatter_sum(t, m, n) / cnt[:, None] + c64(layer.bias))
+    ref = torch.tanh(xr @ P(layer.weight).t() + scatter_sum(t, m, n) / cnt[:, None] + P(layer.bias))
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 3e-5 * be.tol)
+    assert len(P.pairs()) == 4                                                    # nn's W, b and the layer's
+    grads_match(gnn, out, ref, [(xt, xr), (et, er)] + P.pairs(), 3e-5 * be.tol)
 
 
 def test_res_gated_and_cg_conv(gnn, be):
@@ -151,21 +187,28 @@ def test_res_gated_and_cg_conv(gnn, be):
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
     layer = gnn.ResGatedGraphConv(Din, Dout, torch.relu, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     out = layer(g, xt)
-    Aw, Bw, Uw, Vw = (c64(p) for p in (layer.A, layer.B, layer.U, layer.V))
+    Aw, Bw, Uw, Vw = (P(p) for p in (layer.A, layer.B, layer.U, layer.V))
     eta = torch.sigmoid((xr @ Aw.t())[t] + (xr @ Bw.t())[s])
-    ref = torch.relu(xr @ Uw.t() + scatter_sum(t, eta * (xr @ Vw.t())[s], n) + c64(layer.bias))
+    ref = torch.relu(xr @ Uw.t() + scatter_sum(t, eta * (xr @ Vw.t())[s], n) + P(layer.bias))
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 3e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr)] + P.pairs(), 3e-5 * be.tol)
     for ein, residual in ((De, True), (0, False)):
         layer = gnn.CGConv((Din, ein), Dout, torch.tanh, residual=residual, device=be.dev)
         randomise_biases(rng, layer)
-        et = jl(gnn, e, be.dev) if ein else None
+        P = Twins(layer)
+        pairs = [(xt, xr)] + P.pairs()
+        if ein:
+            et, er = jl(gnn, e, be.dev, True), c64(e).requires_grad_(True)
+            pairs.append((et, er))
+        else:
+            et = None
         out = layer(g, xt, et)
-        z = torch.cat([xr[t], xr[s]] + ([c64(e)] if ein else []), dim=1)
-        ref = scatter_sum(t, dense(layer.dense_f, z) * dense(layer.dense_s, z), n) + (xr if residual else 0)
+        z = torch.cat([xr[t], xr[s]] + ([er] if ein else []), dim=1)
+        ref = scatter_sum(t, dense(layer.dense_f, z, P) * dense(layer.dense_s, z, P), n) + (xr if residual else 0)
         assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-        grads_match(gnn, out, xt, ref, xr, 3e-5 * be.tol)
+        grads_match(gnn, out, ref, pairs, 3e-5 * be.tol)
     with pytest.raises(AssertionError):
         layer(g, xt, jl(gnn, e[:-1], be.dev))
 
@@ -176,15 +219,18 @@ def test_megnet_conv(gnn, be):
     n, E, Din, Dout = g.num_nodes, g.num_edges, 3, 5
     layer = gnn.MEGNetConv(Din, Dout, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     x, e = rng.standard_normal((n, Din)), rng.standard_normal((E, Din))
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
-    xbar, ebar = layer(g, xt, jl(gnn, e, be.dev))
-    eb = seq(layer.phi_e, torch.cat([xr[t], xr[s], c64(e)], dim=1))
+    et, er = jl(gnn, e, be.dev, True), c64(e).requires_grad_(True)
+    xbar, ebar = layer(g, xt, et)
+    eb = seq(layer.phi_e, torch.cat([xr[t], xr[s], er], dim=1), P)
     cnt = torch.bincount(t, minlength=n).clamp(min=1).double()
-    xb = seq(layer.phi_v, torch.cat([xr, scatter_sum(t, eb, n) / cnt[:, None]], dim=1))
+    xb = seq(layer.phi_v, torch.cat([xr, scatter_sum(t, eb, n) / cnt[:, None]], dim=1), P)
     assert xbar.shape == (Dout, n) and ebar.shape == (Dout, E)
     assert rel(gnn.rows(ebar), eb) < 3e-6 * be.tol and rel(gnn.rows(xbar), xb) < 3e-6 * be.tol
-    grads_match(gnn, xbar, xt, xb, xr, 3e-5 * be.tol)
+    grads_match(gnn, xbar, xb, [(xt, xr), (et, er)] + P.pairs(), 3e-5 * be.tol)
+    grads_match(gnn, ebar, eb, [(xt, xr), (et, er)] + P.pairs(layer.phi_e), 3e-5 * be.tol)
 
 
 @pytest.mark.parametrize("K,residual", [(1, False), (3, True)])
@@ -195,18 +241,20 @@ def test_gmm_conv(gnn, be, K, residual):
     Dout = Din if residual else 3
     layer = gnn.GMMConv((Din, ein), Dout, torch.tanh, K=K, residual=residual, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     x, e = rng.standard_normal((n, Din)), rng.uniform(-1, 1, (E, ein))
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
-    out = layer(g, xt, jl(gnn, e, be.dev))
-    mu, si = c64(layer.mu), c64(layer.sigma_inv)                                  # (ein, K)
-    wk = torch.exp((((c64(e)[:, :, None] - mu[None]) ** 2) / 2 * si[None] ** 2).sum(1))       # (E, K)
-    xk = (xr @ c64(layer.dense_x.weight).t()).reshape(n, K, Dout)                 # Julia (out, K, N) -> rows (N, K, out)
+    et, er = jl(gnn, e, be.dev, True), c64(e).requires_grad_(True)
+    out = layer(g, xt, et)
+    mu, si = P(layer.mu), P(layer.sigma_inv)                                      # (ein, K)
+    wk = torch.exp((((er[:, :, None] - mu[None]) ** 2) / 2 * si[None] ** 2).sum(1))            # (E, K)
+    xk = (xr @ P(layer.dense_x.weight).t()).reshape(n, K, Dout)                   # Julia (out, K, N) -> rows (N, K, out)
     cnt = torch.bincount(t, minlength=n).clamp(min=1).double()
     m = scatter_sum(t, wk[:, :, None] * xk[s], n) / cnt[:, None, None]
-    ref = torch.tanh(m.mean(1) + c64(layer.bias)) + (xr if residual else 0)
+    ref = torch.tanh(m.mean(1) + P(layer.bias)) + (xr if residual else 0)
     assert out.shape == (Dout, n)
     assert rel(gnn.rows(out), ref) < 3e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 3e-5 * be.tol)
+    grads_match(gnn, out, ref, [(xt, xr), (et, er)] + P.pairs(), 3e-5 * be.tol)
     with pytest.raises(AssertionError, match="Pseudo-cordinate"):
         layer(g, xt, jl(gnn, rng.standard_normal((E, ein + 1)), be.dev))
 
@@ -218,25 +266,31 @@ def test_egnn_conv(gnn, be, ein, residual):
     n, E, hin, Dx = g.num_nodes, g.num_edges, 5, 3
     layer = gnn.EGNNConv((hin, ein), hin, hidden_size=6, residual=residual, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     h, x, e = rng.standard_normal((n, hin)), rng.standard_normal((n, Dx)), rng.standard_normal((E, max(ein, 1)))
     ht, hr = jl(gnn, h, be.dev, True), c64(h).requires_grad_(True)
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
-    et = jl(gnn, e, be.dev) if ein else None
+    inputs = [(ht, hr), (xt, xr)]
+    if ein:
+        et, er = jl(gnn, e, be.dev, True), c64(e).requires_grad_(True)
+        inputs.append((et, er))
+    else:
+        et = None
     hnew, xnew = layer(g, ht, xt, et)
     xd = xr[t] - xr[s]
     sq = (xd ** 2).sum(1, keepdim=True)
     xd = xd / (sq.sqrt() + 1e-6)
-    f = torch.cat([hr[t], hr[s], sq] + ([c64(e)] if ein else []), dim=1)
-    mh = seq(layer.phi_e, f)
-    mx = seq(layer.phi_x, mh) * xd
+    f = torch.cat([hr[t], hr[s], sq] + ([er] if ein else []), dim=1)
+    mh = seq(layer.phi_e, f, P)
+    mx = seq(layer.phi_x, mh, P) * xd
     cnt = torch.bincount(t, minlength=n).clamp(min=1).double()
-    hn = seq(layer.phi_h, torch.cat([hr, scatter_sum(t, mh, n)], dim=1))
+    hn = seq(layer.phi_h, torch.cat([hr, scatter_sum(t, mh, n)], dim=1), P)
     href = hr + hn if residual else hn
     xref = xr + scatter_sum(t, mx, n) / cnt[:, None]
     assert hnew.shape == (hin, n) and xnew.shape == (Dx, n)
     assert rel(gnn.rows(hnew), href) < 5e-6 * be.tol and rel(gnn.rows(xnew), xref) < 5e-6 * be.tol
-    grads_match(gnn, hnew, ht, href, hr, 5e-5 * be.tol)
-    grads_match(gnn, xnew, xt, xref, xr, 5e-5 * be.tol)
+    grads_match(gnn, hnew, href, inputs + P.pairs(layer.phi_e, layer.phi_h), 5e-5 * be.tol)
+    grads_match(gnn, xnew, xref, inputs + P.pairs(layer.phi_e, layer.phi_x), 5e-5 * be.tol)
     if ein:
         with pytest.raises(AssertionError, match="Edge features must be provided"):
             layer(g, ht, xt)
@@ -249,10 +303,16 @@ def test_d_conv(gnn, be, k, weights):
     n, Din, Dout = g.num_nodes, 3, 4
     layer = gnn.DConv(Din, Dout, k, device=be.dev)
     randomise_biases(rng, layer)
+    P = Twins(layer)
     x = rng.standard_normal((n, Din))
     xt, xr = jl(gnn, x, be.dev, True), c64(x).requires_grad_(True)
+    pairs = [(xt, xr)] + P.pairs()
+    if weights:                                                                   # GNNGraph keeps the tensor it is given
+        g.w.requires_grad_(True)
+        pairs.append((g.w, c64(g.w).requires_grad_(True)))
+        A = torch.zeros(n, n, dtype=F64).index_put((s, t), pairs[-1][1], accumulate=True)
     out = layer(g, xt)
-    W = c64(layer.weights)                                                        # (2, k, out, in)
+    W = P(layer.weights)                                                          # (2, k, out, in)
     dout, din = A.sum(1), A.sum(0)
     P_out = lambda v: A.t() @ (dout[:, None] * v)                                 # propagate(w_mul_xj, g, +; xj = v .* deg_out')
     P_in = lambda v: A @ (din[:, None] * v)                                       # the same on the reversed graph
@@ -265,7 +325,7 @@ def test_d_conv(gnn, be, k, weights):
         T2i, T2o = 2 * P_in(T1i) - T0, 2 * P_out(T1o) - T0
         hsum = hsum + T2i @ W[0, i - 1].t() + T2o @ W[1, i - 1].t()
         T1i, T1o = T2i, T2o
-    ref = hsum + c64(layer.bias)
+    ref = hsum + P(layer.bias)
     assert out.shape == (Dout, n)
     assert rel(gnn.rows(out), ref) < 5e-6 * be.tol
-    grads_match(gnn, out, xt, ref, xr, 5e-5 * be.tol)
+    grads_match(gnn, out, ref, pairs, 5e-5 * be.tol)

@@ -1,6 +1,8 @@
 """Graph queries from the device plan (graphneuralnetworks.jl_b200/query.py): the known answers of
 GNNGraphs/test/gnngraph.jl:42-170 (the symmetric 4-cycle and the directed 4-ring) and GNNGraphs/test/query.jl for
 has_self_loops / has_multi_edges / is_bidirected.  CPU test double always; CUDA variants gated until they have run."""
+import numpy as np
+import pytest
 import torch
 
 
@@ -60,3 +62,36 @@ def test_adjacency_list_with_eid_and_flags(gnn, be):        # query.jl:176-198, 
     h = gnn.remove_self_loops(gnn.remove_multi_edges(g))
     assert not gnn.has_self_loops(h) and not gnn.has_multi_edges(h) and h.num_edges == 4
     assert gnn.is_bidirected(gnn.to_bidirected(h))
+
+
+@pytest.mark.parametrize("dir", ["in", "out", "both"])
+def test_weighted_degree_value_and_gradient(gnn, be, dir):
+    """degree(g, T; dir, edge_weight=w) is scatter(+, w, t) / (w, s) / both (GNNGraphs/src/query.jl:359-369), and its
+    gradient in w is scatter's pullback: Δ[t], Δ[s] or their sum — against float64 index_add and autograd"""
+    dev = be.dev
+    rng = np.random.default_rng(3)
+    n, E = 30, 200
+    s, t = rng.integers(1, n + 1, E), rng.integers(1, n - 4, E)           # the last nodes have no in-edge
+    w = rng.uniform(0.5, 1.5, E)
+    g = gnn.GNNGraph(T(s, dev), T(t, dev), num_nodes=n)
+    wt = torch.as_tensor(w, dtype=torch.float32).to(dev).requires_grad_(True)
+    w64 = torch.as_tensor(w).requires_grad_(True)
+
+    def scatter(idx):
+        return torch.zeros(n, dtype=torch.float64).index_add(0, torch.as_tensor(idx - 1), w64)
+
+    ref = {"in": lambda: scatter(t), "out": lambda: scatter(s), "both": lambda: scatter(t) + scatter(s)}[dir]()
+    d = gnn.degree(g, torch.float32, dir=dir, edge_weight=wt)
+    assert d.dtype == torch.float32 and d.requires_grad
+    assert torch.allclose(d.detach().cpu().double(), ref, rtol=1e-6, atol=0)
+    cot = torch.randn(n, dtype=torch.float64, generator=torch.Generator().manual_seed(0))
+    (gw,) = torch.autograd.grad((d.double() * cot.to(dev)).sum(), wt)
+    (rw,) = torch.autograd.grad((ref * cot).sum(), w64)
+    assert torch.allclose(gw.cpu().double(), rw, rtol=1e-6, atol=1e-6)
+    # the graph's own weights take the same path; without grad the result has no history
+    gg = gnn.GNNGraph(T(s, dev), T(t, dev), wt, num_nodes=n)
+    (gw2,) = torch.autograd.grad((gnn.degree(gg, dir=dir).double() * cot.to(dev)).sum(), wt)
+    assert torch.equal(gw2, gw)
+    with torch.no_grad():
+        assert not gnn.degree(g, dir=dir, edge_weight=wt).requires_grad
+    assert not gnn.degree(g, dir=dir, edge_weight=wt.detach()).requires_grad
