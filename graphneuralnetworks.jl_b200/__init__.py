@@ -22,6 +22,7 @@ from .layers_more import (CGConv, ChebConv, DConv, EdgeConv, EGNNConv, GMMConv, 
 from .readout import (broadcast_edges, broadcast_nodes, global_attention_pool, global_pool, reduce_edges, reduce_nodes,
                       softmax_edges, softmax_nodes)
 from .transform import csr, remove_multi_edges, remove_self_loops, sort_edge_index, to_bidirected, unbatch
+from .generate import knn_graph, radius_graph
 from .sampling import NeighborLoader, induced_subgraph, sample_edge_ids, sample_neighbors
 from .query import (adjacency_list, adjacency_matrix, has_multi_edges, has_self_loops, inneighbors, is_bidirected,
                     outneighbors)

@@ -109,6 +109,9 @@ _SIGS = {
     "gnnb_graph_csr_device": (_int, [_vp, _int, _vp, _vp, _vp, _vp]),
     "gnnb_sample_neighbors": (_int, [_vp, _vp, _i64, _int, _int, _i64, _int, _int, C.c_uint64, _vp, _vp, _i64,
                                      C.POINTER(_i64), _vp]),
+    "gnnb_knn": (_int, [_f32p, _i64, _int, _vp, _i64, _int, _int, _vp, _vp]),
+    "gnnb_radius_count": (_int, [_f32p, _i64, _int, _vp, _i64, C.c_float, _int, _vp, C.POINTER(_i64), _vp]),
+    "gnnb_radius_fill": (_int, [_f32p, _i64, _int, _vp, _i64, C.c_float, _int, _vp, _vp, _i64, _vp]),
     "gnnb_sample_positions_host": (_int, [_i32, _i64, _int, C.c_uint64, C.c_uint64, _vp, _i64, C.POINTER(_i64)]),
     "gnnb_propagate_host": (_int, [_vp, _int, _int, _int, _f32p, _f32p, _i64, _f32p]),
     "gnnb_gcn_propagate_host": (_int, [_vp, _int, _f32p, _f32p, _i64, _f32p]),

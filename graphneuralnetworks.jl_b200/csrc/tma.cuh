@@ -54,12 +54,28 @@ __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
                  : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
+// bounded wait on phase `parity`: false if it never completes (then *err is raised) or if another thread already raised
+// *err; a broken pipeline reports a status instead of hanging the kernel
+__device__ __forceinline__ bool mbar_wait_bounded(uint32_t bar, uint32_t parity, int* err) {
+    for (uint32_t spin = 0; spin < (1u << 26); ++spin) {
+        if (mbar_try(bar, parity)) return true;
+        if ((spin & 1023) == 1023 && *(volatile int*)err) return false;
+    }
+    atomicExch(err, 1);
+    return false;
+}
 // columns [col, col + box_cols) of row `row` of the 2-D tensor behind `map` (box_rows = 1) into dst
 __device__ __forceinline__ void load_row(uint32_t dst, const CUtensorMap* map, int col, int row, uint32_t bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(dst), "l"(map), "r"(col), "r"(row), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// 1-D bulk copy (cp.async.bulk, no tensor map) of `bytes` from global `src` into shared `dst`, completion counted on `bar`.
+// src and dst 16 B aligned, bytes a non-zero multiple of 16.
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
 
 }  // namespace tma
 }  // namespace gnnb

@@ -353,6 +353,31 @@ int gnnb_sample_neighbors(gnnb_graph_t g, const void* nodes, int64_t n_nodes, in
 int gnnb_sample_positions_host(int32_t deg, int64_t K, int replace, uint64_t seed, uint64_t j, int64_t* out,
                                int64_t capacity, int64_t* k_out);
 
+/* --------------------------------------------------------- geometric graphs (csrc/knn.cu)
+ * replaces: knn_graph(points, k; graph_indicator, self_loops) (GNNGraphs/src/generate.jl:112-145) and
+ *           radius_graph(points, r; graph_indicator, self_loops) (generate.jl:196-222): a KDTree / BallTree of
+ *           NearestNeighbors.jl on the CPU, graphs of a batch kept apart by a dummy coordinate.  Brute force here, exact.
+ * points: n rows of d contiguous DEVICE floats (Julia's (d, n) matrix).  d2(i,j) = Σ_{f=0..d-1} (p_i[f] - p_j[f])² in
+ * ascending f, every sub / mul / add rounded on its own (no FMA); a NaN d2 counts as +Inf.
+ * seg_ptr: NULL (one segment) or n_seg + 1 non-decreasing DEVICE offsets from 0 to n, validated on the device
+ * (GNNB_EINVAL).  A point's candidates are the points of its own segment.  n < 2^31.
+ * gnnb_knn: nbr (n*k int32, 0-based, row-major) row i = the k candidates j (j == i excluded unless self_loops) with the
+ *   smallest (d2, j), in ascending (d2, j).  k >= 1 and d >= 1 (GNNB_EINVAL); k > 64 or d > 256: GNNB_EUNSUPPORTED.  A
+ *   non-empty segment with fewer than k (+ 1 without self loops) points: GNNB_ESIZE.
+ * gnnb_radius_count: offsets (n + 1 int64) = running counts of the rows {j : sqrt_rn(d2) <= r} (j == i excluded unless
+ *   self_loops); *total_host = offsets[n].  r NaN or negative: GNNB_EINVAL.
+ * gnnb_radius_fill: the rows themselves, row i at nbr[offsets[i] .. offsets[i+1]) in ascending j (0-based int32);
+ *   capacity < offsets[n]: GNNB_ESIZE.  offsets must come from gnnb_radius_count with the same points, r, self_loops
+ *   and segments; a row whose hits differ from offsets[i+1] - offsets[i] gives GNNB_EINVAL.  A row never writes
+ *   outside its own range nor outside [0, capacity).
+ * All three synchronise the stream. */
+int gnnb_knn(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, int k, int self_loops,
+             int32_t* nbr, void* stream);
+int gnnb_radius_count(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,
+                      int self_loops, int64_t* offsets, int64_t* total_host, void* stream);
+int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,
+                     int self_loops, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream);
+
 /* ------------------------------------------------------ host-buffer entries
  * The reference-facing call with HOST arrays (what a CPU-array caller of `propagate` has): copies
  * x (and w) to the device, runs the fused pass, copies `out` back; synchronous.  Used for the

@@ -377,4 +377,103 @@ function coalesce_edge_index(s::CuVector{T}, t::CuVector{T}, n::Integer) where {
     return so[1:nu[]], to[1:nu[]], perm .+ 1, idxs          # 1-based permutation, segment id of every sorted edge
 end
 
+## knn_graph / radius_graph on device points — replace GNNGraphs/src/generate.jl:112-145,196-222 (KDTree / BallTree on
+## the CPU).  Exact fp32 distances within each graph of the batch; rows in (d2, j) order (knn) or ascending j (radius).
+## The indicator is sorted on the device when it is not already non-decreasing, and the rows are mapped back; every step
+## below stays on the device (no scalar indexing, no host copy of the neighbour lists).
+function _knn_segments(graph_indicator, n)
+    graph_indicator === nothing && return nothing, nothing, nothing
+    @assert graph_indicator isa AbstractVector{<:Integer}
+    @assert length(graph_indicator) == n
+    gi = CuVector{Int64}(graph_indicator)
+    n == 0 && return nothing, nothing, nothing
+    order = nothing
+    if !all(gi[2:end] .>= gi[1:end-1])
+        # unique keys (graph, position): the sort is stable whatever algorithm sortperm picks
+        keys = (gi .- minimum(gi)) .* Int64(n) .+ CuVector{Int64}(0:n-1)
+        order = sortperm(keys)
+    end
+    gs = order === nothing ? gi : gi[order]
+    ends = findall(gs[1:end-1] .!= gs[2:end])                 # last position of every graph but the last
+    seg = vcat(CUDA.zeros(Int64, 1), Int64.(ends), CuVector{Int64}([n]))
+    inv = nothing
+    if order !== nothing
+        inv = similar(order)
+        inv[order] .= CuVector{Int64}(1:n)                    # sorted position of each node
+    end
+    return order, inv, seg
+end
+
+_knn_seg_args(seg) = seg === nothing ? (CU_NULL, 1) : (seg, length(seg) - 1)
+
+function _knn_coo(centre, nbr, dir)
+    @assert dir ∈ (:in, :out)
+    return dir == :in ? (nbr, centre) : (centre, nbr)
+end
+
+# centre of every entry of a ragged list with `counts` entries per row (1-based rows), on the device: a +delta at the
+# first entry of every non-empty row, then a running sum
+function _ragged_centres(counts::CuVector{Int64}, total::Integer)
+    centre = CUDA.zeros(Int64, total)
+    total == 0 && return centre
+    nz = findall(counts .> 0)
+    nzv = Int64.(nz)
+    starts = cumsum(counts)[nz] .- counts[nz] .+ 1
+    centre[starts] .= nzv .- vcat(CUDA.zeros(Int64, 1), nzv[1:end-1])
+    return cumsum(centre)
+end
+
+function GNNGraphs.knn_graph(points::CuMatrix{Float32}, k::Int; graph_indicator = nothing, self_loops = false,
+                             dir = :in, kws...)
+    @assert dir ∈ (:in, :out)
+    d, n = size(points)
+    order, inv, seg = _knn_segments(graph_indicator, n)
+    x = order === nothing ? points : points[:, order]
+    sp, ns = _knn_seg_args(seg)
+    nbr = CuMatrix{Int32}(undef, k, n)                        # column i = row i of the C layout
+    check(ccall((:gnnb_knn, LIB), Cint,
+                (CuPtr{Float32}, Int64, Cint, CuPtr{Int64}, Int64, Cint, Cint, CuPtr{Int32}, Ptr{Cvoid}),
+                x, n, d, sp, ns, k, self_loops, nbr, stream()))
+    ids = Int64.(nbr) .+ 1
+    if order !== nothing
+        ids = order[ids[:, inv]]                              # columns back in node order, ids back to node ids
+    end
+    s, t = _knn_coo(repeat(CuVector{Int64}(1:n), inner = k), vec(ids), dir)
+    return GNNGraph((s, t); num_nodes = n, graph_indicator, kws...)
+end
+
+function GNNGraphs.radius_graph(points::CuMatrix{Float32}, r::AbstractFloat; graph_indicator = nothing,
+                                self_loops = false, dir = :in, kws...)
+    @assert dir ∈ (:in, :out)
+    d, n = size(points)
+    order, inv, seg = _knn_segments(graph_indicator, n)
+    x = order === nothing ? points : points[:, order]
+    sp, ns = _knn_seg_args(seg)
+    offsets = CUDA.zeros(Int64, n + 1)
+    total = Ref{Int64}(0)
+    check(ccall((:gnnb_radius_count, LIB), Cint,
+                (CuPtr{Float32}, Int64, Cint, CuPtr{Int64}, Int64, Cfloat, Cint, CuPtr{Int64}, Ref{Int64}, Ptr{Cvoid}),
+                x, n, d, sp, ns, r, self_loops, offsets, total, stream()))
+    E = total[]
+    nbr = CuVector{Int32}(undef, E)
+    E > 0 && check(ccall((:gnnb_radius_fill, LIB), Cint,
+                         (CuPtr{Float32}, Int64, Cint, CuPtr{Int64}, Int64, Cfloat, Cint, CuPtr{Int64}, CuPtr{Int32},
+                          Int64, Ptr{Cvoid}),
+                         x, n, d, sp, ns, r, self_loops, offsets, nbr, E, stream()))
+    ids = Int64.(nbr) .+ 1
+    counts = offsets[2:end] .- offsets[1:end-1]               # row lengths in sorted order
+    if order === nothing
+        centre = _ragged_centres(counts, E)
+    else
+        counts_out = counts[inv]                              # row lengths in node order
+        centre = _ragged_centres(counts_out, E)
+        start_out = cumsum(counts_out) .- counts_out          # 0-based start of each output row
+        pos = CuVector{Int64}(0:E-1) .- start_out[centre]     # position inside the row
+        src = offsets[1:end-1][inv][centre] .+ pos .+ 1       # the same entry in the sorted rows
+        ids = order[ids[src]]
+    end
+    s, t = _knn_coo(centre, ids, dir)
+    return GNNGraph((s, t); num_nodes = n, graph_indicator, kws...)
+end
+
 end # module
