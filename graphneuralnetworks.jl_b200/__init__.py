@@ -23,6 +23,8 @@ from .readout import (broadcast_edges, broadcast_nodes, global_attention_pool, g
                       softmax_edges, softmax_nodes)
 from .transform import csr, remove_multi_edges, remove_self_loops, sort_edge_index, to_bidirected, unbatch
 from .generate import knn_graph, radius_graph
+from .linkpred import (DotDecoder, add_edges, dot_decoder, edge_decoding, edge_encoding, intersect, negative_sample,
+                       perturb_edges, rand_edge_split, rand_graph)
 from .sampling import NeighborLoader, induced_subgraph, sample_edge_ids, sample_neighbors
 from .query import (adjacency_list, adjacency_matrix, has_multi_edges, has_self_loops, inneighbors, is_bidirected,
                     outneighbors)

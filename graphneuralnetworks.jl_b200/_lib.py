@@ -21,6 +21,7 @@ COPY_XJ, W_MUL_XJ = 0, 1
 SUM, MEAN, MAX, MIN = 0, 1, 2, 3
 SRC, DST = 0, 1
 DIR_OUT, DIR_IN, DIR_BOTH = 0, 1, 2
+CODES_DIRECTED, CODES_DIRECTED_NOLOOP, CODES_UNDIRECTED, CODES_UNDIRECTED_NOLOOP, CODES_BIPARTITE = range(5)
 
 
 class GNNBError(RuntimeError):
@@ -112,6 +113,11 @@ _SIGS = {
     "gnnb_knn": (_int, [_f32p, _i64, _int, _vp, _i64, _int, _int, _vp, _vp]),
     "gnnb_radius_count": (_int, [_f32p, _i64, _int, _vp, _i64, C.c_float, _int, _vp, C.POINTER(_i64), _vp]),
     "gnnb_radius_fill": (_int, [_f32p, _i64, _int, _vp, _i64, C.c_float, _int, _vp, _vp, _i64, _vp]),
+    "gnnb_edge_encode": (_int, [_int, _i64, _i64, _vp, _vp, _i64, _int, _vp, _vp]),
+    "gnnb_edge_decode": (_int, [_int, _i64, _i64, _vp, _i64, _int, _vp, _vp, _vp]),
+    "gnnb_edge_codes_sorted": (_int, [_int, _i64, _i64, _vp, _vp, _i64, _int, _vp, C.POINTER(_i64), _vp]),
+    "gnnb_codes_member": (_int, [_vp, _i64, _vp, _i64, _vp, _vp]),
+    "gnnb_sample_codes": (_int, [C.c_uint64, _vp, _i64, _i64, C.c_uint64, _vp, C.POINTER(_i64), _vp]),
     "gnnb_sample_positions_host": (_int, [_i32, _i64, _int, C.c_uint64, C.c_uint64, _vp, _i64, C.POINTER(_i64)]),
     "gnnb_propagate_host": (_int, [_vp, _int, _int, _int, _f32p, _f32p, _i64, _f32p]),
     "gnnb_gcn_propagate_host": (_int, [_vp, _int, _f32p, _f32p, _i64, _f32p]),

@@ -27,12 +27,6 @@ __global__ void mul_vec_kernel(const float* __restrict__ a, const float* __restr
 }
 
 // ---- RMAT (Graph500 a,b,c,d = .57,.19,.19,.05), counter-based, integer thresholds ------------------
-__host__ __device__ static inline uint64_t splitmix64(uint64_t x) {
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
 __global__ void rmat_kernel(int64_t N, int64_t first, int64_t count, uint64_t seed, int scale, int64_t* __restrict__ src,
                             int64_t* __restrict__ dst) {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

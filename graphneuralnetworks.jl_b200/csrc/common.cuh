@@ -45,6 +45,15 @@ extern std::atomic<int64_t> g_launches;
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// splitmix64's output function: the mixer of every counter-based random stream in the library (RMAT, neighbour
+// sampling, the edge-code permutation)
+__host__ __device__ static inline uint64_t splitmix64(uint64_t x) {
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+
 // SMs of the H100 SXM: the block-count caps of the grid-stride and two-stage reduction kernels are multiples of it
 constexpr int kNumSMs = 132;
 
@@ -97,6 +106,8 @@ int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st);
 int ensure_invdeg(gnnb_graph* g, Csr& c, cudaStream_t st);
 int ensure_items(gnnb_graph* g, const Csr& c, cudaStream_t st);            // seglean.cu
 int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st);     // seglean.cu: g->gcn_c and the Csr's es stream
+// transform.cu: flags[k] = 1 where sorted key k starts a run of equal keys (k == 0 or keys[k] != keys[k-1])
+int run_head_flags(const uint64_t* keys, int64_t E, int32_t* flags, cudaStream_t st);
 
 // segreduce.cu
 struct SegArgs {

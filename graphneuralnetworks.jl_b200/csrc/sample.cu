@@ -15,12 +15,6 @@
 
 namespace gnnb {
 
-__host__ __device__ static inline uint64_t mix64(uint64_t x) {
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
 __host__ __device__ static inline uint64_t mulhi64(uint64_t a, uint64_t b) {
 #ifdef __CUDA_ARCH__
     return __umul64hi(a, b);
@@ -30,7 +24,7 @@ __host__ __device__ static inline uint64_t mulhi64(uint64_t a, uint64_t b) {
 }
 // uniform integer in [0, m), m <= 2^31, from the (seed, j, draw) counter
 __host__ __device__ static inline uint32_t rnd_below(uint64_t seed, uint64_t j, uint64_t draw, uint32_t m) {
-    const uint64_t r = mix64(mix64(seed ^ (j * 0xD1342543DE82EF95ull)) + draw);
+    const uint64_t r = splitmix64(splitmix64(seed ^ (j * 0xD1342543DE82EF95ull)) + draw);
     return (uint32_t)mulhi64(r, (uint64_t)m);
 }
 

@@ -124,6 +124,13 @@ static int sort_pairs(const void* u, const void* v, int64_t E, int index_bytes, 
     return GNNB_OK;
 }
 
+int run_head_flags(const uint64_t* keys, int64_t E, int32_t* flags, cudaStream_t st) {
+    if (E == 0) return GNNB_OK;
+    head_flags_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(keys, E, flags);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
 static int check_args(int64_t E, int64_t max_index, int index_bytes) {
     if (index_bytes != 4 && index_bytes != 8) GNNB_FAIL(GNNB_EINVAL, "index_bytes must be 4 or 8 (got %d)", index_bytes);
     if (E < 0 || E >= ((int64_t)1 << 31)) GNNB_FAIL(GNNB_ESIZE, "number of edges %lld outside [0, 2^31)", (long long)E);

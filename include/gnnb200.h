@@ -378,6 +378,62 @@ int gnnb_radius_count(const float* points, int64_t n, int d, const int64_t* seg_
 int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,
                      int self_loops, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream);
 
+/* ------------------------------------------------- edge codes and random edges (csrc/edgegen.cu)
+ * Code spaces of edge_encoding / edge_decoding (GNNGraphs/src/utils.jl:189-268, bipartite :263-268), 0-based here (the
+ * reference's idx - 1), node ids 0-based (s, t < n; bipartite s < n1, t < n2), n1, n2 in [0, 2^31):
+ *   DIRECTED             M = n^2         c = s n + t
+ *   DIRECTED_NOLOOP      M = n(n-1)      c = s (n-1) + t - (t > s)                       (s != t)
+ *   UNDIRECTED           M = n(n+1)/2    c = start(s) + t - s,      start(s) = s(2n+1-s)/2  (s <= t after swapping)
+ *   UNDIRECTED_NOLOOP    M = n(n-1)/2    c = start(s) + t - s - 1,  start(s) = s(2n-1-s)/2  (s < t after swapping)
+ *   BIPARTITE            M = n1 n2       c = s n2 + t
+ * Decoding is integer-exact: the undirected row comes from a float64 sqrt of the exact uint64 discriminant and is then
+ * corrected with integer arithmetic.  n2 is read only for BIPARTITE. */
+typedef enum {
+    GNNB_CODES_DIRECTED = 0,
+    GNNB_CODES_DIRECTED_NOLOOP = 1,
+    GNNB_CODES_UNDIRECTED = 2,
+    GNNB_CODES_UNDIRECTED_NOLOOP = 3,
+    GNNB_CODES_BIPARTITE = 4
+} gnnb_code_space;
+
+/* Rounds of the Feistel network behind gnnb_sample_codes (part of its output contract: changing it changes every
+ * sample). */
+#define GNNB_FEISTEL_ROUNDS 8
+
+/* replaces: edge_encoding(s, t, n; directed, self_loops) (utils.jl:189-227).  s, t: E DEVICE int64 ids with base
+ * index_base (0|1); codes: E DEVICE uint64.  An id out of range, or a self loop in a NOLOOP space: GNNB_EINDEX (the
+ * reference's `@assert all(s .!= t)`).  Synchronises the stream. */
+int gnnb_edge_encode(int space, int64_t n1, int64_t n2, const int64_t* s, const int64_t* t, int64_t num_edges,
+                     int index_base, uint64_t* codes, void* stream);
+/* replaces: edge_decoding(idx, n; directed, self_loops) and edge_decoding(idx, n1, n2) (utils.jl:229-268).  Writes
+ * int64 ids with base index_base; a code >= M: GNNB_EINDEX.  Undirected codes decode to s <= t (s < t).  Synchronises. */
+int gnnb_edge_decode(int space, int64_t n1, int64_t n2, const uint64_t* codes, int64_t num_edges, int index_base,
+                     int64_t* s, int64_t* t, void* stream);
+/* The sorted set of distinct codes of an edge list: encode, device radix sort, one code per run of equal codes.
+ * replaces: the host-side `edge_encoding` + `setdiff!` bookkeeping of negative_sample (GNNGraphs/src/transform.jl:
+ * 899-917) and `intersect(idx1, idx2)` of intersect(g1, g2) (GNNGraphs/src/operators.jl:13-15).  Pairs the space does
+ * not hold (self loops in a NOLOOP space) are skipped; ids out of range: GNNB_EINDEX.  codes_out: DEVICE uint64 with
+ * num_edges entries; *n_out (HOST) = distinct codes written, ascending.  num_edges < 2^31.  Synchronises. */
+int gnnb_edge_codes_sorted(int space, int64_t n1, int64_t n2, const int64_t* s, const int64_t* t, int64_t num_edges,
+                           int index_base, uint64_t* codes_out, int64_t* n_out, void* stream);
+/* flags[k] = 1 if codes[k] is in `set` (x ascending distinct DEVICE uint64), else 0: one binary search per code.
+ * replaces: the membership half of `intersect(idx1, idx2)` (operators.jl:15).  num_codes < 2^31.  Does not
+ * synchronise. */
+int gnnb_codes_member(const uint64_t* codes, int64_t num_codes, const uint64_t* set, int64_t x, uint8_t* flags,
+                      void* stream);
+/* The first m codes of the seeded permutation π of [0, M) that are not in `excl`, in π order.
+ * replaces: the sampling of negative_sample (transform.jl:904-922: randsubseq over all codes, setdiff! against the
+ *           positives, truncation to the first num_neg of an ascending list) and of rand_graph (generate.jl:51-65 via
+ *           _rand_edges, utils.jl:270-284: StatsBase.sample without replacement), and randperm in rand_edge_split
+ *           (transform.jl:948).
+ * π(i): a balanced Feistel network of GNNB_FEISTEL_ROUNDS rounds over [0, 4^h), 4^h the smallest power of four >= M
+ * (h >= 1), cycle-walked until the value is < M.  Round r maps (L, R) -> (R, L ^ (splitmix64(R ^ k_r) & (2^h - 1))),
+ * k_r = splitmix64(splitmix64(seed) + r), value = L 2^h + R.  excl: x ascending distinct DEVICE codes < M (GNNB_EINVAL
+ * otherwise).  out: DEVICE uint64, m entries; writes min(m, M - x) codes and sets *n_out (HOST) to that number.
+ * The output is distinct by construction and a pure function of (M, excl, m, seed).  M < 2^62.  Synchronises. */
+int gnnb_sample_codes(uint64_t M, const uint64_t* excl, int64_t x, int64_t m, uint64_t seed, uint64_t* out,
+                      int64_t* n_out, void* stream);
+
 /* ------------------------------------------------------ host-buffer entries
  * The reference-facing call with HOST arrays (what a CPU-array caller of `propagate` has): copies
  * x (and w) to the device, runs the fused pass, copies `out` back; synchronous.  Used for the

@@ -23,6 +23,7 @@ module GNNlibB200Ext
 
 using CUDA
 using ChainRulesCore
+using Random
 using Statistics: mean
 using GNNlib: GNNlib, propagate, copy_xj, e_mul_xj, w_mul_xj, expand_srcdst, check_num_nodes
 using GNNGraphs: GNNGraphs, GNNGraph, COO_T, edge_index, get_edge_weight
@@ -474,6 +475,141 @@ function GNNGraphs.radius_graph(points::CuMatrix{Float32}, r::AbstractFloat; gra
     end
     s, t = _knn_coo(centre, ids, dir)
     return GNNGraph((s, t); num_nodes = n, graph_indicator, kws...)
+end
+
+## Link prediction on device COO graphs — replace negative_sample (GNNGraphs/src/transform.jl:890-929: a host copy,
+## randsubseq over all n² codes, setdiff!), rand_edge_split (:945-968), perturb_edges (:385-418), intersect
+## (operators.jl:7-20) and edge_encoding / edge_decoding (utils.jl:189-268).  One primitive, gnnb_sample_codes: the first
+## m codes of a seeded permutation of [0, M) outside a sorted exclusion set, in permutation order.  Codes are the
+## reference's idx - 1 (UInt64); randomness comes from `seed` (drawn from `rng` when none is given).
+const CuCOO = Tuple{<:CuVector{<:Integer}, <:CuVector{<:Integer}, <:Any}
+const SPACE = Dict((true, true) => Cint(0), (true, false) => Cint(1), (false, true) => Cint(2), (false, false) => Cint(3))
+_space_size(sp, n) = (n * n, n * (n - 1), n * (n + 1) ÷ 2, n * (n - 1) ÷ 2)[sp + 1]
+_seed(rng, seed) = seed === nothing ? rand(rng, UInt64) : UInt64(seed)
+
+function _encode(sp::Cint, n, s::CuVector{Int64}, t::CuVector{Int64})
+    codes = CuVector{UInt64}(undef, length(s))
+    check(ccall((:gnnb_edge_encode, LIB), Cint,
+                (Cint, Int64, Int64, CuPtr{Int64}, CuPtr{Int64}, Int64, Cint, CuPtr{UInt64}, Ptr{Cvoid}),
+                sp, n, n, s, t, length(s), 1, codes, stream()))
+    codes
+end
+
+function _decode(sp::Cint, n1, n2, codes::CuVector{UInt64})
+    s, t = CuVector{Int64}(undef, length(codes)), CuVector{Int64}(undef, length(codes))
+    check(ccall((:gnnb_edge_decode, LIB), Cint,
+                (Cint, Int64, Int64, CuPtr{UInt64}, Int64, Cint, CuPtr{Int64}, CuPtr{Int64}, Ptr{Cvoid}),
+                sp, n1, n2, codes, length(codes), 1, s, t, stream()))
+    s, t
+end
+
+function _codes_sorted(sp::Cint, n, s::CuVector{Int64}, t::CuVector{Int64})
+    out = CuVector{UInt64}(undef, length(s))
+    cnt = Ref{Int64}(0)
+    check(ccall((:gnnb_edge_codes_sorted, LIB), Cint,
+                (Cint, Int64, Int64, CuPtr{Int64}, CuPtr{Int64}, Int64, Cint, CuPtr{UInt64}, Ref{Int64}, Ptr{Cvoid}),
+                sp, n, n, s, t, length(s), 1, out, cnt, stream()))
+    out[1:cnt[]]
+end
+
+function _sample_codes(M::Integer, m::Integer, excl::Union{Nothing, CuVector{UInt64}}, seed::UInt64)
+    x = excl === nothing ? 0 : length(excl)
+    out = CuVector{UInt64}(undef, max(0, min(m, M - x)))
+    cnt = Ref{Int64}(0)
+    check(ccall((:gnnb_sample_codes, LIB), Cint,
+                (UInt64, CuPtr{UInt64}, Int64, Int64, UInt64, CuPtr{UInt64}, Ref{Int64}, Ptr{Cvoid}),
+                M, excl === nothing ? CU_NULL : excl, x, m, seed, out, cnt, stream()))
+    out[1:cnt[]]
+end
+
+function GNNGraphs.edge_encoding(s::CuVector{<:Integer}, t::CuVector{<:Integer}, n; directed = true, self_loops = true)
+    sp = SPACE[(directed, self_loops)]
+    return _encode(sp, n, CuVector{Int64}(s), CuVector{Int64}(t)) .+ UInt64(1), _space_size(sp, n)
+end
+
+function GNNGraphs.edge_decoding(idx::CuVector{<:Integer}, n; directed = true, self_loops = true)
+    return _decode(SPACE[(directed, self_loops)], n, n, CuVector{UInt64}(idx) .- UInt64(1))
+end
+
+GNNGraphs.edge_decoding(idx::CuVector{<:Integer}, n1, n2) = _decode(Cint(4), n1, n2, CuVector{UInt64}(idx) .- UInt64(1))
+
+function GNNGraphs.negative_sample(g::GNNGraph{<:CuCOO}; max_trials = 3, num_neg_edges = g.num_edges,
+                                   bidirected = GNNGraphs.is_bidirected(g), seed = nothing, rng = Random.default_rng())
+    @assert g.num_graphs == 1
+    n = g.num_nodes
+    @assert n >= 2 "negative_sample needs at least 2 nodes"
+    s, t = CuVector{Int64}.(edge_index(g))
+    sp = bidirected ? Cint(3) : Cint(1)                        # no self loops; undirected pairs when bidirected
+    codes = _sample_codes(_space_size(sp, n), bidirected ? num_neg_edges ÷ 2 : num_neg_edges,
+                          _codes_sorted(sp, n, s, t), _seed(rng, seed))
+    sn, tn = _decode(sp, n, n, codes)
+    if bidirected
+        sn, tn = vcat(sn, tn), vcat(tn, sn)
+    end
+    return GNNGraph(sn, tn, num_nodes = n)
+end
+
+function GNNGraphs.rand_edge_split(g::GNNGraph{<:CuCOO}, frac; bidirected = GNNGraphs.is_bidirected(g),
+                                   seed = nothing, rng = Random.default_rng())
+    @assert 0 <= frac <= 1 "frac must be between 0 and 1"
+    s, t = edge_index(g)
+    if bidirected
+        @assert GNNGraphs.is_bidirected(g)
+        @assert !GNNGraphs.has_self_loops(g)
+        @assert !GNNGraphs.has_multi_edges(g)
+        mask = s .< t
+        s, t = s[mask], t[mask]
+    end
+    ne = length(s)
+    eids = Int64.(_sample_codes(ne, ne, nothing, _seed(rng, seed))) .+ 1
+    size1 = round(Int, ne * frac)
+    e1, e2 = eids[1:size1], eids[(size1 + 1):end]
+    s1, t1, s2, t2 = s[e1], t[e1], s[e2], t[e2]
+    if bidirected
+        s1, t1 = vcat(s1, t1), vcat(t1, s1)
+        s2, t2 = vcat(s2, t2), vcat(t2, s2)
+    end
+    return GNNGraph(s1, t1, num_nodes = g.num_nodes), GNNGraph(s2, t2, num_nodes = g.num_nodes)
+end
+
+function GNNGraphs.perturb_edges(g::GNNGraph{<:CuCOO}, perturb_ratio::AbstractFloat; seed = nothing,
+                                 rng = Random.default_rng())
+    @assert perturb_ratio >= 0 && perturb_ratio <= 1 "perturb_ratio must be between 0 and 1"
+    k = ceil(Int, g.num_edges * perturb_ratio)
+    k == 0 && return g
+    n = g.num_nodes
+    @assert n > 1 "Graph must contain at least 2 nodes to add edges"
+    @assert k <= n * (n - 1)
+    snew, tnew = _decode(Cint(1), n, n, _sample_codes(n * (n - 1), k, nothing, _seed(rng, seed)))
+    return GNNGraphs.add_edges(g, (snew, tnew, nothing))
+end
+
+function Base.intersect(g1::GNNGraph{<:CuCOO}, g2::GNNGraph{<:CuCOO})
+    @assert g1.num_nodes == g2.num_nodes
+    n = g1.num_nodes
+    s1, t1 = CuVector{Int64}.(edge_index(g1))
+    s2, t2 = CuVector{Int64}.(edge_index(g2))
+    (isempty(s1) || isempty(s2)) && return GNNGraph(s1[1:0], t1[1:0]; num_nodes = n)
+    codes1 = _encode(Cint(0), n, s1, t1)
+    set2 = _codes_sorted(Cint(0), n, s2, t2)
+    inb = CuVector{UInt8}(undef, length(codes1))
+    check(ccall((:gnnb_codes_member, LIB), Cint, (CuPtr{UInt64}, Int64, CuPtr{UInt64}, Int64, CuPtr{UInt8}, Ptr{Cvoid}),
+                codes1, length(codes1), set2, length(set2), inb, stream()))
+    # first occurrence of every pair of g1 (Julia's intersect keeps g1's order, each element once): the run heads of the
+    # stable pair sort of gnnb_coalesce_edges
+    E = length(s1)
+    so, to = similar(s1), similar(t1)
+    perm, seg = CuVector{Int64}(undef, E), CuVector{Int64}(undef, E)
+    nu = Ref{Int64}(0)
+    check(ccall((:gnnb_coalesce_edges, LIB), Cint,
+                (CuPtr{Int64}, CuPtr{Int64}, Int64, Int64, Cint, Cint, CuPtr{Int64}, CuPtr{Int64}, CuPtr{Int64},
+                 CuPtr{Int64}, Ref{Int64}, Ptr{Cvoid}),
+                s1, t1, E, n, 8, 1, so, to, perm, seg, nu, stream()))
+    head = vcat(CUDA.ones(Bool, 1), seg[2:end] .!= seg[1:end-1])
+    first = CUDA.zeros(Bool, E)
+    first[perm[head] .+ 1] .= true
+    keep = findall((inb .!= 0) .& first)
+    return GNNGraph(s1[keep], t1[keep]; num_nodes = n)
 end
 
 end # module
