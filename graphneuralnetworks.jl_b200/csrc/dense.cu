@@ -116,6 +116,8 @@ int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* b
                      int64_t K, int64_t Nout, float* y, cudaStream_t st);
 int linear_tf32x3_error();
 int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t Dout, float* dW, cudaStream_t st);
+int linear_bwd_tf32x3(const float* dy, const float* y, const float* x, const float* W, int64_t M, int64_t Din, float* dx,
+                      float* dW, float* db, cudaStream_t st);
 extern int g_tc_enabled;
 
 __global__ void transpose_small_kernel(const float* __restrict__ w, int rows, int cols, float* __restrict__ wt) {
@@ -334,6 +336,10 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
     }
     if (!dy || !W) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     if (relu && (!y || !dpre_ws)) GNNB_FAIL(GNNB_EINVAL, "relu pullback needs the forward output and a (N,Dout) workspace");
+    if (dx && dW && x && Dout == 128) {   // the fused pullback: dpre stays on chip, dpre_ws is not touched
+        const int rc = linear_bwd_tf32x3(dy, relu ? y : nullptr, x, W, N, Din, dx, dW, db, st);
+        if (rc != GNNB_EUNSUPPORTED) return rc;
+    }
     const float* dpre = dy;
     if ((relu || db) && N > 0) {
         if (Dout % 4 != 0 || Dout > 1024 || ((uintptr_t)dy & 15) || (relu && (((uintptr_t)y & 15) || ((uintptr_t)dpre_ws & 15))))

@@ -61,6 +61,10 @@ __device__ __forceinline__ bool bar_wait(uint32_t bar, uint32_t parity, int* err
 }
 __device__ __forceinline__ float tf32_big(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// asks L2 to fetch `bytes` (a multiple of 16) at the 16 B aligned `p` ahead of the register loads that will read them
+__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
+}
 
 // wgmma shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (stride byte offset), leading byte
 // offset unused by this layout.  A step of K = 8 tf32 inside the 128 B swizzle row advances the start address by 32 B.
@@ -126,6 +130,8 @@ struct Params {
     int K, Nout, relu, ldw;
     int* err;
     const float* __restrict__ wimg;  // wide kernel only: W split and swizzled per (quarter, K-block), see tcx::w_image_kernel
+    const float* __restrict__ act;   // linear_bwd_dx_kernel only: forward output for the relu mask, or null (no mask)
+    float* __restrict__ colsum;      // linear_bwd_dx_kernel only: [grid][4 producer warps][128] column sums of dpre, or null
 };
 
 // epilogue of one 64 x 128 accumulator pair: columns col_base + [0, 128) of rows row0 + [0, 64), `ncols` of them valid
@@ -154,9 +160,30 @@ __device__ __forceinline__ void store_tile(const Params& p, const float* dm, con
     }
 }
 
+// consumer warpgroups of the ring kernels: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile of this CTA
+__device__ __forceinline__ void consume_tiles(const Params& p, uint32_t sbase, const float* sbias, int KB, int64_t ntiles) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
+    const int wg = (warp - PRODUCERS / 32) >> 2;
+    float dm[64] = {}, dc[64] = {};
+    uint32_t it = 0;
+    bool alive = true;
+    for (int64_t tile = blockIdx.x; alive && tile < ntiles; tile += gridDim.x) {
+        for (int kb = 0; kb < KB; ++kb, ++it) {
+            const int stage = it % NSTAGE;
+            if (!bar_wait(bar_full + 8 * stage, (it / NSTAGE) & 1, p.err)) { alive = false; break; }
+            const uint32_t a_big = sbase + SMEM_A + stage * 2 * KBLK_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
+            const uint32_t w_big = sbase + SMEM_W_BIG + kb * KBLK_BYTES, w_small = sbase + SMEM_W_SMALL + kb * KBLK_BYTES;
+            mma_kblock(dm, dc, a_big, a_small, w_big, w_small, kb == 0);
+            if (lane == 0) bar_arrive(bar_empty + 8 * stage);   // this warp's reads of the stage are complete
+        }
+        if (alive) store_tile(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
+    }
+}
+
 __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params p) {
     extern __shared__ __align__(1024) unsigned char smem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5;
     const int KB = p.K / BK;                                   // K-blocks per tile (<= 4)
     const int64_t ntiles = (p.M + BM - 1) / BM;
     const uint32_t sbase = s_u32(smem);
@@ -225,22 +252,120 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params 
             for (int i = 0; i < 8; ++i) v[i] = vn[i];
         }
     } else {
-        // ================= consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile =================
-        const int wg = (warp - PRODUCERS / 32) >> 2;
-        float dm[64] = {}, dc[64] = {};
-        uint32_t it = 0;
-        bool alive = true;
-        for (int64_t tile = blockIdx.x; alive && tile < ntiles; tile += gridDim.x) {
-            for (int kb = 0; kb < KB; ++kb, ++it) {
-                const int stage = it % NSTAGE;
-                if (!bar_wait(bar_full + 8 * stage, (it / NSTAGE) & 1, p.err)) { alive = false; break; }
-                const uint32_t a_big = sbase + SMEM_A + stage * 2 * KBLK_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
-                const uint32_t w_big = sbase + SMEM_W_BIG + kb * KBLK_BYTES, w_small = sbase + SMEM_W_SMALL + kb * KBLK_BYTES;
-                mma_kblock(dm, dc, a_big, a_small, w_big, w_small, kb == 0);
-                if (lane == 0) bar_arrive(bar_empty + 8 * stage);   // this warp's reads of the stage are complete
-            }
-            if (alive) store_tile(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
+        consume_tiles(p, sbase, sbias, KB, ntiles);
+    }
+}
+
+// dx = dpre * W for dpre = relu ? (y > 0 ? dy : 0) : dy, Dout = 128 rows of W and Din = Nout <= 128 columns.  The producers
+// form dpre from dy and the forward output y (p.act) in registers, so dpre is never stored, and add it into per-thread
+// column sums for db.  Tiles, images and the MMA sequence are those of linear_tf32x3_kernel run on a transposed copy of W
+// with a zero bias, so dx has the same bits as that composition; W is read transposed straight into the images instead.
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params p) {
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int64_t ntiles = (p.M + BM - 1) / BM;
+    const uint32_t sbase = s_u32(smem);
+    const uint32_t bar_full = sbase + SMEM_BAR;                // [NSTAGE]
+    const uint32_t bar_empty = bar_full + 8 * NSTAGE;          // [NSTAGE]
+    float* sbias = reinterpret_cast<float*>(smem + SMEM_BIAS);
+
+    if (tid == 0) {
+        for (int s = 0; s < NSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (int i = tid; i < BN; i += THREADS) sbias[i] = 0.f;    // (dm + dc) + 0: a -0 sum stores as +0, as in the composition
+    // image row n = column n of W (n < Din), K = the 128 rows of W
+    for (int idx = tid; idx < BN * 32; idx += THREADS) {
+        const int n = idx >> 5, c4 = idx & 31, kb = c4 >> 3, c = c4 & 7;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (n < p.Nout) {
+            const float* col = p.w + (size_t)(4 * c4) * p.Nout + n;
+            v = make_float4(__ldg(col), __ldg(col + p.Nout), __ldg(col + 2 * p.Nout), __ldg(col + 3 * p.Nout));
         }
+        const float4 b = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
+        const float4 s = make_float4(v.x - b.x, v.y - b.y, v.z - b.z, v.w - b.w);
+        const int off = kb * KBLK_BYTES + (n >> 3) * 1024 + (n & 7) * 128 + ((c ^ (n & 7)) << 4);
+        *reinterpret_cast<float4*>(smem + SMEM_W_BIG + off) = b;
+        *reinterpret_cast<float4*>(smem + SMEM_W_SMALL + off) = s;
+    }
+    fence_proxy_async();
+    __syncthreads();
+
+    if (warp < PRODUCERS / 32) {
+        // ================= producers: K = 128, so a tile is 4 K-blocks.  The next item is prefetched into registers, the
+        // next tile into L2.
+        const int c = tid & 7, r16 = tid >> 3, rr = r16 & 7;
+        const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+        // flattened (tile, K-block) sequence of this CTA, as in linear_tf32x3_kernel
+        const int64_t my_tiles = (ntiles > (int64_t)blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+        const int64_t total = my_tiles * 4;
+        auto fetch = [&](int64_t item, float4* g, float4* m) {
+            const int64_t tile = blockIdx.x + (item >> 2) * gridDim.x;
+            const int kb = (int)(item & 3);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int64_t row = tile * BM + r16 + 16 * i;
+                const bool in = item < total && row < p.M;
+                const size_t at = (size_t)row * 128 + kb * BK;
+                g[i] = in ? __ldg(reinterpret_cast<const float4*>(p.x + at) + c) : zero;
+                m[i] = (in && p.act) ? __ldg(reinterpret_cast<const float4*>(p.act + at) + c) : zero;
+            }
+        };
+        // dpre = act ? (act > 0 ? g : 0) : g, applied when the prefetched registers are promoted: holding the mask of the
+        // current item as well would not fit beside the next item's loads
+        auto masked = [&](float4* g, const float4* m) {
+            if (!p.act) return;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                g[i].x = m[i].x > 0.f ? g[i].x : 0.f; g[i].y = m[i].y > 0.f ? g[i].y : 0.f;
+                g[i].z = m[i].z > 0.f ? g[i].z : 0.f; g[i].w = m[i].w > 0.f ? g[i].w : 0.f;
+            }
+        };
+        // column sums of dpre: after each item the 4 threads of a warp that share a column group add theirs in a fixed
+        // order, and lanes 8 kb .. 8 kb + 7 keep the sums of K-block kb (columns 32 kb + 4 c .. + 3)
+        float4 cs = zero;
+        float4 g[8], gn[8], mn[8];
+        fetch(0, g, mn);
+        masked(g, mn);
+        for (int64_t it = 0; it < total; ++it) {
+            const int kb = (int)(it & 3);
+            if (tid == 0 && kb == 0 && it + 4 < total) {       // the next tile of this CTA into L2
+                const int64_t r0 = (blockIdx.x + ((it >> 2) + 1) * gridDim.x) * BM, nr = (p.M - r0 < BM) ? p.M - r0 : BM;
+                prefetch_l2(p.x + (size_t)r0 * 128, (uint32_t)(nr * 512));
+                if (p.act) prefetch_l2(p.act + (size_t)r0 * 128, (uint32_t)(nr * 512));
+            }
+            fetch(it + 1, gn, mn);
+            if (p.colsum) {
+                float4 t = zero;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) { t.x += g[i].x; t.y += g[i].y; t.z += g[i].z; t.w += g[i].w; }
+#pragma unroll
+                for (int o = 8; o <= 16; o <<= 1) {
+                    t.x += __shfl_xor_sync(0xffffffffu, t.x, o); t.y += __shfl_xor_sync(0xffffffffu, t.y, o);
+                    t.z += __shfl_xor_sync(0xffffffffu, t.z, o); t.w += __shfl_xor_sync(0xffffffffu, t.w, o);
+                }
+                if ((lane >> 3) == kb) { cs.x += t.x; cs.y += t.y; cs.z += t.z; cs.w += t.w; }
+            }
+            const int stage = (int)(it % NSTAGE);
+            if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((it / NSTAGE) & 1) ^ 1), p.err)) break;
+            unsigned char* abig = smem + SMEM_A + stage * 2 * KBLK_BYTES;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const float4 b = make_float4(tf32_big(g[i].x), tf32_big(g[i].y), tf32_big(g[i].z), tf32_big(g[i].w));
+                const float4 s = make_float4(g[i].x - b.x, g[i].y - b.y, g[i].z - b.z, g[i].w - b.w);
+                const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
+                *reinterpret_cast<float4*>(abig + off) = b;
+                *reinterpret_cast<float4*>(abig + KBLK_BYTES + off) = s;
+            }
+            fence_proxy_async();
+            bar_arrive(bar_full + 8 * stage);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) g[i] = gn[i];
+            masked(g, mn);
+        }
+        if (p.colsum) reinterpret_cast<float4*>(p.colsum + ((size_t)blockIdx.x * 4 + warp) * 128 + (lane >> 3) * BK)[c] = cs;
+    } else {
+        consume_tiles(p, sbase, sbias, 128 / BK, ntiles);
     }
 }
 }  // namespace tc
@@ -265,20 +390,25 @@ constexpr int SMEM_BARW = WSTAGE * STAGE_BYTES;
 constexpr int SMEM_TOTALW = SMEM_BARW + 64;
 
 struct ParamsW {
-    const float* __restrict__ dpre;   // [M][128]
+    const float* __restrict__ dpre;   // [M][128] (dy in the fused pullback)
     const float* __restrict__ x;      // [M][Din]
     float* __restrict__ partial;      // [grid][128][Din]
     int64_t M, rows_per_cta;
     int Din;
     int* err;
+    const float* __restrict__ act;    // linear_bwd_dw_kernel only: forward output y, dpre = y > 0 ? dy : 0; null: dpre = dy
 };
+constexpr int L2_AHEAD = 3;           // linear_bwd_dw_kernel: row blocks prefetched into L2 ahead of the register loads
 
 // byte offset of element (row n, k) of a K-major SWIZZLE_128B image, k < 32
 __device__ __forceinline__ int kmajor_off(int n, int k) {
     return (n >> 3) * 1024 + (n & 7) * 128 + ((((k >> 2) ^ (n & 7))) << 4) + (k & 3) * 4;
 }
 
-__global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) {
+// FUSED: the fused pullback's variant, which forms dpre from dy and the relu mask of p.act in the producers and prefetches
+// the rows L2_AHEAD blocks ahead into L2; otherwise p.dpre is read as it is
+template <bool FUSED>
+__device__ __forceinline__ void dw_body(const ParamsW& p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t sbase = s_u32(smem);
@@ -300,16 +430,14 @@ __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) 
     if (warp < PRODUCERS / 32) {
         // ---- producers: 32 rows of dPre (128 floats) and of X (Din floats) per stage, transposed + split + swizzled
         const int rl = lane >> 2, fl = lane & 3;
-        auto fetch = [&](int64_t blk, float4* va, float4* vb) {
-            const int64_t r0 = r_begin + blk * 32;
+        // the 8 float4 this thread covers in row block blk of src (row stride ld floats, nf float4 per row)
+        auto load = [&](const float* src, int ld, int nf, int64_t blk, float4* v) {
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
-                const int64_t r = r0 + rl + 8 * (q & 3);
+                const int64_t r = r_begin + blk * 32 + rl + 8 * (q & 3);
                 const int f = 4 * (warp + 4 * (q >> 2)) + fl;
-                const bool in = blk < nblk && r < r_end;
-                va[q] = in ? __ldg(reinterpret_cast<const float4*>(p.dpre + (size_t)r * 128) + f) : make_float4(0.f, 0.f, 0.f, 0.f);
-                vb[q] = (in && f < nfB) ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)r * p.Din) + f)
-                                        : make_float4(0.f, 0.f, 0.f, 0.f);
+                v[q] = (blk < nblk && r < r_end && f < nf) ? __ldg(reinterpret_cast<const float4*>(src + (size_t)r * ld) + f)
+                                                           : make_float4(0.f, 0.f, 0.f, 0.f);
             }
         };
         auto put1 = [&](unsigned char* big, int n, int k, float e) {
@@ -321,12 +449,9 @@ __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) 
         auto put = [&](unsigned char* big, int n0, int k, float4 v) {
             put1(big, n0, k, v.x); put1(big, n0 + 1, k, v.y); put1(big, n0 + 2, k, v.z); put1(big, n0 + 3, k, v.w);
         };
-        float4 va[8], vb[8], na[8], nb[8];
-        fetch(0, va, vb);
-        for (int64_t blk = 0; blk < nblk; ++blk) {
-            fetch(blk + 1, na, nb);
+        auto stage_in = [&](int64_t blk, const float4* va, const float4* vb) {
             const int stage = (int)(blk % WSTAGE);
-            if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((blk / WSTAGE) & 1) ^ 1), p.err)) break;
+            if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((blk / WSTAGE) & 1) ^ 1), p.err)) return false;
             unsigned char* st = smem + stage * STAGE_BYTES;
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
@@ -337,8 +462,50 @@ __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) 
             }
             fence_proxy_async();
             bar_arrive(bar_full + 8 * stage);
+            return true;
+        };
+        if constexpr (!FUSED) {
+            float4 va[8], vb[8], na[8], nb[8];
+            load(p.dpre, 128, 32, 0, va);
+            load(p.x, p.Din, nfB, 0, vb);
+            for (int64_t blk = 0; blk < nblk; ++blk) {
+                load(p.dpre, 128, 32, blk + 1, na);
+                load(p.x, p.Din, nfB, blk + 1, nb);
+                if (!stage_in(blk, va, vb)) break;
 #pragma unroll
-            for (int q = 0; q < 8; ++q) { va[q] = na[q]; vb[q] = nb[q]; }
+                for (int q = 0; q < 8; ++q) { va[q] = na[q]; vb[q] = nb[q]; }
+            }
+        } else {
+            // dy and y are loaded one block ahead into registers and the mask is applied when they are promoted; x is
+            // loaded when its block is staged, from L2, where it was prefetched L2_AHEAD blocks ahead (dy, y and x all one
+            // block ahead would not fit the registers)
+            float4 va[8], vb[8], na[8], nm[8];
+            auto promote = [&]() {
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    va[q] = na[q];
+                    if (p.act) {
+                        va[q].x = nm[q].x > 0.f ? va[q].x : 0.f; va[q].y = nm[q].y > 0.f ? va[q].y : 0.f;
+                        va[q].z = nm[q].z > 0.f ? va[q].z : 0.f; va[q].w = nm[q].w > 0.f ? va[q].w : 0.f;
+                    }
+                }
+            };
+            load(p.dpre, 128, 32, 0, na);
+            if (p.act) load(p.act, 128, 32, 0, nm);
+            promote();
+            for (int64_t blk = 0; blk < nblk; ++blk) {
+                if (tid == 0 && blk + L2_AHEAD < nblk) {
+                    const int64_t ra = r_begin + 32 * (blk + L2_AHEAD), nr = (r_end - ra < 32) ? r_end - ra : 32;
+                    prefetch_l2(p.dpre + (size_t)ra * 128, (uint32_t)(nr * 512));
+                    if (p.act) prefetch_l2(p.act + (size_t)ra * 128, (uint32_t)(nr * 512));
+                    prefetch_l2(p.x + (size_t)ra * p.Din, (uint32_t)(nr * p.Din * 4));
+                }
+                load(p.dpre, 128, 32, blk + 1, na);
+                if (p.act) load(p.act, 128, 32, blk + 1, nm);
+                load(p.x, p.Din, nfB, blk, vb);
+                if (!stage_in(blk, va, vb)) break;
+                promote();
+            }
         }
     } else {
         // ---- consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of dW (M = 128), N = Din (padded to 128)
@@ -373,12 +540,22 @@ __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) 
     }
 }
 
-__global__ void dw_reduce_kernel(const float* __restrict__ partial, int nparts, int n, float* __restrict__ dW) {
+__global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) { dw_body<false>(p); }
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_kernel(const ParamsW p) { dw_body<true>(p); }
+
+// dW[i] = sum of the n-float partials; with db: threads n .. n + 127 add the 128-float column-sum partials into db
+__global__ void dw_reduce_kernel(const float* __restrict__ partial, int nparts, int n, float* __restrict__ dW,
+                                 const float* __restrict__ colsum = nullptr, int ncolsum = 0, float* __restrict__ db = nullptr) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    float acc = 0.f;
-    for (int b = 0; b < nparts; ++b) acc += partial[(size_t)b * n + i];     // fixed order: deterministic
-    dW[i] = acc;
+    if (i < n) {
+        float acc = 0.f;
+        for (int b = 0; b < nparts; ++b) acc += partial[(size_t)b * n + i];     // fixed order: deterministic
+        dW[i] = acc;
+    } else if (db && i < n + 128) {
+        float acc = 0.f;
+        for (int b = 0; b < ncolsum; ++b) acc += colsum[(size_t)b * 128 + i - n];
+        db[i - n] = acc;
+    }
 }
 }  // namespace tcw
 
@@ -552,7 +729,7 @@ int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* b
     }
     tc::Params p;
     p.x = x; p.w = W; p.bias = bias; p.addend = addend; p.y = y; p.M = M; p.K = (int)K; p.Nout = (int)Nout; p.relu = relu;
-    p.ldw = (int)ldw; p.err = g_tc_err; p.wimg = nullptr;
+    p.ldw = (int)ldw; p.err = g_tc_err; p.wimg = nullptr; p.act = nullptr; p.colsum = nullptr;
     if (wide) {
         // the split, swizzled image of W (2 x its size), rebuilt per call: W changes between training steps
         static float* wimg = nullptr; static size_t wimg_elems = 0;
@@ -593,7 +770,7 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
     }
     if (M == 0) { GNNB_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)(Dout * Din), st)); return GNNB_OK; }
     tcw::ParamsW p;
-    p.dpre = dpre; p.x = x; p.partial = partial; p.M = M; p.Din = (int)Din; p.err = g_tc_err;
+    p.dpre = dpre; p.x = x; p.partial = partial; p.M = M; p.Din = (int)Din; p.err = g_tc_err; p.act = nullptr;
     int64_t rpc = ceil_div(M, nsm);
     rpc = ceil_div(rpc, 32) * 32;
     p.rows_per_cta = rpc;
@@ -602,6 +779,51 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
     GNNB_LAUNCHED();
     const int n = (int)(128 * Din);
     tcw::dw_reduce_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(partial, grid, n, dW);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
+// The dense layer's whole pullback for Dout = 128, Din in {32, 64, 96, 128}: dpre = y > 0 ? dy : 0 (y non-null, relu) or
+// dy, dx = dpre W, dW = dpre^T x and db = column sums of dpre (db may be null), in three launches that read dy, y and x
+// once each per product and never store dpre.  dx has the bits of linear_tf32x3 on dpre and W^T, dW those of dw_tf32x3
+// on dpre; GNNB_EUNSUPPORTED for anything else.
+int linear_bwd_tf32x3(const float* dy, const float* y, const float* x, const float* W, int64_t M, int64_t Din, float* dx,
+                      float* dW, float* db, cudaStream_t st) {
+    if (!g_tc_enabled) return GNNB_EUNSUPPORTED;
+    if (Din % 32 != 0 || Din > 128 || Din < 32 || M <= 0) return GNNB_EUNSUPPORTED;
+    if (((uintptr_t)dy & 15) || ((uintptr_t)y & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dx & 15)) return GNNB_EUNSUPPORTED;
+    static bool configured = false;
+    static int nsm = 0;
+    static float *partial = nullptr, *colsum = nullptr;
+    if (!configured) {
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
+        int dev = 0;
+        GNNB_CUDA(cudaGetDevice(&dev));
+        GNNB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
+        GNNB_CUDA(cudaMalloc(&partial, sizeof(float) * (size_t)nsm * 128 * 128));
+        GNNB_CUDA(cudaMalloc(&colsum, sizeof(float) * (size_t)nsm * 4 * 128));
+        if (!g_tc_err) { GNNB_CUDA(cudaMalloc(&g_tc_err, sizeof(int))); GNNB_CUDA(cudaMemset(g_tc_err, 0, sizeof(int))); }
+        configured = true;
+    }
+    // dx and the column sums of dpre: one CTA per SM over 128-row tiles
+    tc::Params p;
+    p.x = dy; p.w = W; p.bias = nullptr; p.addend = nullptr; p.y = dx; p.M = M; p.K = 128; p.Nout = (int)Din; p.relu = 0;
+    p.ldw = 128; p.err = g_tc_err; p.wimg = nullptr; p.act = y; p.colsum = db ? colsum : nullptr;
+    const int64_t ntiles = ceil_div(M, tc::BM);
+    const int grid_dx = (int)(ntiles < nsm ? ntiles : nsm);
+    tc::linear_bwd_dx_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
+    GNNB_LAUNCHED();
+    // dW: the split-K partition of dw_tf32x3
+    tcw::ParamsW pw;
+    pw.dpre = dy; pw.x = x; pw.partial = partial; pw.M = M; pw.Din = (int)Din; pw.err = g_tc_err; pw.act = y;
+    const int64_t rpc = ceil_div(ceil_div(M, nsm), 32) * 32;
+    pw.rows_per_cta = rpc;
+    const int grid_dw = (int)ceil_div(M, rpc);
+    tcw::linear_bwd_dw_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw);
+    GNNB_LAUNCHED();
+    const int n = (int)(128 * Din);
+    tcw::dw_reduce_kernel<<<(unsigned)ceil_div(n + 128, 256), 256, 0, st>>>(partial, grid_dw, n, dW, colsum, grid_dx * 4, db);
     GNNB_LAUNCHED();
     return GNNB_OK;
 }

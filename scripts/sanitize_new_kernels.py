@@ -12,7 +12,7 @@ y = torch.empty(N, Nout, device="cuda")
 gnn._lib.check(lib.gnnb_linear(x.data_ptr(), W.data_ptr(), b.data_ptr(), 1, N, K, Nout, y.data_ptr(), None))
 ref = (x.double() @ W.double().t() + b.double()).clamp(min=0)
 print("wide linear err", float((y.double() - ref).norm() / ref.norm()), "tc_error", lib.gnnb_dense_tc_error())
-# narrow linear kernel (tail tile, Nout < 128) and its pullback: dx through the same kernel, dW through the split-K kernel
+# narrow linear kernel (tail tile, Nout < 128) and its pullback through the fused kernels
 N, K, Nout = 1000 + 13, 96, 128
 x = torch.randn(N, K, device="cuda"); W = torch.randn(Nout, K, device="cuda") / K ** 0.5; b = torch.randn(Nout, device="cuda")
 y = torch.empty(N, Nout, device="cuda")
@@ -24,6 +24,16 @@ gnn._lib.check(lib.gnnb_linear_bwd(dy.data_ptr(), y.data_ptr(), x.data_ptr(), W.
 dpre = dy.double() * (y > 0)
 print("narrow linear dx err", float((dx.double() - dpre @ W.double()).norm() / (dpre @ W.double()).norm()),
       "dW err", float((dW.double() - dpre.t() @ x.double()).norm() / (dpre.t() @ x.double()).norm()),
+      "tc_error", lib.gnnb_dense_tc_error())
+# the fused pullback (linear_bwd_dx_kernel, linear_bwd_dw_kernel) at a ragged N: one row past a CTA's split-K range,
+# no relu, no db
+N, K = 132 * 32 + 1, 128
+x = torch.randn(N, K, device="cuda"); W = torch.randn(Nout, K, device="cuda") / K ** 0.5
+dy = torch.randn(N, Nout, device="cuda"); dx = torch.empty_like(x); dW = torch.empty_like(W)
+gnn._lib.check(lib.gnnb_linear_bwd(dy.data_ptr(), None, x.data_ptr(), W.data_ptr(), 0, N, K, Nout, None, dx.data_ptr(),
+                                   dW.data_ptr(), None, None))
+print("fused pullback dx err", float((dx.double() - dy.double() @ W.double()).norm() / (dy.double() @ W.double()).norm()),
+      "dW err", float((dW.double() - dy.double().t() @ x.double()).norm() / (dy.double().t() @ x.double()).norm()),
       "tc_error", lib.gnnb_dense_tc_error())
 # closing line
 D = 36
