@@ -73,6 +73,9 @@ _SIGS = {
     "gnnb_graph_create": (_int, [C.POINTER(_vp), _vp, _vp, _i64, _i64, _i64, _int, _int, _int, _vp]),
     "gnnb_graph_destroy": (_int, [_vp]),
     "gnnb_graph_add_self_loops": (_int, [_vp, C.POINTER(_vp), _vp]),
+    "gnnb_graph_subgraph": (_int, [_vp, _vp, _vp, _i64, C.POINTER(_vp), _vp, _vp, C.POINTER(_i64), C.POINTER(_i64),
+                                   _vp]),
+    "gnnb_bernoulli_keep": (_int, [_i64, C.c_double, C.c_uint64, _vp, _vp]),
     "gnnb_graph_info": (_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "gnnb_graph_csr": (_int, [_vp, _int, _vp, _vp, _vp, _vp]),
     "gnnb_degree": (_int, [_vp, _int, _f32p, _f32p, _vp]),

@@ -7,6 +7,8 @@
 // the CPU); it rebuilds a CSC from COO on every fused CPU call (GNNGraphs/src/query.jl:227).
 #include "common.cuh"
 #include <cub/cub.cuh>
+#include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 
 namespace gnnb {
 
@@ -87,6 +89,83 @@ __global__ void selfloop_rows_kernel(const int32_t* __restrict__ rowptr, int32_t
         ncol[pos] = (int32_t)r;
         neid[pos] = E + (int32_t)r;
     }
+}
+
+// ---- subgraph plans (remove_edges / remove_nodes / getgraph / add_nodes) ----------------------------
+// A kept set of nodes renumbered in ascending old id is a monotone map, and the plan's sort is stable, so compacting
+// the parent's sorted arrays (keeping their order) gives exactly the arrays a fresh stable sort of the child's COO
+// gives.  Every position comes from an exclusive scan of 0/1 flags over n + 1 (or E + 1) items whose last flag is 0:
+// entry [n] (or [E]) of the scan is the kept count, and item i is kept iff scan[i + 1] != scan[i].
+struct NodeKeepFlag {        // node i is kept (keep == NULL keeps all)
+    const uint8_t* keep;
+    int64_t n;
+    __host__ __device__ int32_t operator()(int64_t i) const { return (i < n && (!keep || keep[i])) ? 1 : 0; }
+};
+struct EdgeKeepFlag {        // COO edge e is kept: its mask (NULL keeps all) and both of its endpoints
+    const uint8_t* ekeep;
+    const uint8_t* nkeep;
+    const int32_t* src;
+    const int32_t* dst;
+    int64_t E;
+    __host__ __device__ int32_t operator()(int64_t e) const {
+        if (e >= E || (ekeep && !ekeep[e])) return 0;
+        return (!nkeep || (nkeep[src[e]] && nkeep[dst[e]])) ? 1 : 0;
+    }
+};
+struct SortedKeepFlag {      // sorted position k of a parent CSR holds a kept edge
+    const int32_t* eid;
+    const int32_t* newid;    // exclusive scan of EdgeKeepFlag, E + 1 entries
+    int64_t E;
+    __host__ __device__ int32_t operator()(int64_t k) const {
+        if (k >= E) return 0;
+        const int32_t e = eid[k];
+        return newid[e + 1] - newid[e];
+    }
+};
+template <typename F>
+using FlagIter = thrust::transform_iterator<F, thrust::counting_iterator<int64_t>, int32_t>;
+template <typename F>
+static FlagIter<F> flag_iter(F f) { return FlagIter<F>(thrust::counting_iterator<int64_t>(0), f); }
+
+__global__ void node_map_kernel(const uint8_t* __restrict__ keep, const int32_t* __restrict__ scan, int64_t n,
+                                int32_t* __restrict__ node_map) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) node_map[i] = (!keep || keep[i]) ? scan[i] : -1;
+}
+
+__global__ void subgraph_coo_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst, int64_t E,
+                                    const int32_t* __restrict__ newid, const int32_t* __restrict__ map,
+                                    int32_t* __restrict__ nsrc, int32_t* __restrict__ ndst,
+                                    int64_t* __restrict__ kept_eids) {
+    int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= E) return;
+    const int32_t p = newid[e];
+    if (newid[e + 1] == p) return;
+    nsrc[p] = map[src[e]];
+    ndst[p] = map[dst[e]];
+    if (kept_eids) kept_eids[p] = e;
+}
+
+__global__ void subgraph_csr_kernel(const int32_t* __restrict__ row, const int32_t* __restrict__ col,
+                                    const int32_t* __restrict__ eid, int64_t E, const int32_t* __restrict__ pos,
+                                    const int32_t* __restrict__ newid, const int32_t* __restrict__ map,
+                                    int32_t* __restrict__ nrow, int32_t* __restrict__ ncol,
+                                    int32_t* __restrict__ neid) {
+    int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= E) return;
+    const int32_t p = pos[k];
+    if (pos[k + 1] == p) return;
+    nrow[p] = map[row[k]];
+    ncol[p] = map[col[k]];
+    neid[p] = newid[eid[k]];
+}
+
+// keep[i] = !(u_i < p), u_i = (splitmix64(splitmix64(seed) + i) >> 11) * 2^-53
+__global__ void bernoulli_keep_kernel(int64_t n, double p, uint64_t key, uint8_t* __restrict__ keep) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double u = (double)(splitmix64(key + (uint64_t)i) >> 11) * 0x1.0p-53;
+    keep[i] = (u < p) ? 0 : 1;
 }
 
 // ---- helpers ------------------------------------------------------------------------------------
@@ -348,6 +427,132 @@ int gnnb_graph_add_self_loops(gnnb_graph_t g, gnnb_graph_t* out, void* stream) {
     } while (0);
     if (status != GNNB_OK) { gnnb_graph_destroy(h); return status; }
     *out = h;
+    return GNNB_OK;
+}
+
+}  // extern "C"
+
+namespace gnnb {
+
+struct SubgraphScratch {
+    void* p[4] = {nullptr, nullptr, nullptr, nullptr};
+    ~SubgraphScratch() {
+        for (void* q : p) cudaFree(q);
+    }
+};
+
+template <typename F>
+static int exclusive_scan_flags(F f, int64_t items, int32_t* out, void* tmp, size_t tmp_bytes, cudaStream_t st) {
+    GNNB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag_iter(f), out, (int)items, st));
+    g_launches.fetch_add(2, std::memory_order_relaxed);  // tile-state init + scan (library kernels)
+    return GNNB_OK;
+}
+
+// one direction of the child: compact the parent's sorted (row, col, eid), renumbered, then rowptr and long rows
+static int derive_subgraph_csr(const Csr& o, Csr& c, int64_t E, int64_t E2, int32_t nrows, const int32_t* newid,
+                               const int32_t* map, int32_t* pos, void* tmp, size_t tmp_bytes, int32_t chunk,
+                               cudaStream_t st) {
+    GNNB_TRY(alloc_csr(c, E2, nrows, nrows, chunk));
+    if (E2 > 0) {
+        GNNB_TRY(exclusive_scan_flags(SortedKeepFlag{o.eid, newid, E}, E + 1, pos, tmp, tmp_bytes, st));
+        subgraph_csr_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(o.row, o.col, o.eid, E, pos, newid, map, c.row,
+                                                                        c.col, c.eid);
+        GNNB_LAUNCHED();
+    }
+    rowptr_kernel<<<(unsigned)ceil_div(E2 + 1, 256), 256, 0, st>>>(c.row, E2, nrows, c.rowptr);
+    GNNB_LAUNCHED();
+    GNNB_TRY(find_long_rows(c, chunk, st));
+    c.built = true;
+    return GNNB_OK;
+}
+
+static int subgraph_into(gnnb_graph* g, const uint8_t* node_keep, const uint8_t* edge_keep, int64_t extra_nodes,
+                         gnnb_graph* h, int32_t* node_map, int64_t* kept_eids, cudaStream_t st) {
+    const int64_t n = g->n_src, E = g->E;
+    GNNB_TRY(ensure_csr(g, false, st));
+    SubgraphScratch sc;
+    GNNB_CUDA(cudaMalloc(&sc.p[0], sizeof(int32_t) * (size_t)(n + 1)));
+    GNNB_CUDA(cudaMalloc(&sc.p[1], sizeof(int32_t) * (size_t)(E + 1)));
+    GNNB_CUDA(cudaMalloc(&sc.p[2], sizeof(int32_t) * (size_t)(E + 1)));
+    int32_t* map = (int32_t*)sc.p[0];      // exclusive scan of the node flags: new id of each kept node, count at [n]
+    int32_t* newid = (int32_t*)sc.p[1];    // exclusive scan of the COO edge flags: child COO id, count at [E]
+    int32_t* pos = (int32_t*)sc.p[2];      // exclusive scan of the flags in one parent direction's sorted order
+    const NodeKeepFlag nf{node_keep, n};
+    const EdgeKeepFlag ef{edge_keep, node_keep, g->coo_src, g->coo_dst, E};
+    const SortedKeepFlag sf{g->by_dst.eid, newid, E};
+    size_t b0 = 0, b1 = 0, b2 = 0;
+    GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b0, flag_iter(nf), map, (int)(n + 1), st));
+    GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b1, flag_iter(ef), newid, (int)(E + 1), st));
+    GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b2, flag_iter(sf), pos, (int)(E + 1), st));
+    const size_t tmp_bytes = std::max(b0, std::max(b1, b2)) + 1;
+    GNNB_CUDA(cudaMalloc(&sc.p[3], tmp_bytes));
+    void* tmp = sc.p[3];
+
+    GNNB_TRY(exclusive_scan_flags(nf, n + 1, map, tmp, tmp_bytes, st));
+    GNNB_TRY(exclusive_scan_flags(ef, E + 1, newid, tmp, tmp_bytes, st));
+    int32_t counts[2] = {0, 0};
+    GNNB_CUDA(cudaMemcpyAsync(&counts[0], map + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaMemcpyAsync(&counts[1], newid + E, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    const int64_t n2 = (int64_t)counts[0] + extra_nodes, E2 = counts[1];
+    if (n2 >= ((int64_t)1 << 31) - 1)
+        GNNB_FAIL(GNNB_ESIZE, "kept nodes + extra_nodes = %lld must be < 2^31-1", (long long)n2);
+    if (node_map && n > 0) {
+        node_map_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(node_keep, map, n, node_map);
+        GNNB_LAUNCHED();
+    }
+    h->E = E2;
+    h->n_src = h->n_dst = (int32_t)n2;
+    const size_t nE = (size_t)(E2 > 0 ? E2 : 1);
+    GNNB_CUDA(cudaMalloc(&h->coo_src, sizeof(int32_t) * nE));
+    GNNB_CUDA(cudaMalloc(&h->coo_dst, sizeof(int32_t) * nE));
+    if (E > 0) {
+        subgraph_coo_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(g->coo_src, g->coo_dst, E, newid, map,
+                                                                        h->coo_src, h->coo_dst, kept_eids);
+        GNNB_LAUNCHED();
+    }
+    GNNB_TRY(derive_subgraph_csr(g->by_dst, h->by_dst, E, E2, (int32_t)n2, newid, map, pos, tmp, tmp_bytes, h->chunk,
+                                 st));
+    if (g->by_src.built)
+        GNNB_TRY(derive_subgraph_csr(g->by_src, h->by_src, E, E2, (int32_t)n2, newid, map, pos, tmp, tmp_bytes,
+                                     h->chunk, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    return GNNB_OK;
+}
+
+}  // namespace gnnb
+
+extern "C" {
+
+int gnnb_graph_subgraph(gnnb_graph_t g, const uint8_t* node_keep, const uint8_t* edge_keep, int64_t extra_nodes,
+                        gnnb_graph_t* out, int32_t* node_map, int64_t* kept_eids, int64_t* num_nodes_out,
+                        int64_t* num_edges_out, void* stream) {
+    if (!g || !out) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    *out = nullptr;
+    if (g->n_src != g->n_dst) GNNB_FAIL(GNNB_ESIZE, "subgraph needs num_src == num_dst (no bipartite plans)");
+    if (extra_nodes < 0) GNNB_FAIL(GNNB_EINVAL, "extra_nodes must be >= 0 (got %lld)", (long long)extra_nodes);
+    gnnb_graph* h = new gnnb_graph();
+    h->chunk = g->chunk;
+    h->device = g->device;
+    const int status = subgraph_into(g, node_keep, edge_keep, extra_nodes, h, node_map, kept_eids,
+                                     (cudaStream_t)stream);
+    if (status != GNNB_OK) {
+        gnnb_graph_destroy(h);
+        return status;
+    }
+    if (num_nodes_out) *num_nodes_out = h->n_src;
+    if (num_edges_out) *num_edges_out = h->E;
+    *out = h;
+    return GNNB_OK;
+}
+
+int gnnb_bernoulli_keep(int64_t n, double p, uint64_t seed, uint8_t* keep, void* stream) {
+    if (!(p >= 0.0 && p <= 1.0)) GNNB_FAIL(GNNB_EINVAL, "drop probability p = %g must lie in [0, 1]", p);
+    if (n < 0 || n >= ((int64_t)1 << 31) - 1) GNNB_FAIL(GNNB_ESIZE, "n = %lld must lie in [0, 2^31-1)", (long long)n);
+    if (n == 0) return GNNB_OK;
+    if (!keep) GNNB_FAIL(GNNB_EINVAL, "keep is NULL");
+    bernoulli_keep_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(n, p, splitmix64(seed), keep);
+    GNNB_LAUNCHED();
     return GNNB_OK;
 }
 

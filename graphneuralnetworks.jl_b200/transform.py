@@ -7,16 +7,40 @@
     to_bidirected(g)                 GNNGraphs/src/transform.jl:495-510
     unbatch(g)                       GNNGraphs/src/transform.jl:741-778
     csr(g; transposed)               the plan's COO -> CSR conversion as an API (the reference has no CSR type)
+    remove_edges(g, edges_or_p)      GNNGraphs/src/transform.jl:121-147   (DropEdge)
+    remove_nodes(g, nodes_or_p)      GNNGraphs/src/transform.jl:212-276   (DropNode)
+    getgraph(g, i; nmap)             GNNGraphs/src/transform.jl:825-888
+    add_nodes(g, n; ndata)           GNNGraphs/src/transform.jl:553-563
 
 The index work (pair encoding, stable radix sort, duplicate runs) is csrc/transform.cu; the feature aggregation of
 `remove_multi_edges` is the library's segmented scatter over the run ids it returns — the same kernels as
 `aggregate_neighbors`.  Graphs given on the CPU are staged to the current CUDA device and the result lives there.
+
+The four graph-editing functions share one entry, `gnnb_graph_subgraph` (csrc/plan.cu): kept nodes are renumbered in
+ascending old id, which is monotone, and the plan's sort is stable, so a compaction of the parent's sorted arrays is
+the child's plan — no new sort.  When g's plan exists and g has at most _DERIVE_MAX_EDGES edges, the child gets that
+derived plan; otherwise the child stays lazy and its plan is a fresh sort when first needed (building the parent's plan
+only to derive from it costs more than that sort, and above that size the derivation's gathers miss L2 and lose to the
+sort).  Both routes give the same bits.
+Random drops are `gnnb_bernoulli_keep`, keyed by a `seed` keyword or by a seed drawn from torch's default generator.
+
+Deliberate differences from the reference:
+1. The random draws are counter-based and keyed by `seed`, so they agree with the reference's `rand() < p` in
+   distribution only.
+2. remove_nodes slices `graph_indicator`; the reference keeps the old vector, which has the wrong length once nodes are
+   gone.
+3. add_nodes on a batched graph appends the new nodes to the last graph, so the indicator stays sorted and has length
+   num_nodes; the reference leaves it short.
+4. getgraph keeps an edge only when both of its endpoints are kept.  The reference tests only the source: on a batched
+   graph the two rules agree, and on other graphs the reference throws a KeyError.
+5. Ids out of range raise AssertionError instead of BoundsError.
 """
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import operator
-from typing import List
+from typing import List, Optional
 
 import torch
 
@@ -24,7 +48,7 @@ from . import _lib
 from . import graph as _graph
 from . import readout as _readout
 from ._lib import lib
-from .graph import GNNGraph, _as_index, _stream, rows, unrows
+from .graph import GNNGraph, _as_index, _Plan, _ptr, _stream, colmajor, rows, unrows
 from .msgpass import mean
 
 
@@ -138,3 +162,170 @@ def csr(g: GNNGraph, transposed: bool = False):
         _lib.check(lib.gnnb_graph_csr_device(p.h, int(bool(transposed)), rowptr.data_ptr(), col.data_ptr(),
                                              eid.data_ptr(), _stream(p.device)))
     return rowptr, col, eid
+
+
+# ---------------------------------------------------------------------------------------------- graph editing
+def _device(g: GNNGraph) -> torch.device:
+    return g._plan.device if g._plan is not None else _graph._compute_device(g.s)
+
+
+def _drop_mask(k: int, p, seed, dev) -> torch.Tensor:
+    """keep[i] = !(u_i < p): the reference's `rand() < p` drop rule on a counter-based stream (gnnb_bernoulli_keep)"""
+    from .linkpred import _seed                      # linkpred imports query, which imports this module
+    keep = torch.empty(k, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.gnnb_bernoulli_keep(k, float(p), _seed(seed), _ptr(keep) if k else None, _stream(dev)))
+    return keep
+
+
+def _id_mask(ids, k: int, dev, what: str) -> torch.Tensor:
+    """keep mask of k items without the 1-based `ids` (repeats allowed)"""
+    ids = _as_index(ids).reshape(-1).to(device=dev, dtype=torch.int64)
+    keep = torch.ones(k, dtype=torch.uint8, device=dev)
+    if ids.numel():
+        assert int(ids.min()) >= 1 and int(ids.max()) <= k, f"{what} id out of range 1:{k}"
+        keep[ids - 1] = 0
+    return keep
+
+
+def _is_probability(x) -> bool:
+    return isinstance(x, numbers.Real) or (isinstance(x, torch.Tensor) and x.dim() == 0)
+
+
+def _is_integral_scalar(x) -> bool:
+    return isinstance(x, numbers.Integral) or (isinstance(x, torch.Tensor) and x.dim() == 0 and
+                                               not x.is_floating_point())
+
+
+# The child's plan is derived from the parent's only when the parent has at most this many edges.  A derived direction
+# gathers newid[eid[k]] (4 B per parent edge, in the parent's sorted order) for every parent edge; while that array fits
+# in the H100's 50 MB L2 the gathers hit L2 and derivation beats a fresh sort of the child, at every keep share and for
+# every function measured, and at 100 M edges in random order it loses to the sort at every keep share (DESIGN.md §7).
+_DERIVE_MAX_EDGES = 1 << 23
+
+
+def _subgraph(g: GNNGraph, node_keep: Optional[torch.Tensor], edge_keep: Optional[torch.Tensor], extra_nodes: int = 0):
+    """The child of g that keeps the nodes of `node_keep` (uint8 mask, None = all) renumbered in ascending old id, then
+    `extra_nodes` isolated nodes, and the edges of `edge_keep` (None = all) whose two endpoints are kept, in COO order.
+    Returns (s, t, num_nodes, kept_eids (0-based int64), plan or None).  With g's plan built and at most _DERIVE_MAX_EDGES
+    edges in g, the child's plan is derived from g's (gnnb_graph_subgraph); otherwise the child stays lazy (its plan is a fresh sort when first needed) and the same arrays come from the
+    masks.  Both routes give the same bits."""
+    dev = _device(g)
+    n, E = g.num_nodes, g.num_edges
+    s0, t0 = g.s.to(dev), g.t.to(dev)
+    if g._plan is not None and E <= _DERIVE_MAX_EDGES:
+        p = g._plan
+        kept = torch.empty(E, dtype=torch.int64, device=dev)
+        nmap = None if node_keep is None else torch.empty(n, dtype=torch.int32, device=dev)
+        h, n2, e2 = C.c_void_p(), C.c_int64(0), C.c_int64(0)
+        with torch.cuda.device(dev):
+            _lib.check(lib.gnnb_graph_subgraph(p.h, _ptr(node_keep), _ptr(edge_keep), int(extra_nodes), C.byref(h),
+                                               _ptr(nmap), _ptr(kept) if E else None, C.byref(n2), C.byref(e2),
+                                               _stream(dev)))
+        plan, n2, kept = _Plan(h.value, dev), int(n2.value), kept[:int(e2.value)]
+    else:
+        ek = torch.ones(E, dtype=torch.bool, device=dev) if edge_keep is None else edge_keep.bool()
+        nmap, n2 = None, n + int(extra_nodes)
+        if node_keep is not None:
+            nk = node_keep.bool()
+            ek = ek & nk[s0.long() - 1] & nk[t0.long() - 1]
+            nmap = torch.where(nk, torch.cumsum(nk, 0, dtype=torch.int32) - 1, -1).to(torch.int32)
+            n2 = int(nk.sum()) + int(extra_nodes)
+        assert n2 < 2 ** 31 - 1, f"kept nodes + extra nodes = {n2} must be < 2^31-1"
+        plan, kept = None, ek.nonzero().reshape(-1)
+    s, t = s0[kept], t0[kept]
+    if nmap is not None:
+        s = (nmap[s.long() - 1] + 1).to(g.s.dtype)
+        t = (nmap[t.long() - 1] + 1).to(g.s.dtype)
+    return s, t, n2, kept, plan
+
+
+def _with_plan(h: GNNGraph, plan: Optional[_Plan]) -> GNNGraph:
+    h._plan = plan
+    return h
+
+
+def _take(x: Optional[torch.Tensor], idx: torch.Tensor) -> Optional[torch.Tensor]:
+    """getobs along the last dimension (edges, nodes or graphs)"""
+    return None if x is None else _take_edges(x, idx.to(x.device))
+
+
+def remove_edges(g: GNNGraph, edges_or_p=0.5, *, seed=None) -> GNNGraph:
+    """DropEdge — transform.jl:121-147.  A vector of 1-based edge ids (repeats allowed) removes those edges; a number p
+    drops each edge independently with probability p (gnnb_bernoulli_keep, keyed by `seed`).  Weights and edge
+    features follow the kept edges; nodes are unchanged."""
+    dev = _device(g)
+    if _is_probability(edges_or_p):
+        keep = _drop_mask(g.num_edges, edges_or_p, seed, dev)
+    else:
+        keep = _id_mask(edges_or_p, g.num_edges, dev, "edge")
+    s, t, n, kept, plan = _subgraph(g, None, keep)
+    return _with_plan(GNNGraph(s, t, _take(g.w, kept), num_nodes=n, ndata=g.ndata,
+                               edata={k: _take(x, kept) for k, x in g.edata.items()}, gdata=g.gdata,
+                               num_graphs=g.num_graphs, graph_indicator=g.graph_indicator), plan)
+
+
+def remove_nodes(g: GNNGraph, nodes_or_p, *, seed=None) -> GNNGraph:
+    """DropNode — transform.jl:212-276.  A vector of 1-based node ids (de-duplicated) or a drop probability p per node
+    (keyed by `seed`).  The edges touching a removed node go too; the kept nodes are renumbered in ascending old id.
+    Node features and graph_indicator are sliced, weights and edge features follow the kept edges."""
+    if _is_integral_scalar(nodes_or_p):      # the reference has remove_nodes(g, p::AbstractFloat) and a vector method
+        raise TypeError("remove_nodes takes a vector of node ids or a float drop probability; to remove node i, pass [i]")
+    dev = _device(g)
+    if _is_probability(nodes_or_p):
+        keep = _drop_mask(g.num_nodes, nodes_or_p, seed, dev)
+    else:
+        keep = _id_mask(nodes_or_p, g.num_nodes, dev, "node")
+    s, t, n, kept, plan = _subgraph(g, keep, None)
+    nodes = keep.bool().nonzero().reshape(-1)
+    return _with_plan(GNNGraph(s, t, _take(g.w, kept), num_nodes=n,
+                               ndata={k: _take(x, nodes) for k, x in g.ndata.items()},
+                               edata={k: _take(x, kept) for k, x in g.edata.items()}, gdata=g.gdata,
+                               num_graphs=g.num_graphs, graph_indicator=_take(g.graph_indicator, nodes)), plan)
+
+
+def getgraph(g: GNNGraph, i, *, nmap: bool = False):
+    """The graphs `i` (1-based, an int or a vector) of a batched graph, as one graph — transform.jl:825-888.  The
+    indicator is renumbered by position in `i` and gdata is sliced by `i`; with nmap=True also the 1-based old ids of
+    the kept nodes.  A graph without graph_indicator is its own only component: getgraph(g, 1) is g itself."""
+    ids = [int(v) for v in (i.reshape(-1).tolist() if isinstance(i, torch.Tensor) else
+                            ([i] if isinstance(i, numbers.Integral) else i))]
+    if g.graph_indicator is None:
+        assert ids == [1], "a graph without graph_indicator has only graph 1"
+        return (g, torch.arange(1, g.num_nodes + 1, device=g.s.device)) if nmap else g
+    assert all(1 <= v <= g.num_graphs for v in ids), f"graph id out of range 1:{g.num_graphs}"
+    dev = _device(g)
+    lut = torch.zeros(g.num_graphs + 1, dtype=torch.int64)
+    for pos, v in enumerate(ids):                  # the reference's Dict: a repeated id takes its last position
+        lut[v] = pos + 1
+    gi = lut.to(dev)[g.graph_indicator.to(dev).long()]
+    keep = (gi > 0).to(torch.uint8)
+    s, t, n, kept, plan = _subgraph(g, keep, None)
+    nodes = keep.bool().nonzero().reshape(-1)
+    gidx = torch.tensor(ids, dtype=torch.int64) - 1
+    h = _with_plan(GNNGraph(s, t, _take(g.w, kept), num_nodes=n,
+                            ndata={k: _take(x, nodes) for k, x in g.ndata.items()},
+                            edata={k: _take(x, kept) for k, x in g.edata.items()},
+                            gdata={k: _take(x, gidx) for k, x in g.gdata.items()}, num_graphs=len(ids),
+                            graph_indicator=gi[nodes].to(g.graph_indicator.dtype)), plan)
+    return (h, nodes + 1) if nmap else h
+
+
+def add_nodes(g: GNNGraph, n: int, *, ndata=None) -> GNNGraph:
+    """n isolated nodes after the existing ones — transform.jl:553-563.  `ndata` (a tensor is named x) must have the
+    keys of g.ndata, with n columns each.  On a batched graph the new nodes join the last graph."""
+    n = int(n)
+    assert n >= 0, "the number of nodes to add must be >= 0"
+    new = {} if ndata is None else ({"x": ndata} if isinstance(ndata, torch.Tensor) else dict(ndata))
+    assert sorted(new) == sorted(g.ndata), "cannot concatenate feature data with different keys"
+    nd = {}
+    for k, x in g.ndata.items():
+        y = torch.as_tensor(new[k]).to(device=x.device, dtype=x.dtype)
+        assert y.shape[-1] == n, f"ndata[{k}] of the new nodes must have {n} columns"
+        nd[k] = torch.cat([colmajor(x), colmajor(y)], dim=-1)
+    s, t, num_nodes, kept, plan = _subgraph(g, None, None, n)
+    gi = g.graph_indicator
+    if gi is not None:
+        gi = torch.cat([gi, torch.full((n,), g.num_graphs, dtype=gi.dtype, device=gi.device)])
+    return _with_plan(GNNGraph(s, t, g.w, num_nodes=num_nodes, ndata=nd, edata=g.edata, gdata=g.gdata,
+                               num_graphs=g.num_graphs, graph_indicator=gi), plan)

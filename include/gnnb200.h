@@ -89,6 +89,31 @@ int gnnb_graph_destroy(gnnb_graph_t g);
  * Requires num_src == num_dst (GNNB_ESIZE otherwise). */
 int gnnb_graph_add_self_loops(gnnb_graph_t g, gnnb_graph_t* out, void* stream);
 
+/* replaces: the index work of remove_edges, remove_nodes, getgraph and add_nodes (GNNGraphs/src/transform.jl:121-147,
+ *           212-276, 553-563, 825-888): a NEW plan for the subgraph of a square plan (num_src == num_dst, else
+ *           GNNB_ESIZE), derived from the parent's CSR without a sort.
+ * node_keep: n DEVICE bytes or NULL (keep all).  Kept nodes are renumbered 0.. in ascending old id, and extra_nodes >= 0
+ *            (GNNB_EINVAL otherwise) isolated nodes are appended after them (add_nodes).
+ * edge_keep: E DEVICE bytes, COO order, or NULL (keep all).  Edge e is kept iff edge_keep[e] != 0 and both of its
+ *            endpoints are kept.
+ * The child's COO is the kept edges in parent COO order, renumbered.  Its CSR-by-target is derived from the parent's,
+ * and so is its CSR-by-source when the parent has built one.  Both are bit-identical to what gnnb_graph_create builds
+ * from the child's COO at the same chunk size.  The child inherits the parent's chunk.
+ * node_map (n int32, DEVICE, or NULL): new 0-based id, or -1 if the node was removed.
+ * kept_eids (E int64, DEVICE, or NULL): 0-based parent COO ids of the kept edges, ascending.  Capacity is the parent's
+ *            E, so no count-then-fill round trip is needed.
+ * num_nodes_out, num_edges_out: HOST (NULL = skip).  Kept nodes + extra_nodes must be < 2^31-1 (GNNB_ESIZE).
+ * One count read-back; synchronises like gnnb_graph_add_self_loops. */
+int gnnb_graph_subgraph(gnnb_graph_t g, const uint8_t* node_keep, const uint8_t* edge_keep, int64_t extra_nodes,
+                        gnnb_graph_t* out, int32_t* node_map, int64_t* kept_eids,
+                        int64_t* num_nodes_out, int64_t* num_edges_out, void* stream);
+
+/* keep[i] = !(u_i < p), u_i = (splitmix64(splitmix64(seed) + i) >> 11) * 2^-53, for i < n (DEVICE bytes).
+ * replaces: the reference's `rand() < p` drop rule of remove_edges(g, p) / remove_nodes(g, p)
+ *           (transform.jl:143-147, 273-276), drawn from a counter-based stream.
+ * p must lie in [0, 1] (GNNB_EINVAL otherwise); n < 2^31-1 (GNNB_ESIZE).  Does not synchronise. */
+int gnnb_bernoulli_keep(int64_t n, double p, uint64_t seed, uint8_t* keep, void* stream);
+
 /* num_edges, num_src, num_dst of a plan */
 int gnnb_graph_info(gnnb_graph_t g, int64_t* num_edges, int64_t* num_src, int64_t* num_dst);
 

@@ -612,4 +612,139 @@ function Base.intersect(g1::GNNGraph{<:CuCOO}, g2::GNNGraph{<:CuCOO})
     return GNNGraph(s1[keep], t1[keep]; num_nodes = n)
 end
 
+## Graph editing on device COO graphs — replace remove_edges (GNNGraphs/src/transform.jl:121-147), remove_nodes
+## (:212-276), getgraph (:825-888) and add_nodes (:553-563).  One entry, gnnb_graph_subgraph: kept nodes renumbered in
+## ascending old id, kept edges in COO order, and, when the parent has a plan and at most DERIVE_MAX_EDGES edges, the child's
+## plan derived from the parent's CSR (no sort) and registered in the plan cache under the child's index arrays; the
+## same arrays come from the masks otherwise (the Python mirror's policy).  Drops with probability p are gnnb_bernoulli_keep, keyed by `seed`
+## (drawn from `rng` when none is given).  The deliberate differences of the Python mirror hold here too
+## (graphneuralnetworks.jl_b200/transform.py): graph_indicator is sliced by remove_nodes and extended by add_nodes, and
+## getgraph keeps an edge only when both of its endpoints are kept.
+function _drop_mask(k::Integer, p, seed::UInt64)
+    keep = CuVector{UInt8}(undef, k)
+    check(ccall((:gnnb_bernoulli_keep, LIB), Cint, (Int64, Cdouble, UInt64, CuPtr{UInt8}, Ptr{Cvoid}),
+                k, Float64(p), seed, k == 0 ? CU_NULL : keep, stream()))
+    keep
+end
+
+function _id_mask(ids, k::Integer)
+    keep = CUDA.ones(UInt8, k)
+    if !isempty(ids)
+        @assert 1 <= minimum(ids) && maximum(ids) <= k "id out of range 1:$k"
+        keep[CuVector{Int64}(ids)] .= 0x00
+    end
+    keep
+end
+
+# the plan of g if one is cached, without building one
+function cached_plan(g::GNNGraph{<:COO_T})
+    s, t = edge_index(g)
+    lock(PLANS_LOCK) do
+        for en in get(PLANS, s, PlanEntry[])
+            (en.t.value === t && en.num_nodes == g.num_nodes && en.num_edges == g.num_edges) && return en.plan
+        end
+        return nothing
+    end
+end
+
+# Derive the child's plan only when g has one and at most this many edges (the Python mirror's
+# transform._DERIVE_MAX_EDGES, measured in DESIGN.md §7); otherwise the child's plan is a fresh sort when first used.
+const DERIVE_MAX_EDGES = 1 << 23
+
+# (s, t, num_nodes, kept edge ids (1-based), old ids of the kept nodes (1-based)); a derived plan goes into the cache
+function _subgraph(g::GNNGraph{<:CuCOO}, node_keep, edge_keep, extra::Integer)
+    n, E = g.num_nodes, g.num_edges
+    s, t = edge_index(g)
+    p = cached_plan(g)
+    if p !== nothing && E <= DERIVE_MAX_EDGES
+        nmap = CuVector{Int32}(undef, n)
+        kept = CuVector{Int64}(undef, E)
+        h, n2, e2 = Ref{Ptr{Cvoid}}(C_NULL), Ref{Int64}(0), Ref{Int64}(0)
+        check(ccall((:gnnb_graph_subgraph, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{UInt8}, CuPtr{UInt8}, Int64, Ref{Ptr{Cvoid}}, CuPtr{Int32}, CuPtr{Int64},
+                     Ref{Int64}, Ref{Int64}, Ptr{Cvoid}),
+                    p.h, cuptr(node_keep), cuptr(edge_keep), extra, h, n == 0 ? CU_NULL : nmap,
+                    E == 0 ? CU_NULL : kept, n2, e2, stream()))
+        child, num_nodes = Plan(h[]), Int(n2[])
+        kept = kept[1:e2[]] .+ 1
+    else
+        child = nothing
+        ek = edge_keep === nothing ? CUDA.ones(Bool, E) : edge_keep .!= 0x00
+        num_nodes = n + extra
+        if node_keep !== nothing
+            nk = node_keep .!= 0x00
+            ek = ek .& nk[s] .& nk[t]
+            nmap = Int32.(cumsum(nk)) .- Int32(1)
+            num_nodes = Int(sum(nk)) + extra
+        end
+        @assert num_nodes < 2^31 - 1 "kept nodes + extra nodes = $num_nodes must be < 2^31-1"
+        kept = findall(ek)
+    end
+    s, t = s[kept], t[kept]
+    if node_keep !== nothing
+        s, t = eltype(s).(nmap[s] .+ 1), eltype(t).(nmap[t] .+ 1)
+    end
+    if child !== nothing
+        lock(PLANS_LOCK) do
+            push!(get!(() -> PlanEntry[], PLANS, s), PlanEntry(WeakRef(t), num_nodes, length(s), child))
+        end
+    end
+    nodes = node_keep === nothing ? CuVector{Int64}(1:n) : findall(node_keep .!= 0x00)
+    return s, t, num_nodes, kept, nodes
+end
+
+_take(x::Nothing, idx) = nothing
+_take(x, idx) = GNNGraphs.getobs(x, idx)
+
+function GNNGraphs.remove_edges(g::GNNGraph{<:CuCOO}, edges_to_remove::AbstractVector{<:Integer})
+    s, t, n, kept, _ = _subgraph(g, nothing, _id_mask(edges_to_remove, g.num_edges), 0)
+    return GNNGraph((s, t, _take(get_edge_weight(g), kept)), n, length(s), g.num_graphs, g.graph_indicator, g.ndata,
+                    _take(g.edata, kept), g.gdata)
+end
+
+function GNNGraphs.remove_edges(g::GNNGraph{<:CuCOO}, p::AbstractFloat; seed = nothing, rng = Random.default_rng())
+    s, t, n, kept, _ = _subgraph(g, nothing, _drop_mask(g.num_edges, p, _seed(rng, seed)), 0)
+    return GNNGraph((s, t, _take(get_edge_weight(g), kept)), n, length(s), g.num_graphs, g.graph_indicator, g.ndata,
+                    _take(g.edata, kept), g.gdata)
+end
+
+function _remove_nodes(g::GNNGraph{<:CuCOO}, keep)
+    s, t, n, kept, nodes = _subgraph(g, keep, nothing, 0)
+    gi = g.graph_indicator === nothing ? nothing : g.graph_indicator[nodes]
+    return GNNGraph((s, t, _take(get_edge_weight(g), kept)), n, length(s), g.num_graphs, gi, _take(g.ndata, nodes),
+                    _take(g.edata, kept), g.gdata)
+end
+
+GNNGraphs.remove_nodes(g::GNNGraph{<:CuCOO}, nodes_to_remove::AbstractVector{<:Integer}) =
+    _remove_nodes(g, _id_mask(nodes_to_remove, g.num_nodes))
+
+GNNGraphs.remove_nodes(g::GNNGraph{<:CuCOO}, p::AbstractFloat; seed = nothing, rng = Random.default_rng()) =
+    _remove_nodes(g, _drop_mask(g.num_nodes, p, _seed(rng, seed)))
+
+function GNNGraphs.getgraph(g::GNNGraph{<:CuCOO}, i::AbstractVector{Int}; nmap = false)
+    if g.graph_indicator === nothing
+        @assert i == [1]
+        return nmap ? (g, 1:(g.num_nodes)) : g
+    end
+    @assert all(1 .<= i .<= g.num_graphs) "graph id out of range 1:$(g.num_graphs)"
+    lut = zeros(Int, g.num_graphs)
+    for (pos, v) in enumerate(i)                               # the reference's Dict: a repeated id takes its last position
+        lut[v] = pos
+    end
+    gi = CuVector(lut)[g.graph_indicator]
+    keep = UInt8.(gi .> 0)
+    s, t, n, kept, nodes = _subgraph(g, keep, nothing, 0)
+    gnew = GNNGraph((s, t, _take(get_edge_weight(g), kept)), n, length(s), length(i), gi[nodes], _take(g.ndata, nodes),
+                    _take(g.edata, kept), _take(g.gdata, i))
+    return nmap ? (gnew, nodes) : gnew
+end
+
+function GNNGraphs.add_nodes(g::GNNGraph{<:CuCOO}, n::Integer; ndata = (;))
+    ndata = GNNGraphs.normalize_graphdata(ndata, default_name = :x, n = n)
+    ndata = GNNGraphs.cat_features(g.ndata, ndata)
+    s, t, num_nodes, _, _ = _subgraph(g, nothing, nothing, n)
+    gi = g.graph_indicator === nothing ? nothing : vcat(g.graph_indicator, fill!(similar(g.graph_indicator, n), g.num_graphs))
+    return GNNGraph((s, t, get_edge_weight(g)), num_nodes, length(s), g.num_graphs, gi, ndata, g.edata, g.gdata)
+end
+
 end # module

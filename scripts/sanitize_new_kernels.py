@@ -1,5 +1,5 @@
-"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback and the TMA-staged reduce
-(variant 13), meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
+"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the TMA-staged reduce
+(variant 13), the subgraph plans and the drop mask, meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gnnb200 as gnn
@@ -62,5 +62,21 @@ try:
 finally:
     lib.gnnb_set_kernel_variant(0)
 print("variant 13 bit-identical", bool(torch.equal(ref, got)))
+# subgraph plans (gnnb_graph_subgraph) and the drop mask (gnnb_bernoulli_keep): the hub graph with both CSRs built, an
+# empty graph, every edge removed, every node removed, extra nodes
+gnn.csr(g, transposed=True)
+e0 = torch.zeros(0, dtype=torch.int64, device="cuda")
+g0 = gnn.GNNGraph(e0, e0, num_nodes=5)
+g0.plan()
+subs = [gnn.remove_edges(g, 0.3, seed=1), gnn.remove_nodes(g, 0.1, seed=2), gnn.remove_edges(g, 1.0),
+        gnn.remove_nodes(g, 1.0), gnn.add_nodes(g, 9), gnn.remove_edges(g0, 0.5), gnn.remove_nodes(g0, [2]),
+        gnn.add_nodes(g0, 3)]
+for h in subs:
+    f = gnn.GNNGraph(h.s, h.t, num_nodes=h.num_nodes)
+    same = all(torch.equal(a, b) for tr in (False, True) for a, b in zip(gnn.csr(h, tr), gnn.csr(f, tr)))
+    print("subgraph", h.num_nodes, h.num_edges, "derived == fresh", same)
+keep = torch.empty(1001, dtype=torch.uint8, device="cuda")
+gnn._lib.check(lib.gnnb_bernoulli_keep(1001, 0.5, 3, keep.data_ptr(), None))
+print("bernoulli kept", int(keep.sum()), "of 1001")
 torch.cuda.synchronize()
 print("done")
