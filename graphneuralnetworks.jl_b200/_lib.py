@@ -149,8 +149,8 @@ for _name, (_res, _args) in _SIGS.items():
     _fn.argtypes = _args
 
 
-if os.environ.get("GNNB_KERNEL_VARIANT"):          # A/B runs of the whole test-suite on one kernel variant
-    lib.gnnb_set_kernel_variant(int(os.environ["GNNB_KERNEL_VARIANT"]))
+if os.environ.get("GNNB_KERNEL_VARIANT"):          # the whole test-suite on the reference kernels (12)
+    check(lib.gnnb_set_kernel_variant(int(os.environ["GNNB_KERNEL_VARIANT"])))
 
 
 def device_count() -> int:

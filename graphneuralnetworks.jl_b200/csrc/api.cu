@@ -15,7 +15,7 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-extern int g_variant;   // segreduce.cu
+extern bool g_reference_kernels;   // segreduce.cu
 int edge_dot(gnnb_graph* g, const float* dout, const float* x, const float* cs, const float* ct, int64_t D,
              float* dw_coo, cudaStream_t st);
 int maxmin_bwd(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
@@ -89,8 +89,8 @@ int gnnb_device_count(void) {
 }
 int64_t gnnb_launch_count(void) { return g_launches.load(); }
 int gnnb_set_kernel_variant(int v) {
-    if (v != 0 && v != 1 && v != 5 && v != 10 && v != 12 && v != 13) GNNB_FAIL(GNNB_EINVAL, "kernel variant must be one of 0, 1, 5, 10, 12, 13");
-    gnnb::g_variant = v;
+    if (v != 0 && v != 12) GNNB_FAIL(GNNB_EINVAL, "kernel variant must be 0 (default) or 12 (reference kernels), got %d", v);
+    gnnb::g_reference_kernels = v == 12;
     return GNNB_OK;
 }
 

@@ -66,7 +66,6 @@ struct Csr {
     int32_t* long_rows = nullptr;  // rows with more than `chunk` edges (unordered)
     int32_t n_long = 0;
     int32_t nrows = 0;  // reduction rows (targets; sources when transposed)
-    int32_t ncols = 0;  // gathered nodes
     float* invdeg = nullptr;  // lazily: 1/max(deg,1) per row (for MEAN)
     // lazily (seglean.cu): the chunk decomposition as a compact list of work items {e_begin, e_end, slot, 0}: slot < 0 = whole
     // rows (stored at every row end), slot >= 0 = one piece of a long row (raw partial into workspace slot `slot`)
@@ -111,7 +110,7 @@ int run_head_flags(const uint64_t* keys, int64_t E, int32_t* flags, cudaStream_t
 
 // segreduce.cu
 struct SegArgs {
-    const float* x = nullptr;   // gathered rows, [ncols][D]
+    const float* x = nullptr;   // gathered rows, [gathered nodes][D]
     const float* x2 = nullptr;  // optional second base for gathered nodes >= split (halo rows)
     int32_t split = 0;
     const float* w = nullptr;   // per-edge weight in PLAN order or nullptr

@@ -158,7 +158,6 @@ int gnnb_scatter(gnnb_graph_t g, int which, int aggr, const float* m, int64_t D,
     GNNB_TRY(ensure_csr(g, which == GNNB_SRC, st));
     Csr view = which == GNNB_SRC ? g->by_src : g->by_dst;
     view.col = view.eid;  // "gather" the edge's own message row: m[:, eid]
-    view.ncols = (int32_t)g->E;
     SegArgs a;
     a.x = m; a.out = out; a.D = D; a.aggr = aggr;
     return seg_reduce(g, view, a, st);

@@ -22,7 +22,7 @@
 
 namespace gnnb {
 
-extern int g_variant;   // segreduce.cu: 0 = lean work-item kernels, 12 = the round-1 chunk kernels
+extern bool g_reference_kernels;   // segreduce.cu: the round-1 chunk kernels for every shape
 
 struct GatParams {
     const int32_t* __restrict__ rowptr;
@@ -726,7 +726,7 @@ int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const f
         GNNB_TRY(ensure_ws(g, sizeof(float) * (size_t)2 * p.nchunks * (D + 2 * H + 4)));
         p.ws = g->ws;
     }
-    const bool lean = g_variant == 0 && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && H <= 64;
+    const bool lean = !g_reference_kernels && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && H <= 64;
     if (lean) {                                    // the work-item kernel (one warp per whole row, logits once per edge)
         GNNB_TRY(ensure_items(g, c, st));
         p.items = reinterpret_cast<const int4*>(c.items); p.n_items = c.n_items;
@@ -807,7 +807,7 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
         GNNB_TRY(ensure_ws(g, sizeof(float) * (size_t)2 * p.nchunks * (D + H + 4)));
         p.ws = g->ws;
     }
-    const bool lean = g_variant == 0 && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && C <= 128 && H <= 64;
+    const bool lean = !g_reference_kernels && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && C <= 128 && H <= 64;
     if (lean) {
         GNNB_TRY(ensure_items(g, c, st));
         p.items = reinterpret_cast<const int4*>(c.items); p.n_items = c.n_items;

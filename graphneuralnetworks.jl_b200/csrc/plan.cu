@@ -175,9 +175,8 @@ static void free_csr(Csr& c) {
     c = Csr();
 }
 
-static int alloc_csr(Csr& c, int64_t E, int32_t nrows, int32_t ncols, int32_t chunk) {
+static int alloc_csr(Csr& c, int64_t E, int32_t nrows, int32_t chunk) {
     c.nrows = nrows;
-    c.ncols = ncols;
     GNNB_CUDA(cudaMalloc(&c.rowptr, sizeof(int32_t) * ((size_t)nrows + 1)));
     GNNB_CUDA(cudaMalloc(&c.col, sizeof(int32_t) * (size_t)(E > 0 ? E : 1)));
     GNNB_CUDA(cudaMalloc(&c.row, sizeof(int32_t) * (size_t)(E > 0 ? E : 1)));
@@ -208,10 +207,9 @@ int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st) {
     if (c.built) return GNNB_OK;
     const int64_t E = g->E;
     const int32_t nrows = transposed ? g->n_src : g->n_dst;
-    const int32_t ncols = transposed ? g->n_dst : g->n_src;
     const int32_t* keys = transposed ? g->coo_src : g->coo_dst;
     const int32_t* other = transposed ? g->coo_dst : g->coo_src;
-    GNNB_TRY(alloc_csr(c, E, nrows, ncols, g->chunk));
+    GNNB_TRY(alloc_csr(c, E, nrows, g->chunk));
     if (E > 0) {
         int32_t* iota = nullptr;
         GNNB_CUDA(cudaMalloc(&iota, sizeof(int32_t) * (size_t)E));
@@ -378,7 +376,7 @@ int gnnb_graph_info(gnnb_graph_t g, int64_t* num_edges, int64_t* num_src, int64_
 }
 
 static int derive_self_loop_csr(const Csr& o, Csr& c, int64_t E, int32_t n, int32_t chunk, cudaStream_t st) {
-    GNNB_TRY(alloc_csr(c, E + n, n, n, chunk));
+    GNNB_TRY(alloc_csr(c, E + n, n, chunk));
     if (E > 0) {
         selfloop_edges_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(o.row, o.col, o.eid, E, c.row, c.col, c.eid);
         GNNB_LAUNCHED();
@@ -452,7 +450,7 @@ static int exclusive_scan_flags(F f, int64_t items, int32_t* out, void* tmp, siz
 static int derive_subgraph_csr(const Csr& o, Csr& c, int64_t E, int64_t E2, int32_t nrows, const int32_t* newid,
                                const int32_t* map, int32_t* pos, void* tmp, size_t tmp_bytes, int32_t chunk,
                                cudaStream_t st) {
-    GNNB_TRY(alloc_csr(c, E2, nrows, nrows, chunk));
+    GNNB_TRY(alloc_csr(c, E2, nrows, chunk));
     if (E2 > 0) {
         GNNB_TRY(exclusive_scan_flags(SortedKeepFlag{o.eid, newid, E}, E + 1, pos, tmp, tmp_bytes, st));
         subgraph_csr_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(o.row, o.col, o.eid, E, pos, newid, map, c.row,

@@ -18,13 +18,10 @@
 // Reference semantics: NNlib.gather -> message -> NNlib.scatter (GNNlib/src/msgpass.jl:75-79,121-129,145-149).
 #include "common.cuh"
 #include "segwalk.cuh"
-#include "tma.cuh"
 #include <cub/cub.cuh>
 #include <math_constants.h>
 
 namespace gnnb {
-
-extern int g_variant;   // segreduce.cu
 
 struct LeanParams {
     const int4* __restrict__ items;
@@ -149,7 +146,9 @@ __device__ __forceinline__ float4 lcomb(float4 a, float4 v, float s1, float s2, 
 // KV float4 per lane: one warp covers a row of KV*128 floats.  SMODE 0: no gathered-node scale, 1: per-edge stream es,
 // 2: gather cs[col].  HALO 0: one source base; 1: nodes >= split live in x2 (the halo rows of a shard).
 // (Staging the most gathered rows in a persisting-L2 window, with or without cache-streaming loads for the rest, was
-// measured slower.)  Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
+// measured slower.  So was staging every row in shared memory by TMA, one 2-D tensor-map tile load per row: on an H100 at
+// 700 W the forward GCN propagate took 19.3 / 35.8 / 28.3 ms against 16.5 / 35.4 / 27.9 ms here at D = 128 / 256 / 512;
+// DESIGN.md §4.)  Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
 // compiler keeps the loop free of divergence handling; shuffles are never executed under a lane-dependent condition.
 template <int KV, int SMODE, bool HAS_W, int HALO, int AGG>
 __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
@@ -250,155 +249,6 @@ __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
         float* o = p.ws + (int64_t)it.z * STRIDE + lane * 4;
 #pragma unroll
         for (int i = 0; i < KV; ++i) *reinterpret_cast<float4*>(o + i * 128) = acc[i];
-    }
-}
-
-// ---- A/B variant 13: the same pass with the rows staged in shared memory by TMA (D = 128, SUM) ---------------------------
-// BASELINE's north_star asks for "TMA staging of node-feature tiles into shared memory".  Round 1 measured one
-// cp.async.bulk per 512 B row, which the TMA unit's request rate bounds.  This variant stages the rows through a 2-D tensor
-// map instead: one cp.async.bulk.tensor.2d tile load (box = one row) per gathered row, four rows per mbarrier.
-// Persistent CTAs (one per SM, 8 warps); every warp is its own producer and consumer: lane 0 issues the loads of the
-// next four edges into the warp's private ring of 8 stages (16 KB, 32 rows in flight per warp, 256 per SM — no registers
-// held by loads in flight), all lanes wait on the stage's mbarrier (complete_tx) and reduce the four rows with LDS.128.
-// A stage is refilled with the NEXT batch's rows as soon as it has been consumed.  Same items, same arithmetic order:
-// bit-identical to the register-staged kernel.
-// Rows of KV*128 floats: a group of four edges is 4 x 512 B (KV = 1), 4 x 1 KB (KV = 2) or 4 x 2 KB in two column halves
-// (KV = 4: a TMA box is at most 256 elements wide), all on the group's one barrier.  128 KB of ring per CTA in every case.
-template <int KV> struct G4 {
-    static constexpr int WARPS = KV == 4 ? 4 : 8;
-    static constexpr int STAGES = KV == 1 ? 8 : 4;                // groups in flight per warp
-    static constexpr int REQS = KV == 4 ? 2 : 1;                  // column halves per row
-    static constexpr int BOX_COLS = KV * 128 / REQS;
-    static constexpr int ROW_BYTES = KV * 512;
-    static constexpr int STAGE_BYTES = 4 * ROW_BYTES;
-    static constexpr int SMEM = WARPS * STAGES * STAGE_BYTES + WARPS * STAGES * 8;
-};
-
-template <int KV, int SMODE>
-__global__ void __launch_bounds__(G4<KV>::WARPS * 32, 1) seg_gather4_kernel(const LeanParams p, const __grid_constant__ CUtensorMap map) {
-    using C = G4<KV>;
-    constexpr unsigned FULL = 0xffffffffu;
-    constexpr int S = C::STAGES;
-    constexpr int64_t STRIDE = (int64_t)KV * 128;
-    extern __shared__ __align__(1024) unsigned char g4smem[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned char* ring = g4smem + warp * (S * C::STAGE_BYTES);
-    const uint32_t ring_u = tma::smem_u32(ring);
-    const uint32_t bar0 = tma::smem_u32(g4smem + C::WARPS * S * C::STAGE_BYTES) + warp * S * 8;
-    if (lane == 0) {
-        for (int s = 0; s < S; ++s) tma::mbar_init(bar0 + 8 * s, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        tma::fence_proxy_async();
-    }
-    __syncwarp();
-    uint32_t par = 0;                                  // parity of every stage's next completion
-
-    // the four rows of group q (edges 4q .. 4q+3) of a batch whose gathered nodes sit in `c` (nv valid edges) into stage st
-    auto issue = [&](int st, int q, int c, int nv) {
-        const int last = nv - 1;
-        const int k = 4 * q;
-        const int c0 = __shfl_sync(FULL, c, k <= last ? k : last);
-        const int c1 = __shfl_sync(FULL, c, k + 1 <= last ? k + 1 : last);
-        const int c2 = __shfl_sync(FULL, c, k + 2 <= last ? k + 2 : last);
-        const int c3 = __shfl_sync(FULL, c, k + 3 <= last ? k + 3 : last);
-        if (lane == 0) {
-            tma::fence_proxy_async();                  // the stage was read through the generic proxy
-            tma::mbar_expect_tx(bar0 + 8 * st, C::STAGE_BYTES);
-#pragma unroll
-            for (int rq = 0; rq < C::REQS; ++rq) {     // column half rq lands its 4 x BOX_COLS block after the previous one
-                const uint32_t dst = ring_u + st * C::STAGE_BYTES + rq * (4 * C::BOX_COLS * 4);
-                tma::load_row(dst, &map, rq * C::BOX_COLS, c0, bar0 + 8 * st);
-                tma::load_row(dst + C::BOX_COLS * 4, &map, rq * C::BOX_COLS, c1, bar0 + 8 * st);
-                tma::load_row(dst + 2 * C::BOX_COLS * 4, &map, rq * C::BOX_COLS, c2, bar0 + 8 * st);
-                tma::load_row(dst + 3 * C::BOX_COLS * 4, &map, rq * C::BOX_COLS, c3, bar0 + 8 * st);
-            }
-        }
-    };
-
-    for (int item = blockIdx.x * C::WARPS + warp; item < p.n_items; item += gridDim.x * C::WARPS) {
-        const int4 it = __ldg(p.items + item);
-        const int e_end = it.y;
-        const bool partial = __any_sync(FULL, it.z >= 0);
-        auto load_lane = [&](int e0, int& c, int& r, float& s1, bool& last) {
-            const int my = e0 + lane;
-            c = 0; r = 0; s1 = 1.f; last = false;
-            if (my < e_end) {
-                c = __ldg(p.col + my);
-                r = __ldg(p.row + my);
-                if (SMODE == 1) s1 = __ldg(p.es + my);
-                last = (my + 1 == e_end) || (__ldg(p.row + my + 1) != r);
-                if (SMODE == 2) s1 = __ldg(p.cs + c);
-            }
-        };
-        float4 acc[KV];
-#pragma unroll
-        for (int i = 0; i < KV; ++i) acc[i] = f4(0.f);
-        int e = it.x;
-        int c_n, r_n; float s1_n; bool last_n;
-        load_lane(e, c_n, r_n, s1_n, last_n);
-        {
-            const int nv = (e_end - e) < 32 ? (e_end - e) : 32;
-            for (int q = 0; q < S && 4 * q < nv; ++q) issue(q, q, c_n, nv);
-        }
-        bool more = true;
-        while (more) {
-            const int c_l = c_n, r_l = r_n;
-            const float s1_l = s1_n;
-            const unsigned vmask = __ballot_sync(FULL, e + lane < e_end);
-            const unsigned bmask = partial ? 0u : __ballot_sync(FULL, last_n);
-            float sc_l = 1.f;
-            if (!partial && e + lane < e_end && p.ct) sc_l = __ldg(p.ct + r_l);
-            more = __any_sync(FULL, e + 32 < e_end);
-            if (more) load_lane(e + 32, c_n, r_n, s1_n, last_n);
-            const int nv = (e_end - e) < 32 ? (e_end - e) : 32;
-            const int nn = more ? ((e_end - e - 32) < 32 ? (e_end - e - 32) : 32) : 0;
-#pragma unroll 1
-            for (int q = 0; q < 8 && 4 * q < nv; ++q) {
-                const int st = q % S;                  // 8 groups per batch, S divides 8: the stage of group q
-                const uint32_t bar = bar0 + 8 * st;
-                const uint32_t ph = (par >> st) & 1u;
-                {   // bounded: a request that never completes aborts the kernel instead of hanging the GPU
-                    uint32_t spin = 0;
-                    while (!tma::mbar_try(bar, ph)) { if (++spin > (1u << 24)) __trap(); }
-                }
-                par ^= 1u << st;
-                const unsigned char* sbase = ring + st * C::STAGE_BYTES;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int j = 4 * q + u;
-                    const float s1 = (SMODE != 0) ? __shfl_sync(FULL, s1_l, j) : 1.f;
-                    if ((vmask >> j) & 1u) {
-#pragma unroll
-                        for (int i = 0; i < KV; ++i) {
-                            // float f = i*128 + lane*4 of row u: request f / BOX_COLS, inside it row u, column f % BOX_COLS
-                            const int f = i * 128 + lane * 4;
-                            const float4 v = *reinterpret_cast<const float4*>(sbase + (f / C::BOX_COLS) * (4 * C::BOX_COLS * 4) +
-                                                                              u * (C::BOX_COLS * 4) + (f % C::BOX_COLS) * 4);
-                            acc[i] = lcomb<SMODE, false, AG_SUM>(acc[i], v, s1, 1.f, 1.f);
-                        }
-                    }
-                    if ((bmask >> j) & 1u) {
-                        const int rj = __shfl_sync(FULL, r_l, j);
-                        const float sc = __shfl_sync(FULL, sc_l, j);
-#pragma unroll
-                        for (int i = 0; i < KV; ++i) {
-                            *reinterpret_cast<float4*>(p.out + (int64_t)rj * STRIDE + i * 128 + lane * 4) =
-                                make_float4(acc[i].x * sc, acc[i].y * sc, acc[i].z * sc, acc[i].w * sc);
-                            acc[i] = f4(0.f);
-                        }
-                    }
-                }
-                __syncwarp();                          // every lane is done with the stage
-                // refill it with the group S ahead: of this batch, or of the next one
-                if (q + S < 8) { if (4 * (q + S) < nv) issue(st, q + S, c_l, nv); }
-                else if (4 * (q + S - 8) < nn) issue(st, q + S - 8, c_n, nn);
-            }
-            e += 32;
-        }
-        if (partial) {
-#pragma unroll
-            for (int i = 0; i < KV; ++i) *reinterpret_cast<float4*>(p.ws + (int64_t)it.z * STRIDE + i * 128 + lane * 4) = acc[i];
-        }
     }
 }
 
@@ -507,30 +357,6 @@ __global__ void __launch_bounds__(256, 2) maxmin_bwd_lean_kernel(const MaxBwdPar
     }
 }
 
-template <int KV>
-int launch_gather4(const LeanParams& p, int smode, const float* x, int32_t ncols, cudaStream_t st) {
-    using C = G4<KV>;
-    CUtensorMap map;
-    if (tma::make_map_2d_f32(&map, x, (uint64_t)ncols, (uint64_t)KV * 128, (uint64_t)C::ROW_BYTES, C::BOX_COLS, 1) != 0)
-        GNNB_FAIL(GNNB_ECUDA, "cuTensorMapEncodeTiled failed for the gather4 variant");
-    static int nsm = 0;
-    if (!nsm) {
-        int dev = 0;
-        GNNB_CUDA(cudaGetDevice(&dev));
-        GNNB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-        GNNB_CUDA(cudaFuncSetAttribute(seg_gather4_kernel<KV, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-        GNNB_CUDA(cudaFuncSetAttribute(seg_gather4_kernel<KV, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-        GNNB_CUDA(cudaFuncSetAttribute(seg_gather4_kernel<KV, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-    }
-    const int64_t want = ceil_div((int64_t)p.n_items, C::WARPS);
-    const unsigned blocks = (unsigned)(want < nsm ? want : nsm);
-    if (smode == 0) seg_gather4_kernel<KV, 0><<<blocks, C::WARPS * 32, C::SMEM, st>>>(p, map);
-    else if (smode == 1) seg_gather4_kernel<KV, 1><<<blocks, C::WARPS * 32, C::SMEM, st>>>(p, map);
-    else seg_gather4_kernel<KV, 2><<<blocks, C::WARPS * 32, C::SMEM, st>>>(p, map);
-    GNNB_LAUNCHED();
-    return GNNB_OK;
-}
-
 template <int KV, int SMODE, bool HAS_W, int HALO, int AGG>
 int launch_lean3(const LeanParams& p, cudaStream_t st) {
     const unsigned blocks = (unsigned)ceil_div(p.n_items, 8);
@@ -624,15 +450,15 @@ int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) {
 }
 
 // the lean path: D in {128, 256, 512}, 16 B-aligned operands.  GNNB_EUNSUPPORTED = not this kernel's shape (the caller
-// falls back to seg_reduce_kernel).  `use_es`: take the per-edge scale stream a.es instead of gathering a.cs.
-int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, bool use_es, cudaStream_t st) {
+// falls back to seg_reduce_kernel).
+int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, cudaStream_t st) {
     if (a.D != 128 && a.D != 256 && a.D != 512) return GNNB_EUNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(a.x) & 15) || (reinterpret_cast<uintptr_t>(a.x2) & 15) ||
         (reinterpret_cast<uintptr_t>(a.out) & 15))
         return GNNB_EUNSUPPORTED;
     const bool ismax = (a.aggr == GNNB_MAX || a.aggr == GNNB_MIN);
     const int agg = ismax ? AG_MAX : (a.aggr == GNNB_MEAN ? AG_MEAN : AG_SUM);
-    const int smode = (a.cs == nullptr) ? 0 : ((use_es && a.es != nullptr) ? 1 : 2);
+    const int smode = (a.cs == nullptr) ? 0 : (a.es != nullptr ? 1 : 2);
     const bool halo = a.x2 != nullptr;
     if (agg != AG_SUM && (smode != 0 || halo)) return GNNB_EUNSUPPORTED;
     GNNB_TRY(ensure_items(g, c, st));
@@ -651,11 +477,6 @@ int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, bo
     p.sign = (a.aggr == GNNB_MIN) ? -1.f : 1.f;
     if (p.n_items == 0) return GNNB_OK;
     const int use_halo = halo ? 1 : 0;
-    if (g_variant == 13 && agg == AG_SUM && !halo && a.w == nullptr) {      // rows staged by TMA tile loads (A/B variant)
-        if (a.D == 128) return launch_gather4<1>(p, smode, a.x, c.ncols, st);
-        if (a.D == 256) return launch_gather4<2>(p, smode, a.x, c.ncols, st);
-        return launch_gather4<4>(p, smode, a.x, c.ncols, st);
-    }
     int rc;
     if (a.D == 128) rc = launch_lean1<1>(p, smode, a.w != nullptr, use_halo, agg, st);
     else if (a.D == 256) rc = launch_lean1<2>(p, smode, a.w != nullptr, use_halo, agg, st);

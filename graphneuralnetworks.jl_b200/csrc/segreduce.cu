@@ -30,13 +30,13 @@ namespace gnnb {
 
 // SegParams: segparams.cuh
 
-// kernel variant (gnnb_set_kernel_variant, A/B runs): 0 = default: the lean work-item kernel (seglean.cu) for rows of
-// 128 / 256 / 512 floats, taking the per-edge scale stream when the caller has one, and seg_reduce_kernel below for every
-// other shape; 10 = the lean kernel gathering cs[col] itself; 12 = seg_reduce_kernel everywhere (the round-1 default);
-// 5 = the same without the 64-register cap; 1 = shared-memory ring filled by cp.async.bulk (segbulk.cu);
-// 13 = the lean pass with the rows staged by TMA tile loads (D = 128 sums; seglean.cu), everything else as 0.
-// Round 1's LDGSTS rings (2..4) and round 2's index-prefetch variants (6..9) were measured slower and removed.
-int g_variant = 0;
+// Reference mode (gnnb_set_kernel_variant(12)): by default (variant 0) rows of 128 / 256 / 512 floats take the lean
+// work-item kernels (seglean.cu, and their GAT counterparts in gat.cu) and every other shape takes seg_reduce_kernel below
+// and the round-1 GAT kernels.  Variant 12 sends every shape to the round-1 kernels.  It stays because it is the
+// reference the tests hold the lean kernels to, bit for bit.  Round 1's LDGSTS rings, round 2's index-prefetch variants,
+// the TMA-staged rings, the lean kernel gathering cs[col] instead of the per-edge scale stream and the uncapped build
+// below were measured no faster than the default and removed (DESIGN.md §4, §7).
+bool g_reference_kernels = false;
 
 template <int VEC> struct VecT;
 template <> struct VecT<4> { using T = float4; };
@@ -248,15 +248,11 @@ template <int VEC, int TPR, int K, bool ISMAX>
 static int launch_seg(const SegParams& p, cudaStream_t st) {
     const int gpb = 256 / TPR;  // groups per block
     dim3 grid((unsigned)ceil_div(p.nchunks, gpb), (unsigned)ceil_div(p.D, (int64_t)VEC * TPR * K));
-    // One warp per 512 B row (D = 128 fp32): throughput follows the number of resident warps, not the loads per warp:
-    // cap the kernel at 64 registers => 4 CTAs x 8 warps per SM.  Variant 5 keeps the
-    // uncapped build (77 registers, 24 warps) for A/B runs.
-    if (VEC == 4 && TPR == 32 && K == 1 && g_variant != 5) {
-        seg_reduce_kernel<4, 32, 1, ISMAX, 8, 4><<<grid, 256, 0, st>>>(p);
-        GNNB_LAUNCHED();
-        return GNNB_OK;
-    }
-    seg_reduce_kernel<VEC, TPR, K, ISMAX><<<grid, 256, 0, st>>>(p);
+    // One warp per 512 B row (D = 128 fp32): capped at 64 registers => 4 CTAs x 8 warps per SM (uncapped it takes 77
+    // registers, 24 warps).  On an H100 at 700 W the uncapped build was 1 % faster in the GCN propagate at 10 M / 100 M
+    // (17.84 against 18.02 ms, DESIGN.md §7); the lean kernel, which serves that shape by default, takes 16.5 ms.
+    constexpr bool ROW512 = VEC == 4 && TPR == 32 && K == 1;
+    seg_reduce_kernel<VEC, TPR, K, ISMAX, ROW512 ? 8 : 0, ROW512 ? 4 : 1><<<grid, 256, 0, st>>>(p);
     GNNB_LAUNCHED();
     return GNNB_OK;
 }
@@ -278,8 +274,7 @@ static int pow2ceil(int64_t v) {
     return p;
 }
 
-int seg_reduce_bulk(const Csr& c, const SegArgs& a, int64_t E, int chunk, float* ws, int fill, int cfg, cudaStream_t st);
-int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, bool use_es, cudaStream_t st);   // seglean.cu
+int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, cudaStream_t st);   // seglean.cu
 
 int seg_reduce(gnnb_graph* g, const Csr& c, const SegArgs& a, cudaStream_t st) {
     if (a.D <= 0) GNNB_FAIL(GNNB_ESIZE, "feature dimension must be positive (got %lld)", (long long)a.D);
@@ -307,8 +302,8 @@ int seg_reduce(gnnb_graph* g, const Csr& c, const SegArgs& a, cudaStream_t st) {
     }
     // the lean work-item kernel (seglean.cu) for rows of 128 / 256 / 512 floats
     int lean_rc = GNNB_EUNSUPPORTED;
-    if (g_variant == 0 || g_variant == 10 || g_variant == 13) {
-        lean_rc = seg_reduce_lean(g, c, a, p.ws, g_variant != 10, st);
+    if (!g_reference_kernels) {
+        lean_rc = seg_reduce_lean(g, c, a, p.ws, st);
         if (lean_rc != GNNB_OK && lean_rc != GNNB_EUNSUPPORTED) return lean_rc;
     }
     if (lean_rc != GNNB_OK && (int64_t)c.nrows > 4 * g->E) {
@@ -322,13 +317,8 @@ int seg_reduce(gnnb_graph* g, const Csr& c, const SegArgs& a, cudaStream_t st) {
                       ((reinterpret_cast<uintptr_t>(a.x2) & 15) == 0) &&
                       ((reinterpret_cast<uintptr_t>(a.out) & 15) == 0);
     int tpr, k;
-    int bulk_rc = GNNB_EUNSUPPORTED;
-    if (lean_rc != GNNB_OK && vec4 && g_variant == 1) {
-        bulk_rc = seg_reduce_bulk(c, a, g->E, g->chunk, p.ws, p.fill, 0, st);
-        if (bulk_rc != GNNB_OK && bulk_rc != GNNB_EUNSUPPORTED) return bulk_rc;
-    }
-    if (lean_rc == GNNB_OK || bulk_rc == GNNB_OK) {
-        // done by the lean kernel (seglean.cu) or a shared-memory-staged kernel (segbulk.cu)
+    if (lean_rc == GNNB_OK) {
+        // done by the lean kernel
     } else if (vec4) {
         int64_t nv = a.D / 4;
         tpr = (int)(nv >= 32 ? 32 : pow2ceil(nv));

@@ -495,12 +495,10 @@ int gnnb_rmat_edges_range(int64_t num_nodes, int64_t first_edge, int64_t count, 
 /* tuning knob for experiments: edges per work chunk of the segmented-reduce kernels (default 128;
  * power of two in [32, 4096]); affects plans created afterwards. */
 int gnnb_set_chunk_edges(int chunk);
-/* A/B switch for the fused segmented reduce on fp32 rows of 128/256/512 floats (results are bit-identical):
- * 0 = default: the lean work-item kernel (csrc/seglean.cu), taking the plan's per-edge scale stream when there is one;
- * 10 = the lean kernel gathering cs[col] per edge;  12 = seg_reduce_kernel (the round-1 default: register-staged
- * LDG.128, 64-register cap);  5 = the same without the register cap;  1 = TMA-staged: one cp.async.bulk (UBLKCP) per
- * row into a shared-memory ring, mbarrier completion;  13 = the lean pass with rows staged by TMA 2-D tile loads (one
- * row per request, four rows per mbarrier, into a per-warp shared-memory ring; D = 128 sums). */
+/* kernels of the fused segmented reduce and of the fused GAT passes (results are bit-identical):
+ * 0 = default: the lean work-item kernels (csrc/seglean.cu, csrc/gat.cu) for rows of 128/256/512 floats, the round-1
+ * chunk kernels for every other shape;  12 = the round-1 chunk kernels (seg_reduce_kernel, gat_fwd_kernel,
+ * gat_bwd_kernel) for every shape: the reference the lean kernels are tested against.  Any other value: GNNB_EINVAL. */
 int gnnb_set_kernel_variant(int v);
 
 #ifdef __cplusplus

@@ -1,5 +1,5 @@
-"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the TMA-staged reduce
-(variant 13), the subgraph plans and the drop mask, meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
+"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans and the
+drop mask, meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gnnb200 as gnn
@@ -53,15 +53,6 @@ for Dm in (128, 256):
     dy = torch.where(torch.isfinite(ym), torch.randn_like(ym), torch.zeros_like(ym))
     ym.backward(dy)
     print("max pullback D", Dm, float(xm.grad.abs().sum()))
-# rows staged by TMA tile loads (variant 13) against the default kernel: same bits
-xs = gnn.unrows(torch.randn(n, 128, device="cuda"))
-ref = gnn.propagate(gnn.copy_xj, g, "+", xj=xs)
-lib.gnnb_set_kernel_variant(13)
-try:
-    got = gnn.propagate(gnn.copy_xj, g, "+", xj=xs)
-finally:
-    lib.gnnb_set_kernel_variant(0)
-print("variant 13 bit-identical", bool(torch.equal(ref, got)))
 # subgraph plans (gnnb_graph_subgraph) and the drop mask (gnnb_bernoulli_keep): the hub graph with both CSRs built, an
 # empty graph, every edge removed, every node removed, extra nodes
 gnn.csr(g, transposed=True)

@@ -44,5 +44,10 @@ def test_argument_errors_map_to_reference_exceptions(gnn):
     with pytest.raises(ValueError):
         gnn._lib.check(lib.gnnb_set_chunk_edges(100))
     assert lib.gnnb_set_chunk_edges(128) == 0
+    for v in (1, 5, 10, 13):            # removed kernel variants: only 0 (default) and 12 (reference) exist
+        with pytest.raises(ValueError):
+            gnn._lib.check(lib.gnnb_set_kernel_variant(v))
+    assert lib.gnnb_set_kernel_variant(12) == 0
+    assert lib.gnnb_set_kernel_variant(0) == 0
     assert lib.gnnb_graph_destroy(None) == 0
     assert b"chunk" in lib.gnnb_last_error() or True
