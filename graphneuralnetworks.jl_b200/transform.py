@@ -11,6 +11,7 @@
     remove_nodes(g, nodes_or_p)      GNNGraphs/src/transform.jl:212-276   (DropNode)
     getgraph(g, i; nmap)             GNNGraphs/src/transform.jl:825-888
     add_nodes(g, n; ndata)           GNNGraphs/src/transform.jl:553-563
+    random_walk_pe(g, walk_length)   GNNGraphs/src/transform.jl:975-990   (per-graph walks, csrc/rwpe.cu)
 
 The index work (pair encoding, stable radix sort, duplicate runs) is csrc/transform.cu; the feature aggregation of
 `remove_multi_edges` is the library's segmented scatter over the run ids it returns — the same kernels as
@@ -34,6 +35,9 @@ Deliberate differences from the reference:
 4. getgraph keeps an edge only when both of its endpoints are kept.  The reference tests only the source: on a batched
    graph the two rules agree, and on other graphs the reference throws a KeyError.
 5. Ids out of range raise AssertionError instead of BoundsError.
+6. random_walk_pe sums each walk step in the plan's edge order instead of forming dense matrix products, so it agrees
+   with the reference to rounding; walk_length < 1 raises AssertionError (the reference throws BoundsError or
+   ArgumentError).
 """
 from __future__ import annotations
 
@@ -329,3 +333,111 @@ def add_nodes(g: GNNGraph, n: int, *, ndata=None) -> GNNGraph:
         gi = torch.cat([gi, torch.full((n,), g.num_graphs, dtype=gi.dtype, device=gi.device)])
     return _with_plan(GNNGraph(s, t, g.w, num_nodes=num_nodes, ndata=nd, edata=g.edata, gdata=g.gdata,
                                num_graphs=g.num_graphs, graph_indicator=gi), plan)
+
+
+# ---------------------------------------------------------------------------------------------- random-walk encoding
+# Segments of at most this many nodes walk in shared memory (gnnb_random_walk_pe, csrc/rwpe.cu); larger ones are composed
+# from the fused propagate.  Must not exceed GNNB_RWPE_SMEM_MAX_NODES (include/gnnb200.h), whose rows the kernel leaves
+# untouched; lowering it (tests do) routes more segments to the propagate route, which overwrites their rows.
+_RWPE_KERNEL_MAX_NODES = 896      # GNNB_RWPE_SMEM_MAX_NODES
+_RWPE_SMEM_MAX_NODES = _RWPE_KERNEL_MAX_NODES
+_RWPE_BLOCK = 128          # sources per propagate pass: D = 128 is the lean kernel's row width
+
+
+def _rwpe_segments(g: GNNGraph, dev) -> Optional[torch.Tensor]:
+    """seg_ptr (int64, on dev) of the runs of equal graph_indicator values, or None (the whole graph is one segment)
+    when there is no indicator, it is not non-decreasing, or an edge joins two graphs."""
+    if g.graph_indicator is None:
+        return None
+    from .generate import _segments
+    order, seg_ptr, _, gi = _segments(g.graph_indicator, g.num_nodes, dev)
+    if order is not None or seg_ptr is None:
+        return None
+    gi = gi.to(device=dev, dtype=torch.int64)
+    if g.num_edges and not bool((gi[g.s.long() - 1] == gi[g.t.long() - 1]).all()):
+        return None
+    return seg_ptr
+
+
+def _rwpe_propagate(g: GNNGraph, w: Optional[torch.Tensor], dinv: torch.Tensor, K: int, out: torch.Tensor) -> None:
+    """out (n, K) = the walks of g (one segment) from `walk_length` launches of the fused propagate per block of
+    _RWPE_BLOCK sources: a one-hot (n, 128) state, u_k = dinv .* propagate(w_mul_xj | copy_xj, g, +; u_{k-1})."""
+    p = g.plan()
+    n, D = g.num_nodes, _RWPE_BLOCK
+    if w is not None and w.numel() == 0:            # a segment without edges: no weights to multiply
+        w = None
+    x = torch.zeros((n, D), dtype=torch.float32, device=p.device)
+    y = torch.empty_like(x)
+    msg = _lib.W_MUL_XJ if w is not None else _lib.COPY_XJ
+    for b0 in range(0, n, D):
+        nb = min(D, n - b0)
+        cols = torch.arange(nb, device=p.device)
+        x.zero_()
+        x[b0 + cols, cols] = 1.0
+        for k in range(K):
+            with torch.cuda.device(p.device):
+                _lib.check(lib.gnnb_propagate(p.h, 0, msg, _lib.SUM, x.data_ptr(), _ptr(w), None, dinv.data_ptr(), D,
+                                              y.data_ptr(), _stream(p.device)))
+            out[b0:b0 + nb, k] = y[b0 + cols, cols]
+            x, y = y, x
+
+
+def random_walk_pe(g: GNNGraph, walk_length: int) -> torch.Tensor:
+    """The random-walk structural encoding — transform.jl:975-990: a (walk_length, num_nodes) float32 matrix with
+    PE[k, j] = (RW^k)[j, j], k = 1..walk_length, RW[i, j] = A[i, j] * dinv[j].  A[i, j] is the summed weight of the
+    edges i -> j (g.w, or 1 without weights; multi-edges add up, self loops count), dinv = 1 / weighted out-degree with
+    +-Inf set to 0: the reference's orientation, the out-degree scales the column node.  Node-major in memory (Julia's
+    (K, N) matrix), on g's compute device.  Not differentiable, like the reference.
+
+    The walk from node j is the row recurrence u_0 = e_j, u_k[t] = dinv[t] * Σ_{edges s -> t} w_e u_{k-1}[s] on the CSR
+    by target (each product and sum rounded, plan order), PE[k, j] = u_k[j]: E_graph multiply-adds per step and per
+    source instead of the reference's K dense N x N products (212 GB per matrix for a batch of 10 000 molecules).
+    Walks never leave a graph, so a batched graph is split into segments, one per run of equal graph_indicator values,
+    when the indicator is non-decreasing and no edge joins two graphs; otherwise the whole graph is one segment.
+      * Segments of at most _RWPE_SMEM_MAX_NODES (896) nodes: gnnb_random_walk_pe, the walk state in shared memory
+        (32 sources per warp or CTA), one launch for all segments of up to 32 nodes and one for the larger ones.
+      * Larger segments, one after the other: per block of 128 sources, walk_length launches of the fused propagate at
+        D = 128 on the segment's plan (derived from g's, no sort).  Memory 2 * n_seg * 128 * 4 bytes; time
+        ceil(n_seg / 128) * walk_length propagates over the segment's edges — seconds for 10^5 nodes, hours for 10^7.
+        No size cap.  Each propagate is followed by two small torch indexing launches, and each such segment first
+        derives its plan in a pass over all of g's nodes and edges, so a batch of many graphs just above the bound costs
+        (number of such graphs) x (N + E) in bookkeeping on top and is bound by launches, not by the propagates.
+    Both routes give the same bits for every row of at most the plan's chunk edges (longer rows are reduced piecewise by
+    the propagate).  Against the reference the only difference is the summation order, so the two agree to rounding."""
+    assert isinstance(walk_length, numbers.Integral) and not isinstance(walk_length, bool) and walk_length >= 1, \
+        f"walk_length = {walk_length} must be an integer >= 1"
+    K = int(walk_length)
+    g = _on_device(g)
+    dev, n = g.s.device, g.num_nodes
+    out = torch.empty((n, K), dtype=torch.float32, device=dev)
+    if n == 0:
+        return unrows(out)
+    p = g.plan()
+    w = None if g.w is None else g.w.to(device=p.device, dtype=torch.float32).contiguous()
+    deg = torch.empty(n, dtype=torch.float32, device=p.device)
+    with torch.cuda.device(p.device):
+        _lib.check(lib.gnnb_degree(p.h, _lib.DIR_OUT, _ptr(w), deg.data_ptr(), _stream(p.device)))
+    dinv = torch.reciprocal(deg)
+    dinv[torch.isinf(dinv)] = 0.0
+    seg_ptr = _rwpe_segments(g, p.device)
+    n_seg = 1 if seg_ptr is None else int(seg_ptr.numel()) - 1
+    bound = min(_RWPE_SMEM_MAX_NODES, _RWPE_KERNEL_MAX_NODES)
+    if seg_ptr is None:
+        big = [] if n <= bound else [0]
+    else:
+        big = ((seg_ptr[1:] - seg_ptr[:-1]) > bound).nonzero().reshape(-1).tolist()
+    if len(big) < n_seg:
+        with torch.cuda.device(p.device):
+            _lib.check(lib.gnnb_random_walk_pe(p.h, _ptr(w), dinv.data_ptr(), _ptr(seg_ptr), n_seg, K, out.data_ptr(),
+                                               _stream(p.device)))
+    for i in big:
+        if n_seg == 1:
+            _rwpe_propagate(g, w, dinv, K, out)
+            continue
+        a, b = int(seg_ptr[i]), int(seg_ptr[i + 1])
+        keep = torch.zeros(n, dtype=torch.uint8, device=p.device)
+        keep[a:b] = 1
+        s, t, n2, kept, plan = _subgraph(g, keep, None)
+        h = _with_plan(GNNGraph(s, t, None if w is None else w[kept], num_nodes=n2), plan)
+        _rwpe_propagate(h, h.w, dinv[a:b].contiguous(), K, out[a:b])
+    return unrows(out)

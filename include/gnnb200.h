@@ -403,6 +403,26 @@ int gnnb_radius_count(const float* points, int64_t n, int d, const int64_t* seg_
 int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,
                      int self_loops, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream);
 
+/* --------------------------------------------------------- random-walk structural encoding (csrc/rwpe.cu)
+ * replaces: random_walk_pe(g, walk_length) (GNNGraphs/src/transform.jl:975-990): K products of the dense N x N matrix
+ *           RW = A * Diagonal(deg_inv), whose diagonals are kept.  Here the walk of each segment runs in shared memory.
+ * PE[k, j] = (RW^k)[j, j] for k = 1..K, RW[i, j] = A[i, j] * dinv[j], A[i, j] = summed weight of the edges i -> j.
+ * Row formulation on the plan's CSR by target: u_0 = e_j, u_k[t] = dinv[t] * Σ_{edges s -> t, plan order} w_e u_{k-1}[s],
+ * each product and sum rounded on its own, a row without edges 0; PE[k, j] = u_k[j].  For rows of at most the plan's
+ * chunk edges that is gnnb_propagate(W_MUL_XJ | COPY_XJ, SUM, ct = dinv) bit for bit.
+ * g: a square plan (GNNB_ESIZE otherwise).  w: E DEVICE floats in COO order, or NULL (every weight 1).  dinv: n DEVICE
+ * floats, 1 / weighted out-degree (gnnb_degree(GNNB_DIR_OUT, w)) with +-Inf replaced by 0 — the caller computes it.
+ * seg_ptr: NULL (one segment) or n_seg + 1 non-decreasing DEVICE offsets from 0 to n, validated on the device
+ * (GNNB_EINVAL).  The walks of a segment never leave it: an edge into a segment this entry walks whose source lies
+ * outside that segment gives GNNB_EINVAL, and nothing is read or written outside a segment.  Edges into the segments
+ * it leaves untouched (below) are not looked at.
+ * out: n x walk_length DEVICE floats, node-major (row j holds PE[1..K, j]).  Rows of segments with more than
+ * GNNB_RWPE_SMEM_MAX_NODES nodes are left untouched: the caller composes those walks from gnnb_propagate.
+ * walk_length >= 1 (GNNB_EINVAL).  Synchronises the stream. */
+#define GNNB_RWPE_SMEM_MAX_NODES 896
+int gnnb_random_walk_pe(gnnb_graph_t g, const float* w, const float* dinv, const int64_t* seg_ptr, int64_t n_seg,
+                        int walk_length, float* out, void* stream);
+
 /* ------------------------------------------------- edge codes and random edges (csrc/edgegen.cu)
  * Code spaces of edge_encoding / edge_decoding (GNNGraphs/src/utils.jl:189-268, bipartite :263-268), 0-based here (the
  * reference's idx - 1), node ids 0-based (s, t < n; bipartite s < n1, t < n2), n1, n2 in [0, 2^31):

@@ -747,4 +747,83 @@ function GNNGraphs.add_nodes(g::GNNGraph{<:CuCOO}, n::Integer; ndata = (;))
     return GNNGraph((s, t, get_edge_weight(g)), num_nodes, length(s), g.num_graphs, gi, ndata, g.edata, g.gdata)
 end
 
+## random_walk_pe on device COO graphs — replaces GNNGraphs/src/transform.jl:975-990 (K products of the dense N x N
+## matrix RW = A * Diagonal(deg_inv), which for a batch of 10 000 molecules is 212 GB per matrix).  The walks of each graph
+## of the batch run in shared memory (gnnb_random_walk_pe); a graph above RWPE_SMEM_MAX_NODES is composed from the fused
+## propagate on its derived plan, 128 sources at a time.  Same routing and same bits as the Python mirror
+## (graphneuralnetworks.jl_b200/transform.py): segments = runs of a non-decreasing graph_indicator that no edge crosses,
+## otherwise the whole graph.
+const RWPE_SMEM_MAX_NODES = 896                               # GNNB_RWPE_SMEM_MAX_NODES
+
+function _rwpe_propagate!(out::CuMatrix{Float32}, p::Plan, n::Integer, w, dinv::CuVector{Float32}, K::Integer)
+    D = 128
+    w = (w === nothing || isempty(w)) ? nothing : w
+    x, y = CUDA.zeros(Float32, D, n), CUDA.zeros(Float32, D, n)
+    for b0 in 0:D:(n - 1)
+        nb = min(D, n - b0)
+        lin = CuVector{Int64}((b0 .+ (0:nb-1)) .* D .+ (1:nb))  # x[c, b0 + c] in column-major (D, n)
+        fill!(x, 0f0)
+        x[lin] .= 1f0
+        for k in 1:K
+            check(ccall((:gnnb_propagate, LIB), Cint,
+                        (Ptr{Cvoid}, Cint, Cint, Cint, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32},
+                         Int64, CuPtr{Float32}, Ptr{Cvoid}),
+                        p.h, 0, w === nothing ? 0 : 1, 0, x, cuptr(w), CU_NULL, dinv, D, y, stream()))
+            out[k, (b0 + 1):(b0 + nb)] .= y[lin]
+            x, y = y, x
+        end
+    end
+    return out
+end
+
+function GNNGraphs.random_walk_pe(g::GNNGraph{<:CuCOO}, walk_length::Int)
+    @assert walk_length >= 1 "walk_length = $walk_length must be >= 1"
+    n, K = g.num_nodes, walk_length
+    out = CuMatrix{Float32}(undef, K, n)                      # column j = PE[1:K, j]: node-major, as the entry writes it
+    n == 0 && return out
+    p = plan(g)
+    w = get_edge_weight(g)
+    w = w === nothing ? nothing : CuVector{Float32}(w)
+    deg = CUDA.zeros(Float32, n)
+    check(ccall((:gnnb_degree, LIB), Cint, (Ptr{Cvoid}, Cint, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                p.h, 0, cuptr(w), deg, stream()))
+    dinv = inv.(deg)
+    dinv[isinf.(dinv)] .= 0f0
+    seg = nothing
+    if g.graph_indicator !== nothing
+        order, _, sg = _knn_segments(g.graph_indicator, n)
+        gi = CuVector{Int64}(g.graph_indicator)
+        s, t = edge_index(g)
+        if order === nothing && sg !== nothing && all(gi[s] .== gi[t])
+            seg = sg
+        end
+    end
+    sp, ns = _knn_seg_args(seg)
+    sizes = seg === nothing ? [n] : Array(seg[2:end] .- seg[1:end-1])
+    big = findall(sizes .> RWPE_SMEM_MAX_NODES)
+    if length(big) < ns
+        check(ccall((:gnnb_random_walk_pe, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Int64}, Int64, Cint, CuPtr{Float32}, Ptr{Cvoid}),
+                    p.h, cuptr(w), dinv, sp, ns, K, out, stream()))
+    end
+    for i in big
+        if seg === nothing
+            _rwpe_propagate!(out, p, n, w, dinv, K)
+            continue
+        end
+        a, b = Array(seg[i:i+1])
+        keep = CUDA.zeros(UInt8, n)
+        keep[(a + 1):b] .= 0x01
+        s, t, m, kept, _ = _subgraph(g, keep, nothing, 0)
+        h = GNNGraph(s, t; num_nodes = m)
+        ws = w === nothing ? nothing : w[kept]
+        sub = view(out, :, (a + 1):b)
+        tmp = CuMatrix{Float32}(undef, K, m)
+        _rwpe_propagate!(tmp, plan(h), m, ws, dinv[(a + 1):b], K)
+        sub .= tmp
+    end
+    return out
+end
+ChainRulesCore.@non_differentiable GNNGraphs.random_walk_pe(::Any...)
+
 end # module

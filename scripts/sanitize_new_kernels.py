@@ -1,5 +1,5 @@
-"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans and the
-drop mask, meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
+"""small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans, the
+drop mask and the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gnnb200 as gnn
@@ -69,5 +69,24 @@ for h in subs:
 keep = torch.empty(1001, dtype=torch.uint8, device="cuda")
 gnn._lib.check(lib.gnnb_bernoulli_keep(1001, 0.5, 3, keep.data_ptr(), None))
 print("bernoulli kept", int(keep.sum()), "of 1001")
+# random_walk_pe: segments of 1, 5, 32 (small launch), 33 and 896 (medium launch) and 897 (propagate route), weighted
+sizes = [1, 5, 32, 33, 896, 897]
+S, T, off = [], [], 0
+for m in sizes:
+    S.append(torch.randint(0, m, (3 * m,), device="cuda") + off); T.append(torch.randint(0, m, (3 * m,), device="cuda") + off)
+    off += m
+s_, t_ = torch.cat(S), torch.cat(T)
+gi = torch.repeat_interleave(torch.arange(1, len(sizes) + 1, device="cuda"), torch.tensor(sizes, device="cuda"))
+gw = gnn.GNNGraph(s_ + 1, t_ + 1, torch.rand(s_.numel(), device="cuda") + 0.5, num_nodes=off, num_graphs=len(sizes),
+                  graph_indicator=gi)
+pe = gnn.random_walk_pe(gw, 6)
+print("random_walk_pe", tuple(pe.shape), "finite", bool(torch.isfinite(pe).all()))
+gx = gnn.GNNGraph(torch.cat([s_, torch.tensor([0], device="cuda")]) + 1, torch.cat([t_, torch.tensor([3], device="cuda")]) + 1,
+                  num_nodes=off)                                   # an edge from the first segment into the second
+deg = gnn.degree(gx, torch.float32, dir="out"); dinv = torch.where(deg != 0, 1 / deg, torch.zeros_like(deg))
+seg = torch.cat([torch.zeros(1, dtype=torch.int64, device="cuda"), torch.cumsum(torch.tensor(sizes, device="cuda"), 0)])
+out = torch.empty(off * 6, device="cuda")
+rc = lib.gnnb_random_walk_pe(gx.plan().h, None, dinv.data_ptr(), seg.data_ptr(), len(sizes), 6, out.data_ptr(), None)
+print("random_walk_pe crossing edge rejected", rc == gnn._lib.EINVAL)
 torch.cuda.synchronize()
 print("done")
