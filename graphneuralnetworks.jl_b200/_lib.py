@@ -96,6 +96,8 @@ _SIGS = {
     "gnnb_bias_act": (_int, [_f32p, _f32p, _int, _i64, _i64, _f32p, _vp]),
     "gnnb_bias_act_bwd": (_int, [_f32p, _f32p, _int, _i64, _i64, _f32p, _f32p, _vp]),
     "gnnb_linear_bwd": (_int, [_f32p, _f32p, _f32p, _f32p, _int, _i64, _i64, _i64, _f32p, _f32p, _f32p, _f32p, _vp]),
+    "gnnb_linear_relu_mask": (_int, [_f32p, _f32p, _f32p, _i64, _i64, _i64, _f32p, _vp, _vp]),
+    "gnnb_linear_bwd_mask": (_int, [_f32p, _vp, _f32p, _f32p, _i64, _i64, _i64, _f32p, _f32p, _f32p, _vp]),
     "gnnb_dense_set_emulation": (_int, [_int]),
     "gnnb_dense_set_tensor_core_kernel": (_int, [_int]),
     "gnnb_dense_tc_error": (_int, []),

@@ -258,7 +258,7 @@ int gnnb_gcn_conv_step_host(gnnb_graph_t g, const float* x_host, const float* W_
     const int64_t Dp = Din;                                // width at which the graph is traversed
     // device staging, carved from one plan-owned allocation: x, p (propagated / pre-propagated), y, dy, dpre, dp, dx, W, b, dW, db
     const size_t nx = (size_t)N * Din, np_ = (size_t)N * Dp, ny = (size_t)N * Dout;
-    const size_t words = nx + np_ + ny + (bwd ? (ny + ny + np_ + nx) : 0) + 2 * (size_t)(Dout * Din) + 2 * (size_t)Dout + 64;
+    const size_t words = nx + np_ + ny + (bwd ? (ny + ny + np_ + nx + (size_t)N * 4) : 0) + 2 * (size_t)(Dout * Din) + 2 * (size_t)Dout + 64;
     if (g->host_ws_bytes < words * sizeof(float)) {
         if (g->host_ws) { cudaDeviceSynchronize(); cudaFree(g->host_ws); g->host_ws = nullptr; g->host_ws_bytes = 0; }
         GNNB_CUDA(cudaMalloc(&g->host_ws, words * sizeof(float)));
@@ -269,6 +269,9 @@ int gnnb_gcn_conv_step_host(gnnb_graph_t g, const float* x_host, const float* W_
     float *x = take(nx), *p = take(np_), *y = take(ny);
     float *dy = bwd ? take(ny) : nullptr, *dpre = bwd ? take(ny) : nullptr, *dp = bwd ? take(np_) : nullptr, *dx = bwd ? take(nx) : nullptr;
     float *W = take((size_t)(Dout * Din)), *b = take((size_t)Dout), *dW = take((size_t)(Dout * Din)), *db = take((size_t)Dout);
+    // the relu mask of y (N x 4 words, 16 B aligned like every carve): the pullback reads it instead of y where it can
+    uint32_t* mask = bwd ? reinterpret_cast<uint32_t*>(take((size_t)N * 4)) : nullptr;
+    bool masked = false;
     cudaStream_t s_main = nullptr, s_in = nullptr, s_out = nullptr;
     cudaEvent_t ev_x = nullptr, ev_dy = nullptr, ev_y = nullptr, ev_dx = nullptr;
     int status = GNNB_OK;
@@ -292,13 +295,22 @@ int gnnb_gcn_conv_step_host(gnnb_graph_t g, const float* x_host, const float* W_
     }
     HP(cudaStreamWaitEvent(s_main, ev_x, 0));
     HT(gnnb_gcn_propagate(g, 0, x, nullptr, nullptr, Dp, p, s_main));                     // p = Â x
-    HT(gnnb_linear(p, W, b_host ? b : nullptr, relu, N, Din, Dout, y, s_main));           // y = act(W p + b)
+    if (bwd && relu && Dout == 128) {                                                     // y = relu(W p + b) + mask
+        const int rc = gnnb_linear_relu_mask(p, W, b_host ? b : nullptr, N, Din, Dout, y, mask, s_main);
+        if (rc != GNNB_OK && rc != GNNB_EUNSUPPORTED) HT(rc);
+        masked = rc == GNNB_OK;
+    }
+    if (!masked) HT(gnnb_linear(p, W, b_host ? b : nullptr, relu, N, Din, Dout, y, s_main));  // y = act(W p + b)
     HP(cudaEventRecord(ev_y, s_main));
     HP(cudaStreamWaitEvent(s_out, ev_y, 0));
     HP(cudaMemcpyAsync(y_host, y, sizeof(float) * ny, cudaMemcpyDeviceToHost, s_out));
     if (bwd) {
         HP(cudaStreamWaitEvent(s_main, ev_dy, 0));
-        HT(gnnb_linear_bwd(dy, y, p, W, relu, N, Din, Dout, dpre, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
+        if (masked) {
+            HT(gnnb_linear_bwd_mask(dy, mask, p, W, N, Din, Dout, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
+        } else {
+            HT(gnnb_linear_bwd(dy, y, p, W, relu, N, Din, Dout, dpre, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
+        }
         HT(gnnb_gcn_propagate(g, 1, dp, nullptr, nullptr, Dp, dx, s_main));               // dx = Â' dp
         HP(cudaEventRecord(ev_dx, s_main));
         HP(cudaStreamWaitEvent(s_out, ev_dx, 0));

@@ -116,8 +116,10 @@ int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* b
                      int64_t K, int64_t Nout, float* y, cudaStream_t st);
 int linear_tf32x3_error();
 int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t Dout, float* dW, cudaStream_t st);
-int linear_bwd_tf32x3(const float* dy, const float* y, const float* x, const float* W, int64_t M, int64_t Din, float* dx,
-                      float* dW, float* db, cudaStream_t st);
+int linear_relu_mask_tf32x3(const float* x, const float* W, const float* bias, int64_t M, int64_t K, float* y, uint32_t* mask,
+                            cudaStream_t st);
+int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, const float* x, const float* W, int64_t M,
+                      int64_t Din, float* dx, float* dW, float* db, cudaStream_t st);
 extern int g_tc_enabled;
 
 __global__ void transpose_small_kernel(const float* __restrict__ w, int rows, int cols, float* __restrict__ wt) {
@@ -337,7 +339,7 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
     if (!dy || !W) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     if (relu && (!y || !dpre_ws)) GNNB_FAIL(GNNB_EINVAL, "relu pullback needs the forward output and a (N,Dout) workspace");
     if (dx && dW && x && Dout == 128) {   // the fused pullback: dpre stays on chip, dpre_ws is not touched
-        const int rc = linear_bwd_tf32x3(dy, relu ? y : nullptr, x, W, N, Din, dx, dW, db, st);
+        const int rc = linear_bwd_tf32x3(dy, relu ? y : nullptr, nullptr, x, W, N, Din, dx, dW, db, st);
         if (rc != GNNB_EUNSUPPORTED) return rc;
     }
     const float* dpre = dy;
@@ -384,6 +386,35 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
         GNNB_TRY(lt::matmul(CUBLAS_OP_N, CUBLAS_OP_T, Din, Dout, N, x, Din, dpre, Dout, dW, Din, nullptr, 0, st));
     }
     return GNNB_OK;
+}
+
+int gnnb_linear_relu_mask(const float* x, const float* W, const float* bias, int64_t N, int64_t Din, int64_t Dout, float* y,
+                          uint32_t* mask, void* stream) {
+    if (N < 0 || Din <= 0 || Dout <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
+    if (Dout != 128) GNNB_FAIL(GNNB_EUNSUPPORTED, "linear_relu_mask: Dout must be 128");
+    if (N > 0 && (!x || !W || !y || !mask)) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    const int rc = linear_relu_mask_tf32x3(x, W, bias, N, Din, y, mask, (cudaStream_t)stream);
+    if (rc == GNNB_EUNSUPPORTED)
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "linear_relu_mask: Din must be 32, 64, 96 or 128, operands 16 B aligned, tensor-core kernels on");
+    return rc;
+}
+
+int gnnb_linear_bwd_mask(const float* dy, const uint32_t* mask, const float* x, const float* W, int64_t N, int64_t Din,
+                         int64_t Dout, float* dx, float* dW, float* db, void* stream) {
+    if (N < 0 || Din <= 0 || Dout <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
+    if (Dout != 128 || Din % 32 != 0 || Din > 128 || !g_tc_enabled)
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "linear_bwd_mask: Dout must be 128, Din 32, 64, 96 or 128, tensor-core kernels on");
+    if (!dx || !dW) GNNB_FAIL(GNNB_EINVAL, "linear_bwd_mask computes dx and dW together: both are required");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (N == 0) {
+        GNNB_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)(Din * Dout), st));
+        if (db) GNNB_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * (size_t)Dout, st));
+        return GNNB_OK;
+    }
+    if (!dy || !mask || !x || !W) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    const int rc = linear_bwd_tf32x3(dy, nullptr, mask, x, W, N, Din, dx, dW, db, st);
+    if (rc == GNNB_EUNSUPPORTED) GNNB_FAIL(GNNB_EUNSUPPORTED, "linear_bwd_mask: operands must be 16 B aligned");
+    return rc;
 }
 
 }  // extern "C"

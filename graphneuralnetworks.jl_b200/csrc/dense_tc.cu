@@ -132,13 +132,24 @@ struct Params {
     const float* __restrict__ wimg;  // wide kernel only: W split and swizzled per (quarter, K-block), see tcx::w_image_kernel
     const float* __restrict__ act;   // linear_bwd_dx_kernel only: forward output for the relu mask, or null (no mask)
     float* __restrict__ colsum;      // linear_bwd_dx_kernel only: [grid][4 producer warps][128] column sums of dpre, or null
+    uint32_t* __restrict__ mask;     // linear_relu_mask_kernel: [M][4] relu mask words written beside y;
+                                     // linear_bwd_dx_mask_kernel: read in place of act
 };
 
-// epilogue of one 64 x 128 accumulator pair: columns col_base + [0, 128) of rows row0 + [0, 64), `ncols` of them valid
+// The relu mask of a 128-wide layer output, 4 words (16 B) per row: bit 2j + c of word w of row r is (y[r][8j + 2w + c] > 0)
+// for j < 16, c < 2; equivalently column n is bit 2 (n >> 3) + (n & 1) of word (n >> 1) & 3.  This is the accumulator
+// fragment's own order (register 4j + 2h + c of lane l is column 8j + 2(l%4) + c), so lane l of the epilogue owns word l%4
+// of each of its rows whole, and a warp's stores for one h are 8 rows x 16 B, contiguous.  The bit is taken from the value
+// y holds after the relu, so it agrees with `y > 0` on y as stored (-0 and NaN inputs give 0).
+
+// epilogue of one 64 x 128 accumulator pair: columns col_base + [0, 128) of rows row0 + [0, 64), `ncols` of them valid.
+// MASK: also the relu mask words of the rows (relu on, col_base 0, ncols = Nout = 128)
+template <bool MASK = false>
 __device__ __forceinline__ void store_tile(const Params& p, const float* dm, const float* dc, const float* sbias, int64_t row0,
                                            int col_base, int ncols) {
     const int lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3;
     const int64_t r0 = row0 + w4 * 16 + (lane >> 2);
+    uint32_t mw[2] = {0u, 0u};
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
         const int c = 8 * j + 2 * (lane & 3);
@@ -156,11 +167,20 @@ __device__ __forceinline__ void store_tile(const Params& p, const float* dm, con
             }
             if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
             *reinterpret_cast<float2*>(p.y + at) = o;
+            if (MASK) mw[h] |= ((uint32_t)(o.x > 0.f) << (2 * j)) | ((uint32_t)(o.y > 0.f) << (2 * j + 1));
+        }
+    }
+    if (MASK) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t row = r0 + 8 * h;
+            if (row < p.M) p.mask[(size_t)row * 4 + (lane & 3)] = mw[h];
         }
     }
 }
 
 // consumer warpgroups of the ring kernels: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile of this CTA
+template <bool MASK = false>
 __device__ __forceinline__ void consume_tiles(const Params& p, uint32_t sbase, const float* sbias, int KB, int64_t ntiles) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
@@ -177,11 +197,13 @@ __device__ __forceinline__ void consume_tiles(const Params& p, uint32_t sbase, c
             mma_kblock(dm, dc, a_big, a_small, w_big, w_small, kb == 0);
             if (lane == 0) bar_arrive(bar_empty + 8 * stage);   // this warp's reads of the stage are complete
         }
-        if (alive) store_tile(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
+        if (alive) store_tile<MASK>(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
     }
 }
 
-__global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params p) {
+// MASK: linear_relu_mask_kernel, which also writes the relu mask of y (Nout = 128, relu on)
+template <bool MASK>
+__device__ __forceinline__ void linear_body(const Params& p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5;
     const int KB = p.K / BK;                                   // K-blocks per tile (<= 4)
@@ -252,15 +274,21 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params 
             for (int i = 0; i < 8; ++i) v[i] = vn[i];
         }
     } else {
-        consume_tiles(p, sbase, sbias, KB, ntiles);
+        consume_tiles<MASK>(p, sbase, sbias, KB, ntiles);
     }
 }
+
+__global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params p) { linear_body<false>(p); }
+__global__ void __launch_bounds__(THREADS, 1) linear_relu_mask_kernel(const Params p) { linear_body<true>(p); }
 
 // dx = dpre * W for dpre = relu ? (y > 0 ? dy : 0) : dy, Dout = 128 rows of W and Din = Nout <= 128 columns.  The producers
 // form dpre from dy and the forward output y (p.act) in registers, so dpre is never stored, and add it into per-thread
 // column sums for db.  Tiles, images and the MMA sequence are those of linear_tf32x3_kernel run on a transposed copy of W
 // with a zero bias, so dx has the same bits as that composition; W is read transposed straight into the images instead.
-__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params p) {
+// MASK: linear_bwd_dx_mask_kernel, which reads the relu mask bits (p.mask, always on) in place of y: the same dpre, from
+// 16 B per row instead of 512.
+template <bool MASK>
+__device__ __forceinline__ void bwd_dx_body(const Params& p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t ntiles = (p.M + BM - 1) / BM;
@@ -299,7 +327,10 @@ __global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params 
         // flattened (tile, K-block) sequence of this CTA, as in linear_tf32x3_kernel
         const int64_t my_tiles = (ntiles > (int64_t)blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
         const int64_t total = my_tiles * 4;
-        auto fetch = [&](int64_t item, float4* g, float4* m) {
+        // the relu mask of the 4 columns 32 kb + 4 c .. + 3 a thread loads: MASK, words 2 (c & 1) and 2 (c & 1) + 1 of the
+        // row's mask (bits 8 kb + 2 (c >> 1) and the next of each); otherwise the 4 floats of y
+        using MaskReg = typename std::conditional<MASK, uint2, float4>::type;
+        auto fetch = [&](int64_t item, float4* g, MaskReg* m) {
             const int64_t tile = blockIdx.x + (item >> 2) * gridDim.x;
             const int kb = (int)(item & 3);
 #pragma unroll
@@ -308,31 +339,42 @@ __global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params 
                 const bool in = item < total && row < p.M;
                 const size_t at = (size_t)row * 128 + kb * BK;
                 g[i] = in ? __ldg(reinterpret_cast<const float4*>(p.x + at) + c) : zero;
-                m[i] = (in && p.act) ? __ldg(reinterpret_cast<const float4*>(p.act + at) + c) : zero;
+                if constexpr (MASK) m[i] = in ? __ldg(reinterpret_cast<const uint2*>(p.mask + (size_t)row * 4) + (c & 1)) : make_uint2(0u, 0u);
+                else m[i] = (in && p.act) ? __ldg(reinterpret_cast<const float4*>(p.act + at) + c) : zero;
             }
         };
         // dpre = act ? (act > 0 ? g : 0) : g, applied when the prefetched registers are promoted: holding the mask of the
-        // current item as well would not fit beside the next item's loads
-        auto masked = [&](float4* g, const float4* m) {
-            if (!p.act) return;
+        // current item as well would not fit beside the next item's loads.  kb: the K-block of the item in g
+        auto masked = [&](float4* g, const MaskReg* m, int kb) {
+            if constexpr (MASK) {
+                const int s = 8 * kb + 2 * (c >> 1);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                g[i].x = m[i].x > 0.f ? g[i].x : 0.f; g[i].y = m[i].y > 0.f ? g[i].y : 0.f;
-                g[i].z = m[i].z > 0.f ? g[i].z : 0.f; g[i].w = m[i].w > 0.f ? g[i].w : 0.f;
+                for (int i = 0; i < 8; ++i) {
+                    g[i].x = (m[i].x >> s) & 1u ? g[i].x : 0.f; g[i].y = (m[i].x >> (s + 1)) & 1u ? g[i].y : 0.f;
+                    g[i].z = (m[i].y >> s) & 1u ? g[i].z : 0.f; g[i].w = (m[i].y >> (s + 1)) & 1u ? g[i].w : 0.f;
+                }
+            } else {
+                if (!p.act) return;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    g[i].x = m[i].x > 0.f ? g[i].x : 0.f; g[i].y = m[i].y > 0.f ? g[i].y : 0.f;
+                    g[i].z = m[i].z > 0.f ? g[i].z : 0.f; g[i].w = m[i].w > 0.f ? g[i].w : 0.f;
+                }
             }
         };
         // column sums of dpre: after each item the 4 threads of a warp that share a column group add theirs in a fixed
         // order, and lanes 8 kb .. 8 kb + 7 keep the sums of K-block kb (columns 32 kb + 4 c .. + 3)
         float4 cs = zero;
-        float4 g[8], gn[8], mn[8];
+        float4 g[8], gn[8];
+        MaskReg mn[8];
         fetch(0, g, mn);
-        masked(g, mn);
+        masked(g, mn, 0);
         for (int64_t it = 0; it < total; ++it) {
             const int kb = (int)(it & 3);
             if (tid == 0 && kb == 0 && it + 4 < total) {       // the next tile of this CTA into L2
                 const int64_t r0 = (blockIdx.x + ((it >> 2) + 1) * gridDim.x) * BM, nr = (p.M - r0 < BM) ? p.M - r0 : BM;
                 prefetch_l2(p.x + (size_t)r0 * 128, (uint32_t)(nr * 512));
-                if (p.act) prefetch_l2(p.act + (size_t)r0 * 128, (uint32_t)(nr * 512));
+                if (!MASK && p.act) prefetch_l2(p.act + (size_t)r0 * 128, (uint32_t)(nr * 512));
             }
             fetch(it + 1, gn, mn);
             if (p.colsum) {
@@ -361,13 +403,16 @@ __global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params 
             bar_arrive(bar_full + 8 * stage);
 #pragma unroll
             for (int i = 0; i < 8; ++i) g[i] = gn[i];
-            masked(g, mn);
+            masked(g, mn, (kb + 1) & 3);
         }
         if (p.colsum) reinterpret_cast<float4*>(p.colsum + ((size_t)blockIdx.x * 4 + warp) * 128 + (lane >> 3) * BK)[c] = cs;
     } else {
         consume_tiles(p, sbase, sbias, 128 / BK, ntiles);
     }
 }
+
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params p) { bwd_dx_body<false>(p); }
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_mask_kernel(const Params p) { bwd_dx_body<true>(p); }
 }  // namespace tc
 
 // =====================================================================================================================
@@ -397,6 +442,7 @@ struct ParamsW {
     int Din;
     int* err;
     const float* __restrict__ act;    // linear_bwd_dw_kernel only: forward output y, dpre = y > 0 ? dy : 0; null: dpre = dy
+    const uint32_t* __restrict__ mask;  // linear_bwd_dw_mask_kernel only: [M][4] relu mask of y (layout: above tc::store_tile)
 };
 constexpr int L2_AHEAD = 3;           // linear_bwd_dw_kernel: row blocks prefetched into L2 ahead of the register loads
 
@@ -406,8 +452,9 @@ __device__ __forceinline__ int kmajor_off(int n, int k) {
 }
 
 // FUSED: the fused pullback's variant, which forms dpre from dy and the relu mask of p.act in the producers and prefetches
-// the rows L2_AHEAD blocks ahead into L2; otherwise p.dpre is read as it is
-template <bool FUSED>
+// the rows L2_AHEAD blocks ahead into L2; otherwise p.dpre is read as it is.  MASK (with FUSED): the relu mask comes from
+// the bits of p.mask instead of y.
+template <bool FUSED, bool MASK = false>
 __device__ __forceinline__ void dw_body(const ParamsW& p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -474,6 +521,44 @@ __device__ __forceinline__ void dw_body(const ParamsW& p) {
                 if (!stage_in(blk, va, vb)) break;
 #pragma unroll
                 for (int q = 0; q < 8; ++q) { va[q] = na[q]; vb[q] = nb[q]; }
+            }
+        } else if constexpr (MASK) {
+            // as below with the mask bits in place of y: the 4 columns 4 f .. 4 f + 3 of a thread's float4 f are bits
+            // 2 (f >> 1) and the next of words 2 (fl & 1) and 2 (fl & 1) + 1 of the row's mask (f & 1 == fl & 1), so
+            // the two float4 of one row (q and q + 4) share one 8 B load
+            float4 va[8], vb[8], na[8];
+            uint2 nm[4];
+            auto load_mask = [&](int64_t blk) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int64_t r = r_begin + blk * 32 + rl + 8 * q;
+                    nm[q] = (blk < nblk && r < r_end) ? __ldg(reinterpret_cast<const uint2*>(p.mask + (size_t)r * 4) + (fl & 1))
+                                                      : make_uint2(0u, 0u);
+                }
+            };
+            auto promote = [&]() {
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const uint2 m = nm[q & 3];
+                    const int s = 4 * (warp + 4 * (q >> 2)) + 2 * (fl >> 1);
+                    va[q].x = (m.x >> s) & 1u ? na[q].x : 0.f; va[q].y = (m.x >> (s + 1)) & 1u ? na[q].y : 0.f;
+                    va[q].z = (m.y >> s) & 1u ? na[q].z : 0.f; va[q].w = (m.y >> (s + 1)) & 1u ? na[q].w : 0.f;
+                }
+            };
+            load(p.dpre, 128, 32, 0, na);
+            load_mask(0);
+            promote();
+            for (int64_t blk = 0; blk < nblk; ++blk) {
+                if (tid == 0 && blk + L2_AHEAD < nblk) {
+                    const int64_t ra = r_begin + 32 * (blk + L2_AHEAD), nr = (r_end - ra < 32) ? r_end - ra : 32;
+                    prefetch_l2(p.dpre + (size_t)ra * 128, (uint32_t)(nr * 512));
+                    prefetch_l2(p.x + (size_t)ra * p.Din, (uint32_t)(nr * p.Din * 4));
+                }
+                load(p.dpre, 128, 32, blk + 1, na);
+                load_mask(blk + 1);
+                load(p.x, p.Din, nfB, blk, vb);
+                if (!stage_in(blk, va, vb)) break;
+                promote();
             }
         } else {
             // dy and y are loaded one block ahead into registers and the mask is applied when they are promoted; x is
@@ -542,6 +627,7 @@ __device__ __forceinline__ void dw_body(const ParamsW& p) {
 
 __global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) { dw_body<false>(p); }
 __global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_kernel(const ParamsW p) { dw_body<true>(p); }
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_mask_kernel(const ParamsW p) { dw_body<true, true>(p); }
 
 // dW[i] = sum of the n-float partials; with db: threads n .. n + 127 add the 128-float column-sum partials into db
 __global__ void dw_reduce_kernel(const float* __restrict__ partial, int nparts, int n, float* __restrict__ dW,
@@ -702,9 +788,21 @@ int linear_tf32x3(const float* x, const float* W, const float* bias, int relu, i
                   cudaStream_t st) {
     return linear_tf32x3_ex(x, W, K, bias, nullptr, relu, M, K, Nout, y, st);
 }
+static int linear_launch(const float* x, const float* W, int64_t ldw, const float* bias, const float* addend, int relu,
+                         int64_t M, int64_t K, int64_t Nout, float* y, uint32_t* mask, cudaStream_t st);
 // W rows `ldw` floats apart (a column block of a wider matrix); addend (M, Nout) added before the activation
 int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* bias, const float* addend, int relu, int64_t M,
                      int64_t K, int64_t Nout, float* y, cudaStream_t st) {
+    return linear_launch(x, W, ldw, bias, addend, relu, M, K, Nout, y, nullptr, st);
+}
+// y = relu(x W^T + bias) and its relu mask (M, 4 words; layout above tc::store_tile) for Nout = 128, K in {32, 64, 96, 128}
+int linear_relu_mask_tf32x3(const float* x, const float* W, const float* bias, int64_t M, int64_t K, float* y, uint32_t* mask,
+                            cudaStream_t st) {
+    if (K % 32 != 0 || K < 32 || K > 128 || ((uintptr_t)mask & 15)) return GNNB_EUNSUPPORTED;
+    return linear_launch(x, W, K, bias, nullptr, 1, M, K, 128, y, mask, st);
+}
+static int linear_launch(const float* x, const float* W, int64_t ldw, const float* bias, const float* addend, int relu,
+                         int64_t M, int64_t K, int64_t Nout, float* y, uint32_t* mask, cudaStream_t st) {
     if (!g_tc_enabled) return GNNB_EUNSUPPORTED;
     const bool wide = K > 128 || Nout > 128;
     if (wide) {
@@ -719,6 +817,7 @@ int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* b
     static int nsm = 0;
     if (!configured) {
         GNNB_CUDA(cudaFuncSetAttribute(tc::linear_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_relu_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
         GNNB_CUDA(cudaFuncSetAttribute(tcx::linear_wide_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcx::SMEM_TOTAL_X));
         int dev = 0;
         GNNB_CUDA(cudaGetDevice(&dev));
@@ -729,7 +828,7 @@ int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* b
     }
     tc::Params p;
     p.x = x; p.w = W; p.bias = bias; p.addend = addend; p.y = y; p.M = M; p.K = (int)K; p.Nout = (int)Nout; p.relu = relu;
-    p.ldw = (int)ldw; p.err = g_tc_err; p.wimg = nullptr; p.act = nullptr; p.colsum = nullptr;
+    p.ldw = (int)ldw; p.err = g_tc_err; p.wimg = nullptr; p.act = nullptr; p.colsum = nullptr; p.mask = mask;
     if (wide) {
         // the split, swizzled image of W (2 x its size), rebuilt per call: W changes between training steps
         static float* wimg = nullptr; static size_t wimg_elems = 0;
@@ -746,6 +845,7 @@ int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* b
     const int64_t ntiles = ceil_div(M, tc::BM);
     const unsigned grid = (unsigned)(ntiles < nsm ? ntiles : nsm);
     if (wide) tcx::linear_wide_tf32x3_kernel<<<grid, tc::THREADS, tcx::SMEM_TOTAL_X, st>>>(p);
+    else if (mask) tc::linear_relu_mask_kernel<<<grid, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
     else tc::linear_tf32x3_kernel<<<grid, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
     GNNB_LAUNCHED();
     return GNNB_OK;
@@ -770,7 +870,7 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
     }
     if (M == 0) { GNNB_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)(Dout * Din), st)); return GNNB_OK; }
     tcw::ParamsW p;
-    p.dpre = dpre; p.x = x; p.partial = partial; p.M = M; p.Din = (int)Din; p.err = g_tc_err; p.act = nullptr;
+    p.dpre = dpre; p.x = x; p.partial = partial; p.M = M; p.Din = (int)Din; p.err = g_tc_err; p.act = nullptr; p.mask = nullptr;
     int64_t rpc = ceil_div(M, nsm);
     rpc = ceil_div(rpc, 32) * 32;
     p.rows_per_cta = rpc;
@@ -786,18 +886,22 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
 // The dense layer's whole pullback for Dout = 128, Din in {32, 64, 96, 128}: dpre = y > 0 ? dy : 0 (y non-null, relu) or
 // dy, dx = dpre W, dW = dpre^T x and db = column sums of dpre (db may be null), in three launches that read dy, y and x
 // once each per product and never store dpre.  dx has the bits of linear_tf32x3 on dpre and W^T, dW those of dw_tf32x3
-// on dpre; GNNB_EUNSUPPORTED for anything else.
-int linear_bwd_tf32x3(const float* dy, const float* y, const float* x, const float* W, int64_t M, int64_t Din, float* dx,
-                      float* dW, float* db, cudaStream_t st) {
+// on dpre; GNNB_EUNSUPPORTED for anything else.  mask (non-null, y null): the relu mask linear_relu_mask_tf32x3 wrote beside
+// y, read in place of y by the *_mask_kernel variants, with the same bits in every output.
+int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, const float* x, const float* W, int64_t M,
+                      int64_t Din, float* dx, float* dW, float* db, cudaStream_t st) {
     if (!g_tc_enabled) return GNNB_EUNSUPPORTED;
     if (Din % 32 != 0 || Din > 128 || Din < 32 || M <= 0) return GNNB_EUNSUPPORTED;
-    if (((uintptr_t)dy & 15) || ((uintptr_t)y & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dx & 15)) return GNNB_EUNSUPPORTED;
+    if (((uintptr_t)dy & 15) || ((uintptr_t)y & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dx & 15) || ((uintptr_t)mask & 15))
+        return GNNB_EUNSUPPORTED;
     static bool configured = false;
     static int nsm = 0;
     static float *partial = nullptr, *colsum = nullptr;
     if (!configured) {
         GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
         GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
         int dev = 0;
         GNNB_CUDA(cudaGetDevice(&dev));
         GNNB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
@@ -810,17 +914,20 @@ int linear_bwd_tf32x3(const float* dy, const float* y, const float* x, const flo
     tc::Params p;
     p.x = dy; p.w = W; p.bias = nullptr; p.addend = nullptr; p.y = dx; p.M = M; p.K = 128; p.Nout = (int)Din; p.relu = 0;
     p.ldw = 128; p.err = g_tc_err; p.wimg = nullptr; p.act = y; p.colsum = db ? colsum : nullptr;
+    p.mask = const_cast<uint32_t*>(mask);
     const int64_t ntiles = ceil_div(M, tc::BM);
     const int grid_dx = (int)(ntiles < nsm ? ntiles : nsm);
-    tc::linear_bwd_dx_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
+    if (mask) tc::linear_bwd_dx_mask_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
+    else tc::linear_bwd_dx_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
     GNNB_LAUNCHED();
     // dW: the split-K partition of dw_tf32x3
     tcw::ParamsW pw;
-    pw.dpre = dy; pw.x = x; pw.partial = partial; pw.M = M; pw.Din = (int)Din; pw.err = g_tc_err; pw.act = y;
+    pw.dpre = dy; pw.x = x; pw.partial = partial; pw.M = M; pw.Din = (int)Din; pw.err = g_tc_err; pw.act = y; pw.mask = mask;
     const int64_t rpc = ceil_div(ceil_div(M, nsm), 32) * 32;
     pw.rows_per_cta = rpc;
     const int grid_dw = (int)ceil_div(M, rpc);
-    tcw::linear_bwd_dw_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw);
+    if (mask) tcw::linear_bwd_dw_mask_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw);
+    else tcw::linear_bwd_dw_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw);
     GNNB_LAUNCHED();
     const int n = (int)(128 * Din);
     tcw::dw_reduce_kernel<<<(unsigned)ceil_div(n + 128, 256), 256, 0, st>>>(partial, grid_dw, n, dW, colsum, grid_dx * 4, db);

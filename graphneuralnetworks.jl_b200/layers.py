@@ -65,6 +65,11 @@ def _add_bias(x: torch.Tensor, b) -> torch.Tensor:
     return x + b.reshape(-1, 1)
 
 
+# relu layers whose pullback wants dx and dW keep the relu mask as bits (gnnb_linear_relu_mask, 16 B per node) instead of
+# y for the backward pass, on the shapes that entry serves; False keeps y (the results are the same bits either way)
+RELU_MASK = True
+
+
 class _LinearFn(torch.autograd.Function):
     """σ.(W * x .+ b) for σ ∈ {identity, relu} through gnnb_linear / gnnb_linear_bwd (cuBLASLt GEMM with the bias and
     relu in the epilogue, fp32-emulated on bf16 tensor cores when available; hand-written relu/bias-grad pullback)."""
@@ -75,16 +80,27 @@ class _LinearFn(torch.autograd.Function):
         Dout = W.shape[0]
         y = torch.empty((N, Dout), dtype=torch.float32, device=x_rows.device)
         Wc = W.contiguous()
+        bp = None if bias is None else bias.data_ptr()
+        mask = None
         with torch.cuda.device(x_rows.device):
-            _lib.check(lib.gnnb_linear(x_rows.data_ptr(), Wc.data_ptr(), None if bias is None else bias.data_ptr(),
-                                       int(relu_flag), N, Din, Dout, y.data_ptr(), _stream(x_rows.device)))
-        ctx.relu_flag, ctx.has_bias = bool(relu_flag), bias is not None
-        ctx.save_for_backward(x_rows, Wc, y if relu_flag else None)
+            if relu_flag and RELU_MASK and ctx.needs_input_grad[0] and ctx.needs_input_grad[1]:
+                mask = torch.empty((N, 4), dtype=torch.int32, device=x_rows.device)
+                rc = lib.gnnb_linear_relu_mask(x_rows.data_ptr(), Wc.data_ptr(), bp, N, Din, Dout, y.data_ptr(),
+                                               mask.data_ptr(), _stream(x_rows.device))
+                if rc == _lib.EUNSUPPORTED:
+                    mask = None
+                else:
+                    _lib.check(rc)
+            if mask is None:
+                _lib.check(lib.gnnb_linear(x_rows.data_ptr(), Wc.data_ptr(), bp, int(relu_flag), N, Din, Dout,
+                                           y.data_ptr(), _stream(x_rows.device)))
+        ctx.relu_flag, ctx.has_bias, ctx.masked = bool(relu_flag), bias is not None, mask is not None
+        ctx.save_for_backward(x_rows, Wc, mask if mask is not None else (y if relu_flag else None))
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x_rows, W, y = ctx.saved_tensors
+        x_rows, W, y = ctx.saved_tensors       # y: the relu mask instead when ctx.masked
         dy = dy.contiguous()
         N, Din = x_rows.shape
         Dout = W.shape[0]
@@ -92,9 +108,13 @@ class _LinearFn(torch.autograd.Function):
         dx = torch.empty_like(x_rows) if need_dx else None
         dW = torch.empty_like(W) if need_dW else None
         db = torch.empty(Dout, dtype=torch.float32, device=dy.device) if need_db else None
-        ws = torch.empty_like(dy) if ctx.relu_flag else None
         p = lambda t: None if t is None else t.data_ptr()
         with torch.cuda.device(dy.device):
+            if ctx.masked:
+                _lib.check(lib.gnnb_linear_bwd_mask(dy.data_ptr(), y.data_ptr(), x_rows.data_ptr(), W.data_ptr(), N, Din,
+                                                    Dout, p(dx), p(dW), p(db), _stream(dy.device)))
+                return dx, dW, db, None
+            ws = torch.empty_like(dy) if ctx.relu_flag else None
             _lib.check(lib.gnnb_linear_bwd(dy.data_ptr(), p(y), x_rows.data_ptr(), W.data_ptr(), int(ctx.relu_flag), N, Din,
                                            Dout, p(ws), p(dx), p(dW), p(db), _stream(dy.device)))
         return dx, dW, db, None

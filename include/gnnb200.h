@@ -238,6 +238,15 @@ int gnnb_linear(const float* x, const float* W, const float* bias, int relu, int
  * gradient are one hand-written pass (deterministic two-stage column sum). */
 int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float* W, int relu, int64_t N,
                     int64_t Din, int64_t Dout, float* dpre_ws, float* dx, float* dW, float* db, void* stream);
+/* The relu layer with its mask kept as bits: gnnb_linear (relu = 1) that also writes mask (N x 4 words, 16 B aligned), bit
+ * by bit `y > 0` of y as stored, in a layout private to the library; gnnb_linear_bwd_mask is gnnb_linear_bwd (relu = 1)
+ * reading that mask instead of y, 16 B instead of 512 per node, with the same bits in dx, dW and db.  dx and dW are both
+ * required there, db may be NULL.  Both serve Dout = 128, Din in {32, 64, 96, 128} with 16 B-aligned operands and the
+ * tensor-core kernels on (gnnb_dense_set_tensor_core_kernel); GNNB_EUNSUPPORTED otherwise (use the y entries). */
+int gnnb_linear_relu_mask(const float* x, const float* W, const float* bias, int64_t N, int64_t Din, int64_t Dout, float* y,
+                          uint32_t* mask, void* stream);
+int gnnb_linear_bwd_mask(const float* dy, const uint32_t* mask, const float* x, const float* W, int64_t N, int64_t Din,
+                         int64_t Dout, float* dx, float* dW, float* db, void* stream);
 /* σ.(W * vcat(x1, x2) .+ b) — sage_conv's dense part (GNNlib/src/layers/conv.jl:281) — without the (Din1+Din2, N) vcat
  * temporary: the two column blocks of W (Dout, Din1+Din2, row-major as the layer stores it) meet x1 (Din1,N) and x2 (Din2,N)
  * in two passes of the wgmma kernel, the second adding the first's result before bias / activation.  Pullback: dx1, dx2,

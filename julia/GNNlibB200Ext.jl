@@ -180,7 +180,41 @@ function fused_linear(W::CuMatrix{Float32}, x::CuMatrix{Float32}, b::Union{Nothi
     return y
 end
 
+# relu(W * x .+ b) with its relu mask kept as bits (4 words per node) for the pullback; `nothing` when
+# gnnb_linear_relu_mask does not serve the shape (Dout != 128, Din not 32, 64, 96 or 128)
+function fused_linear_relu_mask(W::CuMatrix{Float32}, x::CuMatrix{Float32}, b::Union{Nothing, CuVector{Float32}})
+    Dout, Din = size(W)
+    N = size(x, 2)
+    Wr = permutedims(W)
+    y = similar(x, Dout, N)
+    mask = CuArray{UInt32}(undef, 4, N)
+    st = ccall((:gnnb_linear_relu_mask, LIB), Cint,
+               (CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64, Int64, CuPtr{Float32}, CuPtr{UInt32}, Ptr{Cvoid}),
+               x, Wr, cuptr(b), N, Din, Dout, y, mask, stream())
+    st == 5 && return nothing                            # GNNB_EUNSUPPORTED
+    check(st)
+    return y, mask
+end
+
 function ChainRulesCore.rrule(::typeof(fused_linear), W, x, b, relu::Bool)
+    ym = relu ? fused_linear_relu_mask(W, x, b) : nothing
+    if ym !== nothing
+        y, mask = ym
+        function fused_linear_mask_pullback(Δ)
+            dy = CuArray{Float32}(unthunk(Δ))
+            Dout, Din = size(W)
+            N = size(x, 2)
+            Wr = permutedims(W)
+            dx, dWr = similar(x), similar(Wr)
+            db = b === nothing ? nothing : similar(b)
+            check(ccall((:gnnb_linear_bwd_mask, LIB), Cint,
+                        (CuPtr{Float32}, CuPtr{UInt32}, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64, Int64,
+                         CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                        dy, mask, x, Wr, N, Din, Dout, dx, dWr, cuptr(db), stream()))
+            return NoTangent(), permutedims(dWr), dx, db === nothing ? NoTangent() : db, NoTangent()
+        end
+        return y, fused_linear_mask_pullback
+    end
     y = fused_linear(W, x, b, relu)
     function fused_linear_pullback(Δ)
         dy = CuArray{Float32}(unthunk(Δ))
