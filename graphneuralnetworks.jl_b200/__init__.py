@@ -21,8 +21,8 @@ from .layers_more import (CGConv, ChebConv, DConv, EdgeConv, EGNNConv, GMMConv, 
                           nn_conv, res_gated_graph_conv)
 from .readout import (broadcast_edges, broadcast_nodes, global_attention_pool, global_pool, reduce_edges, reduce_nodes,
                       softmax_edges, softmax_nodes)
-from .transform import (add_nodes, csr, getgraph, random_walk_pe, remove_edges, remove_multi_edges, remove_nodes,
-                        remove_self_loops, sort_edge_index, to_bidirected, unbatch)
+from .transform import (add_nodes, color_refinement, csr, getgraph, random_walk_pe, remove_edges, remove_multi_edges,
+                        remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
 from .generate import knn_graph, radius_graph
 from .linkpred import (DotDecoder, add_edges, dot_decoder, edge_decoding, edge_encoding, intersect, negative_sample,
                        perturb_edges, rand_edge_split, rand_graph)

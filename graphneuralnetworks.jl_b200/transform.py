@@ -12,6 +12,7 @@
     getgraph(g, i; nmap)             GNNGraphs/src/transform.jl:825-888
     add_nodes(g, n; ndata)           GNNGraphs/src/transform.jl:553-563
     random_walk_pe(g, walk_length)   GNNGraphs/src/transform.jl:975-990   (per-graph walks, csrc/rwpe.cu)
+    color_refinement(g, x0)          GNNGraphs/src/utils.jl:340-389       (1-WL colour refinement, csrc/wl.cu)
 
 The index work (pair encoding, stable radix sort, duplicate runs) is csrc/transform.cu; the feature aggregation of
 `remove_multi_edges` is the library's segmented scatter over the run ids it returns — the same kernels as
@@ -38,6 +39,9 @@ Deliberate differences from the reference:
 6. random_walk_pe sums each walk step in the plan's edge order instead of forming dense matrix products, so it agrees
    with the reference to rounding; walk_length < 1 raises AssertionError (the reference throws BoundsError or
    ArgumentError).
+7. color_refinement refines to the fixed point, renumbers the colours from 1 in every round and groups signatures by
+   a multiset hash of its own; the reference stops after at most two rounds and carries its ids over between rounds
+   (see its docstring).
 """
 from __future__ import annotations
 
@@ -441,3 +445,48 @@ def random_walk_pe(g: GNNGraph, walk_length: int) -> torch.Tensor:
         h = _with_plan(GNNGraph(s, t, None if w is None else w[kept], num_nodes=n2), plan)
         _rwpe_propagate(h, h.w, dinv[a:b].contiguous(), K, out[a:b])
     return unrows(out)
+
+
+def color_refinement(g: GNNGraph, x0=None, *, max_iters: Optional[int] = None):
+    """1-WL colour refinement — utils.jl:340-389: returns (x, num_colors, niters).
+
+    Round r maps node i to its signature (c_i, multiset{c_s : edges s -> i}): the in-neighbours, with multiplicity, a
+    self loop making i its own neighbour, edge weights ignored.  Two nodes get the same new colour iff their
+    signatures are equal, and the colours are numbered 1..k in order of first appearance by node id (the reference's
+    `get!(hashmap, ..., length(hashmap) + 1)` within one round).  A batched graph is refined as one graph, so colours
+    compare across its graphs.  x0 (an integer vector of length num_nodes) matters only through its partition; None
+    starts every node in one class.  The rounds run until one leaves the number of classes unchanged — refinement only
+    splits classes, so that round reproduces the previous colours — or until `max_iters` rounds (an integer >= 1; 2
+    gives the reference's partition and is the h-round form of WL features).  niters counts the rounds computed,
+    the last included; a capped call that has not converged returns niters == max_iters.  x is an int64 tensor on
+    g's compute device; num_colors and niters are Python ints.  An empty graph gives (empty, 0, 1).
+
+    Each round is one pass of gnnb_color_refinement's signature kernel over the in-edges and a stable radix sort of
+    the exact key (c_i, S_1, S_2), S_k = Σ_{edges s -> i} splitmix64(c_s ^ salt_k) mod 2^61 - 1, with one count read
+    back per round.  Deliberate differences from the reference:
+      * the loop runs to the fixed point; the reference stops after at most two rounds (its x and x' alias after the
+        first, so the second ends the loop), and its own test expects niters == 2;
+      * colours are renumbered from 1 in every round, so nothing carries over from earlier rounds (the reference's ids
+        continue across rounds: its known answer starts at 4);
+      * signatures are grouped by the multiset hash above instead of Julia's `hash` of the sorted list.  Both are
+        probabilistic: two different multisets with the same c_i share (S_1, S_2) with probability about 2^-122 per
+        pair under a random-function model of splitmix64.  That bounds chance collisions, not inputs built to collide.
+    Wrong-length x0 or a max_iters that is not an integer >= 1 raise AssertionError."""
+    assert max_iters is None or (isinstance(max_iters, numbers.Integral) and not isinstance(max_iters, bool)
+                                 and max_iters >= 1), f"max_iters = {max_iters} must be None or an integer >= 1"
+    g = _on_device(g)
+    dev, n = g.s.device, g.num_nodes
+    if x0 is not None:
+        x0 = torch.as_tensor(x0)
+        assert x0.dim() == 1 and x0.numel() == n, f"len(x0) = {x0.numel()} must equal num_nodes = {n}"
+        assert not (x0.is_floating_point() or x0.is_complex()), f"x0 must hold integers, not {x0.dtype}"
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    if n == 0:
+        return out, 0, 1
+    p = g.plan()
+    x = None if x0 is None else x0.to(device=p.device, dtype=torch.int64).contiguous()
+    num_colors, niters = C.c_int64(0), C.c_int64(0)
+    with torch.cuda.device(p.device):
+        _lib.check(lib.gnnb_color_refinement(p.h, _ptr(x), 0 if max_iters is None else int(max_iters), out.data_ptr(),
+                                             C.byref(num_colors), C.byref(niters), _stream(p.device)))
+    return out, int(num_colors.value), int(niters.value)

@@ -432,6 +432,24 @@ int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_p
 int gnnb_random_walk_pe(gnnb_graph_t g, const float* w, const float* dinv, const int64_t* seg_ptr, int64_t n_seg,
                         int walk_length, float* out, void* stream);
 
+/* --------------------------------------------------------- 1-WL colour refinement (csrc/wl.cu)
+ * replaces: color_refinement(g, x0) (GNNGraphs/src/utils.jl:340-389): a host loop hashing (x_i, sort(x[in-neighbours]))
+ *           into a Dict once per node per round.
+ * Round r maps node i to its signature (c_i, multiset{c_s : edges s -> i}) (in-neighbours with multiplicity, a self loop
+ * counts, weights ignored); two nodes get the same new colour iff their signatures are equal.  Colours are numbered
+ * 1..k in order of first appearance by node id, afresh every round.  The rounds stop when a round leaves the number of
+ * classes unchanged (refinement only splits classes, so that round reproduces the previous colours) or after max_iters
+ * rounds.  Signatures are grouped by the exact key (c_i, S_1, S_2), S_k = Σ_edges splitmix64(c_s ^ salt_k) mod 2^61 - 1:
+ * two different multisets of the same c_i share it with probability about 2^-122 under a random-function model (chance
+ * collisions only, not inputs built to collide).
+ * g: a square plan (GNNB_ESIZE otherwise).  x0: n DEVICE int64s (any values; only their partition matters), or NULL
+ * for one starting class.  max_iters: 0 = until stable, >= 1 caps the rounds, < 0 is GNNB_EINVAL.
+ * colors: n DEVICE int64s, 1-based.  num_colors, niters: HOST outputs (niters counts the last round; n == 0 gives
+ * num_colors = 0, niters = 1).  Scratch: one allocation of about 92 B per node per call, plus the plan's workspace for
+ * rows of more than the plan's chunk of edges.  Synchronises the stream. */
+int gnnb_color_refinement(gnnb_graph_t g, const int64_t* x0, int64_t max_iters, int64_t* colors, int64_t* num_colors,
+                          int64_t* niters, void* stream);
+
 /* ------------------------------------------------- edge codes and random edges (csrc/edgegen.cu)
  * Code spaces of edge_encoding / edge_decoding (GNNGraphs/src/utils.jl:189-268, bipartite :263-268), 0-based here (the
  * reference's idx - 1), node ids 0-based (s, t < n; bipartite s < n1, t < n2), n1, n2 in [0, 2^31):

@@ -860,4 +860,27 @@ function GNNGraphs.random_walk_pe(g::GNNGraph{<:CuCOO}, walk_length::Int)
 end
 ChainRulesCore.@non_differentiable GNNGraphs.random_walk_pe(::Any...)
 
+## color_refinement on device COO graphs — replaces GNNGraphs/src/utils.jl:340-389 (a host loop that hashes
+## (x_i, sort(x[in-neighbours])) into a Dict and indexes scalars, so it cannot run on a CuArray graph).  One pass of
+## gnnb_color_refinement's signature kernel per round and a stable radix sort of the exact (c_i, S_1, S_2) key.  Same
+## contract as the Python mirror (graphneuralnetworks.jl_b200/transform.py): rounds until the class count stops
+## changing (the reference stops after at most two; `max_iters = 2` gives its partition), colours 1..k by first
+## appearance renumbered every round, signatures grouped by a mod 2^61 - 1 multiset hash.
+function GNNGraphs.color_refinement(g::GNNGraph{<:CuCOO}, x0::AbstractVector{<:Integer} = CUDA.ones(Int, g.num_nodes);
+                                    max_iters::Union{Nothing,Integer} = nothing)
+    @assert length(x0) == g.num_nodes "length(x0) = $(length(x0)) must equal num_nodes = $(g.num_nodes)"
+    @assert max_iters === nothing || max_iters >= 1 "max_iters = $max_iters must be nothing or >= 1"
+    n = g.num_nodes
+    x = CuVector{Int64}(undef, n)
+    n == 0 && return x, 0, 1
+    p = plan(g)
+    xd = CuVector{Int64}(x0)
+    k, it = Ref{Int64}(0), Ref{Int64}(0)
+    check(ccall((:gnnb_color_refinement, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Int64}, Int64, CuPtr{Int64}, Ref{Int64}, Ref{Int64}, Ptr{Cvoid}),
+                p.h, xd, max_iters === nothing ? 0 : max_iters, x, k, it, stream()))
+    return x, Int(k[]), Int(it[])
+end
+ChainRulesCore.@non_differentiable GNNGraphs.color_refinement(::Any...)
+
 end # module

@@ -1,5 +1,7 @@
 """small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans, the
-drop mask and the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), meant to run under `compute-sanitizer --tool memcheck` (or racecheck / synccheck)"""
+drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses) and colour
+refinement (hub rows cut into long-row pieces, a path, a batch), meant to run under `compute-sanitizer --tool memcheck`
+(or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gnnb200 as gnn
@@ -88,5 +90,18 @@ seg = torch.cat([torch.zeros(1, dtype=torch.int64, device="cuda"), torch.cumsum(
 out = torch.empty(off * 6, device="cuda")
 rc = lib.gnnb_random_walk_pe(gx.plan().h, None, dinv.data_ptr(), seg.data_ptr(), len(sizes), 6, out.data_ptr(), None)
 print("random_walk_pe crossing edge rejected", rc == gnn._lib.EINVAL)
+# color_refinement: two hubs of 3 000 in-edges (pieces of 128 and the fix-up), a path of 41 nodes, a batch of small graphs
+hs = torch.randint(0, 500, (6000,), device="cuda"); ht = torch.cat([torch.full((3000,), 7, device="cuda"),
+                                                                   torch.full((3000,), 499, device="cuda")])
+bs, bt = torch.randint(0, 500, (1500,), device="cuda"), torch.randint(0, 500, (1500,), device="cuda")
+gh = gnn.GNNGraph(torch.cat([hs, bs]) + 1, torch.cat([ht, bt]) + 1, num_nodes=500)
+print("color_refinement hubs", gnn.color_refinement(gh)[1:], gnn.color_refinement(gh, torch.arange(500, device="cuda") % 3)[1:])
+a = torch.arange(40, device="cuda")
+print("color_refinement path", gnn.color_refinement(gnn.GNNGraph(torch.cat([a, a + 1]) + 1, torch.cat([a + 1, a]) + 1,
+                                                                 num_nodes=41))[1:])
+ms, mt = torch.randint(0, 23, (200, 50), device="cuda"), torch.randint(0, 23, (200, 50), device="cuda")
+off = (torch.arange(200, device="cuda") * 23)[:, None]
+print("color_refinement batch", gnn.color_refinement(gnn.GNNGraph((ms + off).reshape(-1) + 1, (mt + off).reshape(-1) + 1,
+                                                                  num_nodes=4600), max_iters=2)[1:])
 torch.cuda.synchronize()
 print("done")
