@@ -842,3 +842,23 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
 }
 
 }  // extern "C"
+
+namespace gnnb {
+
+// the forward fix-up with one head (C = D): the long rows' partial slots [acc: D][M][S] combined in chunk order into
+// out = acc / S, seg_max = M, seg_sum = S.  set2set.cu's attention writes its slots in this layout.
+int gat_fwd_fixup_one_head(const Csr& c, int64_t E, int chunk, int64_t D, bool vec4, float* ws, float* out,
+                           float* seg_max, float* seg_sum, cudaStream_t st) {
+    if (c.n_long == 0) return GNNB_OK;
+    GatParams p = {};
+    p.rowptr = c.rowptr; p.ws = ws; p.out = out; p.stat_a = seg_max; p.stat_b = seg_sum;
+    p.D = D; p.C = (int32_t)D; p.H = 1; p.E = (int32_t)E; p.nrows = c.nrows; p.chunk = chunk;
+    p.nchunks = (int32_t)ceil_div(E, chunk);
+    const unsigned fb = nblk((int64_t)c.n_long * (vec4 ? D / 4 : D));
+    if (vec4) gat_fwd_fixup_kernel<4><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
+    else gat_fwd_fixup_kernel<1><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
+}  // namespace gnnb

@@ -347,7 +347,8 @@ int seg_reduce(gnnb_graph* g, const Csr& c, const SegArgs& a, cudaStream_t st) {
     return GNNB_OK;
 }
 
-// the partial slots of the long rows of `c`, added in chunk order into out (plain sums: no scale, no mean)
+// the partial slots of the long rows of `c`, added in chunk order into out (plain sums: no scale, no mean); float4 when D
+// is a multiple of 4 and out, ws are 16 B aligned, scalar otherwise
 int seg_fixup_sum(const Csr& c, int64_t E, int chunk, int64_t D, float* ws, float* out, cudaStream_t st) {
     if (c.n_long == 0) return GNNB_OK;
     SegParams p;
@@ -356,8 +357,10 @@ int seg_fixup_sum(const Csr& c, int64_t E, int chunk, int64_t D, float* ws, floa
     p.D = D; p.E = (int32_t)E; p.nrows = c.nrows; p.chunk = chunk;
     p.nchunks = (int32_t)ceil_div(E, chunk);
     p.mean = 0; p.sign = 1.f; p.fill = 0; p.ws = ws;
-    const int64_t threads = (int64_t)c.n_long * ceil_div(D, 4);
-    seg_fixup_kernel<4, false><<<(unsigned)ceil_div(threads, 256), 256, 0, st>>>(p, c.long_rows, c.n_long);
+    const bool vec4 = D % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(ws) & 15) == 0;
+    const int64_t threads = (int64_t)c.n_long * (vec4 ? D / 4 : D);
+    if (vec4) seg_fixup_kernel<4, false><<<(unsigned)ceil_div(threads, 256), 256, 0, st>>>(p, c.long_rows, c.n_long);
+    else seg_fixup_kernel<1, false><<<(unsigned)ceil_div(threads, 256), 256, 0, st>>>(p, c.long_rows, c.n_long);
     GNNB_LAUNCHED();
     return GNNB_OK;
 }

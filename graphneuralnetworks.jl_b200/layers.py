@@ -711,6 +711,32 @@ class _GRUCell(torch.nn.Module):
         return hn, hn
 
 
+class _LSTMCell(torch.nn.Module):
+    """Flux.LSTMCell(in => out) (Flux 0.16) on Julia-shaped (D, N) arrays; returns (h', (h', c')) like Flux's cell.
+        g = Wi x + Wh h + bias, split into input, forget, cell, output gates (in that order)
+        c' = σ(f) .* c + σ(i) .* tanh(cell);  h' = σ(o) .* tanh(c')
+    h and c may be vectors (out,), broadcast over the columns of x."""
+
+    def __init__(self, ch_in: int, ch_out: int, device=None):
+        super().__init__()
+        self.Wi = torch.nn.Parameter(glorot_uniform(4 * ch_out, ch_in, device=device))
+        self.Wh = torch.nn.Parameter(glorot_uniform(4 * ch_out, ch_out, device=device))
+        self.bias = torch.nn.Parameter(torch.zeros(4 * ch_out, device=device))
+        self.ch_out = ch_out
+
+    def forward(self, x, state):
+        h, c = state
+        if h.dim() == 1:
+            h = h.reshape(-1, 1)
+        if c.dim() == 1:
+            c = c.reshape(-1, 1)
+        o = self.ch_out
+        g = _matmul(self.Wi, x) + _matmul(self.Wh, h) + self.bias.reshape(-1, 1)
+        c_new = torch.sigmoid(g[o:2 * o]) * c + torch.sigmoid(g[:o]) * torch.tanh(g[2 * o:3 * o])
+        h_new = torch.sigmoid(g[3 * o:]) * torch.tanh(c_new)
+        return h_new, (h_new, c_new)
+
+
 def gated_graph_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:218-233: zero-pad x to `dims`, then num_layers rounds of
     m = propagate(copy_xj, g, aggr, xj = W_i * h);  h = gru(m, h).   l.weight is (dims, dims, num_layers)."""

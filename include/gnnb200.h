@@ -450,6 +450,30 @@ int gnnb_random_walk_pe(gnnb_graph_t g, const float* w, const float* dinv, const
 int gnnb_color_refinement(gnnb_graph_t g, const int64_t* x0, int64_t max_iters, int64_t* colors, int64_t* num_colors,
                           int64_t* niters, void* stream);
 
+/* --------------------------------------------------------- Set2Set attention (csrc/set2set.cu)
+ * replaces the per-node part of set2set_pool (GNNlib/src/layers/pool.jl:37-39): broadcast_nodes(g, q), sum(qn .* x),
+ *           softmax_nodes and reduce_nodes(+, g, x .* α), about six passes over D x N floats, in one pass over x:
+ *   s_k = <q[:, t_k], x[:, s_k]>;  M_i = max_k s_k;  S_i = Σ_k exp(s_k − M_i)
+ *   r[:, i] = Σ_k exp(s_k − M_i) x[:, s_k] / S_i          (k over the in-edges of target i, in plan order)
+ * x (D, num_src), q (D, num_dst), r (D, num_dst): DEVICE floats, column i contiguous.  seg_max, seg_sum (num_dst) are
+ * kept for the pullback.  A target with no edges: r = 0 (reduce_nodes' neutral element), seg_max = −Inf, seg_sum = 0.
+ * On the graph-indicator plan (edge k = node k -> its graph) the targets are the graphs of a batch.
+ * 1 <= D (GNNB_ESIZE) <= GNNB_SET2SET_MAX_D (GNNB_EUNSUPPORTED: compose the three readout calls).  A NULL array of
+ * positive size: GNNB_ESIZE.  Rows of more than the plan's chunk of edges are reduced in pieces and combined in a fixed
+ * order: the results are run-to-run bit-identical.  Does not synchronise. */
+#define GNNB_SET2SET_MAX_D 1024
+int gnnb_set2set_attend(gnnb_graph_t g, const float* x, const float* q, int64_t D,
+                        float* r, float* seg_max, float* seg_sum, void* stream);
+/* pullback given dr (D, num_dst): α_k recomputed from seg_max / seg_sum (s_k with the forward's instructions, so α is
+ * the forward's bit for bit), T_i = <dr_i, r_i>,
+ *   ds_k = α_k (<dr[:, t_k], x[:, s_k]> − T_i)
+ *   dxe[:, k] = α_k dr[:, t_k] + ds_k q[:, t_k]      per edge, in COO order: every column written exactly once
+ *   dq[:, i]  = Σ_k ds_k x[:, s_k]                  (0 for a target with no edges)
+ * On the graph-indicator plan dxe is dx.  Same bounds and errors as the forward. */
+int gnnb_set2set_attend_bwd(gnnb_graph_t g, const float* x, const float* q, const float* r,
+                            const float* seg_max, const float* seg_sum, const float* dr, int64_t D,
+                            float* dxe, float* dq, void* stream);
+
 /* ------------------------------------------------- edge codes and random edges (csrc/edgegen.cu)
  * Code spaces of edge_encoding / edge_decoding (GNNGraphs/src/utils.jl:189-268, bipartite :263-268), 0-based here (the
  * reference's idx - 1), node ids 0-based (s, t < n; bipartite s < n1, t < n2), n1, n2 in [0, 2^31):

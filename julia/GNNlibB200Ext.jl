@@ -883,4 +883,67 @@ function GNNGraphs.color_refinement(g::GNNGraph{<:CuCOO}, x0::AbstractVector{<:I
 end
 ChainRulesCore.@non_differentiable GNNGraphs.color_refinement(::Any...)
 
+## set2set_pool on device COO graphs — replaces GNNlib/src/layers/pool.jl:29-43.  Each iteration's attention
+## (broadcast_nodes, sum(qn .* x), softmax_nodes, reduce_nodes: about six passes over D x N floats and three D x N
+## temporaries) is one pass of gnnb_set2set_attend over the graph-indicator plan (node k -> graph indicator[k]); its rrule
+## calls gnnb_set2set_attend_bwd, whose per-edge dxe is dx on that plan, and keeps only graph-sized state besides x and q.
+## Same routing as the Python mirror (graphneuralnetworks.jl_b200/readout.py): n_in above SET2SET_MAX_D takes the
+## reference's composition.
+const SET2SET_MAX_D = 1024                                    # GNNB_SET2SET_MAX_D
+
+function _indicator_plan(g::GNNGraph)
+    n = g.num_nodes
+    gi = g.graph_indicator === nothing ? CUDA.ones(Int64, n) : CuVector{Int64}(g.graph_indicator)
+    src = CuVector{Int64}(1:n)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:gnnb_graph_create, LIB), Cint,
+                (Ref{Ptr{Cvoid}}, CuPtr{Cvoid}, CuPtr{Cvoid}, Int64, Int64, Int64, Cint, Cint, Cint, Ptr{Cvoid}),
+                h, pointer(src), pointer(gi), n, n, g.num_graphs, 8, 1, 1, stream()))
+    return Plan(h[])
+end
+ChainRulesCore.@non_differentiable _indicator_plan(::Any...)
+
+function _set2set_attend(p::Plan, x::CuMatrix{Float32}, q::CuMatrix{Float32})
+    D, G = size(q)
+    r = similar(q)
+    smax, ssum = CuVector{Float32}(undef, G), CuVector{Float32}(undef, G)
+    check(ccall((:gnnb_set2set_attend, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Float32}, CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32},
+                 Ptr{Cvoid}),
+                p.h, x, q, D, r, smax, ssum, stream()))
+    return r, smax, ssum
+end
+
+set2set_attend(p::Plan, x::CuMatrix{Float32}, q::CuMatrix{Float32}) = _set2set_attend(p, x, q)[1]
+
+function ChainRulesCore.rrule(::typeof(set2set_attend), p::Plan, x::CuMatrix{Float32}, q::CuMatrix{Float32})
+    r, smax, ssum = _set2set_attend(p, x, q)
+    function set2set_attend_pullback(Δ)
+        dr = CuMatrix{Float32}(unthunk(Δ))
+        dx, dq = similar(x), similar(q)
+        check(ccall((:gnnb_set2set_attend_bwd, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32},
+                     CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                    p.h, x, q, r, smax, ssum, dr, size(q, 1), dx, dq, stream()))
+        return NoTangent(), NoTangent(), dx, dq
+    end
+    return r, set2set_attend_pullback
+end
+
+function GNNlib.set2set_pool(l, g::GNNGraph{<:CuCOO}, x::CuMatrix{Float32})
+    @assert size(x, 2) == g.num_nodes "x has $(size(x, 2)) columns instead of num_nodes = $(g.num_nodes)"
+    n_in = size(x, 1)
+    n_in > SET2SET_MAX_D && return invoke(GNNlib.set2set_pool, Tuple{Any, GNNGraph, AbstractMatrix}, l, g, x)
+    p = _indicator_plan(g)
+    qstar = CUDA.zeros(Float32, 2 * n_in, g.num_graphs)
+    h = CUDA.zeros(Float32, size(l.lstm.Wh, 2))
+    state = (h, zero(h))
+    for _ in 1:l.num_iters
+        q, state = l.lstm(qstar, state)
+        r = set2set_attend(p, x, CuMatrix{Float32}(q))
+        qstar = vcat(q, r)
+    end
+    return qstar
+end
+
 end # module

@@ -1,6 +1,7 @@
 """small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans, the
-drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses) and colour
-refinement (hub rows cut into long-row pieces, a path, a batch), meant to run under `compute-sanitizer --tool memcheck`
+drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), colour
+refinement (hub rows cut into long-row pieces, a path, a batch) and Set2Set (a graph with no nodes, graphs of chunk +- 1
+nodes, D = 1, 3 and 1024, the composition at D = 1025), meant to run under `compute-sanitizer --tool memcheck`
 (or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -103,5 +104,15 @@ ms, mt = torch.randint(0, 23, (200, 50), device="cuda"), torch.randint(0, 23, (2
 off = (torch.arange(200, device="cuda") * 23)[:, None]
 print("color_refinement batch", gnn.color_refinement(gnn.GNNGraph((ms + off).reshape(-1) + 1, (mt + off).reshape(-1) + 1,
                                                                   num_nodes=4600), max_iters=2)[1:])
+# Set2Set: graphs of 127, 128, 129 nodes (chunk 128) and one without nodes, forward and backward at D = 1, 3, 1024, 1025
+gi = torch.repeat_interleave(torch.tensor([1, 2, 4, 5], device="cuda"), torch.tensor([127, 128, 129, 1], device="cuda"))
+a = torch.arange(1, gi.numel() + 1, device="cuda")
+gs = gnn.GNNGraph(a, a, num_nodes=gi.numel(), num_graphs=5, graph_indicator=gi)
+for Ds in (1, 3, 1024, 1025):
+    l = gnn.Set2Set(Ds, 2, device="cuda")
+    xs = torch.randn(Ds, gi.numel(), device="cuda").requires_grad_(True)
+    ys = l(gs, xs)
+    ys.sum().backward()
+    print("set2set D", Ds, "empty graph r == 0", bool((ys[Ds:, 2] == 0).all()), "grad finite", bool(torch.isfinite(xs.grad).all()))
 torch.cuda.synchronize()
 print("done")
