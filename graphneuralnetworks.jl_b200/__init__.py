@@ -23,6 +23,8 @@ from .readout import (Set2Set, broadcast_edges, broadcast_nodes, global_attentio
                       reduce_nodes, set2set_pool, softmax_edges, softmax_nodes)
 from .transform import (add_nodes, color_refinement, csr, getgraph, random_walk_pe, remove_edges, remove_multi_edges,
                         remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
+from .temporal import (DCGRU, DCGRUCell, EvolveGCNO, EvolveGCNOCell, GConvGRU, GConvGRUCell, GConvLSTM, GConvLSTMCell,
+                       GNNRecurrence, TemporalSnapshotsGNNGraph, TGCN, TGCNCell, initialstates)
 from .generate import knn_graph, radius_graph
 from .linkpred import (DotDecoder, add_edges, dot_decoder, edge_decoding, edge_encoding, intersect, negative_sample,
                        perturb_edges, rand_edge_split, rand_graph)

@@ -122,7 +122,14 @@ _SIGS = {
     "gnnb_color_refinement": (_int, [_vp, _vp, _i64, _vp, C.POINTER(_i64), C.POINTER(_i64), _vp]),
     "gnnb_set2set_attend": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _vp]),
     "gnnb_set2set_attend_bwd": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _vp]),
-    "gnnb_edge_encode": (_int, [_int, _i64, _i64, _vp, _vp, _i64, _int, _vp, _vp]),
+    "gnnb_gru_rz": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _i64, _f32p, _f32p, _f32p, _vp]),
+    "gnnb_gru_out": (_int, [_f32p, _i64, _f32p, _f32p, _f32p, _i64, _i64, _int, _f32p, _f32p, _vp]),
+    "gnnb_gru_out_bwd": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _i64, _int, _f32p, _i64, _f32p, _f32p, _vp]),
+    "gnnb_gru_rz_bwd": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32p, _i64, _f32p, _vp]),
+    "gnnb_lstm_cell": (_int, [_f32p, _i64, _f32p, _f32p, _f32p, _i64, _i64, _f32p, _f32p, _f32p, _vp]),
+    "gnnb_lstm_cell_bwd": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32p, _f32p, _f32p, _f32p,
+                                  _vp]),
+    "gnnb_edge_encode":(_int, [_int, _i64, _i64, _vp, _vp, _i64, _int, _vp, _vp]),
     "gnnb_edge_decode": (_int, [_int, _i64, _i64, _vp, _i64, _int, _vp, _vp, _vp]),
     "gnnb_edge_codes_sorted": (_int, [_int, _i64, _i64, _vp, _vp, _i64, _int, _vp, C.POINTER(_i64), _vp]),
     "gnnb_codes_member": (_int, [_vp, _i64, _vp, _i64, _vp, _vp]),

@@ -197,6 +197,13 @@ __global__ void colsum_final_kernel(const float* __restrict__ partial, int nbloc
     db[c] = acc;
 }
 
+// the final pass of the two-stage column sum over partials written by other kernels (recurrent.cu's peephole gradient)
+int colsum_final(const float* partial, int nblocks, int64_t D, float* out, cudaStream_t st) {
+    colsum_final_kernel<<<(unsigned)ceil_div(D, 128), 128, 0, st>>>(partial, nblocks, (int)D, out);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
 }  // namespace gnnb
 
 using namespace gnnb;

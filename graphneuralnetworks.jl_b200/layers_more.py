@@ -2,6 +2,7 @@
 the reference writes them: dense per-node / per-edge algebra around `propagate`, `apply_edges`, `aggregate_neighbors`.
 
     cheb_conv              conv.jl:83-98        (X·L̃ through the fused propagate; λmax by Lanczos on the device)
+                                                (its basis, cheb_basis, and DConv's, diffusion_basis, also serve temporal.py)
     edge_conv              conv.jl:237-246
     nn_conv                conv.jl:260-273
     res_gated_graph_conv   conv.jl:287-300
@@ -81,10 +82,8 @@ def scaled_laplacian_mul(g: GNNGraph, X: torch.Tensor, c: torch.Tensor, lmax: fl
     return (2.0 / lmax) * (X - _normalized_adjacency_mul(g, X, c)) - X
 
 
-def cheb_conv(l, g: GNNGraph, X: torch.Tensor) -> torch.Tensor:
-    """GNNlib/src/layers/conv.jl:83-98.  l.weight is (out, in, k), k >= 2 as in the reference."""
-    check_num_nodes(g, X)
-    assert X.shape[0] == l.weight.shape[1], "Input feature size must match input channel size."
+def cheb_operator(g: GNNGraph):
+    """(c, λmax) of L̃ = 2/λmax (I - D^-1/2 A D^-1/2) - I: c = 1 ./ sqrt.(out-degree); λmax is cached on the graph"""
     d = degree(g, torch.float32, dir="out")
     assert bool((d != 0).all()), "Graph contains isolated nodes, cannot compute `normalized_adjacency`."
     c = 1.0 / torch.sqrt(d)
@@ -92,12 +91,31 @@ def cheb_conv(l, g: GNNGraph, X: torch.Tensor) -> torch.Tensor:
     if cache is None:
         cache = _lambda_max(g, c)
         g._lmax_cache = cache
+    return c, cache
+
+
+def cheb_basis(g: GNNGraph, X: torch.Tensor, k: int, op=None) -> list:
+    """[Z_0, ..., Z_{k-1}] of cheb_conv (conv.jl:90-97), k >= 2: Z_0 = X, Z_1 = X L̃, Z_j = 2 Z_{j-1} L̃ - Z_{j-2}.
+    X is (D, N): each column of the propagate is reduced on its own, so the basis of a (D·T, N) view is every time
+    step's basis at once, and the basis of a vcat is the vcat of the bases.  op: cheb_operator(g), when known."""
+    c, lmax = cheb_operator(g) if op is None else op
     Z_prev = X
-    Z = scaled_laplacian_mul(g, X, c, cache)
-    Y = _matmul(l.weight[:, :, 0], Z_prev) + _matmul(l.weight[:, :, 1], Z)
+    Z = scaled_laplacian_mul(g, X, c, lmax)
+    basis = [Z_prev, Z]
+    for _ in range(2, int(k)):
+        Z, Z_prev = 2 * scaled_laplacian_mul(g, Z, c, lmax) - Z_prev, Z
+        basis.append(Z)
+    return basis
+
+
+def cheb_conv(l, g: GNNGraph, X: torch.Tensor) -> torch.Tensor:
+    """GNNlib/src/layers/conv.jl:83-98.  l.weight is (out, in, k), k >= 2 as in the reference."""
+    check_num_nodes(g, X)
+    assert X.shape[0] == l.weight.shape[1], "Input feature size must match input channel size."
+    Z = cheb_basis(g, X, int(l.k))
+    Y = _matmul(l.weight[:, :, 0], Z[0]) + _matmul(l.weight[:, :, 1], Z[1])
     for k in range(2, int(l.k)):
-        Z, Z_prev = 2 * scaled_laplacian_mul(g, Z, c, cache) - Z_prev, Z
-        Y = Y + _matmul(l.weight[:, :, k], Z)
+        Y = Y + _matmul(l.weight[:, :, k], Z[k])
     return _add_bias(Y, _bias(l))
 
 
@@ -216,23 +234,44 @@ def egnn_conv(l, g: GNNGraph, h: torch.Tensor, x: torch.Tensor, e: Optional[torc
 
 
 # ------------------------------------------------------------------------------------------------ DConv
-def d_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
-    """GNNlib/src/layers/conv.jl:696-724, statement for statement.  l.weights is (2, k, out, in)."""
-    gt = GNNGraph(g.t, g.s, g.w, num_nodes=g.num_nodes)
+def transposed_graph(g: GNNGraph) -> GNNGraph:
+    """the reversed graph DConv diffuses on (conv.jl:697), with its plan, cached on the (immutable) graph"""
+    gt = getattr(g, "_dconv_gt", None)
+    if gt is None:
+        gt = GNNGraph(g.t, g.s, g.w, num_nodes=g.num_nodes)
+        g._dconv_gt = gt
+    return gt
+
+
+def diffusion_basis(g: GNNGraph, x: torch.Tensor, k: int, gt: Optional[GNNGraph] = None) -> list:
+    """The terms of d_conv (conv.jl:696-724) as [(j, T_in, T_out), ...]: h = Σ W[1, j] T_in + W[2, j] T_out (Julia
+    indices; j 0-based here).  The reference's recurrence keeps T0 = x and applies weights[:, 2] to both the first and
+    the second diffusion step, and so does this.  x is (D, N); see cheb_basis for (D·T, N) views."""
+    if gt is None:
+        gt = GNNGraph(g.t, g.s, g.w, num_nodes=g.num_nodes)
     deg_out = degree(g, torch.float32, dir="out").reshape(1, -1)
     deg_in = degree(g, torch.float32, dir="in").reshape(1, -1)
-    Wt = l.weights
-    h = _matmul(Wt[0, 0], x) + _matmul(Wt[1, 0], x)
     T0 = x
-    if l.k > 1:
+    terms = [(0, T0, T0)]
+    if k > 1:
         T1_out = propagate(w_mul_xj, g, operator.add, xj=T0 * deg_out)
         T1_in = propagate(w_mul_xj, gt, operator.add, xj=T0 * deg_in)
-        h = h + _matmul(Wt[0, 1], T1_in) + _matmul(Wt[1, 1], T1_out)
-    for i in range(2, int(l.k) + 1):
+        terms.append((1, T1_in, T1_out))
+    for i in range(2, int(k) + 1):
         T2_in = 2 * propagate(w_mul_xj, gt, operator.add, xj=T1_in * deg_in) - T0
         T2_out = 2 * propagate(w_mul_xj, g, operator.add, xj=T1_out * deg_out) - T0
-        h = h + _matmul(Wt[0, i - 1], T2_in) + _matmul(Wt[1, i - 1], T2_out)
+        terms.append((i - 1, T2_in, T2_out))
         T1_in, T1_out = T2_in, T2_out
+    return terms
+
+
+def d_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
+    """GNNlib/src/layers/conv.jl:696-724, statement for statement.  l.weights is (2, k, out, in)."""
+    Wt = l.weights
+    terms = diffusion_basis(g, x, int(l.k))
+    h = _matmul(Wt[0, 0], x) + _matmul(Wt[1, 0], x)
+    for j, T_in, T_out in terms[1:]:
+        h = h + _matmul(Wt[0, j], T_in) + _matmul(Wt[1, j], T_out)
     return _add_bias(h, _bias(l))
 
 

@@ -474,6 +474,61 @@ int gnnb_set2set_attend_bwd(gnnb_graph_t g, const float* x, const float* q, cons
                             const float* seg_max, const float* seg_sum, const float* dr, int64_t D,
                             float* dxe, float* dq, void* stream);
 
+/* --------------------------------------------------------- recurrent gates (csrc/recurrent.cu)
+ * The gate arithmetic of the recurrent temporal cells (GraphNeuralNetworks/src/layers/temporalconv.jl), one pass over
+ * node rows per entry instead of about ten broadcasts with their own (out, N) temporaries.  Arrays are DEVICE floats in
+ * node rows (row n of an (N, W) array at n * W), except the x-side pre-activations:
+ *   px: step t's slice of PX, the x-side operator of every gate for all steps at once.  Row n at px + n * ld_px, gate g's
+ *       D floats at column g * D;  ld_px >= G * D (G = 3 for the GRU cells, 4 for the LSTM), so that a (N, T, G·D)
+ *       array is read in place at px = PX + t * G·D, ld_px = T·G·D.
+ * σ(a) = 1 / (1 + expf(−a)) and tanhf: the accurate forms (the reference's sigmoid_fast / tanh_fast approximate).  The
+ * rows are vectorised by float4 when D % 4 == 0 and every row start is 16 B aligned, scalar otherwise; each output float
+ * is written once and no atomics are used, so results are run-to-run bit-identical.
+ * Errors: N < 0, D < 1, ld_px < G * D, or a NULL array of positive size: GNNB_ESIZE.  N == 0 is a no-op (except that
+ * gnnb_lstm_cell_bwd writes dw = 0).  None of the entries synchronises. */
+/* GRU, first half (gate order in px: [r | z | n]); ah (N, 2D) = [ah_r | ah_z], the h-side operators of r and z:
+ *   r = σ(px_r + ah_r);  z = σ(px_z + ah_z);  rh = r ⊙ h
+ * replaces temporalconv.jl:244-249 (GConvGRUCell), :566-569 (DCGRUCell, z = dconv_u), :842-846 (TGCNCell, the r .* h
+ * input of dense_h).  r and z are kept for the pullback; rh is the input of the candidate's h-side operator. */
+int gnnb_gru_rz(const float* px, int64_t ld_px, const float* ah, const float* h, int64_t N, int64_t D, float* r,
+                float* z, float* rh, void* stream);
+/* GRU, second half; ah_n (N, D) the candidate's h-side operator (of rh):
+ *   n = tanh(px_n + ah_n)
+ *   blend 0: h' = (1 − z) ⊙ n + z ⊙ h      GConvGRUCell (temporalconv.jl:250-252), DCGRUCell (:570-573)
+ *   blend 1: h' = (1 − z) ⊙ h + z ⊙ n      TGCNCell (:846-847)
+ * n is kept for the pullback.  blend other than 0 / 1: GNNB_EINVAL. */
+int gnnb_gru_out(const float* px, int64_t ld_px, const float* ah_n, const float* h, const float* z, int64_t N,
+                 int64_t D, int blend, float* n, float* h_new, void* stream);
+/* pullback of gnnb_gru_out given dh' (N, D):
+ *   dn = dh' ⊙ (1 − z) [blend 0] | dh' ⊙ z [blend 1];  dpre_n = dn ⊙ (1 − n²)
+ *   dz = dh' ⊙ (h − n) [blend 0] | dh' ⊙ (n − h) [blend 1];  dh = dh' ⊙ z [blend 0] | dh' ⊙ (1 − z) [blend 1]
+ * dpre_n: row n at dpre_n + n * ld_dpre (>= D: it may be the n block of an (N, 3D) array); dz, dh (N, D). */
+int gnnb_gru_out_bwd(const float* dh_new, const float* h, const float* z, const float* n, int64_t N, int64_t D,
+                     int blend, float* dpre_n, int64_t ld_dpre, float* dz, float* dh, void* stream);
+/* pullback of gnnb_gru_rz given drh (the candidate operator's pullback) and dz:
+ *   dpre_r = drh ⊙ h ⊙ r (1 − r);  dpre_z = dz ⊙ z (1 − z);  dh += drh ⊙ r
+ * dpre_rz: row n at dpre_rz + n * ld_dpre (>= 2D), [dpre_r | dpre_z].  dh (N, D) is read and written. */
+int gnnb_gru_rz_bwd(const float* drh, const float* dz, const float* h, const float* r, const float* z, int64_t N,
+                    int64_t D, float* dpre_rz, int64_t ld_dpre, float* dh, void* stream);
+/* LSTM with peepholes (GConvLSTMCell, temporalconv.jl:425-435), gate order [i | f | c | o]; ah (N, 4D), c (N, D):
+ *   i = σ(px_i + ah_i + w_i ⊙ c);  f = σ(px_f + ah_f + w_f ⊙ c);  g = tanh(px_c + ah_c + w_c ⊙ c)
+ *   c' = f ⊙ c + i ⊙ g;  o = σ(px_o + ah_o + w_o ⊙ c')   (the new c, :431-433);  h' = o ⊙ tanh(c')
+ * w: 4·D floats [w_i | w_f | w_c | w_o], or NULL for no peepholes (Flux's LSTMCell).  gates (N, 4D) = [i | f | g | o]
+ * is kept for the pullback. */
+int gnnb_lstm_cell(const float* px, int64_t ld_px, const float* ah, const float* c, const float* w, int64_t N,
+                   int64_t D, float* gates, float* c_new, float* h_new, void* stream);
+/* pullback given dh', dc' (N, D) and the forward's c, gates, c':
+ *   dpre_o = dh' ⊙ tanh(c') ⊙ o (1 − o);  dc'' = dc' + dh' ⊙ o ⊙ (1 − tanh²(c')) + dpre_o ⊙ w_o
+ *   dpre_i = dc'' ⊙ g ⊙ i (1 − i);  dpre_f = dc'' ⊙ c ⊙ f (1 − f);  dpre_c = dc'' ⊙ i ⊙ (1 − g²)
+ *   dc = dc'' ⊙ f + dpre_i ⊙ w_i + dpre_f ⊙ w_f + dpre_c ⊙ w_c
+ *   dw = Σ_n [dpre_i ⊙ c | dpre_f ⊙ c | dpre_c ⊙ c | dpre_o ⊙ c']       (when w and dw are given)
+ * dpre (N, 4D) serves the x side and the h side alike.  dw is a deterministic two-stage column sum (per-block partials,
+ * then dense.cu's fixed-order final pass): ws holds GNNB_LSTM_DW_SLOTS(N) * 4 * D floats (NULL when dw is NULL). */
+#define GNNB_LSTM_DW_SLOTS(N) ((N) < 65536 ? ((N) + 63) / 64 : 1024)
+int gnnb_lstm_cell_bwd(const float* dh_new, const float* dc_new, const float* c, const float* gates,
+                       const float* c_new, const float* w, int64_t N, int64_t D, float* dpre, float* dc, float* dw,
+                       float* ws, void* stream);
+
 /* ------------------------------------------------- edge codes and random edges (csrc/edgegen.cu)
  * Code spaces of edge_encoding / edge_decoding (GNNGraphs/src/utils.jl:189-268, bipartite :263-268), 0-based here (the
  * reference's idx - 1), node ids 0-based (s, t < n; bipartite s < n1, t < n2), n1, n2 in [0, 2^31):

@@ -946,4 +946,92 @@ function GNNlib.set2set_pool(l, g::GNNGraph{<:CuCOO}, x::CuMatrix{Float32})
     return qstar
 end
 
+## The gates of the recurrent temporal cells (GraphNeuralNetworks/src/layers/temporalconv.jl) — one pass over node
+## columns per call instead of the cells' broadcasts.  px (G·D, N): the x-side pre-activations of the G gates ([r; z; n]
+## for the GRU cells, [i; f; c; o] for the LSTM); ah the h-side ones; every array a dense CuMatrix (node stride = rows).
+## Wiring GConvGRUCell / DCGRUCell / TGCNCell / GConvLSTMCell to these is left to the cells.
+function gru_rz(px::CuMatrix{Float32}, ah::CuMatrix{Float32}, h::CuMatrix{Float32})
+    D, N = size(h)
+    r, z, rh = similar(h), similar(h), similar(h)
+    check(ccall((:gnnb_gru_rz, LIB), Cint,
+                (CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64, CuPtr{Float32}, CuPtr{Float32},
+                 CuPtr{Float32}, Ptr{Cvoid}),
+                px, size(px, 1), ah, h, N, D, r, z, rh, stream()))
+    return r, z, rh
+end
+
+function ChainRulesCore.rrule(::typeof(gru_rz), px::CuMatrix{Float32}, ah::CuMatrix{Float32}, h::CuMatrix{Float32})
+    r, z, rh = gru_rz(px, ah, h)
+    function gru_rz_pullback(Δ)
+        D, N = size(h)
+        drh, dz = CuMatrix{Float32}(unthunk(Δ[3])), CuMatrix{Float32}(unthunk(Δ[2]))
+        dpre, dh = CuMatrix{Float32}(undef, 2D, N), CUDA.zeros(Float32, D, N)
+        check(ccall((:gnnb_gru_rz_bwd, LIB), Cint,
+                    (CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64,
+                     CuPtr{Float32}, Int64, CuPtr{Float32}, Ptr{Cvoid}),
+                    drh, dz, h, r, z, N, D, dpre, 2D, dh, stream()))
+        return NoTangent(), vcat(dpre, CUDA.zeros(Float32, size(px, 1) - 2D, N)), dpre, dh
+    end
+    return (r, z, rh), gru_rz_pullback
+end
+
+function gru_out(px::CuMatrix{Float32}, ah_n::CuMatrix{Float32}, h::CuMatrix{Float32}, z::CuMatrix{Float32}, blend::Int)
+    D, N = size(h)
+    n, hn = similar(h), similar(h)
+    check(ccall((:gnnb_gru_out, LIB), Cint,
+                (CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64, Cint,
+                 CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                px, size(px, 1), ah_n, h, z, N, D, blend, n, hn, stream()))
+    return hn, n
+end
+
+function ChainRulesCore.rrule(::typeof(gru_out), px::CuMatrix{Float32}, ah_n::CuMatrix{Float32}, h::CuMatrix{Float32},
+                              z::CuMatrix{Float32}, blend::Int)
+    hn, n = gru_out(px, ah_n, h, z, blend)
+    function gru_out_pullback(Δ)
+        D, N = size(h)
+        dhn = CuMatrix{Float32}(unthunk(Δ[1]))
+        dpre, dz, dh = similar(h), similar(h), similar(h)
+        check(ccall((:gnnb_gru_out_bwd, LIB), Cint,
+                    (CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64, Cint, CuPtr{Float32},
+                     Int64, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                    dhn, h, z, n, N, D, blend, dpre, D, dz, dh, stream()))
+        return NoTangent(), vcat(CUDA.zeros(Float32, 2D, N), dpre), dpre, dh, dz, NoTangent()
+    end
+    return (hn, n), gru_out_pullback
+end
+
+## w: the peepholes vcat(w_i, w_f, w_c, w_o) (4D), or nothing for Flux's LSTMCell
+function _lstm_cell(px, ah, c::CuMatrix{Float32}, w)
+    D, N = size(c)
+    gates, cn, hn = CuMatrix{Float32}(undef, 4D, N), similar(c), similar(c)
+    check(ccall((:gnnb_lstm_cell, LIB), Cint,
+                (CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Int64, Int64, CuPtr{Float32},
+                 CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                px, size(px, 1), ah, c, w === nothing ? CU_NULL : w, N, D, gates, cn, hn, stream()))
+    return hn, cn, gates
+end
+
+lstm_cell(px::CuMatrix{Float32}, ah::CuMatrix{Float32}, c::CuMatrix{Float32}, w) = _lstm_cell(px, ah, c, w)[1:2]
+
+function ChainRulesCore.rrule(::typeof(lstm_cell), px::CuMatrix{Float32}, ah::CuMatrix{Float32}, c::CuMatrix{Float32}, w)
+    hn, cn, gates = _lstm_cell(px, ah, c, w)
+    function lstm_cell_pullback(Δ)
+        D, N = size(c)
+        dhn = Δ[1] isa AbstractZero ? CUDA.zeros(Float32, D, N) : CuMatrix{Float32}(unthunk(Δ[1]))
+        dcn = Δ[2] isa AbstractZero ? CUDA.zeros(Float32, D, N) : CuMatrix{Float32}(unthunk(Δ[2]))
+        dpre, dc = CuMatrix{Float32}(undef, 4D, N), similar(c)
+        dw = w === nothing ? nothing : similar(w)
+        slots = N < 65536 ? cld(N, 64) : 1024                  # GNNB_LSTM_DW_SLOTS(N)
+        ws = w === nothing ? nothing : CuVector{Float32}(undef, slots * 4D)
+        check(ccall((:gnnb_lstm_cell_bwd, LIB), Cint,
+                    (CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Int64,
+                     Int64, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                    dhn, dcn, c, gates, cn, w === nothing ? CU_NULL : w, N, D, dpre, dc,
+                    dw === nothing ? CU_NULL : dw, ws === nothing ? CU_NULL : ws, stream()))
+        return NoTangent(), dpre, dpre, dc, w === nothing ? NoTangent() : dw
+    end
+    return (hn, cn), lstm_cell_pullback
+end
+
 end # module

@@ -114,5 +114,38 @@ for Ds in (1, 3, 1024, 1025):
     ys = l(gs, xs)
     ys.sum().backward()
     print("set2set D", Ds, "empty graph r == 0", bool((ys[Ds:, 2] == 0).all()), "grad finite", bool(torch.isfinite(xs.grad).all()))
+# recurrent gates: every entry at D = 1, 3, 64, 129 on a strided PX and with a 4-byte offset (the scalar path), then
+# every temporal layer forward and backward on a small graph
+from gnnb200._lib import lib as L, check as chk  # noqa: E402
+st0 = torch.cuda.current_stream().cuda_stream
+for Dr in (1, 3, 64, 129):
+    for off in (0, 1):
+        Nr = 300
+        def rb(n):
+            return torch.randn(n + off, device="cuda")[off:]
+        ld3, ld4 = 3 * Dr + 4, 4 * Dr + 4
+        px3, px4, ah2, ah, ah4, hr, cr, wr = (rb(Nr * ld3), rb(Nr * ld4), rb(Nr * 2 * Dr), rb(Nr * Dr), rb(Nr * 4 * Dr),
+                                              rb(Nr * Dr), rb(Nr * Dr), rb(4 * Dr))
+        r_, z_, rh_, n_, hn_, dz_, dh_ = (rb(Nr * Dr) for _ in range(7))
+        dpx, gates, dpre = rb(Nr * 3 * Dr), rb(Nr * 4 * Dr), rb(Nr * 4 * Dr)
+        dw, ws = rb(4 * Dr), rb(((Nr + 63) // 64) * 4 * Dr)
+        P = lambda t: t.data_ptr()
+        chk(L.gnnb_gru_rz(P(px3), ld3, P(ah2), P(hr), Nr, Dr, P(r_), P(z_), P(rh_), st0))
+        for blend in (0, 1):
+            chk(L.gnnb_gru_out(P(px3), ld3, P(ah), P(hr), P(z_), Nr, Dr, blend, P(n_), P(hn_), st0))
+            chk(L.gnnb_gru_out_bwd(P(hn_), P(hr), P(z_), P(n_), Nr, Dr, blend, P(dpx) + 8 * Dr, 3 * Dr, P(dz_), P(dh_), st0))
+            chk(L.gnnb_gru_rz_bwd(P(rh_), P(dz_), P(hr), P(r_), P(z_), Nr, Dr, P(dpx), 3 * Dr, P(dh_), st0))
+        for peep in (True, False):
+            chk(L.gnnb_lstm_cell(P(px4), ld4, P(ah4), P(cr), P(wr) if peep else None, Nr, Dr, P(gates), P(n_), P(hn_), st0))
+            chk(L.gnnb_lstm_cell_bwd(P(hn_), P(n_), P(cr), P(gates), P(n_), P(wr) if peep else None, Nr, Dr, P(dpre),
+                                     P(dz_), P(dw) if peep else None, P(ws) if peep else None, st0))
+    print("recurrent gates D", Dr, "ok")
+ar = torch.arange(60, device="cuda")
+gr = gnn.GNNGraph(torch.cat([ar, (ar + 1) % 60]) + 1, torch.cat([(ar + 1) % 60, ar]) + 1, num_nodes=60)
+for layer in (gnn.GConvGRU(3, 8, 3, device="cuda"), gnn.GConvLSTM(3, 8, 2, device="cuda"), gnn.DCGRU(3, 8, 2, device="cuda"),
+              gnn.TGCN(3, 8, device="cuda"), gnn.EvolveGCNO(3, 8, device="cuda")):
+    xr = gnn.colmajor(torch.randn(3, 5, 60, device="cuda")).requires_grad_(True)
+    layer(gr, xr).sum().backward()
+    print(repr(layer), "grad finite", bool(torch.isfinite(xr.grad).all()))
 torch.cuda.synchronize()
 print("done")
