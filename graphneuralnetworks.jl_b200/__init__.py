@@ -31,5 +31,7 @@ from .linkpred import (DotDecoder, add_edges, dot_decoder, edge_decoding, edge_e
 from .sampling import NeighborLoader, induced_subgraph, sample_edge_ids, sample_neighbors
 from .query import (adjacency_list, adjacency_matrix, has_multi_edges, has_self_loops, inneighbors, is_bidirected,
                     outneighbors)
+from .hetero import (GNNHeteroGraph, HeteroGraphConv, add_edges, edge_type_subgraph, has_edge, num_edge_types,
+                     num_node_types, rand_bipartite_heterograph, rand_heterograph)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -88,6 +88,7 @@ _SIGS = {
     "gnnb_softmax_edge_neighbors_bwd": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _vp]),
     "gnnb_gcn_norm": (_int, [_vp, _f32p, _f32p, _vp]),
     "gnnb_gcn_propagate": (_int, [_vp, _int, _f32p, _f32p, _f32p, _i64, _f32p, _vp]),
+    "gnnb_gcn_propagate_bipartite": (_int, [_vp, _int, _f32p, _i64, _f32p, _vp]),
     "gnnb_gat_aggregate": (_int, [_vp, _f32p, _f32p, _f32p, _i64, _i64, C.c_float, _f32p, _f32p, _f32p,
                                   _f32p, _vp]),
     "gnnb_gat_aggregate_bwd": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, C.c_float,

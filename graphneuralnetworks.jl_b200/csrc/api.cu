@@ -177,6 +177,23 @@ int gnnb_gcn_propagate(gnnb_graph_t g, int transposed, const float* x, const flo
     return gnnb_propagate(g, transposed, w ? GNNB_W_MUL_XJ : GNNB_COPY_XJ, GNNB_SUM, x, w, c, c, D, out, stream);
 }
 
+int gnnb_gcn_propagate_bipartite(gnnb_graph_t g, int transposed, const float* x, int64_t D, float* out, void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (!x || !out) GNNB_FAIL(GNNB_EINVAL, "x/out is NULL");
+    if (D <= 0) GNNB_FAIL(GNNB_ESIZE, "feature dimension must be positive (got %lld)", (long long)D);
+    cudaStream_t st = (cudaStream_t)stream;
+    GNNB_TRY(ensure_csr(g, transposed != 0, st));
+    GNNB_TRY(ensure_bipartite_gcn_scale(g, transposed != 0, st));
+    const Csr& cc = transposed ? g->by_src : g->by_dst;
+    SegArgs a;
+    // forward: gathered sources scaled by c_src (as the per-edge stream), target rows by c_dst; the pullback swaps them
+    a.x = x; a.out = out; a.D = D; a.aggr = GNNB_SUM;
+    a.cs = transposed ? g->bip_c_dst : g->bip_c_src;
+    a.es = transposed ? g->bip_es_src : g->bip_es_dst;
+    a.ct = transposed ? g->bip_c_src : g->bip_c_dst;
+    return seg_reduce(g, cc, a, st);
+}
+
 // ---- node-partitioned shards ---------------------------------------------------------------------
 int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local, const float* x_halo,
                         int64_t n_local, const float* w, const float* cs, const float* ct, int64_t D, float* out,

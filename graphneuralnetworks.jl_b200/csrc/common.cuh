@@ -93,6 +93,11 @@ struct gnnb_graph {
     float* ws2 = nullptr;
     size_t ws2_bytes = 0;
     float* gcn_c = nullptr;      // lazily: 1/sqrt(in-degree), the default symmetric normalisation (unweighted), plan-owned
+    // lazily: the two-sided (heterograph) GCN normalisation, kept apart from gcn_c / Csr::es so a square plan can serve both
+    float* bip_c_src = nullptr;  // [n_src] 1/sqrt(out-degree)
+    float* bip_c_dst = nullptr;  // [n_dst] 1/sqrt(in-degree)
+    float* bip_es_dst = nullptr; // [E] bip_c_src[col[e]] in by_dst plan order (forward)
+    float* bip_es_src = nullptr; // [E] bip_c_dst[col[e]] in by_src plan order (pullback)
     void* host_ws = nullptr;     // device staging of the *_host entries (grown on demand, freed with the plan)
     size_t host_ws_bytes = 0;
     std::mutex mu;
@@ -105,6 +110,8 @@ int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st);
 int ensure_invdeg(gnnb_graph* g, Csr& c, cudaStream_t st);
 int ensure_items(gnnb_graph* g, const Csr& c, cudaStream_t st);            // seglean.cu
 int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st);     // seglean.cu: g->gcn_c and the Csr's es stream
+int ensure_bipartite_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st);   // seglean.cu: g->bip_* for one direction
+int rsqrt_exact(float* d, int64_t n, cudaStream_t st);                     // edgeops.cu: d = 1/sqrt(d) in place
 // transform.cu: flags[k] = 1 where sorted key k starts a run of equal keys (k == 0 or keys[k] != keys[k-1])
 int run_head_flags(const uint64_t* keys, int64_t E, int32_t* flags, cudaStream_t st);
 

@@ -66,6 +66,12 @@ __global__ void rsqrt_exact_kernel(float* __restrict__ d, int64_t n) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) d[i] = __fdiv_rn(1.0f, __fsqrt_rn(d[i]));
 }
+int rsqrt_exact(float* d, int64_t n, cudaStream_t st) {
+    if (n <= 0) return GNNB_OK;
+    rsqrt_exact_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(d, n);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
 
 // dw_plan[e] = scale * <dout[row[e],:], x[col[e],:]>   (pullback of w_mul_xj w.r.t. the edge weight)
 template <int TPR>

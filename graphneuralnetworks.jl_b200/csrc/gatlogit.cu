@@ -107,6 +107,83 @@ __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_bwd_kernel(const f
     }
 }
 
+// one half per pass (a relation between two node types: el over the targets' W xi, er over the sources' W xj):
+// out[n, h] = sum_c a[off + c, h] Wx[c, h, n], off = 0 (el) or C (er)
+template <int G>
+__global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_half_fwd_kernel(const float* __restrict__ Wx, const float* __restrict__ a,
+                                                                              int64_t N, int C, int H, int off, float* __restrict__ out) {
+    constexpr int HPP = 32 / G;
+    const int lane = threadIdx.x & 31;
+    const int64_t n = (int64_t)blockIdx.x * LOGIT_WARPS + (threadIdx.x >> 5);
+    if (n >= N) return;
+    const int sub = lane / G, c4 = (lane % G) * 4;
+    const float* row = Wx + n * (int64_t)H * C;
+    for (int h0 = 0; h0 < H; h0 += HPP) {
+        const int h = h0 + sub;
+        float p = 0.f;
+        if (h < H) {
+            const float4 w = __ldg(reinterpret_cast<const float4*>(row + h * C + c4));
+            const float4 ah = __ldg(reinterpret_cast<const float4*>(a + (int64_t)h * 2 * C + off + c4));
+            p = ah.x * w.x + ah.y * w.y + ah.z * w.z + ah.w * w.w;
+        }
+#pragma unroll
+        for (int o = G / 2; o > 0; o >>= 1) p += __shfl_xor_sync(0xffffffffu, p, o);
+        if (h < H && (lane % G) == 0) out[n * H + h] = p;
+    }
+}
+
+// pullback of one half: dWx[c,h,n] += d[h,n] a[off+c,h]; the da partial holds sum_n d Wx in its half and 0 in the other
+template <int G, int PASSES>
+__global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_half_bwd_kernel(const float* __restrict__ Wx, const float* __restrict__ a,
+                                                                              const float* __restrict__ dh, int64_t N, int C, int H, int off,
+                                                                              float* __restrict__ dWx, float* __restrict__ partial) {
+    constexpr int HPP = 32 / G;
+    extern __shared__ float sm[];              // [LOGIT_WARPS][2 * H * C]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane / G, c4 = (lane % G) * 4;
+    const int64_t W = (int64_t)gridDim.x * LOGIT_WARPS;
+    float4 acc[PASSES], ah[PASSES];
+#pragma unroll
+    for (int p = 0; p < PASSES; ++p) {
+        acc[p] = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int h = p * HPP + sub;
+        ah[p] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (h < H) ah[p] = __ldg(reinterpret_cast<const float4*>(a + (int64_t)h * 2 * C + off + c4));
+    }
+    for (int64_t n = (int64_t)blockIdx.x * LOGIT_WARPS + warp; n < N; n += W) {
+        const float* row = Wx + n * (int64_t)H * C;
+        float* drow = dWx + n * (int64_t)H * C;
+#pragma unroll
+        for (int p = 0; p < PASSES; ++p) {
+            const int h = p * HPP + sub;
+            if (h < H) {
+                const float d = __ldg(dh + n * H + h);
+                const float4 w = __ldg(reinterpret_cast<const float4*>(row + h * C + c4));
+                float4 v = *reinterpret_cast<const float4*>(drow + h * C + c4);
+                v.x += d * ah[p].x; v.y += d * ah[p].y; v.z += d * ah[p].z; v.w += d * ah[p].w;
+                *reinterpret_cast<float4*>(drow + h * C + c4) = v;
+                acc[p].x += d * w.x; acc[p].y += d * w.y; acc[p].z += d * w.z; acc[p].w += d * w.w;
+            }
+        }
+    }
+    const int A = 2 * H * C;
+    float* mine = sm + warp * A;
+#pragma unroll
+    for (int p = 0; p < PASSES; ++p) {
+        const int h = p * HPP + sub;
+        if (h < H) {
+            *reinterpret_cast<float4*>(mine + h * 2 * C + off + c4) = acc[p];
+            *reinterpret_cast<float4*>(mine + h * 2 * C + (C - off) + c4) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < A; i += blockDim.x) {
+        float s = 0.f;
+        for (int w = 0; w < LOGIT_WARPS; ++w) s += sm[w * A + i];
+        partial[(int64_t)blockIdx.x * A + i] = s;
+    }
+}
+
 __global__ void gat_logit_final_kernel(const float* __restrict__ partial, int nblocks, int A, float* __restrict__ da) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= A) return;
@@ -134,12 +211,21 @@ extern "C" {
 int gnnb_gat_logit_terms(const float* Wx, const float* a, int64_t N, int64_t C, int64_t H, float* el, float* er, void* stream) {
     if (N < 0 || C <= 0 || H <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
     if (N == 0) return GNNB_OK;
-    if (!Wx || !a || !el || !er) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (!Wx || !a || (!el && !er)) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     int G = 0;
     if (!logit_shape(C, H, &G) || ((uintptr_t)Wx & 15) || ((uintptr_t)a & 15))
         GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms: C/4 must be a power of two <= 32, C*H <= 4096, 16 B-aligned operands");
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned blocks = (unsigned)ceil_div(N, LOGIT_WARPS);
+    if (!el || !er) {                          // one half: el (rows 1..C of a) or er (rows C+1..2C)
+        float* out = el ? el : er;
+        const int off = el ? 0 : (int)C;
+#define GNNB_LH(GG) case GG: gat_logit_half_fwd_kernel<GG><<<blocks, LOGIT_WARPS * 32, 0, st>>>(Wx, a, N, (int)C, (int)H, off, out); break;
+        switch (G) { GNNB_LH(1) GNNB_LH(2) GNNB_LH(4) GNNB_LH(8) GNNB_LH(16) GNNB_LH(32) }
+#undef GNNB_LH
+        GNNB_LAUNCHED();
+        return GNNB_OK;
+    }
 #define GNNB_LG(GG) case GG: gat_logit_fwd_kernel<GG><<<blocks, LOGIT_WARPS * 32, 0, st>>>(Wx, a, N, (int)C, (int)H, el, er); break;
     switch (G) { GNNB_LG(1) GNNB_LG(2) GNNB_LG(4) GNNB_LG(8) GNNB_LG(16) GNNB_LG(32) }
 #undef GNNB_LG
@@ -154,7 +240,7 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
     cudaStream_t st = (cudaStream_t)stream;
     const int A = (int)(2 * H * C);
     if (N == 0) { GNNB_CUDA(cudaMemsetAsync(da, 0, sizeof(float) * (size_t)A, st)); return GNNB_OK; }
-    if (!Wx || !a || !del || !der || !dWx_accum) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (!Wx || !a || (!del && !der) || !dWx_accum) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     int G = 0;
     if (!logit_shape(C, H, &G) || ((uintptr_t)Wx & 15) || ((uintptr_t)a & 15) || ((uintptr_t)dWx_accum & 15))
         GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms_bwd: C/4 must be a power of two <= 32, C*H <= 4096, 16 B-aligned operands");
@@ -168,6 +254,24 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
     static float* part_buf = nullptr; static size_t part_bytes = 0;
     const size_t need = sizeof(float) * (size_t)nblocks * A;
     if (part_bytes < need) { if (part_buf) { cudaDeviceSynchronize(); cudaFree(part_buf); } GNNB_CUDA(cudaMalloc(&part_buf, need)); part_bytes = need; }
+    if (!del || !der) {                        // one half: del (target half of da) or der (source half)
+        const float* dh = del ? del : der;
+        const int off = del ? 0 : (int)C;
+#define GNNB_LHB(GG, PP) { auto k = gat_logit_half_bwd_kernel<GG, PP>; \
+        if (smem > 48 * 1024) GNNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        k<<<nblocks, LOGIT_WARPS * 32, smem, st>>>(Wx, a, dh, N, (int)C, (int)H, off, dWx_accum, part_buf); }
+#define GNNB_LHBP(GG) switch (passes) { case 1: GNNB_LHB(GG, 1) break; case 2: GNNB_LHB(GG, 2) break; case 3: case 4: GNNB_LHB(GG, 4) break; default: GNNB_LHB(GG, 8) break; }
+        switch (G) {
+            case 1: GNNB_LHBP(1) break; case 2: GNNB_LHBP(2) break; case 4: GNNB_LHBP(4) break;
+            case 8: GNNB_LHBP(8) break; case 16: GNNB_LHBP(16) break; default: GNNB_LHBP(32) break;
+        }
+#undef GNNB_LHBP
+#undef GNNB_LHB
+        GNNB_LAUNCHED();
+        gat_logit_final_kernel<<<(unsigned)ceil_div((int64_t)A, 128), 128, 0, st>>>(part_buf, nblocks, A, da);
+        GNNB_LAUNCHED();
+        return GNNB_OK;
+    }
 #define GNNB_LB(GG, PP) { auto k = gat_logit_bwd_kernel<GG, PP>; \
         if (smem > 48 * 1024) GNNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         k<<<nblocks, LOGIT_WARPS * 32, smem, st>>>(Wx, a, del, der, N, (int)C, (int)H, dWx_accum, part_buf); }

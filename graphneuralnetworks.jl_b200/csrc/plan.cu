@@ -362,6 +362,10 @@ int gnnb_graph_destroy(gnnb_graph_t g) {
     cudaFree(g->ws);
     cudaFree(g->ws2);
     cudaFree(g->gcn_c);
+    cudaFree(g->bip_c_src);
+    cudaFree(g->bip_c_dst);
+    cudaFree(g->bip_es_dst);
+    cudaFree(g->bip_es_src);
     cudaFree(g->host_ws);
     delete g;
     return GNNB_OK;

@@ -449,6 +449,39 @@ int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) {
     return GNNB_OK;
 }
 
+// the two-sided scales of a relation (heterograph gcn_conv, conv.jl:45-50): c_src = 1/sqrt(out-degree), c_dst =
+// 1/sqrt(in-degree), both IEEE-exact as gnnb_gcn_norm, and for one direction the per-edge stream of the gathered side's
+// scale: forward (by_dst) es[e] = c_src[col[e]], pullback (by_src) es[e] = c_dst[col[e]]
+int ensure_bipartite_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) {
+    float*& es_slot = transposed ? g->bip_es_src : g->bip_es_dst;
+    if (g->bip_c_src != nullptr && g->bip_c_dst != nullptr && (es_slot != nullptr || g->E == 0)) return GNNB_OK;
+    GNNB_TRY(ensure_csr(g, true, st));                   // out-degrees come from the by-source rowptr
+    if (g->bip_c_src == nullptr || g->bip_c_dst == nullptr) {
+        float *cs = nullptr, *cd = nullptr;
+        GNNB_CUDA(cudaMalloc(&cs, sizeof(float) * (size_t)(g->n_src > 0 ? g->n_src : 1)));
+        GNNB_CUDA(cudaMalloc(&cd, sizeof(float) * (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
+        int rc = gnnb_degree(g, GNNB_DIR_OUT, nullptr, cs, st);
+        if (rc == GNNB_OK) rc = gnnb_degree(g, GNNB_DIR_IN, nullptr, cd, st);
+        if (rc == GNNB_OK) rc = rsqrt_exact(cs, g->n_src, st);
+        if (rc == GNNB_OK) rc = rsqrt_exact(cd, g->n_dst, st);
+        if (rc != GNNB_OK) { cudaFree(cs); cudaFree(cd); return rc; }
+        GNNB_CUDA(cudaStreamSynchronize(st));
+        std::lock_guard<std::mutex> lock(g->mu);
+        if (g->bip_c_src == nullptr) { g->bip_c_src = cs; g->bip_c_dst = cd; } else { cudaFree(cs); cudaFree(cd); }
+    }
+    if (es_slot == nullptr && g->E > 0) {
+        const Csr& c = transposed ? g->by_src : g->by_dst;
+        float* es = nullptr;
+        GNNB_CUDA(cudaMalloc(&es, sizeof(float) * (size_t)g->E));
+        gather_scale_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, transposed ? g->bip_c_dst : g->bip_c_src, es);
+        GNNB_LAUNCHED();
+        GNNB_CUDA(cudaStreamSynchronize(st));
+        std::lock_guard<std::mutex> lock(g->mu);
+        if (es_slot == nullptr) es_slot = es; else cudaFree(es);
+    }
+    return GNNB_OK;
+}
+
 // the lean path: D in {128, 256, 512}, 16 B-aligned operands.  GNNB_EUNSUPPORTED = not this kernel's shape (the caller
 // falls back to seg_reduce_kernel).
 int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, cudaStream_t st) {

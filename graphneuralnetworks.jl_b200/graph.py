@@ -199,29 +199,69 @@ class GNNGraph:
         """Build (once) and return the device plan.  Raises AssertionError on out-of-range indices."""
         if self._plan is not None:
             return self._plan
-        if device is None:
-            device = _compute_device(self.s)
-        if _lib.device_count() <= 0:
-            raise _lib.GNNBError(_lib.ECUDA, "no CUDA device: the message-passing engine has no CPU fallback")
-        h = C.c_void_p()
-        on_dev = 1 if self.s.is_cuda else 0
-        with torch.cuda.device(device):
-            _lib.check(lib.gnnb_graph_create(C.byref(h), self.s.data_ptr(), self.t.data_ptr(), self.num_edges,
-                                             self.num_nodes, self.num_nodes, self.s.element_size(), 1, on_dev,
-                                             _stream(device)))
-        self._plan = _Plan(h.value, device)
+        self._plan = _make_plan(self.s, self.t, self.num_edges, self.num_nodes, self.num_nodes, device)
         return self._plan
+
+
+def _make_plan(s: torch.Tensor, t: torch.Tensor, num_edges: int, num_src: int, num_dst: int,
+               device: Optional[torch.device] = None) -> _Plan:
+    """gnnb_graph_create over 1-based (s, t): sources in [1, num_src], targets in [1, num_dst] (AssertionError
+    otherwise)."""
+    if device is None:
+        device = _compute_device(s)
+    if _lib.device_count() <= 0:
+        raise _lib.GNNBError(_lib.ECUDA, "no CUDA device: the message-passing engine has no CPU fallback")
+    h = C.c_void_p()
+    on_dev = 1 if s.is_cuda else 0
+    with torch.cuda.device(device):
+        _lib.check(lib.gnnb_graph_create(C.byref(h), s.data_ptr(), t.data_ptr(), num_edges, num_src, num_dst,
+                                         s.element_size(), 1, on_dev, _stream(device)))
+    return _Plan(h.value, device)
+
+
+def _is_hetero(g) -> bool:
+    return getattr(g, "is_hetero", False)
+
+
+def relation(g):
+    """The one relation message passing runs over: the graph itself for a GNNGraph, the only edge type's relation
+    (``s``, ``t``, ``w``, ``num_edges``, ``plan()``) for a one-relation GNNHeteroGraph (AssertionError otherwise)."""
+    if _is_hetero(g):
+        return g.only_relation()
+    return g
+
+
+def num_src_dst(g) -> tuple:
+    """(num_src, num_dst) of that relation: (num_nodes, num_nodes) for a GNNGraph; the node counts of the source and
+    target types for a one-relation GNNHeteroGraph.  Every array message passing makes is sized by these two."""
+    if _is_hetero(g):
+        r = g.only_relation()
+        return r.num_src, r.num_dst
+    return g.num_nodes, g.num_nodes
+
+
+def homogeneous_only(g, name: str) -> None:
+    """The reference types these layers for GNNGraph only: a heterograph is a TypeError naming the layer."""
+    if _is_hetero(g):
+        raise TypeError(f"{name} needs a GNNGraph; it has no method for a GNNHeteroGraph (use a relation-wise layer "
+                        f"inside HeteroGraphConv)")
 
 
 # --------------------------------------------------------------------------------------------------
 # queries / transforms on the hot path
 # --------------------------------------------------------------------------------------------------
-def edge_index(g: GNNGraph):
-    """(s, t) — GNNGraphs/src/query.jl:12."""
+def edge_index(g: GNNGraph, *args):
+    """(s, t) — GNNGraphs/src/query.jl:12 (heterographs: edge_index(g[, edge_t]), gnnheterograph/query.jl:9-10)."""
+    if _is_hetero(g):
+        from .hetero import edge_index as f
+        return f(g, *args)
     return g.s, g.t
 
 
-def get_edge_weight(g: GNNGraph):
+def get_edge_weight(g: GNNGraph, *args):
+    if _is_hetero(g):
+        from .hetero import get_edge_weight as f
+        return f(g, *args)
     return g.w
 
 
@@ -234,11 +274,15 @@ def set_edge_weight(g: GNNGraph, w: torch.Tensor) -> GNNGraph:
     return h
 
 
-def add_self_loops(g: GNNGraph) -> GNNGraph:
+def add_self_loops(g: GNNGraph, *args) -> GNNGraph:
     """s=[s;1:n], t=[t;1:n], weights padded with 1 — GNNGraphs/src/transform.jl:12-28.
 
     Requires empty edata (the reference asserts it).  The result (and its plan, derived on the device from
-    this graph's CSR without a new sort) is cached on ``g``: graphs are immutable values."""
+    this graph's CSR without a new sort) is cached on ``g``: graphs are immutable values.  Heterographs:
+    add_self_loops(g[, edge_t]) (gnnheterograph/transform.jl:20-76)."""
+    if _is_hetero(g):
+        from .hetero import add_self_loops as f
+        return f(g, *args)
     assert len(g.edata) == 0, "add_self_loops requires empty edata"  # transform.jl:14
     if g._loops is not None:
         return g._loops
@@ -285,11 +329,19 @@ class _WeightedDegreeFn(torch.autograd.Function):
         return dw, None, None, None
 
 
-def degree(g: GNNGraph, T=None, *, dir: str = "out", edge_weight=True) -> torch.Tensor:
+def degree(g: GNNGraph, T=None, *args, dir: str = "out", edge_weight=True) -> torch.Tensor:
     """degree(g, T; dir, edge_weight) — GNNGraphs/src/query.jl:314-331,355-369 (note the reference default dir=:out).
 
     edge_weight: True -> the graph's own weights if any, False/None -> counts, tensor -> those weights.  With weights
-    that require grad the result is differentiable in them (the reference's weighted degree is a scatter(+))."""
+    that require grad the result is differentiable in them (the reference's weighted degree is a scatter(+)).
+    Heterographs: degree(g, edge_t, T=None; dir) (gnnheterograph/query.jl:55-68)."""
+    if _is_hetero(g):
+        if edge_weight is not True:
+            raise TypeError("degree(g::GNNHeteroGraph, edge_t, T; dir) takes no edge_weight (its degrees are unweighted)")
+        from .hetero import degree as f
+        return f(g, T, *args, dir=dir)
+    if args:
+        raise TypeError(f"degree(g::GNNGraph, T; dir, edge_weight) takes one positional argument after g, got {1 + len(args)}")
     assert dir in ("in", "out", "both")  # query.jl:339
     if isinstance(edge_weight, torch.Tensor):
         w = edge_weight
@@ -313,8 +365,11 @@ def degree(g: GNNGraph, T=None, *, dir: str = "out", edge_weight=True) -> torch.
     return out.to(T)
 
 
-def graph_indicator(g: GNNGraph, edges: bool = False) -> torch.Tensor:
-    """GNNGraphs/src/query.jl:500-512."""
+def graph_indicator(g: GNNGraph, edges=False) -> torch.Tensor:
+    """GNNGraphs/src/query.jl:500-512 (heterographs: graph_indicator(g[, node_t]), gnnheterograph/query.jl:81-98)."""
+    if _is_hetero(g):
+        from .hetero import graph_indicator as f
+        return f(g) if edges is False else f(g, edges)
     gi = g.graph_indicator
     if gi is None:
         gi = torch.ones(g.num_nodes, dtype=torch.int64, device=g.s.device)
@@ -328,6 +383,9 @@ def batch(graphs: Sequence[GNNGraph]) -> GNNGraph:
     cumulative node counts, graph_indicator by the cumulative graph counts; edges stay grouped per graph."""
     graphs = list(graphs)
     assert len(graphs) > 0
+    if _is_hetero(graphs[0]):
+        from .hetero import batch as f
+        return f(graphs)
     dev = graphs[0].s.device
     nodesum = np.cumsum([0] + [g.num_nodes for g in graphs])
     graphsum = np.cumsum([0] + [g.num_graphs for g in graphs])

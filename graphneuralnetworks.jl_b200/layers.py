@@ -27,7 +27,7 @@ import torch
 
 from . import _lib
 from ._lib import lib
-from .graph import GNNGraph, _stream, add_self_loops, degree, rows, unrows
+from .graph import GNNGraph, _is_hetero, _stream, add_self_loops, degree, homogeneous_only, num_src_dst, relation, rows, unrows
 from .msgpass import (Fix1, _GCNPropagateFn, _f32, aggregate_neighbors, apply_edges, check_num_nodes, copy_xj,
                       e_mul_xj, expand_srcdst, mean, propagate, softmax_edge_neighbors, w_mul_xj)
 
@@ -212,6 +212,8 @@ def gcn_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor
              norm_fn: Optional[Callable] = None, conv_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:14-72, statement for statement; the unweighted default-norm case runs the
     fused kernel (degree from rowptr, both 1/sqrt(d) scalings folded into the load/store of one pass)."""
+    if _is_hetero(g):
+        return _gcn_conv_hetero(l, g, x, edge_weight, norm_fn, conv_weight)
     check_gcnconv_input(g, edge_weight)
     if conv_weight is None:
         weight = l.weight
@@ -255,6 +257,72 @@ def gcn_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor
     return _bias_act(l, out)
 
 
+class _GCNBipartiteFn(torch.autograd.Function):
+    """c_dst .* propagate(copy_xj, g, +, xj = x .* c_src') with c_src = 1/sqrt(out-degree), c_dst = 1/sqrt(in-degree):
+    gnnb_gcn_propagate_bipartite both ways (the plan keeps both scale vectors and their per-edge streams)."""
+
+    @staticmethod
+    def forward(ctx, x_rows, plan, n_dst):
+        D = math.prod(x_rows.shape[1:])          # x may have no rows (num_src == 0) while out has num_dst
+        out = torch.empty((n_dst,) + tuple(x_rows.shape[1:]), dtype=torch.float32, device=x_rows.device)
+        with torch.cuda.device(plan.device):
+            _lib.check(lib.gnnb_gcn_propagate_bipartite(plan.h, 0, x_rows.data_ptr(), D, out.data_ptr(),
+                                                        _stream(plan.device)))
+        ctx.plan, ctx.D, ctx.n_src = plan, D, x_rows.shape[0]
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        dout = dout.contiguous()
+        dx = torch.empty((ctx.n_src,) + tuple(dout.shape[1:]), dtype=torch.float32, device=dout.device)
+        with torch.cuda.device(ctx.plan.device):
+            _lib.check(lib.gnnb_gcn_propagate_bipartite(ctx.plan.h, 1, dout.data_ptr(), ctx.D, dx.data_ptr(),
+                                                        _stream(ctx.plan.device)))
+        return dx, None, None
+
+
+def _gcn_conv_hetero(l, g, x, edge_weight, norm_fn, conv_weight) -> torch.Tensor:
+    """gcn_conv's heterograph branch (GNNlib/src/layers/conv.jl:14-72): unweighted out- and in-degrees of the one
+    relation scale the sources and the targets, and W is applied after the propagation whatever Dout and Din are.  The
+    default norm_fn without edge weights is one fused pass each way; anything else composes degree and propagate in the
+    reference's order.  A target without in-edges gets 0 (before bias and σ) and a source without out-edges a zero
+    gradient, where the reference's 0 * 1/sqrt(0) gives NaN."""
+    rel = relation(g)
+    check_gcnconv_input(rel, edge_weight)
+    weight = l.weight if conv_weight is None else conv_weight
+    if conv_weight is not None and tuple(weight.shape) != tuple(l.weight.shape):
+        raise ValueError(f"The weight matrix has the wrong size. Expected {tuple(l.weight.shape)} "
+                         f"but got {tuple(weight.shape)}")
+    if l.add_self_loops:
+        g = add_self_loops(g)                  # loops on a relation between nodes of one type only
+        n_loops = relation(g).num_edges - rel.num_edges
+        rel = relation(g)
+        if edge_weight is not None:
+            edge_weight = torch.cat([edge_weight, torch.ones(n_loops, dtype=edge_weight.dtype, device=edge_weight.device)])
+            assert edge_weight.numel() == rel.num_edges
+    xj, xi = expand_srcdst(g, x)
+    check_num_nodes(g, (xj, xi))
+    use_w = bool(getattr(l, "use_edge_weight", False))
+    n_src, n_dst = num_src_dst(g)
+    if edge_weight is None and not use_w and norm_fn is None:
+        plan = rel.plan()
+        out = unrows(_GCNBipartiteFn.apply(_f32(rows(xj), plan.device), plan, n_dst))
+    else:
+        nf = norm_fn or default_norm_fn
+        et = g.etypes[0]
+        cin = nf(degree(g, et, torch.float32, dir="in"))
+        cout = nf(degree(g, et, torch.float32, dir="out"))
+        xs = xj * cout.reshape(1, -1)
+        if edge_weight is not None:
+            out = propagate(e_mul_xj, g, operator.add, xj=xs, e=edge_weight)
+        elif use_w:
+            out = propagate(w_mul_xj, g, operator.add, xj=xs)
+        else:
+            out = propagate(copy_xj, g, operator.add, xj=xs)
+        out = out * cin.reshape(1, -1)
+    return _linear(l, weight, out, True)       # σ.(W * x .+ b)
+
+
 def glorot_uniform(*shape, device=None) -> torch.Tensor:
     """Flux.glorot_uniform: U(-s, s), s = sqrt(24 / (fan_in + fan_out)) / 2... = sqrt(6/(fan_in+fan_out))."""
     fan_out, fan_in = shape[0], shape[1] if len(shape) > 1 else shape[0]
@@ -285,8 +353,9 @@ class _GATAggregateFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, Wx_rows, el_rows, er_rows, plan, slope):
-        N, H, Cc = Wx_rows.shape
-        out = torch.empty_like(Wx_rows)
+        _, H, Cc = Wx_rows.shape
+        N = el_rows.shape[0]                   # targets (num_dst); Wx and er have a row per source
+        out = torch.empty((N, H, Cc), dtype=torch.float32, device=Wx_rows.device)
         smax = torch.empty((N, H), dtype=torch.float32, device=Wx_rows.device)
         ssum = torch.empty((N, H), dtype=torch.float32, device=Wx_rows.device)
         with torch.cuda.device(plan.device):
@@ -356,6 +425,54 @@ class _GATCoreFn(torch.autograd.Function):
         return dWx, da_jl.t(), None, None
 
 
+class _GATPairFn(torch.autograd.Function):
+    """gat_conv's edge part for two projections: Wxj (N_src, H, C) over the sources, Wxi (N_dst, H, C) over the targets.
+    el from Wxi and er from Wxj, one half per gnnb_gat_logit_terms pass, then gnnb_gat_aggregate over the plan.
+    Backward: gnnb_gat_aggregate_bwd gives dWxj, del, der; gnnb_gat_logit_terms_bwd adds the er chain into dWxj and the
+    el chain into dWxi, each with its half of da (the other half zero), and da is their sum."""
+
+    @staticmethod
+    def forward(ctx, Wxj_rows, Wxi_rows, a, plan, slope):
+        Ns, H, Cc = Wxj_rows.shape
+        Nd = Wxi_rows.shape[0]
+        dev = Wxj_rows.device
+        a_jl = a.detach().t().contiguous()                 # Julia (2C, H) column-major memory = rows (H, 2C)
+        el = torch.empty((Nd, H), dtype=torch.float32, device=dev)
+        er = torch.empty((Ns, H), dtype=torch.float32, device=dev)
+        out = torch.empty((Nd, H, Cc), dtype=torch.float32, device=dev)
+        smax, ssum = torch.empty_like(el), torch.empty_like(el)
+        with torch.cuda.device(plan.device):
+            st = _stream(plan.device)
+            _lib.check(lib.gnnb_gat_logit_terms(Wxi_rows.data_ptr(), a_jl.data_ptr(), Nd, Cc, H, el.data_ptr(), None, st))
+            _lib.check(lib.gnnb_gat_logit_terms(Wxj_rows.data_ptr(), a_jl.data_ptr(), Ns, Cc, H, None, er.data_ptr(), st))
+            _lib.check(lib.gnnb_gat_aggregate(plan.h, Wxj_rows.data_ptr(), el.data_ptr(), er.data_ptr(), Cc, H, slope,
+                                              out.data_ptr(), None, smax.data_ptr(), ssum.data_ptr(), st))
+        ctx.plan, ctx.slope, ctx.dims = plan, slope, (Cc, H)
+        ctx.save_for_backward(Wxj_rows, Wxi_rows, a_jl, el, er, smax, ssum, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        Wxj_rows, Wxi_rows, a_jl, el, er, smax, ssum, out = ctx.saved_tensors
+        Cc, H = ctx.dims
+        Ns, Nd = Wxj_rows.shape[0], Wxi_rows.shape[0]
+        dout = dout.contiguous()
+        dWxj = torch.empty_like(Wxj_rows)
+        dWxi = torch.zeros_like(Wxi_rows)
+        del_, der = torch.empty_like(el), torch.empty_like(er)
+        da_r, da_l = torch.empty_like(a_jl), torch.empty_like(a_jl)
+        with torch.cuda.device(ctx.plan.device):
+            st = _stream(ctx.plan.device)
+            _lib.check(lib.gnnb_gat_aggregate_bwd(ctx.plan.h, Wxj_rows.data_ptr(), el.data_ptr(), er.data_ptr(),
+                                                  smax.data_ptr(), ssum.data_ptr(), out.data_ptr(), dout.data_ptr(), Cc, H,
+                                                  ctx.slope, dWxj.data_ptr(), del_.data_ptr(), der.data_ptr(), st))
+            _lib.check(lib.gnnb_gat_logit_terms_bwd(Wxj_rows.data_ptr(), a_jl.data_ptr(), None, der.data_ptr(), Ns, Cc, H,
+                                                    dWxj.data_ptr(), da_r.data_ptr(), st))
+            _lib.check(lib.gnnb_gat_logit_terms_bwd(Wxi_rows.data_ptr(), a_jl.data_ptr(), del_.data_ptr(), None, Nd, Cc, H,
+                                                    dWxi.data_ptr(), da_l.data_ptr(), st))
+        return dWxj, dWxi, (da_l + da_r).t(), None, None
+
+
 def gat_logit_fusable(chout: int, heads: int) -> bool:
     """shapes csrc/gatlogit.cu covers: C/4 a power of two <= 32, C*H <= 4096 (config 3: 64 x 8)"""
     g = chout // 4
@@ -411,7 +528,26 @@ def gat_conv(l, g: GNNGraph, x: torch.Tensor, e: Optional[torch.Tensor] = None, 
     Wxi = Wxj
     if xi is not xj:
         Wxi = _jl_reshape3(l.dense_x(xi), chout, heads)
-    if fused and e is None and xi is xj and gat_fusable(chout, heads) and float(getattr(l, "dropout", 0.0) or 0.0) == 0.0:
+    nodrop = float(getattr(l, "dropout", 0.0) or 0.0) == 0.0
+    if fused and e is None and xi is not xj and gat_fusable(chout, heads) and nodrop:
+        # two projections (the (xj, xi) form; a relation between two node types): el from W xi over the num_dst
+        # targets, er from W xj over the num_src sources, then the fused logits -> leakyrelu -> neighbourhood softmax
+        # -> α-weighted sum over the relation's plan
+        plan = relation(g).plan()
+        Wr = _f32(rows(Wxj), plan.device)                       # (N_src, H, C)
+        if Wr.data_ptr() % 16 != 0:
+            Wr = Wr.clone()
+        Wi = _f32(rows(Wxi), plan.device)                       # (N_dst, H, C)
+        if Wi.data_ptr() % 16 != 0:
+            Wi = Wi.clone()
+        a = l.a
+        if gat_logit_fusable(chout, heads) and a.dtype == torch.float32:
+            out = unrows(_GATPairFn.apply(Wr, Wi, a, plan, float(l.negative_slope)))
+        else:
+            el = (Wi * a[:chout, :].t().unsqueeze(0)).sum(-1)   # rows 1..C of a pair with the target
+            er = (Wr * a[chout:, :].t().unsqueeze(0)).sum(-1)   # rows C+1..2C with the source
+            out = unrows(_GATAggregateFn.apply(Wr, el.contiguous(), er.contiguous(), plan, float(l.negative_slope)))
+    elif fused and e is None and xi is xj and gat_fusable(chout, heads) and nodrop:
         plan = g.plan()
         Wr = _f32(rows(Wxj), plan.device)                       # (N, H, C)
         if Wr.data_ptr() % 16 != 0:                             # a misaligned view: the fused kernels take 16 B-aligned rows
@@ -570,6 +706,7 @@ def gin_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
 def sgc_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:407-448 (SGConv): k rounds of the normalised GCN propagate around one W; the
     unweighted case is k launches of the fused kernel (both 1/sqrt(d) scalings folded in)."""
+    homogeneous_only(g, "sgc_conv")
     if edge_weight is not None:
         assert edge_weight.numel() == g.num_edges, \
             f"Wrong number of edge weights (expected {g.num_edges} but given {edge_weight.numel()})"
@@ -604,6 +741,7 @@ def sgc_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor
 
 def agnn_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:337-352: cosine-similarity attention, neighbourhood softmax, weighted sum."""
+    homogeneous_only(g, "agnn_conv")
     check_num_nodes(g, x)
     if l.add_self_loops:
         g = add_self_loops(g)
@@ -652,6 +790,7 @@ def _loops_and_weights(l, g: GNNGraph, edge_weight):
 
 def sg_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:501-543 (SGConv): W applied on the cheaper side of k normalised propagation rounds."""
+    homogeneous_only(g, "sg_conv")
     g, edge_weight = _loops_and_weights(l, g, edge_weight)
     W = l.weight
     Dout, Din = W.shape
@@ -668,6 +807,7 @@ def sg_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor]
 def tag_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:634-686 (TAGConv), as the reference computes it: after round i the running sum
     S_i = Σ_{j<=i} Â^j x is multiplied by the ONE weight matrix and accumulated:  Σ_i W S_i  (+ bias)."""
+    homogeneous_only(g, "tag_conv")
     g, edge_weight = _loops_and_weights(l, g, edge_weight)
     W = l.weight
     state = {"pow": None, "total": None}
@@ -740,6 +880,7 @@ class _LSTMCell(torch.nn.Module):
 def gated_graph_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:218-233: zero-pad x to `dims`, then num_layers rounds of
     m = propagate(copy_xj, g, aggr, xj = W_i * h);  h = gru(m, h).   l.weight is (dims, dims, num_layers)."""
+    homogeneous_only(g, "gated_graph_conv")
     check_num_nodes(g, x)
     m_in, n = x.shape
     assert m_in <= l.dims, "number of input features must be less or equal to output features."
@@ -813,6 +954,7 @@ def transformer_message_main(xi, xj, e):
 def transformer_conv(l, g: GNNGraph, x: torch.Tensor, e: Optional[torch.Tensor] = None) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:553-612: multi-head dot-product attention over each in-neighbourhood, then the
     root-weight / gating / skip / batch-norm / feed-forward tail (dense per-node work, left to torch like Flux's)."""
+    homogeneous_only(g, "transformer_conv")
     check_num_nodes(g, x)
     if l.add_self_loops:
         g = add_self_loops(g)

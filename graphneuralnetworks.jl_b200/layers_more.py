@@ -24,7 +24,7 @@ from typing import Callable, Optional
 import numpy as np
 import torch
 
-from .graph import GNNGraph, degree, rows, unrows
+from .graph import GNNGraph, degree, homogeneous_only, rows, unrows
 from .layers import (_add_bias, _bias, _Dense, _DenseAct, _jl_reshape3, _matmul, _sigma, glorot_uniform, identity,
                      relu)
 from .msgpass import (Fix1, aggregate_neighbors, apply_edges, check_num_edges, check_num_nodes, e_mul_xj,
@@ -110,6 +110,7 @@ def cheb_basis(g: GNNGraph, X: torch.Tensor, k: int, op=None) -> list:
 
 def cheb_conv(l, g: GNNGraph, X: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:83-98.  l.weight is (out, in, k), k >= 2 as in the reference."""
+    homogeneous_only(g, "cheb_conv")
     check_num_nodes(g, X)
     assert X.shape[0] == l.weight.shape[1], "Input feature size must match input channel size."
     Z = cheb_basis(g, X, int(l.k))
@@ -141,6 +142,7 @@ def nn_conv_message(l, xi, xj, e):
 
 def nn_conv(l, g: GNNGraph, x: torch.Tensor, e: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:260-265"""
+    homogeneous_only(g, "nn_conv")
     check_num_nodes(g, x)
     m = propagate(Fix1(nn_conv_message, l), g, l.aggr, xj=x, e=e)
     return _sigma(l)(_add_bias(_matmul(l.weight, x) + m, _bias(l)))
@@ -171,14 +173,15 @@ def cg_conv(l, g: GNNGraph, x: torch.Tensor, e: Optional[torch.Tensor] = None) -
     if e is not None:
         check_num_edges(g, e)
     m = propagate(Fix1(cg_message, l), g, operator.add, xi=xi, xj=xj, e=e)
-    if l.residual and x.shape[0] == m.shape[0]:                # otherwise the reference only warns
-        m = m + x
+    if l.residual and xi.shape[0] == m.shape[0]:               # otherwise the reference only warns
+        m = m + xi
     return m
 
 
 # ------------------------------------------------------------------------------------------------ MEGNet / GMM / EGNN
 def megnet_conv(l, g: GNNGraph, x: torch.Tensor, e: torch.Tensor):
     """GNNlib/src/layers/conv.jl:356-368: returns (x̄, ē)"""
+    homogeneous_only(g, "megnet_conv")
     check_num_nodes(g, x)
     phi_e = _field(l, "\u03d5e", "\u03c6e", "phi_e")              # ϕe (Python NFKC-normalises ϕ to φ in identifiers)
     phi_v = _field(l, "\u03d5v", "\u03c6v", "phi_v")
@@ -189,6 +192,7 @@ def megnet_conv(l, g: GNNGraph, x: torch.Tensor, e: torch.Tensor):
 
 def gmm_conv(l, g: GNNGraph, x: torch.Tensor, e: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:372-401, statement for statement (including the sign of the exponent)."""
+    homogeneous_only(g, "gmm_conv")
     (nin, ein), out = l.ch
     assert ein == e.shape[0] and g.num_edges == e.shape[1], "Pseudo-cordinate dimension is not equal to (ein,num_edge)"
     w = e.unsqueeze(1)                                         # (ein, 1, E)
@@ -217,6 +221,7 @@ def egnn_message(l, xi, xj, e):
 
 def egnn_conv(l, g: GNNGraph, h: torch.Tensor, x: torch.Tensor, e: Optional[torch.Tensor] = None):
     """GNNlib/src/layers/conv.jl:459-483: returns (h, x)"""
+    homogeneous_only(g, "egnn_conv")
     if l.num_features["edge"] > 0:
         assert e is not None, "Edge features must be provided."
     assert h.shape[0] == l.num_features["in"], "Input features must match layer input size."
@@ -267,6 +272,7 @@ def diffusion_basis(g: GNNGraph, x: torch.Tensor, k: int, gt: Optional[GNNGraph]
 
 def d_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:696-724, statement for statement.  l.weights is (2, k, out, in)."""
+    homogeneous_only(g, "d_conv")
     Wt = l.weights
     terms = diffusion_basis(g, x, int(l.k))
     h = _matmul(Wt[0, 0], x) + _matmul(Wt[1, 0], x)

@@ -25,7 +25,7 @@ import torch
 
 from . import _lib
 from ._lib import lib
-from .graph import GNNGraph, _ptr, _stream, rows, unrows
+from .graph import GNNGraph, _is_hetero, _ptr, _stream, num_src_dst, relation, rows, unrows
 
 # --------------------------------------------------------------------------------------------------
 # aggregation operators: `+`, mean, max, min (NNlib.scatter ops the layers use)
@@ -58,6 +58,14 @@ def _aggr_code(aggr) -> int:
 def check_num_nodes(g: GNNGraph, x) -> bool:
     if x is None:
         return True
+    if _is_hetero(g):
+        # gnnheterograph/utils.jl:1-13: a (xj, xi) pair, xj over the source type and xi over the target type
+        assert isinstance(x, tuple) and len(x) == 2, "a heterograph takes the node features as a (xj, xi) pair"
+        ns, nd = num_src_dst(g)
+        for v, n, side in ((x[0], ns, "source"), (x[1], nd, "target")):
+            if isinstance(v, torch.Tensor):
+                assert v.shape[-1] == n, f"Got {v.shape[-1]} as last dimension size instead of the {side} type's {n} nodes"
+        return True
     if isinstance(x, torch.Tensor):
         assert g.num_nodes == x.shape[-1], \
             f"Got {x.shape[-1]} as last dimension size instead of num_nodes={g.num_nodes}"
@@ -73,8 +81,8 @@ def check_num_edges(g: GNNGraph, e) -> bool:
     if e is None:
         return True
     if isinstance(e, torch.Tensor):
-        assert g.num_edges == e.shape[-1], \
-            f"Got {e.shape[-1]} as last dimension size instead of num_edges={g.num_edges}"
+        E = relation(g).num_edges
+        assert E == e.shape[-1], f"Got {e.shape[-1]} as last dimension size instead of num_edges={E}"
         return True
     if isinstance(e, dict):
         e = tuple(e.values())
@@ -161,12 +169,13 @@ def lib_edges(plan) -> int:
 
 
 class _PropagateFn(torch.autograd.Function):
-    """Fused propagate(copy_xj | w_mul_xj, g, aggr): gnnb_propagate / gnnb_propagate_bwd."""
+    """Fused propagate(copy_xj | w_mul_xj, g, aggr): gnnb_propagate / gnnb_propagate_bwd.  x has num_src rows, the
+    result num_dst (n_out)."""
 
     @staticmethod
-    def forward(ctx, x_rows, w, plan, aggr):
-        N, D = x_rows.shape[0], (x_rows[0].numel() if x_rows.shape[0] else 1)
-        out = torch.empty_like(x_rows)
+    def forward(ctx, x_rows, w, plan, aggr, n_out):
+        D = int(torch.tensor(x_rows.shape[1:]).prod()) if x_rows.dim() > 1 else 1
+        out = torch.empty((n_out,) + tuple(x_rows.shape[1:]), dtype=torch.float32, device=x_rows.device)
         msg = _lib.COPY_XJ if w is None else _lib.W_MUL_XJ
         with torch.cuda.device(plan.device):
             _lib.check(lib.gnnb_propagate(plan.h, 0, msg, aggr, x_rows.data_ptr(), _ptr(w), None, None, D,
@@ -187,7 +196,7 @@ class _PropagateFn(torch.autograd.Function):
             _lib.check(lib.gnnb_propagate_bwd(plan.h, ctx.msg, ctx.aggr, dout.data_ptr(), x_rows.data_ptr(),
                                               _ptr(w), None, None, _ptr(out), ctx.D, _ptr(dx), _ptr(dw),
                                               _stream(plan.device)))
-        return dx, dw, None, None
+        return dx, dw, None, None, None
 
 
 class _GCNPropagateFn(torch.autograd.Function):
@@ -256,21 +265,23 @@ def _map_struct(fn: Callable, x):
 
 
 def _gather(g: GNNGraph, x, which: int):
-    plan = g.plan()
+    rel = relation(g)
+    plan = rel.plan()
 
     def one(a: torch.Tensor):
-        r = _GatherFn.apply(_f32(rows(a), plan.device), plan, which, g.num_edges)
+        r = _GatherFn.apply(_f32(rows(a), plan.device), plan, which, rel.num_edges)
         return unrows(r)
 
     return _map_struct(one, x)
 
 
 def _scatter(g: GNNGraph, aggr, m, which: int = _lib.DST):
-    plan = g.plan()
+    plan = relation(g).plan()
     code = _aggr_code(aggr)
+    n = num_src_dst(g)[1 if which == _lib.DST else 0]
 
     def one(a: torch.Tensor):
-        r = _ScatterFn.apply(_f32(rows(a), plan.device), plan, which, code, g.num_nodes)
+        r = _ScatterFn.apply(_f32(rows(a), plan.device), plan, which, code, n)
         return unrows(r)
 
     return _map_struct(one, m)
@@ -337,7 +348,8 @@ def _fusable(f, xi, xj, e, g) -> Optional[Any]:
     if f is copy_xj:
         return "none"
     if f is w_mul_xj and e is None:
-        return "none" if g.w is None else g.w
+        w = relation(g).w
+        return "none" if w is None else w
     if f is e_mul_xj and isinstance(e, torch.Tensor) and e.dim() == 1:
         return e
     return None
@@ -349,9 +361,9 @@ def propagate(f: Callable, g: GNNGraph, aggr, xi=None, xj=None, e=None):
     if w is not None:
         check_num_nodes(g, (xj, xi))
         check_num_edges(g, e)
-        plan = g.plan()
+        plan = relation(g).plan()
         wt = None if isinstance(w, str) else _f32(w, plan.device)
-        out = _PropagateFn.apply(_f32(rows(xj), plan.device), wt, plan, _aggr_code(aggr))
+        out = _PropagateFn.apply(_f32(rows(xj), plan.device), wt, plan, _aggr_code(aggr), num_src_dst(g)[1])
         return unrows(out)
     m = apply_edges(f, g, xi, xj, e)
     return aggregate_neighbors(g, aggr, m)
@@ -359,8 +371,9 @@ def propagate(f: Callable, g: GNNGraph, aggr, xi=None, xj=None, e=None):
 
 def softmax_edge_neighbors(g: GNNGraph, e: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/utils.jl:84-97: softmax of the edge features over each target's in-neighbourhood."""
-    assert e.shape[-1] == g.num_edges
-    plan = g.plan()
+    rel = relation(g)
+    assert e.shape[-1] == rel.num_edges
+    plan = rel.plan()
     return unrows(_EdgeSoftmaxFn.apply(_f32(rows(e), plan.device), plan))
 
 

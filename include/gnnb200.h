@@ -192,6 +192,16 @@ int gnnb_softmax_edge_neighbors_bwd(gnnb_graph_t g, const float* alpha, const fl
 int gnnb_gcn_norm(gnnb_graph_t g, const float* w, float* c_out, void* stream);
 int gnnb_gcn_propagate(gnnb_graph_t g, int transposed, const float* x, const float* w,
                        const float* c, int64_t D, float* out, void* stream);
+/* The two-sided normalisation of gcn_conv on a one-relation heterograph (GNNlib/src/layers/conv.jl:45-50,58-66):
+ *     c_src = 1 ./ sqrt.(out-degree)   (num_src floats)      c_dst = 1 ./ sqrt.(in-degree)   (num_dst floats)
+ *     out = (propagate(copy_xj, g, +, xj = x .* c_src')) .* c_dst'          (x: num_src rows, out: num_dst rows)
+ * transposed=1 is the pullback: dx (num_src rows) = c_src .* (A^T-propagate(dout .* c_dst)), dout num_dst rows.
+ * Unweighted degrees, as the reference's heterograph branch.  Both scale vectors and their per-edge streams (c_src[s_k]
+ * in the by-target plan order, c_dst[t_k] in the by-source order) are built once and kept with the plan, apart from the
+ * symmetric scales of gnnb_gcn_propagate: a square plan may be asked for both normalisations.  Any num_src / num_dst
+ * (num_src == num_dst included).  A target without in-edges gets a zero row, a source without out-edges a zero
+ * gradient (the reference's 0 * 1/sqrt(0) is NaN there). */
+int gnnb_gcn_propagate_bipartite(gnnb_graph_t g, int transposed, const float* x, int64_t D, float* out, void* stream);
 
 /* --------------------------------------------------------------- GAT core
  * replaces: the edge part of gat_conv + gat_message (GNNlib/src/layers/conv.jl:136-141,152-167):
@@ -218,7 +228,10 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
  * Wx (C,H,N), a (2C,H) column-major as the layer stores it, el / er (H,N).  One pass over Wx.
  * Pullback: dWx_accum (C,H,N) += del[h,n] a[c,h] + der[h,n] a[C+c,h]  IN PLACE (it already holds the dWx of
  * gnnb_gat_aggregate_bwd), da (2C,H) = [sum_n del Wx ; sum_n der Wx] — deterministic (fixed-order reduction).
- * Shapes: C/4 a power of two <= 32, C*H <= 4096 (GNNB_EUNSUPPORTED otherwise). */
+ * Shapes: C/4 a power of two <= 32, C*H <= 4096 (GNNB_EUNSUPPORTED otherwise).
+ * One half per call (GAT across two node types, where el comes from W xi over the targets and er from W xj over the
+ * sources): el or er may be NULL (not both), and the pass computes the other half alone; del or der may be NULL (not
+ * both) in the pullback, which then adds that half's chain into dWx_accum and writes da with zeros in the other half. */
 int gnnb_gat_logit_terms(const float* Wx, const float* a, int64_t N, int64_t C, int64_t H, float* el, float* er, void* stream);
 int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, const float* der, int64_t N, int64_t C,
                              int64_t H, float* dWx_accum, float* da, void* stream);

@@ -297,6 +297,29 @@ function ChainRulesCore.rrule(::typeof(gcn_core), p::Plan, x, c)
     return out, gcn_core_pullback
 end
 
+# gcn_conv on a one-relation GNNHeteroGraph (GNNlib/src/layers/conv.jl:45-50,58-66): sources scaled by 1/sqrt(out-degree),
+# targets by 1/sqrt(in-degree), on the relation's bipartite plan (gnnb_gcn_propagate_bipartite).  x is (D, num_src), the
+# result (D, num_dst); the pullback is the same entry with transposed = 1.
+function gcn_core_bipartite(p::Plan, x::CuMatrix{Float32}, n_dst::Integer)
+    out = CuMatrix{Float32}(undef, size(x, 1), n_dst)
+    check(ccall((:gnnb_gcn_propagate_bipartite, LIB), Cint,
+                (Ptr{Cvoid}, Cint, CuPtr{Float32}, Int64, CuPtr{Float32}, Ptr{Cvoid}),
+                p.h, 0, x, size(x, 1), out, stream()))
+    return out
+end
+function ChainRulesCore.rrule(::typeof(gcn_core_bipartite), p::Plan, x, n_dst)
+    out = gcn_core_bipartite(p, x, n_dst)
+    function gcn_core_bipartite_pullback(Δ)
+        dout = CuArray{Float32}(unthunk(Δ))
+        dx = similar(x)
+        check(ccall((:gnnb_gcn_propagate_bipartite, LIB), Cint,
+                    (Ptr{Cvoid}, Cint, CuPtr{Float32}, Int64, CuPtr{Float32}, Ptr{Cvoid}),
+                    p.h, 1, dout, size(x, 1), dx, stream()))
+        return NoTangent(), NoTangent(), dx, NoTangent()       # the scales depend on the graph only (unweighted)
+    end
+    return out, gcn_core_bipartite_pullback
+end
+
 function in_degree(p::Plan, n::Integer)
     d = CUDA.zeros(Float32, n)
     check(ccall((:gnnb_degree, LIB), Cint, (Ptr{Cvoid}, Cint, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),

@@ -147,5 +147,22 @@ for layer in (gnn.GConvGRU(3, 8, 3, device="cuda"), gnn.GConvLSTM(3, 8, 2, devic
     xr = gnn.colmajor(torch.randn(3, 5, 60, device="cuda")).requires_grad_(True)
     layer(gr, xr).sum().backward()
     print(repr(layer), "grad finite", bool(torch.isfinite(xr.grad).all()))
+# two-sided GCN on relations: num_src >> num_dst, << num_dst, a row longer than the chunk, isolated sources and targets,
+# forward and pullback at D = 3, 128, 1000
+for ns_, nd_ in ((300, 7), (7, 300), (40, 30)):
+    sh = torch.randint(1, ns_, (900,), device="cuda")
+    th = torch.cat([torch.randint(1, nd_, (600,), device="cuda"), torch.ones(300, dtype=torch.int64, device="cuda")])
+    hg = gnn.GNNHeteroGraph({("A", "r", "B"): (sh, th)}, num_nodes={"A": ns_, "B": nd_})
+    for Dh in (3, 128, 1000):
+        lh = gnn.GCNConv(Dh, 8, device="cuda")
+        xh = torch.randn(Dh, ns_, device="cuda").requires_grad_(True)
+        lh(hg, (xh, torch.randn(Dh, nd_, device="cuda"))).sum().backward()
+        print("gcn bipartite", ns_, nd_, Dh, "grad finite", bool(torch.isfinite(xh.grad).all()))
+    for heads_, C_ in ((1, 8), (8, 16), (3, 128)):                 # one-half logit passes, forward and pullback
+        lg = gnn.GATConv(12, C_, heads=heads_, add_self_loops=False, device="cuda")
+        xa = torch.randn(12, ns_, device="cuda").requires_grad_(True)
+        xb = torch.randn(12, nd_, device="cuda").requires_grad_(True)
+        lg(hg, (xa, xb)).sum().backward()
+        print("gat bipartite", ns_, nd_, heads_, C_, "grad finite", bool(torch.isfinite(xa.grad).all() and torch.isfinite(xb.grad).all()))
 torch.cuda.synchronize()
 print("done")
