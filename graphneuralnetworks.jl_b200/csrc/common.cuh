@@ -76,6 +76,19 @@ struct Csr {
     bool built = false;
 };
 
+#ifdef __CUDACC__
+// max(a, b) that returns NaN when either operand is NaN (max.NaN.f32): Julia's `max`, which NNlib's scatter(max) and
+// relu fold with.  fmaxf returns the other operand instead.  Same bits as fmaxf whenever neither operand is NaN.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+    float d;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+    return d;
+}
+// the shift of an online softmax step whose new running max is Mn: Mn itself, or 0 while every logit seen so far is
+// -Inf, so that exp(M - shift) and exp(u - shift) give 0 there instead of exp(-Inf + Inf) = NaN
+__device__ __forceinline__ float softmax_shift(float Mn) { return Mn == -__int_as_float(0x7f800000) ? 0.f : Mn; }
+#endif
+
 }  // namespace gnnb
 
 struct gnnb_graph {

@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(256) bias_act_kernel(const float* __restrict__
             const float4 b = __ldg(reinterpret_cast<const float4*>(bias) + (int)(i % nv));
             v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
         }
-        if (RELU) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+        if (RELU) { v.x = fmax_nan(v.x, 0.f); v.y = fmax_nan(v.y, 0.f); v.z = fmax_nan(v.z, 0.f); v.w = fmax_nan(v.w, 0.f); }
         reinterpret_cast<float4*>(y)[i] = v;
     }
 }

@@ -60,6 +60,12 @@ __device__ __forceinline__ bool bar_wait(uint32_t bar, uint32_t parity, int* err
     return false;
 }
 __device__ __forceinline__ float tf32_big(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+// x - tf32_big(x): exact for finite x; 0 for x = +-Inf, whose big part already is x (Inf - Inf would put a NaN in the
+// cross terms).  A NaN stays NaN.
+__device__ __forceinline__ float tf32_small(float x, float b) { return isinf(x) ? 0.f : x - b; }
+__device__ __forceinline__ float4 tf32_small(float4 v, float4 b) {
+    return make_float4(tf32_small(v.x, b.x), tf32_small(v.y, b.y), tf32_small(v.z, b.z), tf32_small(v.w, b.w));
+}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // asks L2 to fetch `bytes` (a multiple of 16) at the 16 B aligned `p` ahead of the register loads that will read them
 __device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {
@@ -165,7 +171,7 @@ __device__ __forceinline__ void store_tile(const Params& p, const float* dm, con
                 const float2 a = *reinterpret_cast<const float2*>(p.addend + at);
                 o.x += a.x; o.y += a.y;
             }
-            if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+            if (p.relu) { o.x = fmax_nan(o.x, 0.f); o.y = fmax_nan(o.y, 0.f); }   // relu(NaN) = NaN
             *reinterpret_cast<float2*>(p.y + at) = o;
             if (MASK) mw[h] |= ((uint32_t)(o.x > 0.f) << (2 * j)) | ((uint32_t)(o.y > 0.f) << (2 * j + 1));
         }
@@ -226,7 +232,7 @@ __device__ __forceinline__ void linear_body(const Params& p) {
             const float4 v = n < p.Nout ? __ldg(reinterpret_cast<const float4*>(p.w + (size_t)n * p.ldw) + c4)
                                         : make_float4(0.f, 0.f, 0.f, 0.f);
             const float4 b = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
-            const float4 s = make_float4(v.x - b.x, v.y - b.y, v.z - b.z, v.w - b.w);
+            const float4 s = tf32_small(v, b);
             const int off = kb * KBLK_BYTES + (n >> 3) * 1024 + (n & 7) * 128 + ((c ^ (n & 7)) << 4);
             *reinterpret_cast<float4*>(smem + SMEM_W_BIG + off) = b;
             *reinterpret_cast<float4*>(smem + SMEM_W_SMALL + off) = s;
@@ -263,7 +269,7 @@ __device__ __forceinline__ void linear_body(const Params& p) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const float4 b = make_float4(tf32_big(v[i].x), tf32_big(v[i].y), tf32_big(v[i].z), tf32_big(v[i].w));
-                const float4 s = make_float4(v[i].x - b.x, v[i].y - b.y, v[i].z - b.z, v[i].w - b.w);
+                const float4 s = tf32_small(v[i], b);
                 const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
                 *reinterpret_cast<float4*>(abig + off) = b;
                 *reinterpret_cast<float4*>(abig + KBLK_BYTES + off) = s;
@@ -311,7 +317,7 @@ __device__ __forceinline__ void bwd_dx_body(const Params& p) {
             v = make_float4(__ldg(col), __ldg(col + p.Nout), __ldg(col + 2 * p.Nout), __ldg(col + 3 * p.Nout));
         }
         const float4 b = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
-        const float4 s = make_float4(v.x - b.x, v.y - b.y, v.z - b.z, v.w - b.w);
+        const float4 s = tf32_small(v, b);
         const int off = kb * KBLK_BYTES + (n >> 3) * 1024 + (n & 7) * 128 + ((c ^ (n & 7)) << 4);
         *reinterpret_cast<float4*>(smem + SMEM_W_BIG + off) = b;
         *reinterpret_cast<float4*>(smem + SMEM_W_SMALL + off) = s;
@@ -394,7 +400,7 @@ __device__ __forceinline__ void bwd_dx_body(const Params& p) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const float4 b = make_float4(tf32_big(g[i].x), tf32_big(g[i].y), tf32_big(g[i].z), tf32_big(g[i].w));
-                const float4 s = make_float4(g[i].x - b.x, g[i].y - b.y, g[i].z - b.z, g[i].w - b.w);
+                const float4 s = tf32_small(g[i], b);
                 const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
                 *reinterpret_cast<float4*>(abig + off) = b;
                 *reinterpret_cast<float4*>(abig + KBLK_BYTES + off) = s;
@@ -491,7 +497,7 @@ __device__ __forceinline__ void dw_body(const ParamsW& p) {
             const int off = kmajor_off(n, k);
             const float b = tf32_big(e);
             *reinterpret_cast<float*>(big + off) = b;
-            *reinterpret_cast<float*>(big + KBLK_BYTES + off) = e - b;
+            *reinterpret_cast<float*>(big + KBLK_BYTES + off) = tf32_small(e, b);
         };
         auto put = [&](unsigned char* big, int n0, int k, float4 v) {
             put1(big, n0, k, v.x); put1(big, n0 + 1, k, v.y); put1(big, n0 + 2, k, v.z); put1(big, n0 + 3, k, v.w);
@@ -674,7 +680,7 @@ __global__ void w_image_kernel(const float* __restrict__ w, int ldw, int K, int 
     const int nq = n >> 7, nl = n & 127;
     const float4 v = __ldg(reinterpret_cast<const float4*>(w + (size_t)n * ldw) + c4);
     const float4 b = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
-    const float4 sm = make_float4(v.x - b.x, v.y - b.y, v.z - b.z, v.w - b.w);
+    const float4 sm = tf32_small(v, b);
     unsigned char* blk = reinterpret_cast<unsigned char*>(wimg) + (size_t)(nq * KB + kb) * (2 * KBLK_BYTES);
     const int off = (nl >> 3) * 1024 + (nl & 7) * 128 + ((c ^ (nl & 7)) << 4);
     *reinterpret_cast<float4*>(blk + off) = b;
@@ -748,7 +754,7 @@ __global__ void __launch_bounds__(THREADS, 1) linear_wide_tf32x3_kernel(const Pa
                 const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
                 const float4 b = make_float4(tf32_big(va[i].x), tf32_big(va[i].y), tf32_big(va[i].z), tf32_big(va[i].w));
                 *reinterpret_cast<float4*>(sa + off) = b;
-                *reinterpret_cast<float4*>(sa + KBLK_BYTES + off) = make_float4(va[i].x - b.x, va[i].y - b.y, va[i].z - b.z, va[i].w - b.w);
+                *reinterpret_cast<float4*>(sa + KBLK_BYTES + off) = tf32_small(va[i], b);
             }
             fence_proxy_async();
             bar_arrive(bar_full + 8 * stage);

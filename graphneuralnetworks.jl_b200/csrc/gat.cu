@@ -174,8 +174,9 @@ __global__ void __launch_bounds__(128, (K == 1 ? 8 : 1)) gat_fwd_kernel(const Ga
                         const float z = eli[i] + ev[u][i];
                         const float uu = z > 0.f ? z : p.slope * z;
                         const float Mn = fmaxf(M[i], uu);
-                        const float sc = expf(M[i] - Mn);     // exp(-inf) = 0 on the first edge
-                        const float pp = expf(uu - Mn);
+                        const float Ms = softmax_shift(Mn);
+                        const float sc = expf(M[i] - Ms);     // exp(-inf) = 0 on the first edge
+                        const float pp = expf(uu - Ms);
                         S[i] = fmaf(S[i], sc, pp);
                         acc[i] = gfma(acc[i], sc, v[u][i], pp);
                         M[i] = Mn;
@@ -271,8 +272,9 @@ __global__ void __launch_bounds__(256, 2) gat_fwd_lean_kernel(const GatParams p)
                     for (int i = 0; i < KV; ++i) {
                         const float uu = myu[(j0 + u) * H + hd[i]];
                         const float Mn = fmaxf(M[i], uu);
-                        const float sc = __expf(M[i] - Mn);          // exp(-inf) = 0 on the first edge of a row
-                        const float pp = __expf(uu - Mn);
+                        const float Ms = softmax_shift(Mn);
+                        const float sc = __expf(M[i] - Ms);          // exp(-inf) = 0 on the first edge of a row
+                        const float pp = __expf(uu - Ms);
                         S[i] = fmaf(S[i], sc, pp);
                         acc[i] = gfma(acc[i], sc, v[u][i], pp);
                         M[i] = Mn;
@@ -339,7 +341,10 @@ __global__ void __launch_bounds__(256) gat_fwd_fixup_kernel(const GatParams p, c
     const int r = long_rows[li];
     const int rs = p.rowptr[r], re = p.rowptr[r + 1];
     const int k0 = rs / p.chunk, k1 = (re - 1) / p.chunk;
-    V acc = gzero<V>(); float M = -CUDART_INF_F, S = 0.f;
+    // M starts at -FLT_MAX, not -Inf: a piece whose logits are all -Inf (M = -Inf, S = 0, acc = 0) then merges as
+    // exp(-Inf + FLT_MAX) = 0 instead of exp(-Inf + Inf) = NaN.  On finite pieces the result has the same bits, and the
+    // serial chain over the pieces of a long row gets no extra instruction.
+    V acc = gzero<V>(); float M = -__int_as_float(0x7f7fffff), S = 0.f;
     for (int kk = k0; kk <= k1; ++kk) {
         const float* base = p.ws + (size_t)(2 * (int64_t)kk + (kk == k0 ? 1 : 0)) * slot;
         const V a = *reinterpret_cast<const V*>(base + f);

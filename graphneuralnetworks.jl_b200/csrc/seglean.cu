@@ -134,7 +134,7 @@ __device__ __forceinline__ float lcomb1(float acc, float v, float s1, float s2, 
     float m = v;
     if (SMODE != 0) m = __fmul_rn(m, s1);
     if (HAS_W) m = __fmul_rn(m, s2);
-    if (AGG == AG_MAX) return fmaxf(acc, __fmul_rn(m, sign));     // the product with +-1 is exact
+    if (AGG == AG_MAX) return fmax_nan(acc, __fmul_rn(m, sign));  // the product with +-1 is exact
     return __fadd_rn(acc, m);
 }
 template <int SMODE, bool HAS_W, int AGG>

@@ -51,7 +51,7 @@ __device__ __forceinline__ float4 vsplat4(float v) { return make_float4(v, v, v,
 template <bool ISMAX> __device__ __forceinline__ float comb1(float acc, float v, float s1, float s2) {
     // (x * cs) * w, each product rounded, then the reduction: matches  w .* (x .* c')  then  +
     float m = __fmul_rn(__fmul_rn(v, s1), s2);
-    if (ISMAX) return fmaxf(acc, m);
+    if (ISMAX) return fmax_nan(acc, m);     // a NaN message makes the row NaN, as Julia's max does
     return __fadd_rn(acc, m);
 }
 template <bool ISMAX> __device__ __forceinline__ float4 comb(float4 a, float4 v, float s1, float s2) {

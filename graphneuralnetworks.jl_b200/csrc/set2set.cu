@@ -156,8 +156,9 @@ __global__ void __launch_bounds__(256) set2set_fwd_kernel(const S2SParams p) {
                     for (int i = 0; i < K; ++i) s = s2s_dot(qv[i], v[u][i], s);
                     s = warp_sum(s);
                     const float Mn = fmaxf(M, s);
-                    const float sc = expf(M - Mn);     // exp(-inf) = 0 on the first edge of a row
-                    const float pp = expf(s - Mn);
+                    const float Ms = softmax_shift(Mn);
+                    const float sc = expf(M - Ms);     // exp(-inf) = 0 on the first edge of a row
+                    const float pp = expf(s - Ms);
                     S = fmaf(S, sc, pp);
 #pragma unroll
                     for (int i = 0; i < K; ++i) acc[i] = s2s_lin(acc[i], sc, v[u][i], pp);

@@ -20,10 +20,10 @@ void FN(orc_scatter)(int aggr, const T* src, const int64_t* idx, int64_t E, int6
         const T* restrict s = src + k * D;
         if (aggr == ORC_SUM || aggr == ORC_MEAN)
             for (int64_t f = 0; f < D; ++f) d[f] = d[f] + s[f];
-        else if (aggr == ORC_MAX)
-            for (int64_t f = 0; f < D; ++f) d[f] = d[f] > s[f] ? d[f] : s[f];
+        else if (aggr == ORC_MAX)   /* Julia's max and min: NaN when either argument is NaN, whatever the order */
+            for (int64_t f = 0; f < D; ++f) d[f] = s[f] != s[f] ? s[f] : (d[f] > s[f] || d[f] != d[f] ? d[f] : s[f]);
         else
-            for (int64_t f = 0; f < D; ++f) d[f] = d[f] < s[f] ? d[f] : s[f];
+            for (int64_t f = 0; f < D; ++f) d[f] = s[f] != s[f] ? s[f] : (d[f] < s[f] || d[f] != d[f] ? d[f] : s[f]);
     }
     if (aggr == ORC_MEAN) {
         int64_t* cnt = (int64_t*)calloc((size_t)(n > 0 ? n : 1), sizeof(int64_t));
