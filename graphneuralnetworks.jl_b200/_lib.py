@@ -155,6 +155,7 @@ _SIGS = {
     "gnnb_shard_builder_destroy": (_int, [_vp]),
     "gnnb_set_chunk_edges": (_int, [_int]),
     "gnnb_set_kernel_variant": (_int, [_int]),
+    "gnnb_gcn_hot_rows": (_int, [_vp, _int, _vp, _i64, C.POINTER(_i64), C.POINTER(C.c_int32), _vp]),
 }
 
 for _name, (_res, _args) in _SIGS.items():

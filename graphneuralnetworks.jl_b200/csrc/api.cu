@@ -16,6 +16,7 @@ void set_error(const char* fmt, ...) {
 }
 
 extern bool g_reference_kernels;   // segreduce.cu
+extern bool g_l2_policy_forced;    // seglean.cu
 int edge_dot(gnnb_graph* g, const float* dout, const float* x, const float* cs, const float* ct, int64_t D,
              float* dw_coo, cudaStream_t st);
 int maxmin_bwd(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
@@ -89,8 +90,10 @@ int gnnb_device_count(void) {
 }
 int64_t gnnb_launch_count(void) { return g_launches.load(); }
 int gnnb_set_kernel_variant(int v) {
-    if (v != 0 && v != 12) GNNB_FAIL(GNNB_EINVAL, "kernel variant must be 0 (default) or 12 (reference kernels), got %d", v);
+    if (v != 0 && v != 12 && v != 14)
+        GNNB_FAIL(GNNB_EINVAL, "kernel variant must be 0 (default), 12 (reference kernels) or 14 (L2 policy at every size), got %d", v);
     gnnb::g_reference_kernels = v == 12;
+    gnnb::g_l2_policy_forced = v == 14;
     return GNNB_OK;
 }
 
@@ -175,6 +178,14 @@ int gnnb_gcn_propagate(gnnb_graph_t g, int transposed, const float* x, const flo
         return seg_reduce(g, cc, a, st);
     }
     return gnnb_propagate(g, transposed, w ? GNNB_W_MUL_XJ : GNNB_COPY_XJ, GNNB_SUM, x, w, c, c, D, out, stream);
+}
+
+int gnnb_gcn_hot_rows(gnnb_graph_t g, int transposed, int32_t* rows_host, int64_t capacity, int64_t* num_rows,
+                      int32_t* threshold, void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (g->n_src != g->n_dst) GNNB_FAIL(GNNB_ESIZE, "gcn_hot_rows needs num_src == num_dst");
+    if (capacity < 0) GNNB_FAIL(GNNB_ESIZE, "capacity must be >= 0");
+    return gcn_hot_rows(g, transposed != 0, rows_host, capacity, num_rows, threshold, (cudaStream_t)stream);
 }
 
 int gnnb_gcn_propagate_bipartite(gnnb_graph_t g, int transposed, const float* x, int64_t D, float* out, void* stream) {

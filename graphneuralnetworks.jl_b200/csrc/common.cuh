@@ -73,6 +73,9 @@ struct Csr {
     int32_t n_items = 0;
     int32_t n_empty = -1;     // rows without edges (-1 = not counted yet)
     float* es = nullptr;      // lazily: es[e] = node_scale[col[e]] in plan order (the plan-owned GCN normalisation)
+    int32_t hot_min = 0;      // with es: edges whose gathered node is gathered >= hot_min times carry es's sign bit
+    int32_t* hot_rows = nullptr;  // with es: those gathered nodes (unordered), whose rows the propagate demotes after use
+    int32_t n_hot = 0;
     bool built = false;
 };
 
@@ -123,6 +126,8 @@ int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st);
 int ensure_invdeg(gnnb_graph* g, Csr& c, cudaStream_t st);
 int ensure_items(gnnb_graph* g, const Csr& c, cudaStream_t st);            // seglean.cu
 int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st);     // seglean.cu: g->gcn_c and the Csr's es stream
+int gcn_hot_rows(gnnb_graph* g, bool transposed, int32_t* rows_host, int64_t capacity, int64_t* num_rows,
+                 int32_t* threshold, cudaStream_t st);                      // seglean.cu: the hot set of es, read back
 int ensure_bipartite_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st);   // seglean.cu: g->bip_* for one direction
 int rsqrt_exact(float* d, int64_t n, cudaStream_t st);                     // edgeops.cu: d = 1/sqrt(d) in place
 // transform.cu: flags[k] = 1 where sorted key k starts a run of equal keys (k == 0 or keys[k] != keys[k-1])

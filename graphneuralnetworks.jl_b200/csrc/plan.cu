@@ -172,6 +172,7 @@ __global__ void bernoulli_keep_kernel(int64_t n, double p, uint64_t key, uint8_t
 static void free_csr(Csr& c) {
     cudaFree(c.rowptr); cudaFree(c.col); cudaFree(c.row); cudaFree(c.eid);
     cudaFree(c.long_rows); cudaFree(c.invdeg); cudaFree(c.items); cudaFree(c.es);
+    cudaFree(c.hot_rows);
     c = Csr();
 }
 

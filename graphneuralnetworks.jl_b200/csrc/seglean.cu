@@ -40,6 +40,7 @@ struct LeanParams {
     int32_t split;
     int32_t mean;
     float sign;
+    int32_t l2hint;   // SMODE 1: L2 eviction priorities of the row loads (L2_* bits), 0 = plain loads
 };
 
 namespace {
@@ -122,11 +123,67 @@ __global__ void gather_scale_kernel(const int32_t* __restrict__ col, int64_t E, 
     if (e < E) es[e] = __ldg(c + __ldg(col + e));
 }
 
+// ---- plan side: the hot rows of the plan-owned GCN stream -------------------------------------------------------------
+__global__ void count_gathers_kernel(const int32_t* __restrict__ col, int64_t E, int32_t* __restrict__ cnt) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < E) atomicAdd(cnt + __ldg(col + e), 1);
+}
+// es[e] = 1/sqrt(d) is >= 0 or +Inf, never NaN, so its sign bit is free: set, it marks an edge whose gathered node is hot
+__global__ void flag_hot_kernel(const int32_t* __restrict__ col, int64_t E, const int32_t* __restrict__ cnt, int32_t t,
+                                float* __restrict__ es) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < E && __ldg(cnt + __ldg(col + e)) >= t) es[e] = __uint_as_float(__float_as_uint(es[e]) | 0x80000000u);
+}
+// the hot nodes as a list (order irrelevant: it only says which rows to demote)
+__global__ void list_hot_kernel(const int32_t* __restrict__ cnt, int32_t n, int32_t t, int32_t* __restrict__ rows,
+                                int32_t* __restrict__ n_rows) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n && cnt[j] >= t) rows[atomicAdd(n_rows, 1)] = (int32_t)j;
+}
+// after a hinted pass: every 128 B line of a hot row of x back to evict_normal, so that the evict_last priority of the
+// pass does not outlive it (a line no longer in L2 is left alone)
+__global__ void demote_rows_kernel(const int32_t* __restrict__ rows, int32_t n_rows, const float* __restrict__ x) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;      // 4 lines per 512 B row
+    if (i >= (int64_t)n_rows * 4) return;
+    const float* line = x + (int64_t)__ldg(rows + (i >> 2)) * 128 + (i & 3) * 32;
+    asm volatile("applypriority.global.L2::evict_normal [%0], 128;" :: "l"(line) : "memory");
+}
+
 // ---- the kernel ------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float4 f4(float v) { return make_float4(v, v, v, v); }
 
 // aggregation of a kernel instance
 constexpr int AG_SUM = 0, AG_MEAN = 1, AG_MAX = 2;   // AG_MAX serves MIN too: min(m) = -max(-m)
+
+// L2 eviction priorities of the SMODE-1 instances (LeanParams::l2hint): hot rows evict_last, cold rows evict_first,
+// output rows evict_first
+constexpr int L2_HOT_LAST = 1, L2_COLD_FIRST = 2, L2_OUT_FIRST = 4;
+
+__device__ __forceinline__ uint64_t policy_evict_last() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ uint64_t policy_evict_first() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ uint64_t policy_evict_normal() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ float4 ldg_policy(const float* ptr, uint64_t pol) {
+    float4 v;
+    asm("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+        : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(ptr), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ void st_policy(float* ptr, float4 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
+                 :: "l"(ptr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
 
 // message of one edge folded into the accumulator: ((x * s1) * s2) with each product rounded, then + / max
 template <int SMODE, bool HAS_W, int AGG>
@@ -145,10 +202,14 @@ __device__ __forceinline__ float4 lcomb(float4 a, float4 v, float s1, float s2, 
 
 // KV float4 per lane: one warp covers a row of KV*128 floats.  SMODE 0: no gathered-node scale, 1: per-edge stream es,
 // 2: gather cs[col].  HALO 0: one source base; 1: nodes >= split live in x2 (the halo rows of a shard).
-// (Staging the most gathered rows in a persisting-L2 window, with or without cache-streaming loads for the rest, was
-// measured slower.  So was staging every row in shared memory by TMA, one 2-D tensor-map tile load per row: on an H100 at
-// 700 W the forward GCN propagate took 19.3 / 35.8 / 28.3 ms against 16.5 / 35.4 / 27.9 ms here at D = 128 / 256 / 512;
-// DESIGN.md §4.)  Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
+// L2 policy (SMODE 1 at D = 128, the plan-owned GCN stream whose sign bits flag the hot rows): hot rows are loaded
+// evict_last, cold rows evict_first, output rows stored evict_first.  On an H100 at 700 W this took the config-2 pass from
+// 16.6 to 15.0 ms; evict_last alone gave 16.1 ms, so the hot set pays only beside evict_first on everything else.  The
+// evict_last priority would outlive the kernel; seg_reduce_lean demotes the hot rows after each hinted pass.  (A hot
+// set staged in a persisting-L2 window, which takes its set-aside from the normal L2, was measured slower on a B200.  So
+// was staging every row in shared memory by TMA, one 2-D tensor-map tile load per row: on an H100 at 700 W the forward
+// GCN propagate took 19.3 / 35.8 / 28.3 ms against 16.5 / 35.4 / 27.9 ms here at D = 128 / 256 / 512; DESIGN.md §4.)
+// Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
 // compiler keeps the loop free of divergence handling; shuffles are never executed under a lane-dependent condition.
 template <int KV, int SMODE, bool HAS_W, int HALO, int AGG>
 __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
@@ -182,6 +243,13 @@ __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
     float4 acc[KV];
 #pragma unroll
     for (int i = 0; i < KV; ++i) acc[i] = f4(neutral);
+    // the hot set is classified for rows of 128 floats, and a halo base never comes with the plan-owned stream
+    constexpr bool HINTS = SMODE == 1 && KV == 1 && HALO == 0;
+    uint64_t pol_hot = 0, pol_cold = 0;
+    if (HINTS && p.l2hint) {
+        pol_hot = (p.l2hint & L2_HOT_LAST) ? policy_evict_last() : policy_evict_normal();
+        pol_cold = (p.l2hint & L2_COLD_FIRST) ? policy_evict_first() : policy_evict_normal();
+    }
 
     int e = it.x;
     int c_n, r_n;
@@ -194,6 +262,7 @@ __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
         const float s1_l = s1_n, s2_l = s2_n;
         const unsigned vmask = __ballot_sync(FULL, e + lane < e_end);            // edges of this batch
         const unsigned bmask = partial ? 0u : __ballot_sync(FULL, last_n);       // row ends among them
+        const unsigned hmask = HINTS ? __ballot_sync(FULL, __float_as_int(s1_l) < 0) : 0u;   // hot gathered rows
         float sc_l = 1.f, dg_l = 1.f;                 // scale (and edge count) of the row each lane's edge belongs to:
         if (!partial && e + lane < e_end) {           // needed at the first row end, long after these loads went out
             if (p.ct) sc_l = __ldg(p.ct + r_l);
@@ -211,13 +280,21 @@ __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
                 const bool second = HALO != 0 && cj >= p.split;
                 const float* xr = (second ? x2l : xl) + (int64_t)cj * STRIDE;
                 if ((vmask >> (j0 + u)) & 1u) {
+                    if (HINTS && p.l2hint) {
+                        const uint64_t pol = ((hmask >> (j0 + u)) & 1u) ? pol_hot : pol_cold;
 #pragma unroll
-                    for (int i = 0; i < KV; ++i) v[u][i] = __ldg(reinterpret_cast<const float4*>(xr + i * 128));
+                        for (int i = 0; i < KV; ++i) v[u][i] = ldg_policy(xr + i * 128, pol);
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < KV; ++i) v[u][i] = __ldg(reinterpret_cast<const float4*>(xr + i * 128));
+                    }
                 }
             }
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-                const float s1 = (SMODE != 0) ? __shfl_sync(FULL, s1_l, j0 + u) : 1.f;
+                // SMODE 1: the sign bit of es marks a hot row; the scale is the value without it (an exact AND)
+                const float s1 = SMODE == 1 ? __int_as_float(__shfl_sync(FULL, __float_as_int(s1_l), j0 + u) & 0x7fffffff)
+                                            : (SMODE != 0) ? __shfl_sync(FULL, s1_l, j0 + u) : 1.f;
                 const float s2 = HAS_W ? __shfl_sync(FULL, s2_l, j0 + u) : 1.f;
                 if ((vmask >> (j0 + u)) & 1u) {
 #pragma unroll
@@ -237,7 +314,8 @@ __global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
 #pragma unroll
                     for (int i = 0; i < KV; ++i) {
                         const float4 res = make_float4(acc[i].x * sc, acc[i].y * sc, acc[i].z * sc, acc[i].w * sc);
-                        *reinterpret_cast<float4*>(o + i * 128) = res;
+                        if (HINTS && (p.l2hint & L2_OUT_FIRST)) st_policy(o + i * 128, res, policy_evict_first());
+                        else *reinterpret_cast<float4*>(o + i * 128) = res;
                         acc[i] = f4(neutral);
                     }
                 }
@@ -424,7 +502,74 @@ int ensure_items(gnnb_graph* g, const Csr& c, cudaStream_t st) {
     return status;
 }
 
-// g->gcn_c = 1/sqrt(in-degree) (IEEE-exact, as gnnb_gcn_norm) and, for one direction, es[e] = gcn_c[col[e]]
+bool g_l2_policy_forced = false;   // gnnb_set_kernel_variant(14): the L2 policy at every size
+
+// L2 policy of the fused GCN propagate (DESIGN.md §4 "L2 policy").  The hot set of a direction: the nodes gathered at
+// least t times, t the smallest count whose nodes fit kHotL2Fraction of the L2 as rows of 128 floats.  The policy runs
+// at D = 128 when the gathered rows are at least kL2PolicyMinRatio times the L2: when they nearly fit, plain loads
+// already hit.  Wider rows keep plain loads (their hot set would pin 2 or 4 times the bytes).  A hinted pass is followed
+// by demote_rows_kernel over the plan's hot nodes, so that no line keeps the evict_last priority once the pass is done.
+constexpr double kHotL2Fraction = 0.56;
+constexpr int64_t kL2PolicyMinRatio = 8;
+constexpr int kL2Hints = L2_HOT_LAST | L2_COLD_FIRST | L2_OUT_FIRST;
+
+static int l2_bytes(const gnnb_graph* g, int64_t* bytes) {
+    int v = 0;
+    GNNB_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, g->device));
+    *bytes = v;
+    return GNNB_OK;
+}
+
+// count the gathers of each of the n gathered nodes of c, choose t, flag the hot edges in es (plan order of c)
+static int flag_hot_rows(gnnb_graph* g, Csr& c, int32_t n, float* es, int32_t* t_out, int32_t** rows_out,
+                         int32_t* n_rows_out, cudaStream_t st) {
+    int64_t l2 = 0;
+    GNNB_TRY(l2_bytes(g, &l2));
+    int64_t budget = (int64_t)((double)l2 * kHotL2Fraction) / 512;           // rows of 128 floats
+    int32_t *cnt = nullptr, *sorted = nullptr, *rows = nullptr, *d_nrows = nullptr;
+    void* tmp = nullptr;
+    int status = GNNB_OK;
+    do {
+#define LP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s failed: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; break; } }
+        LP(cudaMalloc(&cnt, sizeof(int32_t) * (size_t)n));
+        LP(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)n, st));
+        count_gathers_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, cnt);
+        LP(cudaGetLastError());
+        int32_t t = 1;                          // every gathered node fits
+        if (n > budget) {                       // t = (budget+1)-th largest count + 1: at most `budget` nodes reach it
+            size_t tmp_bytes = 0;
+            LP(cudaMalloc(&sorted, sizeof(int32_t) * (size_t)n));
+            LP(cub::DeviceRadixSort::SortKeysDescending(nullptr, tmp_bytes, cnt, sorted, n, 0, 32, st));
+            LP(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+            LP(cub::DeviceRadixSort::SortKeysDescending(tmp, tmp_bytes, cnt, sorted, n, 0, 32, st));
+            int32_t kth = 0;
+            LP(cudaMemcpyAsync(&kth, sorted + budget, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+            LP(cudaStreamSynchronize(st));
+            t = kth + 1;
+        }
+        flag_hot_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, cnt, t, es);
+        LP(cudaGetLastError());
+        LP(cudaMalloc(&rows, sizeof(int32_t) * (size_t)(n < budget ? n : budget)));
+        LP(cudaMalloc(&d_nrows, sizeof(int32_t)));
+        LP(cudaMemsetAsync(d_nrows, 0, sizeof(int32_t), st));
+        list_hot_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(cnt, n, t, rows, d_nrows);
+        LP(cudaGetLastError());
+        int32_t n_rows = 0;
+        LP(cudaMemcpyAsync(&n_rows, d_nrows, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        LP(cudaStreamSynchronize(st));
+        g_launches.fetch_add(n > budget ? 4 : 3, std::memory_order_relaxed);
+        *t_out = t;
+        *rows_out = rows;
+        *n_rows_out = n_rows;
+        rows = nullptr;
+#undef LP
+    } while (0);
+    cudaFree(cnt); cudaFree(sorted); cudaFree(tmp); cudaFree(rows); cudaFree(d_nrows);
+    return status;
+}
+
+// g->gcn_c = 1/sqrt(in-degree) (IEEE-exact, as gnnb_gcn_norm) and, for one direction, es[e] = gcn_c[col[e]] with the
+// hot edges flagged in the sign bit
 int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) {
     Csr& c = transposed ? g->by_src : g->by_dst;
     if (g->gcn_c != nullptr && (c.es != nullptr || g->E == 0)) return GNNB_OK;
@@ -442,10 +587,26 @@ int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) {
         GNNB_CUDA(cudaMalloc(&es, sizeof(float) * (size_t)g->E));
         gather_scale_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, g->gcn_c, es);
         GNNB_LAUNCHED();
-        GNNB_CUDA(cudaStreamSynchronize(st));
+        int32_t t = 0, n_hot = 0;
+        int32_t* hot = nullptr;
+        const int rc = flag_hot_rows(g, c, transposed ? g->n_dst : g->n_src, es, &t, &hot, &n_hot, st);
+        if (rc != GNNB_OK) { cudaFree(es); return rc; }
         std::lock_guard<std::mutex> lock(g->mu);
-        if (c.es == nullptr) c.es = es; else cudaFree(es);
+        if (c.es == nullptr) { c.es = es; c.hot_min = t; c.hot_rows = hot; c.n_hot = n_hot; } else { cudaFree(es); cudaFree(hot); }
     }
+    return GNNB_OK;
+}
+
+// the hot set of one direction, for inspection: threshold, size and (up to `capacity`) the nodes, unordered, to host
+int gcn_hot_rows(gnnb_graph* g, bool transposed, int32_t* rows_host, int64_t capacity, int64_t* num_rows,
+                 int32_t* threshold, cudaStream_t st) {
+    GNNB_TRY(ensure_csr(g, transposed, st));
+    GNNB_TRY(ensure_gcn_scale(g, transposed, st));
+    const Csr& c = transposed ? g->by_src : g->by_dst;
+    if (num_rows) *num_rows = c.n_hot;
+    if (threshold) *threshold = c.hot_min;
+    const int64_t n = capacity < c.n_hot ? capacity : c.n_hot;
+    if (rows_host && n > 0) GNNB_CUDA(cudaMemcpy(rows_host, c.hot_rows, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost));
     return GNNB_OK;
 }
 
@@ -508,12 +669,22 @@ int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, cu
     p.x = a.x; p.x2 = a.x2; p.split = a.split; p.out = a.out; p.ws = ws;
     p.mean = (a.aggr == GNNB_MEAN);
     p.sign = (a.aggr == GNNB_MIN) ? -1.f : 1.f;
+    p.l2hint = 0;
+    if (smode == 1 && a.es == c.es && c.hot_min > 0 && a.D == 128 && !halo) {   // the plan-owned GCN stream, flagged
+        int64_t l2 = 0;
+        GNNB_TRY(l2_bytes(g, &l2));
+        if (g_l2_policy_forced || (int64_t)g->n_src * a.D * 4 >= kL2PolicyMinRatio * l2) p.l2hint = kL2Hints;
+    }
     if (p.n_items == 0) return GNNB_OK;
     const int use_halo = halo ? 1 : 0;
     int rc;
     if (a.D == 128) rc = launch_lean1<1>(p, smode, a.w != nullptr, use_halo, agg, st);
     else if (a.D == 256) rc = launch_lean1<2>(p, smode, a.w != nullptr, use_halo, agg, st);
     else rc = launch_lean1<4>(p, smode, a.w != nullptr, use_halo, agg, st);
+    if (rc == GNNB_OK && (p.l2hint & L2_HOT_LAST) && c.n_hot > 0) {        // the evict_last priority ends with the pass
+        demote_rows_kernel<<<(unsigned)ceil_div((int64_t)c.n_hot * 4, 256), 256, 0, st>>>(c.hot_rows, c.n_hot, a.x);
+        GNNB_LAUNCHED();
+    }
     return rc;
 }
 

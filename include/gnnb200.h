@@ -192,6 +192,12 @@ int gnnb_softmax_edge_neighbors_bwd(gnnb_graph_t g, const float* alpha, const fl
 int gnnb_gcn_norm(gnnb_graph_t g, const float* w, float* c_out, void* stream);
 int gnnb_gcn_propagate(gnnb_graph_t g, int transposed, const float* x, const float* w,
                        const float* c, int64_t D, float* out, void* stream);
+/* The hot set behind the plan-owned normalisation's L2 policy (built with that stream if it is not yet): the nodes
+ * gathered at least `threshold` times in one direction, `threshold` the smallest count whose nodes fit 0.56 of the
+ * device's L2 as rows of 128 floats.  Writes the threshold and the number of hot nodes, and up to `capacity` of the
+ * nodes (0-based, unordered) to the HOST array rows_host (may be NULL). */
+int gnnb_gcn_hot_rows(gnnb_graph_t g, int transposed, int32_t* rows_host, int64_t capacity, int64_t* num_rows,
+                      int32_t* threshold, void* stream);
 /* The two-sided normalisation of gcn_conv on a one-relation heterograph (GNNlib/src/layers/conv.jl:45-50,58-66):
  *     c_src = 1 ./ sqrt.(out-degree)   (num_src floats)      c_dst = 1 ./ sqrt.(in-degree)   (num_dst floats)
  *     out = (propagate(copy_xj, g, +, xj = x .* c_src')) .* c_dst'          (x: num_src rows, out: num_dst rows)
@@ -637,7 +643,9 @@ int gnnb_set_chunk_edges(int chunk);
 /* kernels of the fused segmented reduce and of the fused GAT passes (results are bit-identical):
  * 0 = default: the lean work-item kernels (csrc/seglean.cu, csrc/gat.cu) for rows of 128/256/512 floats, the round-1
  * chunk kernels for every other shape;  12 = the round-1 chunk kernels (seg_reduce_kernel, gat_fwd_kernel,
- * gat_bwd_kernel) for every shape: the reference the lean kernels are tested against.  Any other value: GNNB_EINVAL. */
+ * gat_bwd_kernel) for every shape: the reference the lean kernels are tested against;  14 = the default kernels with the
+ * fused GCN propagate's L2 eviction priorities at every size (by default only when the gathered rows are at least 8 times
+ * the L2), so that tests reach them on small graphs.  Any other value: GNNB_EINVAL. */
 int gnnb_set_kernel_variant(int v);
 
 #ifdef __cplusplus
