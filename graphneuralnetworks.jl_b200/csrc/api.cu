@@ -72,7 +72,7 @@ static int plan_weights(gnnb_graph* g, const Csr& c, int msg, const float* w, si
                         cudaStream_t st) {
     *out = nullptr;
     if (msg != GNNB_W_MUL_XJ || !w || g->E == 0) return GNNB_OK;
-    GNNB_TRY(ensure_ws2(g, sizeof(float) * ((size_t)g->E + ws2_off_floats)));
+    GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * ((size_t)g->E + ws2_off_floats)));
     float* p = g->ws2 + ws2_off_floats;
     GNNB_TRY(permute_edge_values(c, g->E, w, 1, p, st));
     *out = p;
@@ -133,7 +133,7 @@ int gnnb_propagate_bwd(gnnb_graph_t g, int msg, int aggr, const float* dout, con
     if (aggr == GNNB_MEAN) {
         GNNB_TRY(ensure_invdeg(g, g->by_dst, st));
         if (ct) {
-            GNNB_TRY(ensure_ws2(g, sizeof(float) * ((size_t)g->n_dst + (size_t)g->E)));
+            GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * ((size_t)g->n_dst + (size_t)g->E)));
             if (g->n_dst > 0) {
                 mul_vec_kernel<<<nblk(g->n_dst), 256, 0, st>>>(ct, g->by_dst.invdeg, g->n_dst, g->ws2);
                 GNNB_LAUNCHED();
@@ -226,38 +226,53 @@ int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local,
 }
 
 // ---- host-buffer entries ------------------------------------------------------------------------
+// The streams and events of one *_host call, destroyed on every return path.  A return before `finished` is set (an
+// error) first waits for the device, so that no copy into the caller's host buffers is still in flight.
+struct HostCall {
+    cudaStream_t st[3] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    bool finished = false;
+    HostCall() = default;
+    HostCall(const HostCall&) = delete;
+    HostCall& operator=(const HostCall&) = delete;
+    ~HostCall() {
+        if (!finished) cudaDeviceSynchronize();
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+        for (cudaStream_t q : st)
+            if (q) cudaStreamDestroy(q);
+    }
+};
+
 static int host_pass(gnnb_graph_t g, int transposed, int msg, int aggr, int gcn, const float* x_host,
                      const float* w_host, int64_t D, float* out_host) {
     if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
     if (!x_host || !out_host) GNNB_FAIL(GNNB_EINVAL, "host buffer is NULL");
     if (D <= 0) GNNB_FAIL(GNNB_ESIZE, "feature dimension must be positive");
     const int64_t n_in = transposed ? g->n_dst : g->n_src, n_out = transposed ? g->n_src : g->n_dst;
+    DeviceScratch sc;
+    HostCall hc;
+    GNNB_CUDA(cudaStreamCreateWithFlags(&hc.st[0], cudaStreamNonBlocking));
+    cudaStream_t st = hc.st[0];
     float *dx = nullptr, *dout = nullptr, *dw = nullptr, *dc = nullptr;
-    cudaStream_t st = nullptr;
-    int status = GNNB_OK;
-#define HP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; goto done; } }
-    HP(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    HP(cudaMalloc(&dx, sizeof(float) * (size_t)(n_in * D > 0 ? n_in * D : 1)));
-    HP(cudaMalloc(&dout, sizeof(float) * (size_t)(n_out * D > 0 ? n_out * D : 1)));
-    HP(cudaMemcpyAsync(dx, x_host, sizeof(float) * (size_t)(n_in * D), cudaMemcpyHostToDevice, st));
+    GNNB_TRY(sc.alloc(&dx, (size_t)(n_in * D > 0 ? n_in * D : 1)));
+    GNNB_TRY(sc.alloc(&dout, (size_t)(n_out * D > 0 ? n_out * D : 1)));
+    GNNB_CUDA(cudaMemcpyAsync(dx, x_host, sizeof(float) * (size_t)(n_in * D), cudaMemcpyHostToDevice, st));
     if (w_host && g->E > 0) {
-        HP(cudaMalloc(&dw, sizeof(float) * (size_t)g->E));
-        HP(cudaMemcpyAsync(dw, w_host, sizeof(float) * (size_t)g->E, cudaMemcpyHostToDevice, st));
+        GNNB_TRY(sc.alloc(&dw, (size_t)g->E));
+        GNNB_CUDA(cudaMemcpyAsync(dw, w_host, sizeof(float) * (size_t)g->E, cudaMemcpyHostToDevice, st));
     }
     if (gcn) {
-        HP(cudaMalloc(&dc, sizeof(float) * (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
-        if ((status = gnnb_gcn_norm(g, dw, dc, st))) goto done;
-        if ((status = gnnb_gcn_propagate(g, transposed, dx, dw, dc, D, dout, st))) goto done;
+        GNNB_TRY(sc.alloc(&dc, (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
+        GNNB_TRY(gnnb_gcn_norm(g, dw, dc, st));
+        GNNB_TRY(gnnb_gcn_propagate(g, transposed, dx, dw, dc, D, dout, st));
     } else {
-        if ((status = gnnb_propagate(g, transposed, msg, aggr, dx, dw, nullptr, nullptr, D, dout, st))) goto done;
+        GNNB_TRY(gnnb_propagate(g, transposed, msg, aggr, dx, dw, nullptr, nullptr, D, dout, st));
     }
-    HP(cudaMemcpyAsync(out_host, dout, sizeof(float) * (size_t)(n_out * D), cudaMemcpyDeviceToHost, st));
-    HP(cudaStreamSynchronize(st));
-#undef HP
-done:
-    cudaFree(dx); cudaFree(dout); cudaFree(dw); cudaFree(dc);
-    if (st) cudaStreamDestroy(st);
-    return status;
+    GNNB_CUDA(cudaMemcpyAsync(out_host, dout, sizeof(float) * (size_t)(n_out * D), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    hc.finished = true;
+    return GNNB_OK;
 }
 
 int gnnb_propagate_host(gnnb_graph_t g, int transposed, int msg, int aggr, const float* x_host,
@@ -287,11 +302,7 @@ int gnnb_gcn_conv_step_host(gnnb_graph_t g, const float* x_host, const float* W_
     // device staging, carved from one plan-owned allocation: x, p (propagated / pre-propagated), y, dy, dpre, dp, dx, W, b, dW, db
     const size_t nx = (size_t)N * Din, np_ = (size_t)N * Dp, ny = (size_t)N * Dout;
     const size_t words = nx + np_ + ny + (bwd ? (ny + ny + np_ + nx + (size_t)N * 4) : 0) + 2 * (size_t)(Dout * Din) + 2 * (size_t)Dout + 64;
-    if (g->host_ws_bytes < words * sizeof(float)) {
-        if (g->host_ws) { cudaDeviceSynchronize(); cudaFree(g->host_ws); g->host_ws = nullptr; g->host_ws_bytes = 0; }
-        GNNB_CUDA(cudaMalloc(&g->host_ws, words * sizeof(float)));
-        g->host_ws_bytes = words * sizeof(float);
-    }
+    GNNB_TRY(grow_buffer(&g->host_ws, &g->host_ws_bytes, words * sizeof(float)));
     float* q = (float*)g->host_ws;
     auto take = [&](size_t n) { float* r = q; q += (n + 3) & ~(size_t)3; return r; };
     float *x = take(nx), *p = take(np_), *y = take(ny);
@@ -300,66 +311,49 @@ int gnnb_gcn_conv_step_host(gnnb_graph_t g, const float* x_host, const float* W_
     // the relu mask of y (N x 4 words, 16 B aligned like every carve): the pullback reads it instead of y where it can
     uint32_t* mask = bwd ? reinterpret_cast<uint32_t*>(take((size_t)N * 4)) : nullptr;
     bool masked = false;
-    cudaStream_t s_main = nullptr, s_in = nullptr, s_out = nullptr;
-    cudaEvent_t ev_x = nullptr, ev_dy = nullptr, ev_y = nullptr, ev_dx = nullptr;
-    int status = GNNB_OK;
-#define HP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s: %s", #expr, cudaGetErrorString(_e)); status = GNNB_ECUDA; goto done; } }
-#define HT(expr) { status = (expr); if (status != GNNB_OK) goto done; }
-    HP(cudaStreamCreateWithFlags(&s_main, cudaStreamNonBlocking));
-    HP(cudaStreamCreateWithFlags(&s_in, cudaStreamNonBlocking));
-    HP(cudaStreamCreateWithFlags(&s_out, cudaStreamNonBlocking));
-    HP(cudaEventCreateWithFlags(&ev_x, cudaEventDisableTiming));
-    HP(cudaEventCreateWithFlags(&ev_dy, cudaEventDisableTiming));
-    HP(cudaEventCreateWithFlags(&ev_y, cudaEventDisableTiming));
-    HP(cudaEventCreateWithFlags(&ev_dx, cudaEventDisableTiming));
+    HostCall hc;
+    for (cudaStream_t& q : hc.st) GNNB_CUDA(cudaStreamCreateWithFlags(&q, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : hc.ev) GNNB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    cudaStream_t s_main = hc.st[0], s_in = hc.st[1], s_out = hc.st[2];
+    cudaEvent_t ev_x = hc.ev[0], ev_dy = hc.ev[1], ev_y = hc.ev[2], ev_dx = hc.ev[3];
     // uploads ride s_in, downloads s_out (PCIe is full duplex), kernels s_main
-    HP(cudaMemcpyAsync(W, W_host, sizeof(float) * (size_t)(Dout * Din), cudaMemcpyHostToDevice, s_in));
-    if (b_host) HP(cudaMemcpyAsync(b, b_host, sizeof(float) * (size_t)Dout, cudaMemcpyHostToDevice, s_in));
-    HP(cudaMemcpyAsync(x, x_host, sizeof(float) * nx, cudaMemcpyHostToDevice, s_in));
-    HP(cudaEventRecord(ev_x, s_in));
+    GNNB_CUDA(cudaMemcpyAsync(W, W_host, sizeof(float) * (size_t)(Dout * Din), cudaMemcpyHostToDevice, s_in));
+    if (b_host) GNNB_CUDA(cudaMemcpyAsync(b, b_host, sizeof(float) * (size_t)Dout, cudaMemcpyHostToDevice, s_in));
+    GNNB_CUDA(cudaMemcpyAsync(x, x_host, sizeof(float) * nx, cudaMemcpyHostToDevice, s_in));
+    GNNB_CUDA(cudaEventRecord(ev_x, s_in));
     if (bwd) {
-        HP(cudaMemcpyAsync(dy, dy_host, sizeof(float) * ny, cudaMemcpyHostToDevice, s_in));
-        HP(cudaEventRecord(ev_dy, s_in));
+        GNNB_CUDA(cudaMemcpyAsync(dy, dy_host, sizeof(float) * ny, cudaMemcpyHostToDevice, s_in));
+        GNNB_CUDA(cudaEventRecord(ev_dy, s_in));
     }
-    HP(cudaStreamWaitEvent(s_main, ev_x, 0));
-    HT(gnnb_gcn_propagate(g, 0, x, nullptr, nullptr, Dp, p, s_main));                     // p = Â x
+    GNNB_CUDA(cudaStreamWaitEvent(s_main, ev_x, 0));
+    GNNB_TRY(gnnb_gcn_propagate(g, 0, x, nullptr, nullptr, Dp, p, s_main));                     // p = Â x
     if (bwd && relu && Dout == 128) {                                                     // y = relu(W p + b) + mask
         const int rc = gnnb_linear_relu_mask(p, W, b_host ? b : nullptr, N, Din, Dout, y, mask, s_main);
-        if (rc != GNNB_OK && rc != GNNB_EUNSUPPORTED) HT(rc);
+        if (rc != GNNB_OK && rc != GNNB_EUNSUPPORTED) return rc;
         masked = rc == GNNB_OK;
     }
-    if (!masked) HT(gnnb_linear(p, W, b_host ? b : nullptr, relu, N, Din, Dout, y, s_main));  // y = act(W p + b)
-    HP(cudaEventRecord(ev_y, s_main));
-    HP(cudaStreamWaitEvent(s_out, ev_y, 0));
-    HP(cudaMemcpyAsync(y_host, y, sizeof(float) * ny, cudaMemcpyDeviceToHost, s_out));
+    if (!masked) GNNB_TRY(gnnb_linear(p, W, b_host ? b : nullptr, relu, N, Din, Dout, y, s_main));  // y = act(W p + b)
+    GNNB_CUDA(cudaEventRecord(ev_y, s_main));
+    GNNB_CUDA(cudaStreamWaitEvent(s_out, ev_y, 0));
+    GNNB_CUDA(cudaMemcpyAsync(y_host, y, sizeof(float) * ny, cudaMemcpyDeviceToHost, s_out));
     if (bwd) {
-        HP(cudaStreamWaitEvent(s_main, ev_dy, 0));
+        GNNB_CUDA(cudaStreamWaitEvent(s_main, ev_dy, 0));
         if (masked) {
-            HT(gnnb_linear_bwd_mask(dy, mask, p, W, N, Din, Dout, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
+            GNNB_TRY(gnnb_linear_bwd_mask(dy, mask, p, W, N, Din, Dout, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
         } else {
-            HT(gnnb_linear_bwd(dy, y, p, W, relu, N, Din, Dout, dpre, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
+            GNNB_TRY(gnnb_linear_bwd(dy, y, p, W, relu, N, Din, Dout, dpre, dp, dW, (b_host && db_host) ? db : nullptr, s_main));
         }
-        HT(gnnb_gcn_propagate(g, 1, dp, nullptr, nullptr, Dp, dx, s_main));               // dx = Â' dp
-        HP(cudaEventRecord(ev_dx, s_main));
-        HP(cudaStreamWaitEvent(s_out, ev_dx, 0));
-        HP(cudaMemcpyAsync(dx_host, dx, sizeof(float) * nx, cudaMemcpyDeviceToHost, s_out));
-        HP(cudaMemcpyAsync(dW_host, dW, sizeof(float) * (size_t)(Dout * Din), cudaMemcpyDeviceToHost, s_out));
-        if (b_host && db_host) HP(cudaMemcpyAsync(db_host, db, sizeof(float) * (size_t)Dout, cudaMemcpyDeviceToHost, s_out));
+        GNNB_TRY(gnnb_gcn_propagate(g, 1, dp, nullptr, nullptr, Dp, dx, s_main));               // dx = Â' dp
+        GNNB_CUDA(cudaEventRecord(ev_dx, s_main));
+        GNNB_CUDA(cudaStreamWaitEvent(s_out, ev_dx, 0));
+        GNNB_CUDA(cudaMemcpyAsync(dx_host, dx, sizeof(float) * nx, cudaMemcpyDeviceToHost, s_out));
+        GNNB_CUDA(cudaMemcpyAsync(dW_host, dW, sizeof(float) * (size_t)(Dout * Din), cudaMemcpyDeviceToHost, s_out));
+        if (b_host && db_host) GNNB_CUDA(cudaMemcpyAsync(db_host, db, sizeof(float) * (size_t)Dout, cudaMemcpyDeviceToHost, s_out));
     }
-    HP(cudaStreamSynchronize(s_out));
-    HP(cudaStreamSynchronize(s_main));
-#undef HP
-#undef HT
-done:
-    if (status != GNNB_OK) cudaDeviceSynchronize();
-    if (ev_x) cudaEventDestroy(ev_x);
-    if (ev_dy) cudaEventDestroy(ev_dy);
-    if (ev_y) cudaEventDestroy(ev_y);
-    if (ev_dx) cudaEventDestroy(ev_dx);
-    if (s_main) cudaStreamDestroy(s_main);
-    if (s_in) cudaStreamDestroy(s_in);
-    if (s_out) cudaStreamDestroy(s_out);
-    return status;
+    GNNB_CUDA(cudaStreamSynchronize(s_out));
+    GNNB_CUDA(cudaStreamSynchronize(s_main));
+    hc.finished = true;
+    return GNNB_OK;
 }
 
 int gnnb_rmat_edges_range(int64_t num_nodes, int64_t first_edge, int64_t count, uint64_t seed, int64_t* src_dev,

@@ -6,7 +6,11 @@
 #include <stdarg.h>
 #include <atomic>
 #include <mutex>
+#include <type_traits>
+#include <vector>
 #include "../../include/gnnb200.h"
+
+struct cublasLtContext;  // cublasLtHandle_t points to it
 
 namespace gnnb {
 
@@ -44,6 +48,82 @@ extern std::atomic<int64_t> g_launches;
     } while (0)
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// ---- device memory ----------------------------------------------------------------------------
+// Scoped device temporaries: every buffer alloc() hands out is freed when the scratch goes out of scope, on every return
+// path, unless release() has handed it to a longer-lived owner (a plan) first.  Constructed with a stream, it
+// synchronises that stream before freeing, so that launches an early error return left queued finish first.
+class DeviceScratch {
+  public:
+    DeviceScratch() = default;
+    explicit DeviceScratch(cudaStream_t sync_on_exit) : st_(sync_on_exit), sync_(true) {}
+    DeviceScratch(const DeviceScratch&) = delete;
+    DeviceScratch& operator=(const DeviceScratch&) = delete;
+    ~DeviceScratch() {
+        if (sync_) cudaStreamSynchronize(st_);
+        for (void* q : bufs_) cudaFree(q);
+    }
+    // *p = `count` elements of T (bytes for void); the status and error text of GNNB_CUDA when cudaMalloc fails
+    template <typename T>
+    int alloc(T** p, size_t count) {
+        using Elem = typename std::conditional<std::is_void<T>::value, char, T>::type;
+        void* q = nullptr;
+        *p = nullptr;
+        GNNB_CUDA(cudaMalloc(&q, sizeof(Elem) * count));
+        bufs_.push_back(q);
+        *p = static_cast<T*>(q);
+        return GNNB_OK;
+    }
+    template <typename T>
+    T* release(T* p) {
+        for (void*& q : bufs_)
+            if (q == p) q = nullptr;
+        return p;
+    }
+
+  private:
+    std::vector<void*> bufs_;
+    cudaStream_t st_ = nullptr;
+    bool sync_ = false;
+};
+
+// Grow-only device buffer *p of *cap bytes: reallocated only when `bytes` exceeds *cap, after a device-wide synchronise
+// so that no launch still reads the old one.  Once large enough it neither allocates nor synchronises, which keeps a
+// warmed-up call legal inside CUDA-graph capture.
+template <typename T>
+int grow_buffer(T** p, size_t* cap, size_t bytes) {
+    if (*cap >= bytes) return GNNB_OK;
+    if (*p) {
+        cudaDeviceSynchronize();
+        cudaFree(*p);
+        *p = nullptr;
+        *cap = 0;
+    }
+    GNNB_CUDA(cudaMalloc(p, bytes));
+    *cap = bytes;
+    return GNNB_OK;
+}
+
+// Library-owned state of one device (dense.cu, dense_tc.cu, gatlogit.cu), built on the first call that needs it on that
+// device.  Every call on the device shares it, so calls on one device must be stream-ordered with respect to each other.
+struct DeviceState {
+    int nsm = 0;                      // SMs: the persistent grid of the tensor-core kernels (their attributes are set)
+    int* tc_err = nullptr;            // dense_tc.cu's pipeline watchdog: a bounded mbarrier wait expired
+    cublasLtContext* lt = nullptr;    // cuBLASLt handle and its workspace (lazily, on the first library GEMM)
+    void* lt_ws = nullptr;
+    // grow-only scratch (grow_buffer): pointer and bytes
+    float* w_blk = nullptr; size_t w_blk_bytes = 0;             // gnnb_linear2_bwd: a 128x128 block of W^T / dW
+    float* wt = nullptr; size_t wt_bytes = 0;                   // gnnb_linear_bwd: W^T (<= 128x128) for the wgmma dx
+    float* wt_wide = nullptr; size_t wt_wide_bytes = 0;         // gnnb_linear_bwd: W^T for the wide wgmma dx
+    float* act_part = nullptr; size_t act_part_bytes = 0;       // act_bwd_kernel: per-block column sums
+    float* wimg = nullptr; size_t wimg_bytes = 0;               // the wide kernel's split, swizzled image of W
+    float* dw_part = nullptr; size_t dw_part_bytes = 0;         // dw_tf32x3: split-K partials
+    float* bwd_part = nullptr; size_t bwd_part_bytes = 0;       // linear_bwd_tf32x3: split-K partials of dW
+    float* bwd_colsum = nullptr; size_t bwd_colsum_bytes = 0;   // linear_bwd_tf32x3: column-sum partials of db
+    float* gat_part = nullptr; size_t gat_part_bytes = 0;       // gnnb_gat_logit_terms_bwd: per-block partials of da
+};
+// the current device's state, created (tensor-core kernels configured, watchdog flag allocated) on first use
+int device_state(DeviceState** out);
 
 // splitmix64's output function: the mixer of every counter-based random stream in the library (RMAT, neighbour
 // sampling, the edge-code permutation)
@@ -120,8 +200,6 @@ struct gnnb_graph {
 };
 
 namespace gnnb {
-int ensure_ws(gnnb_graph* g, size_t bytes);
-int ensure_ws2(gnnb_graph* g, size_t bytes);
 int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st);
 int ensure_invdeg(gnnb_graph* g, Csr& c, cudaStream_t st);
 int ensure_items(gnnb_graph* g, const Csr& c, cudaStream_t st);            // seglean.cu

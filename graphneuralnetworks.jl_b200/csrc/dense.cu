@@ -25,16 +25,14 @@ LT_FN(cublasLtMatmulPreferenceDestroy) LT_FN(cublasLtMatmulPreferenceSetAttribut
 LT_FN(cublasLtMatmul) LT_FN(cublasLtGetVersion)
 #undef LT_FN
 static void* handle_lib = nullptr;
-static cublasLtHandle_t handle = nullptr;
-static void* workspace = nullptr;
+static bool loaded = false;   // every symbol above resolved (process-wide: the library is loaded once)
 static const size_t workspace_bytes = (size_t)256 << 20;
 static int emulation = -1;   // -1 unknown, 0 unavailable, 1 in use
 static int want_emulation = 1;
 static std::mutex mu;
 
-static int load() {
-    std::lock_guard<std::mutex> lock(mu);
-    if (handle) return GNNB_OK;
+static int load_symbols() {
+    if (loaded) return GNNB_OK;
     const char* env = getenv("GNNB_CUBLASLT");
     const char* cands[] = {env, "/usr/local/cuda/lib64/libcublasLt.so.12", "/usr/local/cuda/lib64/libcublasLt.so",
                            "libcublasLt.so.12"};
@@ -53,17 +51,30 @@ static int load() {
     LT_LOAD(cublasLtMatmulPreferenceSetAttribute) LT_LOAD(cublasLtMatmulAlgoGetHeuristic) LT_LOAD(cublasLtMatmul)
     LT_LOAD(cublasLtGetVersion)
 #undef LT_LOAD
+    loaded = true;
+    return GNNB_OK;
+}
+
+// the library and the current device's handle and workspace (s->lt, s->lt_ws), loaded on first use
+static int load(DeviceState* s) {
+    std::lock_guard<std::mutex> lock(mu);
+    if (s->lt) return GNNB_OK;
+    GNNB_TRY(load_symbols());
     cublasLtHandle_t h = nullptr;
     if (cublasLtCreate(&h) != CUBLAS_STATUS_SUCCESS) GNNB_FAIL(GNNB_ECUDA, "cublasLtCreate failed");
-    GNNB_CUDA(cudaMalloc(&workspace, workspace_bytes));
-    handle = h;
+    GNNB_CUDA(cudaMalloc(&s->lt_ws, workspace_bytes));
+    s->lt = h;
     return GNNB_OK;
 }
 
 // C(m x n, ldc) = op(A)(m x k) * op(B)(k x n) [+ bias(m)] [relu], all column-major fp32
 static int matmul(cublasOperation_t ta, cublasOperation_t tb, int64_t m, int64_t n, int64_t k, const float* A, int64_t lda,
                   const float* B, int64_t ldb, float* C, int64_t ldc, const float* bias, int relu, cudaStream_t st) {
-    GNNB_TRY(load());
+    DeviceState* ds = nullptr;
+    GNNB_TRY(device_state(&ds));
+    GNNB_TRY(load(ds));
+    cublasLtHandle_t handle = ds->lt;
+    void* workspace = ds->lt_ws;
     if (m == 0 || n == 0) return GNNB_OK;
     if (k == 0 && ldc == m && !bias) { GNNB_CUDA(cudaMemsetAsync(C, 0, sizeof(float) * (size_t)(m * n), st)); return GNNB_OK; }
     const bool try_emu = want_emulation && emulation != 0;
@@ -266,8 +277,10 @@ int gnnb_linear2_bwd(const float* dy, const float* y, const float* x1, const flo
         GNNB_TRY(gnnb_linear_bwd(dy, y, nullptr, W, relu, N, Din1, Dout, dpre_ws, nullptr, nullptr, db, stream));
         if (relu) dpre = dpre_ws;
     }
-    static float* tmp = nullptr;                       // 128x128 transposed block / dW block
-    if (!tmp) GNNB_CUDA(cudaMalloc(&tmp, sizeof(float) * 128 * 128));
+    DeviceState* s = nullptr;
+    GNNB_TRY(device_state(&s));
+    GNNB_TRY(grow_buffer(&s->w_blk, &s->w_blk_bytes, sizeof(float) * 128 * 128));
+    float* tmp = s->w_blk;                             // 128x128 transposed block / dW block
     for (int blk = 0; blk < 2; ++blk) {
         const int64_t Din = blk ? Din2 : Din1;
         const float* Wb = W + (blk ? Din1 : 0);
@@ -296,10 +309,10 @@ static int act_bwd_launch(const float* dy, const float* y, int relu, int64_t N, 
     const int nblocks = (int)ceil_div(N, rows_per_block);
     float* partial = nullptr;
     if (db) {
-        static float* part_buf = nullptr; static size_t part_bytes = 0;
-        const size_t need = sizeof(float) * (size_t)nblocks * D;
-        if (part_bytes < need) { if (part_buf) { cudaDeviceSynchronize(); cudaFree(part_buf); } GNNB_CUDA(cudaMalloc(&part_buf, need)); part_bytes = need; }
-        partial = part_buf;
+        DeviceState* s = nullptr;
+        GNNB_TRY(device_state(&s));
+        GNNB_TRY(grow_buffer(&s->act_part, &s->act_part_bytes, sizeof(float) * (size_t)nblocks * D));
+        partial = s->act_part;
     }
     if (relu) act_bwd_kernel<1><<<nblocks, 256, 0, st>>>(dy, y, N, (int)D, dpre, partial, rows_per_block);
     else act_bwd_kernel<0><<<nblocks, 256, 0, st>>>(dy, y, N, (int)D, nullptr, partial, rows_per_block);
@@ -360,25 +373,23 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
     }
     // dX = dPre * W : rows of dPre (K = Dout) against W^T stored K-major => the same wgmma kernel on a transposed copy of W
     if (dx && g_tc_enabled && Dout % 32 == 0 && Dout <= 128 && Din % 16 == 0 && Din <= 128 && Din >= 16) {
-        static float* wt = nullptr;
-        if (!wt) GNNB_CUDA(cudaMalloc(&wt, sizeof(float) * 128 * 128));
-        transpose_small_kernel<<<(unsigned)ceil_div(Dout * Din, 256), 256, 0, st>>>(W, (int)Dout, (int)Din, wt);
+        DeviceState* s = nullptr;
+        GNNB_TRY(device_state(&s));
+        GNNB_TRY(grow_buffer(&s->wt, &s->wt_bytes, sizeof(float) * 128 * 128));
+        transpose_small_kernel<<<(unsigned)ceil_div(Dout * Din, 256), 256, 0, st>>>(W, (int)Dout, (int)Din, s->wt);
         GNNB_LAUNCHED();
-        const int rc = linear_tf32x3(dpre, wt, nullptr, 0, N, Dout, Din, dx, st);
+        const int rc = linear_tf32x3(dpre, s->wt, nullptr, 0, N, Dout, Din, dx, st);
         if (rc == GNNB_OK) dx = nullptr;
         else if (rc != GNNB_EUNSUPPORTED) return rc;
     } else if (dx && g_tc_enabled && (Dout > 128 || Din > 128) && Dout % 32 == 0 && Dout <= 2048 && Din % 128 == 0 && Din <= 1024 &&
                N >= 2048) {
         // wide shapes: the same product through the wide wgmma kernel on a transposed copy of W (<= 8 MB, kept)
-        static float* wtw = nullptr; static size_t wtw_elems = 0;
-        if (wtw_elems < (size_t)(Dout * Din)) {
-            if (wtw) { cudaDeviceSynchronize(); cudaFree(wtw); wtw = nullptr; wtw_elems = 0; }
-            GNNB_CUDA(cudaMalloc(&wtw, sizeof(float) * (size_t)(Dout * Din)));
-            wtw_elems = (size_t)(Dout * Din);
-        }
-        transpose_small_kernel<<<(unsigned)ceil_div(Dout * Din, 256), 256, 0, st>>>(W, (int)Dout, (int)Din, wtw);
+        DeviceState* s = nullptr;
+        GNNB_TRY(device_state(&s));
+        GNNB_TRY(grow_buffer(&s->wt_wide, &s->wt_wide_bytes, sizeof(float) * (size_t)(Dout * Din)));
+        transpose_small_kernel<<<(unsigned)ceil_div(Dout * Din, 256), 256, 0, st>>>(W, (int)Dout, (int)Din, s->wt_wide);
         GNNB_LAUNCHED();
-        const int rc = linear_tf32x3(dpre, wtw, nullptr, 0, N, Dout, Din, dx, st);
+        const int rc = linear_tf32x3(dpre, s->wt_wide, nullptr, 0, N, Dout, Din, dx, st);
         if (rc == GNNB_OK) dx = nullptr;
         else if (rc != GNNB_EUNSUPPORTED) return rc;
     }

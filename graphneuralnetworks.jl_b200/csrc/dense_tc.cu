@@ -17,6 +17,7 @@
 // The kernel is HBM-bound by design (2 x 4 x K bytes per row against 6 K^2 flops on the TF32 tensor cores).
 // Every mbarrier wait is bounded: a broken pipeline makes the kernel flag an error and drain instead of hanging.
 #include "common.cuh"
+#include <map>
 
 namespace gnnb {
 
@@ -784,8 +785,37 @@ __global__ void __launch_bounds__(THREADS, 1) linear_wide_tf32x3_kernel(const Pa
 }
 }  // namespace tcx
 
-static int* g_tc_err = nullptr;
 int g_tc_enabled = 1;
+
+static std::mutex g_states_mu;
+static std::map<int, DeviceState> g_states;   // by device ordinal; never erased, so a returned pointer stays valid
+
+int device_state(DeviceState** out) {
+    int dev = 0;
+    GNNB_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(g_states_mu);
+    auto it = g_states.find(dev);
+    if (it == g_states.end()) {
+        // the >48 KB dynamic shared memory of the tensor-core kernels is a per-device function attribute
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_relu_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tcx::linear_wide_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcx::SMEM_TOTAL_X));
+        GNNB_CUDA(cudaFuncSetAttribute(tcw::dw_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
+        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
+        GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
+        DeviceState s;
+        GNNB_CUDA(cudaDeviceGetAttribute(&s.nsm, cudaDevAttrMultiProcessorCount, dev));
+        DeviceScratch sc;
+        GNNB_TRY(sc.alloc(&s.tc_err, 1));
+        GNNB_CUDA(cudaMemset(s.tc_err, 0, sizeof(int)));
+        sc.release(s.tc_err);
+        it = g_states.emplace(dev, s).first;
+    }
+    *out = &it->second;
+    return GNNB_OK;
+}
 
 // returns GNNB_EUNSUPPORTED (no error text) when the shape is not covered by the tensor-core kernel
 int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* bias, const float* addend, int relu, int64_t M,
@@ -819,35 +849,19 @@ static int linear_launch(const float* x, const float* W, int64_t ldw, const floa
     }
     if (((uintptr_t)x & 15) || ((uintptr_t)W & 15) || ((uintptr_t)y & 15) || ((uintptr_t)addend & 15)) return GNNB_EUNSUPPORTED;
     if (M == 0) return GNNB_OK;
-    static bool configured = false;
-    static int nsm = 0;
-    if (!configured) {
-        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
-        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_relu_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
-        GNNB_CUDA(cudaFuncSetAttribute(tcx::linear_wide_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcx::SMEM_TOTAL_X));
-        int dev = 0;
-        GNNB_CUDA(cudaGetDevice(&dev));
-        GNNB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-        GNNB_CUDA(cudaMalloc(&g_tc_err, sizeof(int)));
-        GNNB_CUDA(cudaMemset(g_tc_err, 0, sizeof(int)));
-        configured = true;
-    }
+    DeviceState* s = nullptr;
+    GNNB_TRY(device_state(&s));
     tc::Params p;
     p.x = x; p.w = W; p.bias = bias; p.addend = addend; p.y = y; p.M = M; p.K = (int)K; p.Nout = (int)Nout; p.relu = relu;
-    p.ldw = (int)ldw; p.err = g_tc_err; p.wimg = nullptr; p.act = nullptr; p.colsum = nullptr; p.mask = mask;
+    p.ldw = (int)ldw; p.err = s->tc_err; p.wimg = nullptr; p.act = nullptr; p.colsum = nullptr; p.mask = mask;
     if (wide) {
         // the split, swizzled image of W (2 x its size), rebuilt per call: W changes between training steps
-        static float* wimg = nullptr; static size_t wimg_elems = 0;
-        const size_t need = (size_t)2 * K * Nout;
-        if (wimg_elems < need) {
-            if (wimg) { cudaDeviceSynchronize(); cudaFree(wimg); wimg = nullptr; wimg_elems = 0; }
-            GNNB_CUDA(cudaMalloc(&wimg, sizeof(float) * need));
-            wimg_elems = need;
-        }
-        tcx::w_image_kernel<<<(unsigned)ceil_div(Nout * (K / 4), 256), 256, 0, st>>>(W, (int)ldw, (int)K, (int)Nout, wimg);
+        GNNB_TRY(grow_buffer(&s->wimg, &s->wimg_bytes, sizeof(float) * (size_t)2 * K * Nout));
+        tcx::w_image_kernel<<<(unsigned)ceil_div(Nout * (K / 4), 256), 256, 0, st>>>(W, (int)ldw, (int)K, (int)Nout, s->wimg);
         GNNB_LAUNCHED();
-        p.wimg = wimg;
+        p.wimg = s->wimg;
     }
+    const int nsm = s->nsm;
     const int64_t ntiles = ceil_div(M, tc::BM);
     const unsigned grid = (unsigned)(ntiles < nsm ? ntiles : nsm);
     if (wide) tcx::linear_wide_tf32x3_kernel<<<grid, tc::THREADS, tcx::SMEM_TOTAL_X, st>>>(p);
@@ -862,21 +876,14 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
     if (!g_tc_enabled) return GNNB_EUNSUPPORTED;
     if (Dout != 128 || Din % 32 != 0 || Din > 128 || Din < 32) return GNNB_EUNSUPPORTED;
     if (((uintptr_t)dpre & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dW & 15)) return GNNB_EUNSUPPORTED;
-    static bool configured = false;
-    static int nsm = 0;
-    static float* partial = nullptr;
-    if (!configured) {
-        GNNB_CUDA(cudaFuncSetAttribute(tcw::dw_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
-        int dev = 0;
-        GNNB_CUDA(cudaGetDevice(&dev));
-        GNNB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-        GNNB_CUDA(cudaMalloc(&partial, sizeof(float) * (size_t)nsm * 128 * 128));
-        if (!g_tc_err) { GNNB_CUDA(cudaMalloc(&g_tc_err, sizeof(int))); GNNB_CUDA(cudaMemset(g_tc_err, 0, sizeof(int))); }
-        configured = true;
-    }
+    DeviceState* s = nullptr;
+    GNNB_TRY(device_state(&s));
+    const int nsm = s->nsm;
+    GNNB_TRY(grow_buffer(&s->dw_part, &s->dw_part_bytes, sizeof(float) * (size_t)nsm * 128 * 128));
+    float* partial = s->dw_part;
     if (M == 0) { GNNB_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)(Dout * Din), st)); return GNNB_OK; }
     tcw::ParamsW p;
-    p.dpre = dpre; p.x = x; p.partial = partial; p.M = M; p.Din = (int)Din; p.err = g_tc_err; p.act = nullptr; p.mask = nullptr;
+    p.dpre = dpre; p.x = x; p.partial = partial; p.M = M; p.Din = (int)Din; p.err = s->tc_err; p.act = nullptr; p.mask = nullptr;
     int64_t rpc = ceil_div(M, nsm);
     rpc = ceil_div(rpc, 32) * 32;
     p.rows_per_cta = rpc;
@@ -900,26 +907,16 @@ int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, con
     if (Din % 32 != 0 || Din > 128 || Din < 32 || M <= 0) return GNNB_EUNSUPPORTED;
     if (((uintptr_t)dy & 15) || ((uintptr_t)y & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dx & 15) || ((uintptr_t)mask & 15))
         return GNNB_EUNSUPPORTED;
-    static bool configured = false;
-    static int nsm = 0;
-    static float *partial = nullptr, *colsum = nullptr;
-    if (!configured) {
-        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
-        GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
-        GNNB_CUDA(cudaFuncSetAttribute(tc::linear_bwd_dx_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_TOTAL));
-        GNNB_CUDA(cudaFuncSetAttribute(tcw::linear_bwd_dw_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tcw::SMEM_TOTALW));
-        int dev = 0;
-        GNNB_CUDA(cudaGetDevice(&dev));
-        GNNB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-        GNNB_CUDA(cudaMalloc(&partial, sizeof(float) * (size_t)nsm * 128 * 128));
-        GNNB_CUDA(cudaMalloc(&colsum, sizeof(float) * (size_t)nsm * 4 * 128));
-        if (!g_tc_err) { GNNB_CUDA(cudaMalloc(&g_tc_err, sizeof(int))); GNNB_CUDA(cudaMemset(g_tc_err, 0, sizeof(int))); }
-        configured = true;
-    }
+    DeviceState* s = nullptr;
+    GNNB_TRY(device_state(&s));
+    const int nsm = s->nsm;
+    GNNB_TRY(grow_buffer(&s->bwd_part, &s->bwd_part_bytes, sizeof(float) * (size_t)nsm * 128 * 128));
+    GNNB_TRY(grow_buffer(&s->bwd_colsum, &s->bwd_colsum_bytes, sizeof(float) * (size_t)nsm * 4 * 128));
+    float *partial = s->bwd_part, *colsum = s->bwd_colsum;
     // dx and the column sums of dpre: one CTA per SM over 128-row tiles
     tc::Params p;
     p.x = dy; p.w = W; p.bias = nullptr; p.addend = nullptr; p.y = dx; p.M = M; p.K = 128; p.Nout = (int)Din; p.relu = 0;
-    p.ldw = 128; p.err = g_tc_err; p.wimg = nullptr; p.act = y; p.colsum = db ? colsum : nullptr;
+    p.ldw = 128; p.err = s->tc_err; p.wimg = nullptr; p.act = y; p.colsum = db ? colsum : nullptr;
     p.mask = const_cast<uint32_t*>(mask);
     const int64_t ntiles = ceil_div(M, tc::BM);
     const int grid_dx = (int)(ntiles < nsm ? ntiles : nsm);
@@ -928,7 +925,7 @@ int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, con
     GNNB_LAUNCHED();
     // dW: the split-K partition of dw_tf32x3
     tcw::ParamsW pw;
-    pw.dpre = dy; pw.x = x; pw.partial = partial; pw.M = M; pw.Din = (int)Din; pw.err = g_tc_err; pw.act = y; pw.mask = mask;
+    pw.dpre = dy; pw.x = x; pw.partial = partial; pw.M = M; pw.Din = (int)Din; pw.err = s->tc_err; pw.act = y; pw.mask = mask;
     const int64_t rpc = ceil_div(ceil_div(M, nsm), 32) * 32;
     pw.rows_per_cta = rpc;
     const int grid_dw = (int)ceil_div(M, rpc);
@@ -941,12 +938,16 @@ int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, con
     return GNNB_OK;
 }
 
-// pipeline watchdog: non-zero if a bounded mbarrier wait expired in any launch so far (then results are invalid)
+// pipeline watchdog: non-zero if a bounded mbarrier wait expired in any launch so far, on any device (then results are
+// invalid)
 int linear_tf32x3_error() {
-    if (!g_tc_err) return 0;
-    int e = 0;
-    cudaMemcpy(&e, g_tc_err, sizeof(int), cudaMemcpyDeviceToHost);
-    return e;
+    std::lock_guard<std::mutex> lock(g_states_mu);
+    for (const auto& kv : g_states) {
+        int e = 0;
+        cudaMemcpy(&e, kv.second.tc_err, sizeof(int), cudaMemcpyDeviceToHost);
+        if (e) return e;
+    }
+    return 0;
 }
 
 }  // namespace gnnb

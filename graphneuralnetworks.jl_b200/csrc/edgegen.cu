@@ -208,13 +208,6 @@ __global__ void perm_batch_kernel(Feistel f, uint64_t M, uint64_t base, int64_t 
 // largest batch of permuted indices held at once (2 GB of codes + 1 GB of flags and 1 GB of ranks)
 constexpr int64_t kMaxBatch = (int64_t)1 << 28;
 
-struct Scratch {
-    void* p[4] = {nullptr, nullptr, nullptr, nullptr};
-    ~Scratch() {
-        for (void* q : p) cudaFree(q);
-    }
-};
-
 static int check_edges(int64_t E, int index_base) {
     if (E < 0 || E >= ((int64_t)1 << 31)) GNNB_FAIL(GNNB_ESIZE, "number of edges %lld outside [0, 2^31)", (long long)E);
     if (index_base != 0 && index_base != 1) GNNB_FAIL(GNNB_EINVAL, "index_base must be 0 or 1 (got %d)", index_base);
@@ -241,9 +234,9 @@ int gnnb_edge_encode(int space, int64_t n1, int64_t n2, const int64_t* s, const 
     if (num_edges == 0) return GNNB_OK;
     if (!s || !t || !codes) GNNB_FAIL(GNNB_EINVAL, "gnnb_edge_encode: NULL array");
     cudaStream_t st = (cudaStream_t)stream;
-    Scratch sc;
-    GNNB_CUDA(cudaMalloc(&sc.p[0], sizeof(int)));
-    int* bad_dev = (int*)sc.p[0];
+    DeviceScratch sc;
+    int* bad_dev = nullptr;
+    GNNB_TRY(sc.alloc(&bad_dev, 1));
     GNNB_CUDA(cudaMemsetAsync(bad_dev, 0, sizeof(int), st));
     encode_kernel<<<(unsigned)ceil_div(num_edges, 256), 256, 0, st>>>(sp, s, t, num_edges, index_base, 0, codes, bad_dev);
     GNNB_LAUNCHED();
@@ -262,9 +255,9 @@ int gnnb_edge_decode(int space, int64_t n1, int64_t n2, const uint64_t* codes, i
     if (num_edges == 0) return GNNB_OK;
     if (!s || !t || !codes) GNNB_FAIL(GNNB_EINVAL, "gnnb_edge_decode: NULL array");
     cudaStream_t st = (cudaStream_t)stream;
-    Scratch sc;
-    GNNB_CUDA(cudaMalloc(&sc.p[0], sizeof(int)));
-    int* bad_dev = (int*)sc.p[0];
+    DeviceScratch sc;
+    int* bad_dev = nullptr;
+    GNNB_TRY(sc.alloc(&bad_dev, 1));
     GNNB_CUDA(cudaMemsetAsync(bad_dev, 0, sizeof(int), st));
     decode_kernel<<<(unsigned)ceil_div(num_edges, 256), 256, 0, st>>>(sp, codes, num_edges, index_base, s, t, bad_dev);
     GNNB_LAUNCHED();
@@ -288,11 +281,13 @@ int gnnb_edge_codes_sorted(int space, int64_t n1, int64_t n2, const int64_t* s, 
     const unsigned blocks = (unsigned)ceil_div(E, 256);
     int end_bit = 1;                     // codes and the sentinel M fit in end_bit bits
     while (end_bit < 64 && (sp.M >> end_bit) != 0) ++end_bit;
-    Scratch sc;
+    DeviceScratch sc;
     // one allocation for the codes, the sorted codes, the run heads and their ranks
     const size_t nb = (size_t)E;
-    GNNB_CUDA(cudaMalloc(&sc.p[0], nb * (8 + 8 + 4 + 4) + 16));
-    uint64_t* codes = (uint64_t*)sc.p[0];
+    void* buf = nullptr;
+    GNNB_TRY(sc.alloc(&buf, nb * (8 + 8 + 4 + 4) + 16));
+    uint64_t* codes = (uint64_t*)buf;
+
     uint64_t* sorted = codes + nb;
     int32_t* heads = (int32_t*)(sorted + nb);
     int32_t* pos = heads + nb;
@@ -303,11 +298,12 @@ int gnnb_edge_codes_sorted(int space, int64_t n1, int64_t n2, const int64_t* s, 
     size_t sort_bytes = 0, scan_bytes = 0;
     GNNB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, codes, sorted, (int)E, 0, end_bit, st));
     GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, heads, pos, (int)E, st));
-    GNNB_CUDA(cudaMalloc(&sc.p[1], std::max(sort_bytes, scan_bytes) + 1));
-    GNNB_CUDA(cub::DeviceRadixSort::SortKeys(sc.p[1], sort_bytes, codes, sorted, (int)E, 0, end_bit, st));
+    void* tmp = nullptr;
+    GNNB_TRY(sc.alloc(&tmp, std::max(sort_bytes, scan_bytes) + 1));
+    GNNB_CUDA(cub::DeviceRadixSort::SortKeys(tmp, sort_bytes, codes, sorted, (int)E, 0, end_bit, st));
     g_launches.fetch_add(2, std::memory_order_relaxed);
     GNNB_TRY(run_head_flags(sorted, E, heads, st));
-    GNNB_CUDA(cub::DeviceScan::InclusiveSum(sc.p[1], scan_bytes, heads, pos, (int)E, st));
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, scan_bytes, heads, pos, (int)E, st));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     compact_kernel<<<blocks, 256, 0, st>>>(sorted, heads, pos, E, sp.M, E, codes_out);  // the sentinel run is skipped
     GNNB_LAUNCHED();
@@ -344,9 +340,9 @@ int gnnb_sample_codes(uint64_t M, const uint64_t* excl, int64_t x, int64_t m, ui
     if (m < 0) GNNB_FAIL(GNNB_EINVAL, "m = %lld is negative", (long long)m);
     if (x > 0 && !excl) GNNB_FAIL(GNNB_EINVAL, "gnnb_sample_codes: excl is NULL");
     cudaStream_t st = (cudaStream_t)stream;
-    Scratch sc;
-    GNNB_CUDA(cudaMalloc(&sc.p[0], sizeof(int)));
-    int* bad_dev = (int*)sc.p[0];
+    DeviceScratch sc;
+    int* bad_dev = nullptr;
+    GNNB_TRY(sc.alloc(&bad_dev, 1));
     if (x > 0) {                         // the batch sizes below count on excl being a set of codes < M
         GNNB_CUDA(cudaMemsetAsync(bad_dev, 0, sizeof(int), st));
         check_set_kernel<<<(unsigned)ceil_div(x, 256), 256, 0, st>>>(excl, x, M, bad_dev);
@@ -364,6 +360,7 @@ int gnnb_sample_codes(uint64_t M, const uint64_t* excl, int64_t x, int64_t m, ui
     uint64_t base = 0, left = avail;     // left: available codes among the indices not yet permuted
     uint64_t* codes = nullptr;
     int32_t *flags = nullptr, *pos = nullptr;
+    void* tmp = nullptr;
     size_t scan_bytes = 0;
     while (written < want) {             // left > 0 here, so base < M: every pass permutes >= 1 new index
         const double need = (double)(want - written);
@@ -374,18 +371,19 @@ int gnnb_sample_codes(uint64_t M, const uint64_t* excl, int64_t x, int64_t m, ui
         if ((uint64_t)B > M - base) B = (int64_t)(M - base);
         if (cap == 0) {                  // buffers sized by the first batch; later batches reuse them
             cap = B;
-            GNNB_CUDA(cudaMalloc(&sc.p[1], (size_t)cap * (8 + 4 + 4)));
-            codes = (uint64_t*)sc.p[1];
+            void* buf = nullptr;
+            GNNB_TRY(sc.alloc(&buf, (size_t)cap * (8 + 4 + 4)));
+            codes = (uint64_t*)buf;
             flags = (int32_t*)(codes + cap);
             pos = flags + cap;
             GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, flags, pos, (int)cap, st));
-            GNNB_CUDA(cudaMalloc(&sc.p[2], scan_bytes + 1));
+            GNNB_TRY(sc.alloc(&tmp, scan_bytes + 1));
         }
         if (B > cap) B = cap;
         const unsigned blocks = (unsigned)ceil_div(B, 256);
         perm_batch_kernel<<<blocks, 256, 0, st>>>(f, M, base, B, excl, x, codes, flags);
         GNNB_LAUNCHED();
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(sc.p[2], scan_bytes, flags, pos, (int)B, st));
+        GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, scan_bytes, flags, pos, (int)B, st));
         g_launches.fetch_add(1, std::memory_order_relaxed);
         compact_kernel<<<blocks, 256, 0, st>>>(codes, flags, pos, B, M, want - written, out + written);
         GNNB_LAUNCHED();

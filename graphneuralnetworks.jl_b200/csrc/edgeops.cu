@@ -189,7 +189,7 @@ int gnnb_degree(gnnb_graph_t g, int dir, const float* w, float* out, void* strea
         return GNNB_OK;
     }
     if (dir == GNNB_DIR_BOTH) {
-        GNNB_TRY(ensure_ws2(g, sizeof(float) * (size_t)g->n_dst));
+        GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * (size_t)g->n_dst));
         GNNB_TRY(gnnb_scatter(g, GNNB_SRC, GNNB_SUM, w, 1, out, stream));
         GNNB_TRY(gnnb_scatter(g, GNNB_DST, GNNB_SUM, w, 1, g->ws2, stream));
         if (g->n_dst > 0) { add_kernel<<<nblk(g->n_dst), 256, 0, st>>>(out, g->ws2, g->n_dst); GNNB_LAUNCHED(); }
@@ -212,7 +212,7 @@ int gnnb_softmax_edge_neighbors(gnnb_graph_t g, const float* e, int64_t K, float
     cudaStream_t st = (cudaStream_t)stream;
     if (g->E == 0) return GNNB_OK;
     const int64_t n = g->E * K;
-    GNNB_TRY(ensure_ws2(g, sizeof(float) * (size_t)g->n_dst * K));
+    GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * (size_t)g->n_dst * K));
     float* stat = g->ws2;
     GNNB_TRY(gnnb_scatter(g, GNNB_DST, GNNB_MAX, e, K, stat, stream));            // max_ = scatter(max, e, t)
     sm_exp_kernel<<<nblk(n), 256, 0, st>>>(g->coo_dst, g->E, K, e, stat, out);     // num = exp.(e .- gather(max_, t))
@@ -230,7 +230,7 @@ int gnnb_softmax_edge_neighbors_bwd(gnnb_graph_t g, const float* alpha, const fl
     cudaStream_t st = (cudaStream_t)stream;
     if (g->E == 0) return GNNB_OK;
     const int64_t n = g->E * K;
-    GNNB_TRY(ensure_ws2(g, sizeof(float) * (size_t)g->n_dst * K));
+    GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * (size_t)g->n_dst * K));
     float* T = g->ws2;
     mul_kernel<<<nblk(n), 256, 0, st>>>(alpha, dalpha, n, de);
     GNNB_LAUNCHED();

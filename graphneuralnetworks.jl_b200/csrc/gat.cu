@@ -728,7 +728,7 @@ int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const f
     p.D = D; p.C = (int32_t)C; p.H = (int32_t)H; p.E = (int32_t)g->E; p.nrows = c.nrows; p.chunk = g->chunk;
     p.nchunks = (int32_t)ceil_div(g->E, g->chunk); p.fill = 1; p.slope = slope;
     if (c.n_long > 0) {
-        GNNB_TRY(ensure_ws(g, sizeof(float) * (size_t)2 * p.nchunks * (D + 2 * H + 4)));
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * p.nchunks * (D + 2 * H + 4)));
         p.ws = g->ws;
     }
     const bool lean = !g_reference_kernels && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && H <= 64;
@@ -793,7 +793,7 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
         return GNNB_OK;
     }
     // ws2: [T: n_dst*H][dz: E*H]
-    GNNB_TRY(ensure_ws2(g, sizeof(float) * ((size_t)n_dst * H + (size_t)g->E * H)));
+    GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * ((size_t)n_dst * H + (size_t)g->E * H)));
     float* T = g->ws2;
     float* dz = g->ws2 + (size_t)n_dst * H;
     {
@@ -809,7 +809,7 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
     p.D = D; p.C = (int32_t)C; p.H = (int32_t)H; p.E = (int32_t)g->E; p.nrows = c.nrows; p.chunk = g->chunk;
     p.nchunks = (int32_t)ceil_div(g->E, g->chunk); p.fill = 1; p.slope = slope;
     if (c.n_long > 0) {
-        GNNB_TRY(ensure_ws(g, sizeof(float) * (size_t)2 * p.nchunks * (D + H + 4)));
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * p.nchunks * (D + H + 4)));
         p.ws = g->ws;
     }
     const bool lean = !g_reference_kernels && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && C <= 128 && H <= 64;

@@ -251,9 +251,10 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
     if (smem > 200 * 1024) GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms_bwd: 2*H*C too large for the block stage");
     int64_t want = ceil_div(N, LOGIT_WARPS);
     const int nblocks = (int)(want < kNumSMs * 4 ? want : kNumSMs * 4);
-    static float* part_buf = nullptr; static size_t part_bytes = 0;
-    const size_t need = sizeof(float) * (size_t)nblocks * A;
-    if (part_bytes < need) { if (part_buf) { cudaDeviceSynchronize(); cudaFree(part_buf); } GNNB_CUDA(cudaMalloc(&part_buf, need)); part_bytes = need; }
+    DeviceState* s = nullptr;
+    GNNB_TRY(device_state(&s));
+    GNNB_TRY(grow_buffer(&s->gat_part, &s->gat_part_bytes, sizeof(float) * (size_t)nblocks * A));
+    float* part_buf = s->gat_part;
     if (!del || !der) {                        // one half: del (target half of da) or der (source half)
         const float* dh = del ? del : der;
         const int off = del ? 0 : (int)C;

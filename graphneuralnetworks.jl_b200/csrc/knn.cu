@@ -264,65 +264,59 @@ static int query_tile(int d) { return d <= 64 ? 128 : 64; }
 static int run(int mode, const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, int k,
                int self_loops, float r, int32_t* nbr, int64_t* counts, const int64_t* offsets, int64_t capacity,
                cudaStream_t st) {
+    DeviceScratch sc(st);
     int64_t* dseg = nullptr;
     int64_t* tiles = nullptr;   // [n_seg + 1 (+ 2 for the default segment)]: counts, then the scan into tile_ptr
     int* flags = nullptr;       // [0] bad, [1] pipeline stall, [2] fill / count mismatch
     void* tmp = nullptr;
     const int qt = query_tile(d);
-    int rc = [&]() -> int {
-        GNNB_CUDA(cudaMalloc(&tiles, sizeof(int64_t) * (size_t)(2 * n_seg + 3)));
-        GNNB_CUDA(cudaMalloc(&flags, 3 * sizeof(int)));
-        GNNB_CUDA(cudaMemsetAsync(flags, 0, 3 * sizeof(int), st));
-        if (!seg_ptr) {
-            dseg = tiles + 2 * n_seg + 1;
-            const int64_t h[2] = {0, n};
-            GNNB_CUDA(cudaMemcpyAsync(dseg, h, sizeof h, cudaMemcpyHostToDevice, st));
-            seg_ptr = dseg;
-        }
-        int64_t* cnt = tiles;
-        int64_t* tile_ptr = tiles + n_seg;
-        GNNB_CUDA(cudaMemsetAsync(tile_ptr, 0, sizeof(int64_t), st));
-        const int need = mode == KNN ? k + (self_loops ? 0 : 1) : 0;
-        tiles_kernel<<<(unsigned)ceil_div(n_seg, 256), 256, 0, st>>>(seg_ptr, n_seg, n, need, qt, cnt, flags);
-        GNNB_LAUNCHED();
-        size_t tmp_bytes = 0;
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, cnt, tile_ptr + 1, (int)n_seg, st));
-        GNNB_CUDA(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, cnt, tile_ptr + 1, (int)n_seg, st));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        Params p{};
-        p.pts = points; p.seg = seg_ptr; p.tile_ptr = tile_ptr; p.n_seg = (int)n_seg; p.d = d; p.k = k;
-        p.self_loops = self_loops ? 1 : 0; p.ct = BUF_FLOATS / d > 0 ? BUF_FLOATS / d : 1; p.r = r;
-        p.nbr = nbr; p.counts = counts; p.offsets = offsets; p.capacity = capacity;
-        p.err = flags + 1; p.mismatch = flags + 2; p.bad = flags;
-        if (mode == KNN) {
-            if (k <= 8) GNNB_TRY((dispatch_d<KNN, 8>(p, n, n_seg, st)));
-            else if (k <= 16) GNNB_TRY((dispatch_d<KNN, 16>(p, n, n_seg, st)));
-            else if (k <= 32) GNNB_TRY((dispatch_d<KNN, 32>(p, n, n_seg, st)));
-            else GNNB_TRY((dispatch_d<KNN, 64>(p, n, n_seg, st)));
-        } else if (mode == COUNT) {
-            GNNB_TRY((dispatch_d<COUNT, 1>(p, n, n_seg, st)));
-        } else {
-            GNNB_TRY((dispatch_d<FILL, 1>(p, n, n_seg, st)));
-        }
-        int h[3] = {0, 0, 0};
-        GNNB_CUDA(cudaMemcpyAsync(h, flags, sizeof h, cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        if (h[0] & 1)
-            GNNB_FAIL(GNNB_EINVAL, "seg_ptr must hold n_seg + 1 non-decreasing offsets from 0 to n = %lld", (long long)n);
-        if (h[0] & 2)
-            GNNB_FAIL(GNNB_ESIZE, "a segment has fewer than k%s = %d points", self_loops ? "" : " + 1", need);
-        if (h[1]) GNNB_FAIL(GNNB_ECUDA, "knn: the candidate pipeline stalled (mbarrier wait timed out)");
-        if (h[2])
-            GNNB_FAIL(GNNB_EINVAL, "gnnb_radius_fill: offsets do not match the rows of these points, r, self_loops and "
-                                   "segments (nothing was written outside a row's own range)");
-        return GNNB_OK;
-    }();
-    cudaStreamSynchronize(st);
-    cudaFree(tiles);
-    cudaFree(flags);
-    cudaFree(tmp);
-    return rc;
+    GNNB_TRY(sc.alloc(&tiles, (size_t)(2 * n_seg + 3)));
+    GNNB_TRY(sc.alloc(&flags, 3));
+    GNNB_CUDA(cudaMemsetAsync(flags, 0, 3 * sizeof(int), st));
+    if (!seg_ptr) {
+        dseg = tiles + 2 * n_seg + 1;
+        const int64_t h[2] = {0, n};
+        GNNB_CUDA(cudaMemcpyAsync(dseg, h, sizeof h, cudaMemcpyHostToDevice, st));
+        seg_ptr = dseg;
+    }
+    int64_t* cnt = tiles;
+    int64_t* tile_ptr = tiles + n_seg;
+    GNNB_CUDA(cudaMemsetAsync(tile_ptr, 0, sizeof(int64_t), st));
+    const int need = mode == KNN ? k + (self_loops ? 0 : 1) : 0;
+    tiles_kernel<<<(unsigned)ceil_div(n_seg, 256), 256, 0, st>>>(seg_ptr, n_seg, n, need, qt, cnt, flags);
+    GNNB_LAUNCHED();
+    size_t tmp_bytes = 0;
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, cnt, tile_ptr + 1, (int)n_seg, st));
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, cnt, tile_ptr + 1, (int)n_seg, st));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    Params p{};
+    p.pts = points; p.seg = seg_ptr; p.tile_ptr = tile_ptr; p.n_seg = (int)n_seg; p.d = d; p.k = k;
+    p.self_loops = self_loops ? 1 : 0; p.ct = BUF_FLOATS / d > 0 ? BUF_FLOATS / d : 1; p.r = r;
+    p.nbr = nbr; p.counts = counts; p.offsets = offsets; p.capacity = capacity;
+    p.err = flags + 1; p.mismatch = flags + 2; p.bad = flags;
+    if (mode == KNN) {
+        if (k <= 8) GNNB_TRY((dispatch_d<KNN, 8>(p, n, n_seg, st)));
+        else if (k <= 16) GNNB_TRY((dispatch_d<KNN, 16>(p, n, n_seg, st)));
+        else if (k <= 32) GNNB_TRY((dispatch_d<KNN, 32>(p, n, n_seg, st)));
+        else GNNB_TRY((dispatch_d<KNN, 64>(p, n, n_seg, st)));
+    } else if (mode == COUNT) {
+        GNNB_TRY((dispatch_d<COUNT, 1>(p, n, n_seg, st)));
+    } else {
+        GNNB_TRY((dispatch_d<FILL, 1>(p, n, n_seg, st)));
+    }
+    int h[3] = {0, 0, 0};
+    GNNB_CUDA(cudaMemcpyAsync(h, flags, sizeof h, cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    if (h[0] & 1)
+        GNNB_FAIL(GNNB_EINVAL, "seg_ptr must hold n_seg + 1 non-decreasing offsets from 0 to n = %lld", (long long)n);
+    if (h[0] & 2)
+        GNNB_FAIL(GNNB_ESIZE, "a segment has fewer than k%s = %d points", self_loops ? "" : " + 1", need);
+    if (h[1]) GNNB_FAIL(GNNB_ECUDA, "knn: the candidate pipeline stalled (mbarrier wait timed out)");
+    if (h[2])
+        GNNB_FAIL(GNNB_EINVAL, "gnnb_radius_fill: offsets do not match the rows of these points, r, self_loops and "
+                               "segments (nothing was written outside a row's own range)");
+    return GNNB_OK;
 }
 
 static int check_common(const char* who, const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg) {
@@ -370,25 +364,20 @@ int gnnb_radius_count(const float* points, int64_t n, int d, const int64_t* seg_
         GNNB_CUDA(cudaStreamSynchronize(st));
         return GNNB_OK;
     }
+    DeviceScratch sc(st);
     int64_t* counts = nullptr;
     void* tmp = nullptr;
-    int rc = [&]() -> int {
-        GNNB_CUDA(cudaMalloc(&counts, sizeof(int64_t) * (size_t)n));
-        GNNB_TRY(knn::run(knn::COUNT, points, n, d, seg_ptr, seg_ptr ? n_seg : 1, 0, self_loops, r, nullptr, counts,
-                          nullptr, 0, st));
-        size_t tmp_bytes = 0;
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, counts, offsets + 1, (int)n, st));
-        GNNB_CUDA(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, counts, offsets + 1, (int)n, st));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        GNNB_CUDA(cudaMemcpyAsync(total_host, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        return GNNB_OK;
-    }();
-    cudaStreamSynchronize(st);
-    cudaFree(counts);
-    cudaFree(tmp);
-    return rc;
+    GNNB_TRY(sc.alloc(&counts, (size_t)n));
+    GNNB_TRY(knn::run(knn::COUNT, points, n, d, seg_ptr, seg_ptr ? n_seg : 1, 0, self_loops, r, nullptr, counts,
+                      nullptr, 0, st));
+    size_t tmp_bytes = 0;
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, counts, offsets + 1, (int)n, st));
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, counts, offsets + 1, (int)n, st));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    GNNB_CUDA(cudaMemcpyAsync(total_host, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    return GNNB_OK;
 }
 
 int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,

@@ -187,8 +187,9 @@ static int alloc_csr(Csr& c, int64_t E, int32_t nrows, int32_t chunk) {
 }
 
 static int find_long_rows(Csr& c, int32_t chunk, cudaStream_t st) {
+    DeviceScratch sc;
     int32_t* d_count = nullptr;
-    GNNB_CUDA(cudaMalloc(&d_count, sizeof(int32_t)));
+    GNNB_TRY(sc.alloc(&d_count, 1));
     GNNB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(int32_t), st));
     if (c.nrows > 0) {
         long_rows_kernel<<<(unsigned)ceil_div(c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, chunk,
@@ -197,7 +198,6 @@ static int find_long_rows(Csr& c, int32_t chunk, cudaStream_t st) {
     }
     GNNB_CUDA(cudaMemcpyAsync(&c.n_long, d_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     GNNB_CUDA(cudaStreamSynchronize(st));
-    cudaFree(d_count);
     return GNNB_OK;
 }
 
@@ -212,8 +212,9 @@ int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st) {
     const int32_t* other = transposed ? g->coo_dst : g->coo_src;
     GNNB_TRY(alloc_csr(c, E, nrows, g->chunk));
     if (E > 0) {
+        DeviceScratch sc;
         int32_t* iota = nullptr;
-        GNNB_CUDA(cudaMalloc(&iota, sizeof(int32_t) * (size_t)E));
+        GNNB_TRY(sc.alloc(&iota, (size_t)E));
         iota_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(iota, E, 0);
         GNNB_LAUNCHED();
         int end_bit = 1;
@@ -222,15 +223,13 @@ int ensure_csr(gnnb_graph* g, bool transposed, cudaStream_t st) {
         GNNB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, c.row, iota, c.eid, (int)E, 0,
                                                   end_bit, st));
         void* tmp = nullptr;
-        GNNB_CUDA(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+        GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
         GNNB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, c.row, iota, c.eid, (int)E, 0,
                                                   end_bit, st));
         g_launches.fetch_add(4, std::memory_order_relaxed);  // histogram + onesweep passes (library kernels)
         gather_i32_kernel<<<(unsigned)ceil_div(E, 256), 256, 0, st>>>(other, c.eid, E, c.col);
         GNNB_LAUNCHED();
         GNNB_CUDA(cudaStreamSynchronize(st));
-        cudaFree(tmp);
-        cudaFree(iota);
     }
     rowptr_kernel<<<(unsigned)ceil_div(E + 1, 256), 256, 0, st>>>(c.row, E, nrows, c.rowptr);
     GNNB_LAUNCHED();
@@ -243,28 +242,14 @@ int ensure_invdeg(gnnb_graph* g, Csr& c, cudaStream_t st) {
     if (c.invdeg) return GNNB_OK;
     std::lock_guard<std::mutex> lock(g->mu);
     if (c.invdeg) return GNNB_OK;
+    DeviceScratch sc;
     float* p = nullptr;
-    GNNB_CUDA(cudaMalloc(&p, sizeof(float) * (size_t)(c.nrows > 0 ? c.nrows : 1)));
+    GNNB_TRY(sc.alloc(&p, (size_t)(c.nrows > 0 ? c.nrows : 1)));
     if (c.nrows > 0) {
         invdeg_kernel<<<(unsigned)ceil_div(c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, p);
         GNNB_LAUNCHED();
     }
-    c.invdeg = p;
-    return GNNB_OK;
-}
-
-int ensure_ws(gnnb_graph* g, size_t bytes) {
-    if (g->ws_bytes >= bytes) return GNNB_OK;
-    if (g->ws) { cudaDeviceSynchronize(); cudaFree(g->ws); g->ws = nullptr; g->ws_bytes = 0; }
-    GNNB_CUDA(cudaMalloc(&g->ws, bytes));
-    g->ws_bytes = bytes;
-    return GNNB_OK;
-}
-int ensure_ws2(gnnb_graph* g, size_t bytes) {
-    if (g->ws2_bytes >= bytes) return GNNB_OK;
-    if (g->ws2) { cudaDeviceSynchronize(); cudaFree(g->ws2); g->ws2 = nullptr; g->ws2_bytes = 0; }
-    GNNB_CUDA(cudaMalloc(&g->ws2, bytes));
-    g->ws2_bytes = bytes;
+    c.invdeg = sc.release(p);
     return GNNB_OK;
 }
 
@@ -272,9 +257,10 @@ static int convert_indices(const void* p, int64_t n, int index_bytes, int index_
                            int on_device, int32_t* out, int* d_bad, cudaStream_t st) {
     if (n == 0) return GNNB_OK;
     const void* dev = p;
+    DeviceScratch sc;
     void* staged = nullptr;
     if (!on_device) {
-        GNNB_CUDA(cudaMalloc(&staged, (size_t)n * index_bytes));
+        GNNB_TRY(sc.alloc(&staged, (size_t)n * index_bytes));
         GNNB_CUDA(cudaMemcpyAsync(staged, p, (size_t)n * index_bytes, cudaMemcpyHostToDevice, st));
         dev = staged;
     }
@@ -284,11 +270,29 @@ static int convert_indices(const void* p, int64_t n, int index_bytes, int index_
     else
         convert_index_kernel<int32_t><<<blocks, 256, 0, st>>>((const int32_t*)dev, n, index_base, limit, out, d_bad);
     GNNB_LAUNCHED();
-    if (staged) {
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        cudaFree(staged);
-    }
+    if (staged) GNNB_CUDA(cudaStreamSynchronize(st));
     return GNNB_OK;
+}
+
+// the plan of a new graph g (sizes set): its COO converted and range-checked, and the forward CSR
+static int build_plan(gnnb_graph* g, const void* src, const void* dst, int index_bytes, int index_base, int on_device,
+                      cudaStream_t st) {
+    const size_t nE = (size_t)(g->E > 0 ? g->E : 1);
+    GNNB_CUDA(cudaMalloc(&g->coo_src, sizeof(int32_t) * nE));
+    GNNB_CUDA(cudaMalloc(&g->coo_dst, sizeof(int32_t) * nE));
+    DeviceScratch sc;
+    int* d_bad = nullptr;
+    GNNB_TRY(sc.alloc(&d_bad, 1));
+    GNNB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+    GNNB_TRY(convert_indices(src, g->E, index_bytes, index_base, g->n_src, on_device, g->coo_src, d_bad, st));
+    GNNB_TRY(convert_indices(dst, g->E, index_bytes, index_base, g->n_dst, on_device, g->coo_dst, d_bad, st));
+    int bad = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    if (bad)
+        GNNB_FAIL(GNNB_EINDEX, "edge index out of range: every index must lie in [%d, num_nodes%s] (convert.jl:49-54)",
+                  index_base, index_base ? "" : ")");
+    return ensure_csr(g, false, st);
 }
 
 }  // namespace gnnb
@@ -322,30 +326,7 @@ int gnnb_graph_create(gnnb_graph_t* out, const void* src, const void* dst, int64
     g->n_dst = (int32_t)num_dst;
     g->chunk = g_chunk_default;
     cudaGetDevice(&g->device);
-    int status = GNNB_OK;
-    int* d_bad = nullptr;
-    do {
-#define GNNB_STEP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s failed: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; break; } }
-        size_t nE = (size_t)(num_edges > 0 ? num_edges : 1);
-        GNNB_STEP(cudaMalloc(&g->coo_src, sizeof(int32_t) * nE));
-        GNNB_STEP(cudaMalloc(&g->coo_dst, sizeof(int32_t) * nE));
-        GNNB_STEP(cudaMalloc(&d_bad, sizeof(int)));
-        GNNB_STEP(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
-        if ((status = convert_indices(src, num_edges, index_bytes, index_base, num_src, on_device, g->coo_src, d_bad, st))) break;
-        if ((status = convert_indices(dst, num_edges, index_bytes, index_base, num_dst, on_device, g->coo_dst, d_bad, st))) break;
-        int bad = 0;
-        GNNB_STEP(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-        GNNB_STEP(cudaStreamSynchronize(st));
-        if (bad) {
-            set_error("edge index out of range: every index must lie in [%d, num_nodes%s] (convert.jl:49-54)",
-                      index_base, index_base ? "" : ")");
-            status = GNNB_EINDEX;
-            break;
-        }
-        if ((status = ensure_csr(g, false, st))) break;
-#undef GNNB_STEP
-    } while (0);
-    cudaFree(d_bad);
+    const int status = build_plan(g, src, dst, index_bytes, index_base, on_device, st);
     if (status != GNNB_OK) {
         gnnb_graph_destroy(g);
         return status;
@@ -394,6 +375,30 @@ static int derive_self_loop_csr(const Csr& o, Csr& c, int64_t E, int32_t n, int3
     return GNNB_OK;
 }
 
+// h = add_self_loops(g) (sizes set): g's COO with the n loops appended, and the CSR of each direction g has built
+static int self_loops_into(gnnb_graph* g, gnnb_graph* h, cudaStream_t st) {
+    const int32_t n = g->n_src;
+    const int64_t E = g->E;
+    const size_t nE = (size_t)(h->E > 0 ? h->E : 1);
+    GNNB_CUDA(cudaMalloc(&h->coo_src, sizeof(int32_t) * nE));
+    GNNB_CUDA(cudaMalloc(&h->coo_dst, sizeof(int32_t) * nE));
+    if (E > 0) {
+        GNNB_CUDA(cudaMemcpyAsync(h->coo_src, g->coo_src, sizeof(int32_t) * E, cudaMemcpyDeviceToDevice, st));
+        GNNB_CUDA(cudaMemcpyAsync(h->coo_dst, g->coo_dst, sizeof(int32_t) * E, cudaMemcpyDeviceToDevice, st));
+    }
+    if (n > 0) {
+        iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(h->coo_src + E, n, 0);
+        GNNB_LAUNCHED();
+        iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(h->coo_dst + E, n, 0);
+        GNNB_LAUNCHED();
+    }
+    GNNB_TRY(ensure_csr(g, false, st));
+    GNNB_TRY(derive_self_loop_csr(g->by_dst, h->by_dst, E, n, h->chunk, st));
+    if (g->by_src.built) GNNB_TRY(derive_self_loop_csr(g->by_src, h->by_src, E, n, h->chunk, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    return GNNB_OK;
+}
+
 int gnnb_graph_add_self_loops(gnnb_graph_t g, gnnb_graph_t* out, void* stream) {
     if (!g || !out) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     *out = nullptr;
@@ -404,30 +409,7 @@ int gnnb_graph_add_self_loops(gnnb_graph_t g, gnnb_graph_t* out, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     gnnb_graph* h = new gnnb_graph();
     h->E = E2; h->n_src = n; h->n_dst = n; h->chunk = g->chunk; h->device = g->device;
-    int status = GNNB_OK;
-    do {
-        size_t nE = (size_t)(E2 > 0 ? E2 : 1);
-        if (cudaMalloc(&h->coo_src, sizeof(int32_t) * nE) != cudaSuccess ||
-            cudaMalloc(&h->coo_dst, sizeof(int32_t) * nE) != cudaSuccess) {
-            set_error("cudaMalloc failed in add_self_loops"); status = GNNB_ENOMEM; break;
-        }
-        if (E > 0) {
-            cudaMemcpyAsync(h->coo_src, g->coo_src, sizeof(int32_t) * E, cudaMemcpyDeviceToDevice, st);
-            cudaMemcpyAsync(h->coo_dst, g->coo_dst, sizeof(int32_t) * E, cudaMemcpyDeviceToDevice, st);
-        }
-        if (n > 0) {
-            iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(h->coo_src + E, n, 0);
-            iota_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(h->coo_dst + E, n, 0);
-            g_launches.fetch_add(2, std::memory_order_relaxed);
-        }
-        if ((status = ensure_csr(g, false, st))) break;
-        if ((status = derive_self_loop_csr(g->by_dst, h->by_dst, E, n, h->chunk, st))) break;
-        if (g->by_src.built) {
-            if ((status = derive_self_loop_csr(g->by_src, h->by_src, E, n, h->chunk, st))) break;
-        }
-        cudaError_t e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("add_self_loops: %s", cudaGetErrorString(e)); status = GNNB_ECUDA; break; }
-    } while (0);
+    const int status = self_loops_into(g, h, st);
     if (status != GNNB_OK) { gnnb_graph_destroy(h); return status; }
     *out = h;
     return GNNB_OK;
@@ -436,13 +418,6 @@ int gnnb_graph_add_self_loops(gnnb_graph_t g, gnnb_graph_t* out, void* stream) {
 }  // extern "C"
 
 namespace gnnb {
-
-struct SubgraphScratch {
-    void* p[4] = {nullptr, nullptr, nullptr, nullptr};
-    ~SubgraphScratch() {
-        for (void* q : p) cudaFree(q);
-    }
-};
 
 template <typename F>
 static int exclusive_scan_flags(F f, int64_t items, int32_t* out, void* tmp, size_t tmp_bytes, cudaStream_t st) {
@@ -473,13 +448,13 @@ static int subgraph_into(gnnb_graph* g, const uint8_t* node_keep, const uint8_t*
                          gnnb_graph* h, int32_t* node_map, int64_t* kept_eids, cudaStream_t st) {
     const int64_t n = g->n_src, E = g->E;
     GNNB_TRY(ensure_csr(g, false, st));
-    SubgraphScratch sc;
-    GNNB_CUDA(cudaMalloc(&sc.p[0], sizeof(int32_t) * (size_t)(n + 1)));
-    GNNB_CUDA(cudaMalloc(&sc.p[1], sizeof(int32_t) * (size_t)(E + 1)));
-    GNNB_CUDA(cudaMalloc(&sc.p[2], sizeof(int32_t) * (size_t)(E + 1)));
-    int32_t* map = (int32_t*)sc.p[0];      // exclusive scan of the node flags: new id of each kept node, count at [n]
-    int32_t* newid = (int32_t*)sc.p[1];    // exclusive scan of the COO edge flags: child COO id, count at [E]
-    int32_t* pos = (int32_t*)sc.p[2];      // exclusive scan of the flags in one parent direction's sorted order
+    DeviceScratch sc;
+    int32_t* map = nullptr;      // exclusive scan of the node flags: new id of each kept node, count at [n]
+    int32_t* newid = nullptr;    // exclusive scan of the COO edge flags: child COO id, count at [E]
+    int32_t* pos = nullptr;      // exclusive scan of the flags in one parent direction's sorted order
+    GNNB_TRY(sc.alloc(&map, (size_t)(n + 1)));
+    GNNB_TRY(sc.alloc(&newid, (size_t)(E + 1)));
+    GNNB_TRY(sc.alloc(&pos, (size_t)(E + 1)));
     const NodeKeepFlag nf{node_keep, n};
     const EdgeKeepFlag ef{edge_keep, node_keep, g->coo_src, g->coo_dst, E};
     const SortedKeepFlag sf{g->by_dst.eid, newid, E};
@@ -488,8 +463,8 @@ static int subgraph_into(gnnb_graph* g, const uint8_t* node_keep, const uint8_t*
     GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b1, flag_iter(ef), newid, (int)(E + 1), st));
     GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b2, flag_iter(sf), pos, (int)(E + 1), st));
     const size_t tmp_bytes = std::max(b0, std::max(b1, b2)) + 1;
-    GNNB_CUDA(cudaMalloc(&sc.p[3], tmp_bytes));
-    void* tmp = sc.p[3];
+    void* tmp = nullptr;
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes));
 
     GNNB_TRY(exclusive_scan_flags(nf, n + 1, map, tmp, tmp_bytes, st));
     GNNB_TRY(exclusive_scan_flags(ef, E + 1, newid, tmp, tmp_bytes, st));

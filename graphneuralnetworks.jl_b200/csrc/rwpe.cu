@@ -147,65 +147,61 @@ static int run(gnnb_graph* g, const float* w, const float* dinv, const int64_t* 
     const size_t off_med = align256(sizeof(int64_t) * (size_t)(2 * n_seg + 3));
     const size_t off_flags = off_med + align256(sizeof(int32_t) * (size_t)(2 * n_seg + 2));
     const size_t off_tmp = off_flags + 256;
+    DeviceScratch sc(st);
     char* buf = nullptr;
-    int rc = [&]() -> int {
-        GNNB_CUDA(cudaMalloc(&buf, off_tmp + (tmp_bytes ? tmp_bytes : 1)));
-        int64_t* items = reinterpret_cast<int64_t*>(buf);
-        int64_t* item_ptr = items + n_seg;
-        int32_t* med = reinterpret_cast<int32_t*>(buf + off_med);
-        int32_t* small = med + n_seg;
-        int32_t* red = small + n_seg;                       // [0] largest medium segment, [1] any small segment
-        int* flags = reinterpret_cast<int*>(buf + off_flags);
-        void* tmp = buf + off_tmp;
-        GNNB_CUDA(cudaMemsetAsync(flags, 0, 2 * sizeof(int), st));
-        if (!seg_ptr) {
-            int64_t* dseg = item_ptr + n_seg + 1;
-            const int64_t h[2] = {0, n};
-            GNNB_CUDA(cudaMemcpyAsync(dseg, h, sizeof h, cudaMemcpyHostToDevice, st));
-            seg_ptr = dseg;
-        }
-        GNNB_CUDA(cudaMemsetAsync(item_ptr, 0, sizeof(int64_t), st));
-        classify_kernel<<<(unsigned)ceil_div(n_seg, 256), 256, 0, st>>>(seg_ptr, n_seg, n, items, med, small, flags);
-        GNNB_LAUNCHED();
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, scan_bytes, items, item_ptr + 1, (int)n_seg, st));
-        GNNB_CUDA(cub::DeviceReduce::Max(tmp, max_bytes, med, red, (int)n_seg, st));
-        GNNB_CUDA(cub::DeviceReduce::Max(tmp, max_bytes, small, red + 1, (int)n_seg, st));
-        g_launches.fetch_add(3, std::memory_order_relaxed);
-        int64_t n_items = 0;
-        int32_t hred[2] = {0, 0};
-        int bad = 0;
-        GNNB_CUDA(cudaMemcpyAsync(&n_items, item_ptr + n_seg, sizeof n_items, cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaMemcpyAsync(hred, red, sizeof hred, cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaMemcpyAsync(&bad, flags, sizeof bad, cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        if (bad)
-            GNNB_FAIL(GNNB_EINVAL, "seg_ptr must hold n_seg + 1 non-decreasing offsets from 0 to n = %lld", (long long)n);
-        Params p{};
-        p.rowptr = g->by_dst.rowptr; p.col = g->by_dst.col; p.eid = g->by_dst.eid;
-        p.w = w; p.dinv = dinv; p.seg = seg_ptr; p.item_ptr = item_ptr; p.out = out; p.crossed = flags + 1;
-        p.n_seg = (int32_t)n_seg; p.K = K;
-        if (hred[1]) {                                      // small segments: every block of this launch is small
-            p.n_small_blocks = (int32_t)ceil_div(n_seg, WARPS);
-            if (w) GNNB_TRY(launch<true>(p, p.n_small_blocks, SMALL_SMEM, st));
-            else GNNB_TRY(launch<false>(p, p.n_small_blocks, SMALL_SMEM, st));
-        }
-        if (n_items) {                                      // medium segments: every block of this launch is medium
-            p.n_small_blocks = 0;
-            const size_t smem = (size_t)2 * hred[0] * SRC * sizeof(float);
-            if (w) GNNB_TRY(launch<true>(p, n_items, smem, st));
-            else GNNB_TRY(launch<false>(p, n_items, smem, st));
-        }
-        int crossed = 0;
-        GNNB_CUDA(cudaMemcpyAsync(&crossed, flags + 1, sizeof crossed, cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        if (crossed)
-            GNNB_FAIL(GNNB_EINVAL, "gnnb_random_walk_pe: an edge crosses segments of seg_ptr (the rows of its segment are "
-                                   "not valid; nothing was read or written outside a segment)");
-        return GNNB_OK;
-    }();
-    cudaStreamSynchronize(st);
-    cudaFree(buf);
-    return rc;
+    GNNB_TRY(sc.alloc(&buf, off_tmp + (tmp_bytes ? tmp_bytes : 1)));
+    int64_t* items = reinterpret_cast<int64_t*>(buf);
+    int64_t* item_ptr = items + n_seg;
+    int32_t* med = reinterpret_cast<int32_t*>(buf + off_med);
+    int32_t* small = med + n_seg;
+    int32_t* red = small + n_seg;                       // [0] largest medium segment, [1] any small segment
+    int* flags = reinterpret_cast<int*>(buf + off_flags);
+    void* tmp = buf + off_tmp;
+    GNNB_CUDA(cudaMemsetAsync(flags, 0, 2 * sizeof(int), st));
+    if (!seg_ptr) {
+        int64_t* dseg = item_ptr + n_seg + 1;
+        const int64_t h[2] = {0, n};
+        GNNB_CUDA(cudaMemcpyAsync(dseg, h, sizeof h, cudaMemcpyHostToDevice, st));
+        seg_ptr = dseg;
+    }
+    GNNB_CUDA(cudaMemsetAsync(item_ptr, 0, sizeof(int64_t), st));
+    classify_kernel<<<(unsigned)ceil_div(n_seg, 256), 256, 0, st>>>(seg_ptr, n_seg, n, items, med, small, flags);
+    GNNB_LAUNCHED();
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, scan_bytes, items, item_ptr + 1, (int)n_seg, st));
+    GNNB_CUDA(cub::DeviceReduce::Max(tmp, max_bytes, med, red, (int)n_seg, st));
+    GNNB_CUDA(cub::DeviceReduce::Max(tmp, max_bytes, small, red + 1, (int)n_seg, st));
+    g_launches.fetch_add(3, std::memory_order_relaxed);
+    int64_t n_items = 0;
+    int32_t hred[2] = {0, 0};
+    int bad = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&n_items, item_ptr + n_seg, sizeof n_items, cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaMemcpyAsync(hred, red, sizeof hred, cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaMemcpyAsync(&bad, flags, sizeof bad, cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    if (bad)
+        GNNB_FAIL(GNNB_EINVAL, "seg_ptr must hold n_seg + 1 non-decreasing offsets from 0 to n = %lld", (long long)n);
+    Params p{};
+    p.rowptr = g->by_dst.rowptr; p.col = g->by_dst.col; p.eid = g->by_dst.eid;
+    p.w = w; p.dinv = dinv; p.seg = seg_ptr; p.item_ptr = item_ptr; p.out = out; p.crossed = flags + 1;
+    p.n_seg = (int32_t)n_seg; p.K = K;
+    if (hred[1]) {                                      // small segments: every block of this launch is small
+        p.n_small_blocks = (int32_t)ceil_div(n_seg, WARPS);
+        if (w) GNNB_TRY(launch<true>(p, p.n_small_blocks, SMALL_SMEM, st));
+        else GNNB_TRY(launch<false>(p, p.n_small_blocks, SMALL_SMEM, st));
+    }
+    if (n_items) {                                      // medium segments: every block of this launch is medium
+        p.n_small_blocks = 0;
+        const size_t smem = (size_t)2 * hred[0] * SRC * sizeof(float);
+        if (w) GNNB_TRY(launch<true>(p, n_items, smem, st));
+        else GNNB_TRY(launch<false>(p, n_items, smem, st));
+    }
+    int crossed = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&crossed, flags + 1, sizeof crossed, cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    if (crossed)
+        GNNB_FAIL(GNNB_EINVAL, "gnnb_random_walk_pe: an edge crosses segments of seg_ptr (the rows of its segment are "
+                               "not valid; nothing was read or written outside a segment)");
+    return GNNB_OK;
 }
 
 }  // namespace rwpe

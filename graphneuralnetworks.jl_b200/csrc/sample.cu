@@ -140,41 +140,35 @@ int gnnb_sample_neighbors(gnnb_graph_t g, const void* nodes, int64_t n_nodes, in
         return GNNB_OK;
     }
     if (!nodes) GNNB_FAIL(GNNB_EINVAL, "gnnb_sample_neighbors: nodes is NULL");
+    DeviceScratch sc(st);
     int* bad = nullptr;
     int64_t* counts = nullptr;
     void* tmp = nullptr;
     const unsigned blocks = (unsigned)ceil_div(n_nodes, 128);
-    int rc = [&]() -> int {
-        GNNB_CUDA(cudaMalloc(&bad, sizeof(int)));
-        GNNB_CUDA(cudaMalloc(&counts, sizeof(int64_t) * (size_t)n_nodes));
-        GNNB_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
-        sample_count_kernel<<<blocks, 128, 0, st>>>(nodes, n_nodes, index_bytes, index_base, c.rowptr, c.nrows, K, replace,
-                                                    counts, bad);
-        GNNB_LAUNCHED();
-        size_t tmp_bytes = 0;
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, counts, offsets_dev + 1, (int)n_nodes, st));
-        GNNB_CUDA(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, counts, offsets_dev + 1, (int)n_nodes, st));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        int hbad = 0;
-        int64_t total = 0;
-        GNNB_CUDA(cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaMemcpyAsync(&total, offsets_dev + n_nodes, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        if (hbad) GNNB_FAIL(GNNB_EINDEX, "node id outside [%d, %d]", index_base, index_base + c.nrows - 1);
-        *total_host = total;
-        if (!eids_dev || total == 0) return GNNB_OK;
-        if (capacity < total) GNNB_FAIL(GNNB_ESIZE, "eids buffer holds %lld entries, %lld needed", (long long)capacity, (long long)total);
-        sample_fill_kernel<<<blocks, 128, 0, st>>>(nodes, n_nodes, index_bytes, index_base, c.rowptr, c.eid, offsets_dev,
-                                                   replace, seed, eids_dev);
-        GNNB_LAUNCHED();
-        return GNNB_OK;
-    }();
-    cudaStreamSynchronize(st);
-    cudaFree(bad);
-    cudaFree(counts);
-    cudaFree(tmp);
-    return rc;
+    GNNB_TRY(sc.alloc(&bad, 1));
+    GNNB_TRY(sc.alloc(&counts, (size_t)n_nodes));
+    GNNB_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
+    sample_count_kernel<<<blocks, 128, 0, st>>>(nodes, n_nodes, index_bytes, index_base, c.rowptr, c.nrows, K, replace,
+                                                counts, bad);
+    GNNB_LAUNCHED();
+    size_t tmp_bytes = 0;
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, counts, offsets_dev + 1, (int)n_nodes, st));
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, counts, offsets_dev + 1, (int)n_nodes, st));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    int hbad = 0;
+    int64_t total = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaMemcpyAsync(&total, offsets_dev + n_nodes, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    if (hbad) GNNB_FAIL(GNNB_EINDEX, "node id outside [%d, %d]", index_base, index_base + c.nrows - 1);
+    *total_host = total;
+    if (!eids_dev || total == 0) return GNNB_OK;
+    if (capacity < total) GNNB_FAIL(GNNB_ESIZE, "eids buffer holds %lld entries, %lld needed", (long long)capacity, (long long)total);
+    sample_fill_kernel<<<blocks, 128, 0, st>>>(nodes, n_nodes, index_bytes, index_base, c.rowptr, c.eid, offsets_dev,
+                                               replace, seed, eids_dev);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
 }
 
 }  // extern "C"

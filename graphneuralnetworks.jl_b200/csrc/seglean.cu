@@ -466,40 +466,34 @@ int ensure_items(gnnb_graph* g, const Csr& c, cudaStream_t st) {
     std::lock_guard<std::mutex> lock(g->mu);
     if (mc.items != nullptr) return GNNB_OK;
     const int32_t nchunks = (int32_t)ceil_div(g->E, g->chunk);
+    DeviceScratch sc;
     int32_t *counts = nullptr, *offs = nullptr, *d_empty = nullptr;
     void* tmp = nullptr;
     int4* items = nullptr;
-    int status = GNNB_OK;
-    do {
-#define LP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s failed: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; break; } }
-        LP(cudaMalloc(&counts, sizeof(int32_t) * ((size_t)nchunks + 1)));
-        LP(cudaMalloc(&offs, sizeof(int32_t) * ((size_t)nchunks + 1)));
-        LP(cudaMalloc(&d_empty, sizeof(int32_t)));
-        LP(cudaMemsetAsync(counts, 0, sizeof(int32_t) * ((size_t)nchunks + 1), st));
-        LP(cudaMemsetAsync(d_empty, 0, sizeof(int32_t), st));
-        item_count_kernel<<<(unsigned)ceil_div(nchunks, 256), 256, 0, st>>>(c.rowptr, c.row, g->chunk, (int)g->E, nchunks, counts);
-        size_t tmp_bytes = 0;
-        LP(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offs, nchunks + 1, st));
-        LP(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-        LP(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, offs, nchunks + 1, st));
-        count_empty_rows_kernel<<<(unsigned)ceil_div((int64_t)c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, d_empty);
-        int32_t n_items = 0, n_empty = 0;
-        LP(cudaMemcpyAsync(&n_items, offs + nchunks, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        LP(cudaMemcpyAsync(&n_empty, d_empty, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        LP(cudaStreamSynchronize(st));
-        LP(cudaMalloc(&items, sizeof(int4) * (size_t)(n_items > 0 ? n_items : 1)));
-        item_emit_kernel<<<(unsigned)ceil_div(nchunks, 256), 256, 0, st>>>(c.rowptr, c.row, g->chunk, (int)g->E, nchunks, offs, items);
-        LP(cudaGetLastError());
-        LP(cudaStreamSynchronize(st));
-        g_launches.fetch_add(4, std::memory_order_relaxed);
-        mc.n_items = n_items;
-        mc.n_empty = n_empty;
-        mc.items = reinterpret_cast<int32_t*>(items);
-        items = nullptr;
-#undef LP
-    } while (0);
-    cudaFree(counts); cudaFree(offs); cudaFree(d_empty); cudaFree(tmp); cudaFree(items);
-    return status;
+    GNNB_TRY(sc.alloc(&counts, (size_t)nchunks + 1));
+    GNNB_TRY(sc.alloc(&offs, (size_t)nchunks + 1));
+    GNNB_TRY(sc.alloc(&d_empty, 1));
+    GNNB_CUDA(cudaMemsetAsync(counts, 0, sizeof(int32_t) * ((size_t)nchunks + 1), st));
+    GNNB_CUDA(cudaMemsetAsync(d_empty, 0, sizeof(int32_t), st));
+    item_count_kernel<<<(unsigned)ceil_div(nchunks, 256), 256, 0, st>>>(c.rowptr, c.row, g->chunk, (int)g->E, nchunks, counts);
+    size_t tmp_bytes = 0;
+    GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts, offs, nchunks + 1, st));
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, counts, offs, nchunks + 1, st));
+    count_empty_rows_kernel<<<(unsigned)ceil_div((int64_t)c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, d_empty);
+    int32_t n_items = 0, n_empty = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&n_items, offs + nchunks, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaMemcpyAsync(&n_empty, d_empty, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    GNNB_TRY(sc.alloc(&items, (size_t)(n_items > 0 ? n_items : 1)));
+    item_emit_kernel<<<(unsigned)ceil_div(nchunks, 256), 256, 0, st>>>(c.rowptr, c.row, g->chunk, (int)g->E, nchunks, offs, items);
+    GNNB_CUDA(cudaGetLastError());
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    g_launches.fetch_add(4, std::memory_order_relaxed);
+    mc.n_items = n_items;
+    mc.n_empty = n_empty;
+    mc.items = reinterpret_cast<int32_t*>(sc.release(items));
+    return GNNB_OK;
 }
 
 bool g_l2_policy_forced = false;   // gnnb_set_kernel_variant(14): the L2 policy at every size
@@ -520,52 +514,47 @@ static int l2_bytes(const gnnb_graph* g, int64_t* bytes) {
     return GNNB_OK;
 }
 
-// count the gathers of each of the n gathered nodes of c, choose t, flag the hot edges in es (plan order of c)
-static int flag_hot_rows(gnnb_graph* g, Csr& c, int32_t n, float* es, int32_t* t_out, int32_t** rows_out,
-                         int32_t* n_rows_out, cudaStream_t st) {
+// count the gathers of each of the n gathered nodes of c, choose t, flag the hot edges in es (plan order of c); the list
+// of hot nodes is allocated in the caller's `keep`
+static int flag_hot_rows(gnnb_graph* g, Csr& c, int32_t n, float* es, DeviceScratch& keep, int32_t* t_out,
+                         int32_t** rows_out, int32_t* n_rows_out, cudaStream_t st) {
     int64_t l2 = 0;
     GNNB_TRY(l2_bytes(g, &l2));
     int64_t budget = (int64_t)((double)l2 * kHotL2Fraction) / 512;           // rows of 128 floats
+    DeviceScratch sc;
     int32_t *cnt = nullptr, *sorted = nullptr, *rows = nullptr, *d_nrows = nullptr;
     void* tmp = nullptr;
-    int status = GNNB_OK;
-    do {
-#define LP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s failed: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; break; } }
-        LP(cudaMalloc(&cnt, sizeof(int32_t) * (size_t)n));
-        LP(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)n, st));
-        count_gathers_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, cnt);
-        LP(cudaGetLastError());
-        int32_t t = 1;                          // every gathered node fits
-        if (n > budget) {                       // t = (budget+1)-th largest count + 1: at most `budget` nodes reach it
-            size_t tmp_bytes = 0;
-            LP(cudaMalloc(&sorted, sizeof(int32_t) * (size_t)n));
-            LP(cub::DeviceRadixSort::SortKeysDescending(nullptr, tmp_bytes, cnt, sorted, n, 0, 32, st));
-            LP(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-            LP(cub::DeviceRadixSort::SortKeysDescending(tmp, tmp_bytes, cnt, sorted, n, 0, 32, st));
-            int32_t kth = 0;
-            LP(cudaMemcpyAsync(&kth, sorted + budget, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-            LP(cudaStreamSynchronize(st));
-            t = kth + 1;
-        }
-        flag_hot_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, cnt, t, es);
-        LP(cudaGetLastError());
-        LP(cudaMalloc(&rows, sizeof(int32_t) * (size_t)(n < budget ? n : budget)));
-        LP(cudaMalloc(&d_nrows, sizeof(int32_t)));
-        LP(cudaMemsetAsync(d_nrows, 0, sizeof(int32_t), st));
-        list_hot_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(cnt, n, t, rows, d_nrows);
-        LP(cudaGetLastError());
-        int32_t n_rows = 0;
-        LP(cudaMemcpyAsync(&n_rows, d_nrows, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        LP(cudaStreamSynchronize(st));
-        g_launches.fetch_add(n > budget ? 4 : 3, std::memory_order_relaxed);
-        *t_out = t;
-        *rows_out = rows;
-        *n_rows_out = n_rows;
-        rows = nullptr;
-#undef LP
-    } while (0);
-    cudaFree(cnt); cudaFree(sorted); cudaFree(tmp); cudaFree(rows); cudaFree(d_nrows);
-    return status;
+    GNNB_TRY(sc.alloc(&cnt, (size_t)n));
+    GNNB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)n, st));
+    count_gathers_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, cnt);
+    GNNB_CUDA(cudaGetLastError());
+    int32_t t = 1;                          // every gathered node fits
+    if (n > budget) {                       // t = (budget+1)-th largest count + 1: at most `budget` nodes reach it
+        size_t tmp_bytes = 0;
+        GNNB_TRY(sc.alloc(&sorted, (size_t)n));
+        GNNB_CUDA(cub::DeviceRadixSort::SortKeysDescending(nullptr, tmp_bytes, cnt, sorted, n, 0, 32, st));
+        GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+        GNNB_CUDA(cub::DeviceRadixSort::SortKeysDescending(tmp, tmp_bytes, cnt, sorted, n, 0, 32, st));
+        int32_t kth = 0;
+        GNNB_CUDA(cudaMemcpyAsync(&kth, sorted + budget, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        GNNB_CUDA(cudaStreamSynchronize(st));
+        t = kth + 1;
+    }
+    flag_hot_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, cnt, t, es);
+    GNNB_CUDA(cudaGetLastError());
+    GNNB_TRY(keep.alloc(&rows, (size_t)(n < budget ? n : budget)));
+    GNNB_TRY(sc.alloc(&d_nrows, 1));
+    GNNB_CUDA(cudaMemsetAsync(d_nrows, 0, sizeof(int32_t), st));
+    list_hot_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(cnt, n, t, rows, d_nrows);
+    GNNB_CUDA(cudaGetLastError());
+    int32_t n_rows = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&n_rows, d_nrows, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    g_launches.fetch_add(n > budget ? 4 : 3, std::memory_order_relaxed);
+    *t_out = t;
+    *rows_out = rows;
+    *n_rows_out = n_rows;
+    return GNNB_OK;
 }
 
 // g->gcn_c = 1/sqrt(in-degree) (IEEE-exact, as gnnb_gcn_norm) and, for one direction, es[e] = gcn_c[col[e]] with the
@@ -573,26 +562,25 @@ static int flag_hot_rows(gnnb_graph* g, Csr& c, int32_t n, float* es, int32_t* t
 int ensure_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) {
     Csr& c = transposed ? g->by_src : g->by_dst;
     if (g->gcn_c != nullptr && (c.es != nullptr || g->E == 0)) return GNNB_OK;
+    DeviceScratch sc;   // what another thread's call installed first is freed here
     if (g->gcn_c == nullptr) {
         float* buf = nullptr;
-        GNNB_CUDA(cudaMalloc(&buf, sizeof(float) * (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
-        int rc = gnnb_gcn_norm(g, nullptr, buf, st);
-        if (rc != GNNB_OK) { cudaFree(buf); return rc; }
+        GNNB_TRY(sc.alloc(&buf, (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
+        GNNB_TRY(gnnb_gcn_norm(g, nullptr, buf, st));
         GNNB_CUDA(cudaStreamSynchronize(st));
         std::lock_guard<std::mutex> lock(g->mu);
-        if (g->gcn_c == nullptr) g->gcn_c = buf; else cudaFree(buf);
+        if (g->gcn_c == nullptr) g->gcn_c = sc.release(buf);
     }
     if (c.es == nullptr && g->E > 0) {
         float* es = nullptr;
-        GNNB_CUDA(cudaMalloc(&es, sizeof(float) * (size_t)g->E));
+        GNNB_TRY(sc.alloc(&es, (size_t)g->E));
         gather_scale_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, g->gcn_c, es);
         GNNB_LAUNCHED();
         int32_t t = 0, n_hot = 0;
         int32_t* hot = nullptr;
-        const int rc = flag_hot_rows(g, c, transposed ? g->n_dst : g->n_src, es, &t, &hot, &n_hot, st);
-        if (rc != GNNB_OK) { cudaFree(es); return rc; }
+        GNNB_TRY(flag_hot_rows(g, c, transposed ? g->n_dst : g->n_src, es, sc, &t, &hot, &n_hot, st));
         std::lock_guard<std::mutex> lock(g->mu);
-        if (c.es == nullptr) { c.es = es; c.hot_min = t; c.hot_rows = hot; c.n_hot = n_hot; } else { cudaFree(es); cudaFree(hot); }
+        if (c.es == nullptr) { c.es = sc.release(es); c.hot_min = t; c.hot_rows = sc.release(hot); c.n_hot = n_hot; }
     }
     return GNNB_OK;
 }
@@ -617,28 +605,28 @@ int ensure_bipartite_gcn_scale(gnnb_graph* g, bool transposed, cudaStream_t st) 
     float*& es_slot = transposed ? g->bip_es_src : g->bip_es_dst;
     if (g->bip_c_src != nullptr && g->bip_c_dst != nullptr && (es_slot != nullptr || g->E == 0)) return GNNB_OK;
     GNNB_TRY(ensure_csr(g, true, st));                   // out-degrees come from the by-source rowptr
+    DeviceScratch sc;   // what another thread's call installed first is freed here
     if (g->bip_c_src == nullptr || g->bip_c_dst == nullptr) {
         float *cs = nullptr, *cd = nullptr;
-        GNNB_CUDA(cudaMalloc(&cs, sizeof(float) * (size_t)(g->n_src > 0 ? g->n_src : 1)));
-        GNNB_CUDA(cudaMalloc(&cd, sizeof(float) * (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
-        int rc = gnnb_degree(g, GNNB_DIR_OUT, nullptr, cs, st);
-        if (rc == GNNB_OK) rc = gnnb_degree(g, GNNB_DIR_IN, nullptr, cd, st);
-        if (rc == GNNB_OK) rc = rsqrt_exact(cs, g->n_src, st);
-        if (rc == GNNB_OK) rc = rsqrt_exact(cd, g->n_dst, st);
-        if (rc != GNNB_OK) { cudaFree(cs); cudaFree(cd); return rc; }
+        GNNB_TRY(sc.alloc(&cs, (size_t)(g->n_src > 0 ? g->n_src : 1)));
+        GNNB_TRY(sc.alloc(&cd, (size_t)(g->n_dst > 0 ? g->n_dst : 1)));
+        GNNB_TRY(gnnb_degree(g, GNNB_DIR_OUT, nullptr, cs, st));
+        GNNB_TRY(gnnb_degree(g, GNNB_DIR_IN, nullptr, cd, st));
+        GNNB_TRY(rsqrt_exact(cs, g->n_src, st));
+        GNNB_TRY(rsqrt_exact(cd, g->n_dst, st));
         GNNB_CUDA(cudaStreamSynchronize(st));
         std::lock_guard<std::mutex> lock(g->mu);
-        if (g->bip_c_src == nullptr) { g->bip_c_src = cs; g->bip_c_dst = cd; } else { cudaFree(cs); cudaFree(cd); }
+        if (g->bip_c_src == nullptr) { g->bip_c_src = sc.release(cs); g->bip_c_dst = sc.release(cd); }
     }
     if (es_slot == nullptr && g->E > 0) {
         const Csr& c = transposed ? g->by_src : g->by_dst;
         float* es = nullptr;
-        GNNB_CUDA(cudaMalloc(&es, sizeof(float) * (size_t)g->E));
+        GNNB_TRY(sc.alloc(&es, (size_t)g->E));
         gather_scale_kernel<<<(unsigned)ceil_div(g->E, 256), 256, 0, st>>>(c.col, g->E, transposed ? g->bip_c_dst : g->bip_c_src, es);
         GNNB_LAUNCHED();
         GNNB_CUDA(cudaStreamSynchronize(st));
         std::lock_guard<std::mutex> lock(g->mu);
-        if (es_slot == nullptr) es_slot = es; else cudaFree(es);
+        if (es_slot == nullptr) es_slot = sc.release(es);
     }
     return GNNB_OK;
 }
@@ -708,7 +696,7 @@ int maxmin_bwd_lean(gnnb_graph* g, const float* w_plan_src, const float* x, cons
     p.n_items = c.n_items;
     p.col = c.col; p.row = c.row; p.w = w_plan_src; p.x = x; p.dout = dout; p.of = out_fwd; p.dx = dx; p.ws = nullptr;
     if (c.n_long > 0) {
-        GNNB_TRY(ensure_ws(g, (size_t)2 * ceil_div(g->E, g->chunk) * D * sizeof(float)));
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, (size_t)2 * ceil_div(g->E, g->chunk) * D * sizeof(float)));
         p.ws = g->ws;
     }
     if (p.n_items > 0) {

@@ -297,7 +297,7 @@ int seg_reduce(gnnb_graph* g, const Csr& c, const SegArgs& a, cudaStream_t st) {
     p.fill = 1;
     p.ws = nullptr;
     if (c.n_long > 0) {
-        GNNB_TRY(ensure_ws(g, (size_t)2 * p.nchunks * a.D * sizeof(float)));
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, (size_t)2 * p.nchunks * a.D * sizeof(float)));
         p.ws = g->ws;
     }
     // the lean work-item kernel (seglean.cu) for rows of 128 / 256 / 512 floats

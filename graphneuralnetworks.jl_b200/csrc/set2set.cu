@@ -354,7 +354,7 @@ int gnnb_set2set_attend(gnnb_graph_t g, const float* x, const float* q, int64_t 
     p.x = x; p.q = q; p.out = r; p.out_max = seg_max; p.out_sum = seg_sum;
     p.D = D; p.slot = (D + 2 + 3) & ~(int64_t)3;       // gat_fwd_fixup_kernel's slot with H = 1
     if (c.n_long > 0) {
-        GNNB_TRY(ensure_ws(g, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * p.slot));
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * p.slot));
         p.ws = g->ws;
     }
     GNNB_TRY(launch(false, vec4, p, st));
@@ -386,7 +386,7 @@ int gnnb_set2set_attend_bwd(gnnb_graph_t g, const float* x, const float* q, cons
     p.x = x; p.q = q; p.r = r; p.smax = seg_max; p.ssum = seg_sum; p.dr = dr; p.out = dq; p.dxe = dxe;
     p.D = D; p.slot = D;                               // seg_fixup_kernel's slot
     if (c.n_long > 0) {
-        GNNB_TRY(ensure_ws(g, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * D));
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * D));
         p.ws = g->ws;
     }
     GNNB_TRY(launch(true, vec4, p, st));

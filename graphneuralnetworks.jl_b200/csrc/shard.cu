@@ -296,88 +296,80 @@ int gnnb_shard_builder_finish(gnnb_shard_builder_t b, int direction, int add_sel
     const int64_t n = d.n;
     const int32_t lo = (int32_t)b->first[b->rank], hi = (int32_t)b->first[b->rank + 1];
     const int32_t n_local = b->n_local;
-    int32_t *flags = nullptr, *offs = nullptr, *rem = nullptr, *rem_s = nullptr, *halo = nullptr, *row = nullptr, *col = nullptr;
-    int64_t* counts = nullptr;
-    void* tmp = nullptr;
-    int64_t n_halo = 0;
-    int status = GNNB_OK;
     const int64_t n_loops = add_self_loops ? n_local : 0;
-    do {
-#define SP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s failed: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; break; } }
+    const int64_t ne = n + n_loops;
+    DeviceScratch sc;                 // the halo, the renamed edges and the receive counts: until the plan is built
+    int32_t *halo = nullptr, *row = nullptr, *col = nullptr;
+    int64_t* counts = nullptr;
+    int64_t n_halo = 0;
+    {
+        DeviceScratch edge_sc;        // the remote-source flags, their scan and the sorted remote sources
         if (n > 0) {
-            SP(cudaMalloc(&flags, sizeof(int32_t) * (size_t)n));
-            SP(cudaMalloc(&offs, sizeof(int32_t) * (size_t)n));
+            int32_t *flags = nullptr, *offs = nullptr, *rem = nullptr, *rem_s = nullptr;
+            void* tmp = nullptr;
+            GNNB_TRY(edge_sc.alloc(&flags, (size_t)n));
+            GNNB_TRY(edge_sc.alloc(&offs, (size_t)n));
             remote_flag_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(d.other, n, lo, hi, flags);
             size_t bytes = 0;
-            SP(cub::DeviceScan::ExclusiveSum(nullptr, bytes, flags, offs, (int)n, st));
-            SP(cudaMalloc(&tmp, bytes ? bytes : 1));
-            SP(cub::DeviceScan::ExclusiveSum(tmp, bytes, flags, offs, (int)n, st));
+            GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, flags, offs, (int)n, st));
+            GNNB_TRY(edge_sc.alloc(&tmp, bytes ? bytes : 1));
+            GNNB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, bytes, flags, offs, (int)n, st));
             int32_t lf = 0, lo_ = 0;
-            SP(cudaMemcpyAsync(&lf, flags + (n - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-            SP(cudaMemcpyAsync(&lo_, offs + (n - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-            SP(cudaStreamSynchronize(st));
+            GNNB_CUDA(cudaMemcpyAsync(&lf, flags + (n - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+            GNNB_CUDA(cudaMemcpyAsync(&lo_, offs + (n - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+            GNNB_CUDA(cudaStreamSynchronize(st));
             const int64_t n_rem = (int64_t)lf + lo_;
-            cudaFree(tmp); tmp = nullptr;
             if (n_rem > 0) {
-                SP(cudaMalloc(&rem, sizeof(int32_t) * (size_t)n_rem));
-                SP(cudaMalloc(&rem_s, sizeof(int32_t) * (size_t)n_rem));
+                GNNB_TRY(edge_sc.alloc(&rem, (size_t)n_rem));
+                GNNB_TRY(edge_sc.alloc(&rem_s, (size_t)n_rem));
                 compact_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(d.other, flags, offs, n, rem);
                 int end_bit = 1;
                 while (end_bit < 31 && ((int64_t)1 << end_bit) < b->N) ++end_bit;
-                SP(cub::DeviceRadixSort::SortKeys(nullptr, bytes, rem, rem_s, (int)n_rem, 0, end_bit, st));
-                SP(cudaMalloc(&tmp, bytes ? bytes : 1));
-                SP(cub::DeviceRadixSort::SortKeys(tmp, bytes, rem, rem_s, (int)n_rem, 0, end_bit, st));
-                cudaFree(tmp); tmp = nullptr;
+                GNNB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, rem, rem_s, (int)n_rem, 0, end_bit, st));
+                GNNB_TRY(edge_sc.alloc(&tmp, bytes ? bytes : 1));
+                GNNB_CUDA(cub::DeviceRadixSort::SortKeys(tmp, bytes, rem, rem_s, (int)n_rem, 0, end_bit, st));
                 // unique: head flags -> scan -> compact (flags / offs are reused: n_rem <= n)
                 head_flag_kernel<<<(unsigned)ceil_div(n_rem, 256), 256, 0, st>>>(rem_s, n_rem, flags);
-                SP(cub::DeviceScan::ExclusiveSum(nullptr, bytes, flags, offs, (int)n_rem, st));
-                SP(cudaMalloc(&tmp, bytes ? bytes : 1));
-                SP(cub::DeviceScan::ExclusiveSum(tmp, bytes, flags, offs, (int)n_rem, st));
-                SP(cudaMemcpyAsync(&lf, flags + (n_rem - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-                SP(cudaMemcpyAsync(&lo_, offs + (n_rem - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-                SP(cudaStreamSynchronize(st));
+                GNNB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, flags, offs, (int)n_rem, st));
+                GNNB_TRY(edge_sc.alloc(&tmp, bytes ? bytes : 1));
+                GNNB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, bytes, flags, offs, (int)n_rem, st));
+                GNNB_CUDA(cudaMemcpyAsync(&lf, flags + (n_rem - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+                GNNB_CUDA(cudaMemcpyAsync(&lo_, offs + (n_rem - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+                GNNB_CUDA(cudaStreamSynchronize(st));
                 n_halo = (int64_t)lf + lo_;
-                SP(cudaMalloc(&halo, sizeof(int32_t) * (size_t)n_halo));
+                GNNB_TRY(sc.alloc(&halo, (size_t)n_halo));
                 compact_kernel<<<(unsigned)ceil_div(n_rem, 256), 256, 0, st>>>(rem_s, flags, offs, n_rem, halo);
-                cudaFree(tmp); tmp = nullptr;
-                cudaFree(rem); rem = nullptr;
             }
             g_launches.fetch_add(8, std::memory_order_relaxed);
         }
-        const int64_t ne = n + n_loops;
-        SP(cudaMalloc(&row, sizeof(int32_t) * (size_t)(ne > 0 ? ne : 1)));
-        SP(cudaMalloc(&col, sizeof(int32_t) * (size_t)(ne > 0 ? ne : 1)));
+        GNNB_TRY(sc.alloc(&row, (size_t)(ne > 0 ? ne : 1)));
+        GNNB_TRY(sc.alloc(&col, (size_t)(ne > 0 ? ne : 1)));
         if (ne > 0) {
             rename_kernel<<<(unsigned)ceil_div(ne, 256), 256, 0, st>>>(d.key, d.other, n, lo, hi, halo, n_halo, n_local, n_loops, row, col);
             g_launches.fetch_add(1, std::memory_order_relaxed);
         }
-        SP(cudaMalloc(&counts, sizeof(int64_t) * (size_t)(b->world + 1)));
+        GNNB_TRY(sc.alloc(&counts, (size_t)(b->world + 1)));
         cudaFree(d.halo_local); d.halo_local = nullptr;
-        SP(cudaMalloc(&d.halo_local, sizeof(int32_t) * (size_t)(n_halo > 0 ? n_halo : 1)));
+        GNNB_CUDA(cudaMalloc(&d.halo_local, sizeof(int32_t) * (size_t)(n_halo > 0 ? n_halo : 1)));
         {
             const int64_t threads = n_halo > b->world + 1 ? n_halo : b->world + 1;
             halo_owner_kernel<<<(unsigned)ceil_div(threads, 256), 256, 0, st>>>(halo, n_halo, b->d_first, b->world, d.halo_local, counts);
             g_launches.fetch_add(1, std::memory_order_relaxed);
         }
         std::vector<int64_t> hc(b->world + 1);
-        SP(cudaMemcpyAsync(hc.data(), counts, sizeof(int64_t) * (size_t)(b->world + 1), cudaMemcpyDeviceToHost, st));
-        SP(cudaGetLastError());
-        SP(cudaStreamSynchronize(st));
+        GNNB_CUDA(cudaMemcpyAsync(hc.data(), counts, sizeof(int64_t) * (size_t)(b->world + 1), cudaMemcpyDeviceToHost, st));
+        GNNB_CUDA(cudaGetLastError());
+        GNNB_CUDA(cudaStreamSynchronize(st));
         if (recv_counts_host) for (int q = 0; q < b->world; ++q) recv_counts_host[q] = hc[q + 1] - hc[q];
         d.n_halo = n_halo;
         // the edge arrays of this direction are no longer needed: the plan keeps its own copies
         cudaFree(d.key); cudaFree(d.other); d.key = nullptr; d.other = nullptr; d.cap = 0; d.n = 0;
-        cudaFree(flags); flags = nullptr; cudaFree(offs); offs = nullptr; cudaFree(rem_s); rem_s = nullptr;
-        status = gnnb_graph_create(plan_out, col, row, ne, (int64_t)n_local + n_halo, n_local, 4, 0, 1, stream);
-        if (status != GNNB_OK) break;
-        if (n_local_out) *n_local_out = n_local;
-        if (n_halo_out) *n_halo_out = n_halo;
-        if (num_edges_out) *num_edges_out = ne;
-#undef SP
-    } while (0);
-    cudaFree(flags); cudaFree(offs); cudaFree(rem); cudaFree(rem_s); cudaFree(halo); cudaFree(row); cudaFree(col);
-    cudaFree(counts); cudaFree(tmp);
-    return status;
+    }
+    GNNB_TRY(gnnb_graph_create(plan_out, col, row, ne, (int64_t)n_local + n_halo, n_local, 4, 0, 1, stream));
+    if (n_local_out) *n_local_out = n_local;
+    if (n_halo_out) *n_halo_out = n_halo;
+    if (num_edges_out) *num_edges_out = ne;
+    return GNNB_OK;
 }
 
 // ---- 'balanced' ownership: degree histogram over the chunks, then the nodes dealt to the ranks by decreasing degree ------
@@ -401,27 +393,22 @@ int gnnb_balanced_relabel(const int32_t* cost_dev, int64_t num_nodes, int world,
     if (!cost_dev || !relabel_dev || !order_dev) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     cudaStream_t st = (cudaStream_t)stream;
     const int n = (int)num_nodes;
+    DeviceScratch sc;
     int32_t *ids = nullptr, *cost_s = nullptr, *by_degree = nullptr;
     void* tmp = nullptr;
-    int status = GNNB_OK;
-    do {
-#define SP(expr) { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error("%s failed: %s", #expr, cudaGetErrorString(_e)); status = (_e == cudaErrorMemoryAllocation) ? GNNB_ENOMEM : GNNB_ECUDA; break; } }
-        SP(cudaMalloc(&ids, sizeof(int32_t) * (size_t)n));
-        SP(cudaMalloc(&cost_s, sizeof(int32_t) * (size_t)n));
-        SP(cudaMalloc(&by_degree, sizeof(int32_t) * (size_t)n));
-        iota32_kernel<<<(unsigned)ceil_div((int64_t)n, 256), 256, 0, st>>>(ids, n);
-        size_t bytes = 0;                                        // stable: ties keep id order, identical on every rank
-        SP(cub::DeviceRadixSort::SortPairsDescending(nullptr, bytes, cost_dev, cost_s, ids, by_degree, n, 0, 32, st));
-        SP(cudaMalloc(&tmp, bytes ? bytes : 1));
-        SP(cub::DeviceRadixSort::SortPairsDescending(tmp, bytes, cost_dev, cost_s, ids, by_degree, n, 0, 32, st));
-        deal_kernel<<<(unsigned)ceil_div((int64_t)n, 256), 256, 0, st>>>(by_degree, n, world, relabel_dev, order_dev);
-        SP(cudaGetLastError());
-        SP(cudaStreamSynchronize(st));
-        g_launches.fetch_add(4, std::memory_order_relaxed);
-#undef SP
-    } while (0);
-    cudaFree(ids); cudaFree(cost_s); cudaFree(by_degree); cudaFree(tmp);
-    return status;
+    GNNB_TRY(sc.alloc(&ids, (size_t)n));
+    GNNB_TRY(sc.alloc(&cost_s, (size_t)n));
+    GNNB_TRY(sc.alloc(&by_degree, (size_t)n));
+    iota32_kernel<<<(unsigned)ceil_div((int64_t)n, 256), 256, 0, st>>>(ids, n);
+    size_t bytes = 0;                                        // stable: ties keep id order, identical on every rank
+    GNNB_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, bytes, cost_dev, cost_s, ids, by_degree, n, 0, 32, st));
+    GNNB_TRY(sc.alloc(&tmp, bytes ? bytes : 1));
+    GNNB_CUDA(cub::DeviceRadixSort::SortPairsDescending(tmp, bytes, cost_dev, cost_s, ids, by_degree, n, 0, 32, st));
+    deal_kernel<<<(unsigned)ceil_div((int64_t)n, 256), 256, 0, st>>>(by_degree, n, world, relabel_dev, order_dev);
+    GNNB_CUDA(cudaGetLastError());
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    g_launches.fetch_add(4, std::memory_order_relaxed);
+    return GNNB_OK;
 }
 
 int gnnb_shard_builder_halo(gnnb_shard_builder_t b, int direction, int32_t* halo_local_dev, void* stream) {

@@ -78,47 +78,36 @@ static int bits_for(int64_t span) {  // bits needed for values in [0, span)
     return b;
 }
 
-struct SortScratch {
-    uint64_t *keys = nullptr, *keys_sorted = nullptr;
-    int32_t *iota = nullptr, *perm = nullptr;
-    int* bad = nullptr;
-    void* tmp = nullptr;
-    ~SortScratch() {
-        cudaFree(keys);
-        cudaFree(keys_sorted);
-        cudaFree(iota);
-        cudaFree(perm);
-        cudaFree(bad);
-        cudaFree(tmp);
-    }
-};
-
-// keys_sorted / perm <- stable sort of the pairs by (u, v); values must lie in [lo, hi)
+// *keys_sorted / *perm <- stable sort of the pairs by (u, v), in the caller's scratch; values must lie in [lo, hi)
 static int sort_pairs(const void* u, const void* v, int64_t E, int index_bytes, int64_t lo, int64_t hi, int vbits,
-                      SortScratch& s, cudaStream_t st) {
-    GNNB_CUDA(cudaMalloc(&s.keys, sizeof(uint64_t) * (size_t)E));
-    GNNB_CUDA(cudaMalloc(&s.keys_sorted, sizeof(uint64_t) * (size_t)E));
-    GNNB_CUDA(cudaMalloc(&s.iota, sizeof(int32_t) * (size_t)E));
-    GNNB_CUDA(cudaMalloc(&s.perm, sizeof(int32_t) * (size_t)E));
-    GNNB_CUDA(cudaMalloc(&s.bad, sizeof(int)));
-    GNNB_CUDA(cudaMemsetAsync(s.bad, 0, sizeof(int), st));
+                      DeviceScratch& sc, uint64_t** keys_sorted, int32_t** perm, cudaStream_t st) {
+    uint64_t* keys = nullptr;
+    int32_t* iota = nullptr;
+    int* d_bad = nullptr;
+    void* tmp = nullptr;
+    GNNB_TRY(sc.alloc(&keys, (size_t)E));
+    GNNB_TRY(sc.alloc(keys_sorted, (size_t)E));
+    GNNB_TRY(sc.alloc(&iota, (size_t)E));
+    GNNB_TRY(sc.alloc(perm, (size_t)E));
+    GNNB_TRY(sc.alloc(&d_bad, 1));
+    GNNB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
     const unsigned blocks = (unsigned)ceil_div(E, 256);
     if (index_bytes == 8)
         encode_pairs_kernel<int64_t><<<blocks, 256, 0, st>>>((const int64_t*)u, (const int64_t*)v, E, lo, hi, vbits,
-                                                             s.keys, s.iota, s.bad);
+                                                             keys, iota, d_bad);
     else
         encode_pairs_kernel<int32_t><<<blocks, 256, 0, st>>>((const int32_t*)u, (const int32_t*)v, E, lo, hi, vbits,
-                                                             s.keys, s.iota, s.bad);
+                                                             keys, iota, d_bad);
     GNNB_LAUNCHED();
     size_t tmp_bytes = 0;
-    GNNB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, s.keys, s.keys_sorted, s.iota, s.perm, (int)E, 0,
+    GNNB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, *keys_sorted, iota, *perm, (int)E, 0,
                                               2 * vbits, st));
-    GNNB_CUDA(cudaMalloc(&s.tmp, tmp_bytes ? tmp_bytes : 1));
-    GNNB_CUDA(cub::DeviceRadixSort::SortPairs(s.tmp, tmp_bytes, s.keys, s.keys_sorted, s.iota, s.perm, (int)E, 0,
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, *keys_sorted, iota, *perm, (int)E, 0,
                                               2 * vbits, st));
     g_launches.fetch_add(2, std::memory_order_relaxed);  // histogram + onesweep passes (library kernels)
     int bad = 0;
-    GNNB_CUDA(cudaMemcpyAsync(&bad, s.bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
     GNNB_CUDA(cudaStreamSynchronize(st));
     if (bad) GNNB_FAIL(GNNB_EINDEX, "edge index outside [%lld, %lld)", (long long)lo, (long long)hi);
     return GNNB_OK;
@@ -153,14 +142,16 @@ int gnnb_sort_edge_index(const void* u, const void* v, int64_t num_edges, int64_
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t lo = 0, hi = max_index + 1;  // values in [0, max_index]: works for 0- and 1-based ids alike
     const int vbits = bits_for(hi);
-    SortScratch s;
-    GNNB_TRY(sort_pairs(u, v, num_edges, index_bytes, lo, hi, vbits, s, st));
+    DeviceScratch sc;
+    uint64_t* keys_sorted = nullptr;
+    int32_t* perm = nullptr;
+    GNNB_TRY(sort_pairs(u, v, num_edges, index_bytes, lo, hi, vbits, sc, &keys_sorted, &perm, st));
     const unsigned blocks = (unsigned)ceil_div(num_edges, 256);
     if (index_bytes == 8)
-        decode_pairs_kernel<int64_t><<<blocks, 256, 0, st>>>(s.keys_sorted, s.perm, num_edges, lo, vbits, (int64_t*)u_out,
+        decode_pairs_kernel<int64_t><<<blocks, 256, 0, st>>>(keys_sorted, perm, num_edges, lo, vbits, (int64_t*)u_out,
                                                              (int64_t*)v_out, perm_out);
     else
-        decode_pairs_kernel<int32_t><<<blocks, 256, 0, st>>>(s.keys_sorted, s.perm, num_edges, lo, vbits, (int32_t*)u_out,
+        decode_pairs_kernel<int32_t><<<blocks, 256, 0, st>>>(keys_sorted, perm, num_edges, lo, vbits, (int32_t*)u_out,
                                                              (int32_t*)v_out, perm_out);
     GNNB_LAUNCHED();
     GNNB_CUDA(cudaStreamSynchronize(st));  // scratch is freed on return
@@ -180,41 +171,33 @@ int gnnb_coalesce_edges(const void* src, const void* dst, int64_t num_edges, int
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t lo = index_base, hi = index_base + num_nodes;
     const int vbits = bits_for(num_nodes);
-    SortScratch s;
-    GNNB_TRY(sort_pairs(src, dst, num_edges, index_bytes, lo, hi, vbits, s, st));
-    int32_t *flags = nullptr, *seg = nullptr;
+    DeviceScratch sc;
+    uint64_t* keys_sorted = nullptr;
+    int32_t *perm = nullptr, *flags = nullptr, *seg = nullptr;
     void* tmp = nullptr;
-    auto cleanup = [&]() {
-        cudaFree(flags);
-        cudaFree(seg);
-        cudaFree(tmp);
-    };
+    GNNB_TRY(sort_pairs(src, dst, num_edges, index_bytes, lo, hi, vbits, sc, &keys_sorted, &perm, st));
     const unsigned blocks = (unsigned)ceil_div(num_edges, 256);
-    int rc = [&]() -> int {
-        GNNB_CUDA(cudaMalloc(&flags, sizeof(int32_t) * (size_t)num_edges));
-        GNNB_CUDA(cudaMalloc(&seg, sizeof(int32_t) * (size_t)num_edges));
-        head_flags_kernel<<<blocks, 256, 0, st>>>(s.keys_sorted, num_edges, flags);
-        GNNB_LAUNCHED();
-        size_t tmp_bytes = 0;
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, flags, seg, (int)num_edges, st));
-        GNNB_CUDA(cudaMalloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-        GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, flags, seg, (int)num_edges, st));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        if (index_bytes == 8)
-            emit_unique_kernel<int64_t><<<blocks, 256, 0, st>>>(s.keys_sorted, flags, seg, s.perm, num_edges, lo, vbits,
-                                                                (int64_t*)src_out, (int64_t*)dst_out, perm_out, seg_out);
-        else
-            emit_unique_kernel<int32_t><<<blocks, 256, 0, st>>>(s.keys_sorted, flags, seg, s.perm, num_edges, lo, vbits,
-                                                                (int32_t*)src_out, (int32_t*)dst_out, perm_out, seg_out);
-        GNNB_LAUNCHED();
-        int32_t last = 0;
-        GNNB_CUDA(cudaMemcpyAsync(&last, seg + (num_edges - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        *num_unique = last;
-        return GNNB_OK;
-    }();
-    cleanup();
-    return rc;
+    GNNB_TRY(sc.alloc(&flags, (size_t)num_edges));
+    GNNB_TRY(sc.alloc(&seg, (size_t)num_edges));
+    head_flags_kernel<<<blocks, 256, 0, st>>>(keys_sorted, num_edges, flags);
+    GNNB_LAUNCHED();
+    size_t tmp_bytes = 0;
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, flags, seg, (int)num_edges, st));
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, flags, seg, (int)num_edges, st));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if (index_bytes == 8)
+        emit_unique_kernel<int64_t><<<blocks, 256, 0, st>>>(keys_sorted, flags, seg, perm, num_edges, lo, vbits,
+                                                            (int64_t*)src_out, (int64_t*)dst_out, perm_out, seg_out);
+    else
+        emit_unique_kernel<int32_t><<<blocks, 256, 0, st>>>(keys_sorted, flags, seg, perm, num_edges, lo, vbits,
+                                                            (int32_t*)src_out, (int32_t*)dst_out, perm_out, seg_out);
+    GNNB_LAUNCHED();
+    int32_t last = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&last, seg + (num_edges - 1), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    *num_unique = last;
+    return GNNB_OK;
 }
 
 int gnnb_graph_csr_device(gnnb_graph_t g, int transposed, int32_t* rowptr_dev, int32_t* col_dev, int32_t* eid_dev,

@@ -182,7 +182,7 @@ __global__ void wl_output_kernel(const int32_t* __restrict__ c, int64_t n, int64
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 static int bits_of(int64_t x) { int b = 0; while (x > 0) { ++b; x >>= 1; } return b; }
 
-struct Scratch {
+struct Arrays {   // the per-call arrays, carved from one allocation
     Key* keys[2];
     int32_t *iota, *v, *c, *flag, *rank, *hp, *headpos;
     uint64_t* s;           // [2][n]: S_1 then S_2
@@ -191,7 +191,7 @@ struct Scratch {
 };
 
 // sort keys[0] (end_bit bits), renumber into sc.c by first appearance; *count = number of classes
-static int relabel(const Scratch& sc, int64_t n, int end_bit, int64_t* count, cudaStream_t st) {
+static int relabel(const Arrays& sc, int64_t n, int end_bit, int64_t* count, cudaStream_t st) {
     const unsigned blocks = (unsigned)ceil_div(n, 256);
     size_t b = sc.tmp_bytes;
     GNNB_CUDA(cub::DeviceRadixSort::SortPairs(sc.tmp, b, sc.keys[0], sc.keys[1], sc.iota, sc.v, (int)n, KeyBits{}, 0,
@@ -218,7 +218,8 @@ static int run(gnnb_graph* g, const int64_t* x0, int64_t max_iters, int64_t* col
     const int64_t n = g->n_dst;
     const Csr& csr = g->by_dst;
     GNNB_TRY(ensure_items(g, csr, st));
-    if (csr.n_long > 0) GNNB_TRY(ensure_ws(g, (size_t)2 * ceil_div(g->E, g->chunk) * 2 * sizeof(uint64_t)));
+    if (csr.n_long > 0)
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, (size_t)2 * ceil_div(g->E, g->chunk) * 2 * sizeof(uint64_t)));
     uint64_t* ws = reinterpret_cast<uint64_t*>(g->ws);
 
     // CUB temporary storage: the sort at its widest bit range (fewer bits never need more), the two scans
@@ -232,63 +233,59 @@ static int run(gnnb_graph* g, const int64_t* x0, int64_t max_iters, int64_t* col
     const size_t tmp_bytes = std::max(sort_bytes, std::max(sum_bytes, max_bytes)) + 1;
     const size_t key_b = align256(sizeof(Key) * (size_t)n), s_b = align256(2 * sizeof(uint64_t) * (size_t)n);
     const size_t i_b = align256(sizeof(int32_t) * (size_t)(n + 1));
+    DeviceScratch scratch(st);
     char* buf = nullptr;
-    int rc = [&]() -> int {
-        GNNB_CUDA(cudaMalloc(&buf, 2 * key_b + s_b + 7 * i_b + tmp_bytes));
-        Scratch sc;
-        char* q = buf;
-        sc.keys[0] = reinterpret_cast<Key*>(q); q += key_b;
-        sc.keys[1] = reinterpret_cast<Key*>(q); q += key_b;
-        sc.s = reinterpret_cast<uint64_t*>(q); q += s_b;
-        int32_t** ints[7] = {&sc.iota, &sc.v, &sc.c, &sc.flag, &sc.rank, &sc.hp, &sc.headpos};
-        for (int32_t** a : ints) { *a = reinterpret_cast<int32_t*>(q); q += i_b; }
-        sc.tmp = q;
-        sc.tmp_bytes = tmp_bytes;
-        const unsigned blocks = (unsigned)ceil_div(n, 256);
-        GNNB_CUDA(cudaMemsetAsync(sc.flag + n, 0, sizeof(int32_t), st));   // the scan's n + 1-th item
-        // round 0: the iota values, and x0's partition (or one class)
-        wl_pack_x0_kernel<<<blocks, 256, 0, st>>>(x0, n, sc.keys[0], sc.iota);
-        GNNB_LAUNCHED();
-        int64_t count = 1;
-        if (x0) GNNB_TRY(relabel(sc, n, 64, &count, st));
-        else GNNB_CUDA(cudaMemsetAsync(sc.c, 0, sizeof(int32_t) * (size_t)n, st));
-        SigParams p;
-        p.items = reinterpret_cast<const int4*>(csr.items);
-        p.col = csr.col; p.row = csr.row; p.c = sc.c;
-        p.s1 = sc.s; p.s2 = sc.s + n; p.ws = ws;
-        p.n_items = csr.n_items;
-        const bool zero_fill = g->E == 0 || csr.n_empty != 0;     // rows without in-edges keep S = (0, 0)
-        int64_t round = 0;
-        for (;;) {
-            ++round;
-            if (zero_fill) GNNB_CUDA(cudaMemsetAsync(sc.s, 0, 2 * sizeof(uint64_t) * (size_t)n, st));
-            if (p.n_items > 0) {
-                wl_signature_kernel<<<(unsigned)ceil_div(p.n_items, 8), 256, 0, st>>>(p);
-                GNNB_LAUNCHED();
-            }
-            if (csr.n_long > 0) {
-                wl_fixup_kernel<<<(unsigned)ceil_div(csr.n_long, 256), 256, 0, st>>>(
-                    csr.long_rows, csr.n_long, csr.rowptr, g->chunk, ws, p.s1, p.s2);
-                GNNB_LAUNCHED();
-            }
-            wl_pack_kernel<<<blocks, 256, 0, st>>>(sc.c, p.s1, p.s2, n, sc.keys[0]);
+    GNNB_TRY(scratch.alloc(&buf, 2 * key_b + s_b + 7 * i_b + tmp_bytes));
+    Arrays sc;
+    char* q = buf;
+    sc.keys[0] = reinterpret_cast<Key*>(q); q += key_b;
+    sc.keys[1] = reinterpret_cast<Key*>(q); q += key_b;
+    sc.s = reinterpret_cast<uint64_t*>(q); q += s_b;
+    int32_t** ints[7] = {&sc.iota, &sc.v, &sc.c, &sc.flag, &sc.rank, &sc.hp, &sc.headpos};
+    for (int32_t** a : ints) { *a = reinterpret_cast<int32_t*>(q); q += i_b; }
+    sc.tmp = q;
+    sc.tmp_bytes = tmp_bytes;
+    const unsigned blocks = (unsigned)ceil_div(n, 256);
+    GNNB_CUDA(cudaMemsetAsync(sc.flag + n, 0, sizeof(int32_t), st));   // the scan's n + 1-th item
+    // round 0: the iota values, and x0's partition (or one class)
+    wl_pack_x0_kernel<<<blocks, 256, 0, st>>>(x0, n, sc.keys[0], sc.iota);
+    GNNB_LAUNCHED();
+    int64_t count = 1;
+    if (x0) GNNB_TRY(relabel(sc, n, 64, &count, st));
+    else GNNB_CUDA(cudaMemsetAsync(sc.c, 0, sizeof(int32_t) * (size_t)n, st));
+    SigParams p;
+    p.items = reinterpret_cast<const int4*>(csr.items);
+    p.col = csr.col; p.row = csr.row; p.c = sc.c;
+    p.s1 = sc.s; p.s2 = sc.s + n; p.ws = ws;
+    p.n_items = csr.n_items;
+    const bool zero_fill = g->E == 0 || csr.n_empty != 0;     // rows without in-edges keep S = (0, 0)
+    int64_t round = 0;
+    for (;;) {
+        ++round;
+        if (zero_fill) GNNB_CUDA(cudaMemsetAsync(sc.s, 0, 2 * sizeof(uint64_t) * (size_t)n, st));
+        if (p.n_items > 0) {
+            wl_signature_kernel<<<(unsigned)ceil_div(p.n_items, 8), 256, 0, st>>>(p);
             GNNB_LAUNCHED();
-            int64_t next = 0;
-            GNNB_TRY(relabel(sc, n, 122 + bits_of(count - 1), &next, st));
-            const bool stable = next == count;
-            count = next;
-            if (stable || round == max_iters) break;
         }
-        wl_output_kernel<<<blocks, 256, 0, st>>>(sc.c, n, colors);
+        if (csr.n_long > 0) {
+            wl_fixup_kernel<<<(unsigned)ceil_div(csr.n_long, 256), 256, 0, st>>>(
+                csr.long_rows, csr.n_long, csr.rowptr, g->chunk, ws, p.s1, p.s2);
+            GNNB_LAUNCHED();
+        }
+        wl_pack_kernel<<<blocks, 256, 0, st>>>(sc.c, p.s1, p.s2, n, sc.keys[0]);
         GNNB_LAUNCHED();
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        *num_colors = count;
-        *niters = round;
-        return GNNB_OK;
-    }();
-    cudaStreamSynchronize(st);
-    cudaFree(buf);
-    return rc;
+        int64_t next = 0;
+        GNNB_TRY(relabel(sc, n, 122 + bits_of(count - 1), &next, st));
+        const bool stable = next == count;
+        count = next;
+        if (stable || round == max_iters) break;
+    }
+    wl_output_kernel<<<blocks, 256, 0, st>>>(sc.c, n, colors);
+    GNNB_LAUNCHED();
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    *num_colors = count;
+    *niters = round;
+    return GNNB_OK;
 }
 
 }  // namespace wl

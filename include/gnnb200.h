@@ -19,6 +19,11 @@
  *     caller-visible memory and never free caller memory.  The only library-owned object is the
  *     opaque graph plan.  "_host" entry points take HOST pointers and do the H2D/D2H themselves.
  *   - there is no CPU fallback: without a CUDA device every compute entry returns GNNB_ECUDA.
+ *   - concurrency: scratch the library owns is per device (a plan's workspaces; the dense and
+ *     attention-logit buffers, the cuBLASLt handle and the tensor-core watchdog flag of each device,
+ *     which grow only).  Calls on one device must therefore be stream-ordered with respect to each
+ *     other.  Once warm, the dense, propagate and attention entries neither allocate nor
+ *     synchronise, so a step of them can be captured in a CUDA graph.
  */
 #ifndef GNNB200_H
 #define GNNB200_H
