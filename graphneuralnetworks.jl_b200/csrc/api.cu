@@ -210,8 +210,9 @@ int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local,
                         int64_t n_local, const float* w, const float* cs, const float* ct, int64_t D, float* out,
                         void* stream) {
     GNNB_TRY(check_common(g, msg, aggr, D, w));
-    if (!out) GNNB_FAIL(GNNB_EINVAL, "out is NULL");
     if (n_local < 0 || n_local > g->n_src) GNNB_FAIL(GNNB_ESIZE, "n_local must be in [0, num_src]");
+    if (g->n_dst == 0) return GNNB_OK;   // a rank that owns no node: no row to reduce, out may be NULL
+    if (!out) GNNB_FAIL(GNNB_EINVAL, "out is NULL");
     if (n_local > 0 && !x_local) GNNB_FAIL(GNNB_EINVAL, "x_local is NULL");
     if (n_local < g->n_src && !x_halo) GNNB_FAIL(GNNB_EINVAL, "x_halo is NULL but the shard has halo sources");
     cudaStream_t st = (cudaStream_t)stream;

@@ -422,7 +422,8 @@ int gnnb_linear_bwd_mask(const float* dy, const uint32_t* mask, const float* x, 
     if (N < 0 || Din <= 0 || Dout <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
     if (Dout != 128 || Din % 32 != 0 || Din > 128 || !g_tc_enabled)
         GNNB_FAIL(GNNB_EUNSUPPORTED, "linear_bwd_mask: Dout must be 128, Din 32, 64, 96 or 128, tensor-core kernels on");
-    if (!dx || !dW) GNNB_FAIL(GNNB_EINVAL, "linear_bwd_mask computes dx and dW together: both are required");
+    // dx of an empty batch has no element (torch hands over NULL for it: a rank that owns no node)
+    if ((!dx && N > 0) || !dW) GNNB_FAIL(GNNB_EINVAL, "linear_bwd_mask computes dx and dW together: both are required");
     cudaStream_t st = (cudaStream_t)stream;
     if (N == 0) {
         GNNB_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)(Din * Dout), st));

@@ -199,7 +199,9 @@ int gnnb_degree(gnnb_graph_t g, int dir, const float* w, float* out, void* strea
 }
 
 int gnnb_gcn_norm(gnnb_graph_t g, const float* w, float* c_out, void* stream) {
-    if (!g || !c_out) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (g->n_dst == 0) return GNNB_OK;   // no targets (an empty rank's shard): nothing to write, c_out may be NULL
+    if (!c_out) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     cudaStream_t st = (cudaStream_t)stream;
     GNNB_TRY(gnnb_degree(g, GNNB_DIR_IN, w, c_out, stream));
     if (g->n_dst > 0) { rsqrt_exact_kernel<<<nblk(g->n_dst), 256, 0, st>>>(c_out, g->n_dst); GNNB_LAUNCHED(); }

@@ -310,7 +310,8 @@ int gnnb_gather_rows(const int32_t* idx_dev, int64_t n, const float* x, int64_t 
                      void* stream);
 /* gnnb_propagate_halo: gnnb_propagate (forward direction of the shard plan) with the gathered rows split
  * over two buffers: node ids < n_local read x_local, the others read x_halo + (id - n_local)*D.
- * cs (optional) has num_src entries ([local | halo] order), ct num_dst. */
+ * cs (optional) has num_src entries ([local | halo] order), ct num_dst.  A shard without targets (num_dst = 0, a rank
+ * that owns no node) has nothing to write: out may be NULL then, and so may gnnb_gcn_norm's c_out. */
 int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local, const float* x_halo,
                         int64_t n_local, const float* w, const float* cs, const float* ct, int64_t D,
                         float* out, void* stream);
