@@ -8,15 +8,22 @@
 // and the two cross terms (2^-11 smaller) in a second one; the epilogue adds the two.
 //
 // Shape: one persistent CTA per SM, 384 threads.  W (<= 128 x 128) is split once into two K-major 128B-swizzled
-// shared-memory images (w_big, w_small).  Row tiles of 128 rows of X stream through a 3-stage ring, one 32-float K-block
-// per stage:
-//   warps 0-3    producers : coalesced LDG.128 of the K-block, split in registers, st.shared into the canonical K-major
-//                            SWIZZLE_128B layout (x_big, x_small), fence.proxy.async, arrive on full[stage]
-//   warps 4-11   consumers : two warpgroups, 64 rows of the tile each: 12 wgmma.m64n128k8.tf32 per K-block from shared
-//                            memory into registers, then + bias, relu, stores straight from the accumulator fragment
+// shared-memory images (w_big, w_small).  Row tiles of 128 rows of X stream through a TMA ring, one 32-float K-block
+// (a 32 x 128 box, SWIZZLE_128B: the raw fp32 values in the canonical K-major layout) per stage:
+//   warp 0, lane 0 : cp.async.bulk.tensor.2d of each box into its stage, completed on full[stage] by complete_tx;
+//                    the fused pullback's producer warps also read every stage for the column sums of db
+//   warps 4-11     : two warpgroups, 64 rows of the tile each: ld.shared of the thread's A fragments, split into big and
+//                    small in registers, 12 wgmma.m64n128k8.tf32 per K-block with A from registers and W from shared
+//                    memory, one wgmma group kept in flight; then + bias, relu, stores straight from the accumulator
+// The ring holds raw tiles only (the small image never goes to shared memory), so it is RING_BYTES = 96 KB deep: 6
+// stages of 16 KB in the forward (5 of 18 KB, 3 of 32 KB in the pullback), up to 80-96 KB per SM in flight from HBM.  The producer warpgroup gives its registers to the consumers
+// (setmaxnreg), which hold two accumulators and two K-blocks of A fragments.
 // The kernel is HBM-bound by design (2 x 4 x K bytes per row against 6 K^2 flops on the TF32 tensor cores).
-// Every mbarrier wait is bounded: a broken pipeline makes the kernel flag an error and drain instead of hanging.
+// Every mbarrier wait is bounded: a broken pipeline makes the kernel flag an error and drain instead of hanging, and the
+// thread that issues the TMA copies waits (bounded) for its last ones to land before it exits (ring_drain).
 #include "common.cuh"
+#include "tma.cuh"
+#include <cudaTypedefs.h>
 #include <map>
 
 namespace gnnb {
@@ -25,7 +32,6 @@ namespace tc {
 constexpr int BM = 128;           // rows per tile (two warpgroups x wgmma M = 64)
 constexpr int BK = 32;            // floats per K-block = one 128 B swizzle row
 constexpr int BN = 128;           // wgmma N: W images hold 128 rows, zero beyond Nout
-constexpr int NSTAGE = 3;
 constexpr int PRODUCERS = 128;    // warps 0-3
 constexpr int CONSUMER_WARPS = 8; // warps 4-11 = warpgroups 1 and 2
 constexpr int THREADS = PRODUCERS + CONSUMER_WARPS * 32;
@@ -33,10 +39,17 @@ constexpr int KBLK_BYTES = BM * 128;          // one operand image of a K-block:
 constexpr int W_BYTES = 4 * KBLK_BYTES;       // up to K = 128: 64 KB per image
 constexpr int SMEM_W_BIG = 0;
 constexpr int SMEM_W_SMALL = W_BYTES;
-constexpr int SMEM_A = 2 * W_BYTES;           // stages: [big 16 KB][small 16 KB]
-constexpr int SMEM_BIAS = SMEM_A + NSTAGE * 2 * KBLK_BYTES;
+constexpr int SMEM_A = 2 * W_BYTES;           // the TMA ring: stages of raw boxes (see ring_stage_bytes)
+constexpr int RING_BYTES = 6 * KBLK_BYTES;
+constexpr int MAX_STAGES = 6;
+constexpr int MASK_BYTES = BM * 16;           // the relu mask words of a tile, beside its dy box (linear_bwd_dx_mask_kernel)
+constexpr int SMEM_BIAS = SMEM_A + RING_BYTES;
 constexpr int SMEM_BAR = SMEM_BIAS + 512;
-constexpr int SMEM_TOTAL = SMEM_BAR + 64;
+constexpr int SMEM_TOTAL = SMEM_BAR + 16 * MAX_STAGES;
+constexpr int PRODUCER_REGS = 56;             // setmaxnreg: 128 x 56 + 256 x 224 <= 64 K registers
+constexpr int CONSUMER_REGS = 224;
+static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory of the ring kernels");
+static_assert(PRODUCERS * PRODUCER_REGS + CONSUMER_WARPS * 32 * CONSUMER_REGS <= 65536, "register split");
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bar_init(uint32_t bar, uint32_t count) {
@@ -68,10 +81,6 @@ __device__ __forceinline__ float4 tf32_small(float4 v, float4 b) {
     return make_float4(tf32_small(v.x, b.x), tf32_small(v.y, b.y), tf32_small(v.z, b.z), tf32_small(v.w, b.w));
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// asks L2 to fetch `bytes` (a multiple of 16) at the 16 B aligned `p` ahead of the register loads that will read them
-__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
 
 // wgmma shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (stride byte offset), leading byte
 // offset unused by this layout.  A step of K = 8 tf32 inside the 128 B swizzle row advances the start address by 32 B.
@@ -125,6 +134,43 @@ __device__ __forceinline__ void mma_kblock(float* dm, float* dc, uint32_t a_big,
     wgmma_wait_all();
     fence_acc(dm);
     fence_acc(dc);
+}
+
+// as wgmma_tf32 with A (64 x 8) from registers: a[e] of thread (warp w of the warpgroup, lane l) is row 16w + l/4 + 8(e&1),
+// column l%4 + 4(e>>1)
+__device__ __forceinline__ void wgmma_tf32_rs(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+        "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// mma_kblock with the A fragments of the K-block in registers (ab / as: big / small, 4 per K = 8 step; dc == dm: one
+// accumulator), committed as one group and not waited for: the same 12 instructions in the same order on the same operand values
+__device__ __forceinline__ void mma_kblock_rs(float* dm, float* dc, const uint32_t* ab, const uint32_t* as, uint32_t b_big,
+                                              uint32_t b_small, bool first) {
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t o = j * 32;
+        const uint32_t acc = (first && j == 0) ? 0u : 1u;
+        wgmma_tf32_rs(dc, as + 4 * j, gmma_desc(b_big + o), acc);
+        wgmma_tf32_rs(dc, ab + 4 * j, gmma_desc(b_small + o), 1u);
+        wgmma_tf32_rs(dm, ab + 4 * j, gmma_desc(b_big + o), dm == dc ? 1u : acc);
+    }
+    wgmma_commit();
 }
 
 struct Params {
@@ -186,46 +232,116 @@ __device__ __forceinline__ void store_tile(const Params& p, const float* dm, con
     }
 }
 
-// consumer warpgroups of the ring kernels: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile of this CTA
-template <bool MASK = false>
-__device__ __forceinline__ void consume_tiles(const Params& p, uint32_t sbase, const float* sbias, int KB, int64_t ntiles) {
+// The ring: stage s of the CTA's flattened (tile, K-block) sequence holds the K-block's raw boxes, 1024 B aligned as
+// SWIZZLE_128B wants: [x or dy 16 KB] and, in the pullback, [y 16 KB] (relu from y) or [the tile's mask words 2 KB] (relu
+// from the mask bits).  full[s] completes on the TMA transaction bytes, empty[s] when every warp reading it has arrived.
+__host__ __device__ constexpr int ring_stage_bytes(int boxes, bool mask) { return boxes * KBLK_BYTES + (mask ? MASK_BYTES : 0); }
+__host__ __device__ constexpr int ring_stages(int stage_bytes) {
+    return RING_BYTES / stage_bytes < MAX_STAGES ? RING_BYTES / stage_bytes : MAX_STAGES;
+}
+
+// consumer warpgroups of the ring kernels: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile of this CTA.  Each
+// thread reads its A fragments of a K-block from the stage (rows r0, r0 + 8, columns 8 j + t, 8 j + t + 4, conflict-free
+// in the swizzled layout), releases the stage, splits them into big and small and issues the K-block's 12 wgmma; the
+// group of K-block i runs while the fragments of K-block i + 1 are read, so the two fragment sets alternate.
+// DPRE (the dense pullback): A = dpre, from the dy box and the mask words beside it (1) or the y box (2, when p.act).
+template <bool MASK_OUT, int DPRE>
+__device__ __forceinline__ void consume_ring(const Params& p, unsigned char* smem, const float* sbias, int KB, int64_t ntiles,
+                                             int ns, int stage_bytes) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * NSTAGE;
-    const int wg = (warp - PRODUCERS / 32) >> 2;
+    const int wg = (warp - PRODUCERS / 32) >> 2, g = lane >> 2, t = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + g;
+    const uint32_t sbase = s_u32(smem);
+    const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * MAX_STAGES;
+    const int64_t my_tiles = (ntiles > (int64_t)blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+    const int64_t total = my_tiles * KB;
     float dm[64] = {}, dc[64] = {};
-    uint32_t it = 0;
+    uint32_t ab0[16], as0[16], ab1[16], as1[16];
+    int stage = 0, kb = 0;
+    uint32_t phase = 0;
+    int64_t tile = blockIdx.x;
     bool alive = true;
-    for (int64_t tile = blockIdx.x; alive && tile < ntiles; tile += gridDim.x) {
-        for (int kb = 0; kb < KB; ++kb, ++it) {
-            const int stage = it % NSTAGE;
-            if (!bar_wait(bar_full + 8 * stage, (it / NSTAGE) & 1, p.err)) { alive = false; break; }
-            const uint32_t a_big = sbase + SMEM_A + stage * 2 * KBLK_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
-            const uint32_t w_big = sbase + SMEM_W_BIG + kb * KBLK_BYTES, w_small = sbase + SMEM_W_SMALL + kb * KBLK_BYTES;
-            mma_kblock(dm, dc, a_big, a_small, w_big, w_small, kb == 0);
-            if (lane == 0) bar_arrive(bar_empty + 8 * stage);   // this warp's reads of the stage are complete
+    auto step = [&](uint32_t* ab, uint32_t* as) {
+        if (!bar_wait(bar_full + 8 * stage, phase, p.err)) { alive = false; return; }
+        const unsigned char* st = smem + SMEM_A + stage * stage_bytes;
+        uint32_t mw[4];   // element e of a fragment: row r0 + 8 (e & 1), word (t >> 1) + 2 (e >> 1) of that row's mask
+        if constexpr (DPRE == 1) {
+            const uint32_t* m = reinterpret_cast<const uint32_t*>(st + KBLK_BYTES) + (t >> 1);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) mw[e] = m[(r0 + 8 * (e & 1)) * 4 + 2 * (e >> 1)];
         }
-        if (alive) store_tile<MASK>(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int off = (r0 + 8 * (e & 1)) * 128 + (((2 * j + (e >> 1)) ^ g) << 4) + 4 * t;
+                float v = *reinterpret_cast<const float*>(st + off);
+                if constexpr (DPRE == 1) v = (mw[e] >> (8 * kb + 2 * j + (t & 1))) & 1u ? v : 0.f;
+                if constexpr (DPRE == 2) {
+                    if (p.act) v = *reinterpret_cast<const float*>(st + KBLK_BYTES + off) > 0.f ? v : 0.f;
+                }
+                const float b = tf32_big(v);
+                ab[4 * j + e] = __float_as_uint(b);
+                as[4 * j + e] = __float_as_uint(tf32_small(v, b));
+            }
+        }
+        __syncwarp();
+        if (lane == 0) bar_arrive(bar_empty + 8 * stage);   // this warp's reads of the stage are complete
+        fence_acc(dm);
+        fence_acc(dc);
+        mma_kblock_rs(dm, dc, ab, as, sbase + SMEM_W_BIG + kb * KBLK_BYTES, sbase + SMEM_W_SMALL + kb * KBLK_BYTES, kb == 0);
+        wgmma_wait_1();                                     // the previous K-block's group, and so its fragment set, is done
+        if (++stage == ns) { stage = 0; phase ^= 1; }
+        if (++kb == KB) {
+            wgmma_wait_all();
+            fence_acc(dm);
+            fence_acc(dc);
+            store_tile<MASK_OUT>(p, dm, dc, sbias, tile * BM + wg * 64, 0, p.Nout);
+            kb = 0;
+            tile += gridDim.x;
+        }
+    };
+    for (int64_t it = 0; alive && it < total; it += 2) {
+        step(ab0, as0);
+        if (alive && it + 1 < total) step(ab1, as1);
+    }
+    wgmma_wait_all();
+}
+
+// the ring kernels' one-time setup: barriers (full: the TMA issue's arrive + bytes; empty: `readers` warps), bias
+__device__ __forceinline__ void ring_init(unsigned char* smem, const float* bias, int nbias, int readers) {
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        const uint32_t bar_full = s_u32(smem + SMEM_BAR), bar_empty = bar_full + 8 * MAX_STAGES;
+        for (int s = 0; s < MAX_STAGES; ++s) { bar_init(bar_full + 8 * s, 1); bar_init(bar_empty + 8 * s, readers); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    float* sbias = reinterpret_cast<float*>(smem + SMEM_BIAS);
+    for (int i = tid; i < BN; i += THREADS) sbias[i] = (bias && i < nbias) ? bias[i] : 0.f;
+}
+
+// the issuing thread's last act: wait, bounded but regardless of the error flag, until the copies of the last `issued`
+// (at most ns) items have landed, so that no bulk copy into this CTA's shared memory outlives it when a broken pipeline
+// made the readers stop early.  (stage, phase): the ring position the next item would have taken.
+__device__ __forceinline__ void ring_drain(uint32_t bar_full, int ns, int stage, uint32_t phase, int64_t issued) {
+    for (int k = 0; k < ns && k < issued; ++k) {
+        if (--stage < 0) { stage = ns - 1; phase ^= 1; }
+        for (uint32_t spin = 0; spin < (1u << 22) && !bar_try(bar_full + 8 * stage, phase); ++spin) {}
     }
 }
 
 // MASK: linear_relu_mask_kernel, which also writes the relu mask of y (Nout = 128, relu on)
 template <bool MASK>
-__device__ __forceinline__ void linear_body(const Params& p) {
+__device__ __forceinline__ void linear_body(const Params& p, const CUtensorMap* tm_x) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5;
     const int KB = p.K / BK;                                   // K-blocks per tile (<= 4)
     const int64_t ntiles = (p.M + BM - 1) / BM;
     const uint32_t sbase = s_u32(smem);
-    const uint32_t bar_full = sbase + SMEM_BAR;                // [NSTAGE]
-    const uint32_t bar_empty = bar_full + 8 * NSTAGE;          // [NSTAGE]
-    float* sbias = reinterpret_cast<float*>(smem + SMEM_BIAS);
+    constexpr int stage_bytes = ring_stage_bytes(1, false), ns = ring_stages(stage_bytes);
 
     // ---- one-time setup: barriers, bias, W split into the two swizzled K-major images (rows >= Nout zero)
-    if (tid == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    for (int i = tid; i < BN; i += THREADS) sbias[i] = (p.bias && i < p.Nout) ? p.bias[i] : 0.f;
+    ring_init(smem, p.bias, p.Nout, CONSUMER_WARPS);
     {
         const int kv = p.K >> 2;                               // float4 per row of W
         for (int idx = tid; idx < BN * kv; idx += THREADS) {
@@ -243,72 +359,52 @@ __device__ __forceinline__ void linear_body(const Params& p) {
     __syncthreads();
 
     if (warp < PRODUCERS / 32) {
-        // ================= producers =================
-        const int c = tid & 7, r16 = tid >> 3, rr = r16 & 7;
-        // flattened (tile, K-block) sequence of this CTA; the next item is prefetched into registers while the current
-        // one waits for its shared-memory slot
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+        if (tid != 0) return;
+        // ================= one thread issues the CTA's (tile, K-block) boxes into the ring =================
+        const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * MAX_STAGES;
         const int64_t my_tiles = (ntiles > (int64_t)blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-        const int64_t total = my_tiles * KB;
-        auto fetch = [&](int64_t item, float4* v) {
-            const int64_t tile = blockIdx.x + (item / KB) * gridDim.x;
-            const int kb = (int)(item % KB);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int64_t row = tile * BM + r16 + 16 * i;
-                v[i] = (item < total && row < p.M)
-                           ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)row * p.K + kb * BK) + c)
-                           : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-        };
-        float4 v[8], vn[8];
-        fetch(0, v);
-        for (int64_t it = 0; it < total; ++it) {
-            fetch(it + 1, vn);
-            const int stage = (int)(it % NSTAGE);
-            if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((it / NSTAGE) & 1) ^ 1), p.err)) break;
-            unsigned char* abig = smem + SMEM_A + stage * 2 * KBLK_BYTES;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float4 b = make_float4(tf32_big(v[i].x), tf32_big(v[i].y), tf32_big(v[i].z), tf32_big(v[i].w));
-                const float4 s = tf32_small(v[i], b);
-                const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
-                *reinterpret_cast<float4*>(abig + off) = b;
-                *reinterpret_cast<float4*>(abig + KBLK_BYTES + off) = s;
-            }
-            fence_proxy_async();
-            bar_arrive(bar_full + 8 * stage);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = vn[i];
+        int stage = 0, kb = 0;
+        uint32_t phase = 0;
+        int64_t tile = blockIdx.x, it = 0;
+        for (; it < my_tiles * KB; ++it) {
+            if (!bar_wait(bar_empty + 8 * stage, phase ^ 1, p.err)) break;
+            tma::mbar_expect_tx(bar_full + 8 * stage, KBLK_BYTES);
+            tma::tensor_load_2d(sbase + SMEM_A + stage * stage_bytes, tm_x, kb * BK, (int)(tile * BM), bar_full + 8 * stage);
+            if (++stage == ns) { stage = 0; phase ^= 1; }
+            if (++kb == KB) { kb = 0; tile += gridDim.x; }
         }
+        ring_drain(bar_full, ns, stage, phase, it);
     } else {
-        consume_tiles<MASK>(p, sbase, sbias, KB, ntiles);
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+        consume_ring<MASK, 0>(p, smem, reinterpret_cast<float*>(smem + SMEM_BIAS), KB, ntiles, ns, stage_bytes);
     }
 }
 
-__global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params p) { linear_body<false>(p); }
-__global__ void __launch_bounds__(THREADS, 1) linear_relu_mask_kernel(const Params p) { linear_body<true>(p); }
+__global__ void __launch_bounds__(THREADS, 1) linear_tf32x3_kernel(const Params p, const __grid_constant__ CUtensorMap tm_x) {
+    linear_body<false>(p, &tm_x);
+}
+__global__ void __launch_bounds__(THREADS, 1) linear_relu_mask_kernel(const Params p, const __grid_constant__ CUtensorMap tm_x) {
+    linear_body<true>(p, &tm_x);
+}
 
-// dx = dpre * W for dpre = relu ? (y > 0 ? dy : 0) : dy, Dout = 128 rows of W and Din = Nout <= 128 columns.  The producers
-// form dpre from dy and the forward output y (p.act) in registers, so dpre is never stored, and add it into per-thread
-// column sums for db.  Tiles, images and the MMA sequence are those of linear_tf32x3_kernel run on a transposed copy of W
-// with a zero bias, so dx has the same bits as that composition; W is read transposed straight into the images instead.
+// dx = dpre * W for dpre = relu ? (y > 0 ? dy : 0) : dy, Dout = 128 rows of W and Din = Nout <= 128 columns.  The
+// consumers form dpre from the dy box and the relu source in their stage (y, or the mask words) in registers, so dpre is
+// never stored; the four producer warps read the same stages for the column sums of db.  Tiles, images and the MMA
+// sequence are those of linear_tf32x3_kernel run on a transposed copy of W with a zero bias, so dx has the same bits as
+// that composition; W is read transposed straight into the images instead.
 // MASK: linear_bwd_dx_mask_kernel, which reads the relu mask bits (p.mask, always on) in place of y: the same dpre, from
 // 16 B per row instead of 512.
 template <bool MASK>
-__device__ __forceinline__ void bwd_dx_body(const Params& p) {
+__device__ __forceinline__ void bwd_dx_body(const Params& p, const CUtensorMap* tm_dy, const CUtensorMap* tm_y) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t ntiles = (p.M + BM - 1) / BM;
     const uint32_t sbase = s_u32(smem);
-    const uint32_t bar_full = sbase + SMEM_BAR;                // [NSTAGE]
-    const uint32_t bar_empty = bar_full + 8 * NSTAGE;          // [NSTAGE]
-    float* sbias = reinterpret_cast<float*>(smem + SMEM_BIAS);
+    const int boxes = (!MASK && p.act) ? 2 : 1;
+    const int stage_bytes = ring_stage_bytes(boxes, MASK), ns = ring_stages(stage_bytes);
 
-    if (tid == 0) {
-        for (int s = 0; s < NSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    for (int i = tid; i < BN; i += THREADS) sbias[i] = 0.f;    // (dm + dc) + 0: a -0 sum stores as +0, as in the composition
+    ring_init(smem, nullptr, 0, CONSUMER_WARPS + PRODUCERS / 32);   // (dm + dc) + 0: a -0 sum stores as +0, as in the composition
     // image row n = column n of W (n < Din), K = the 128 rows of W
     for (int idx = tid; idx < BN * 32; idx += THREADS) {
         const int n = idx >> 5, c4 = idx & 31, kb = c4 >> 3, c = c4 & 7;
@@ -327,107 +423,105 @@ __device__ __forceinline__ void bwd_dx_body(const Params& p) {
     __syncthreads();
 
     if (warp < PRODUCERS / 32) {
-        // ================= producers: K = 128, so a tile is 4 K-blocks.  The next item is prefetched into registers, the
-        // next tile into L2.
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+        // ================= producers: K = 128, so a tile is 4 K-blocks.  Thread 0 issues the boxes ns - 1 items ahead of
+        // the item the four warps read; each warp reads 32 rows x 128 B of every stage for the column sums.
+        const uint32_t bar_full = sbase + SMEM_BAR, bar_empty = bar_full + 8 * MAX_STAGES;
         const int c = tid & 7, r16 = tid >> 3, rr = r16 & 7;
-        const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
-        // flattened (tile, K-block) sequence of this CTA, as in linear_tf32x3_kernel
         const int64_t my_tiles = (ntiles > (int64_t)blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
         const int64_t total = my_tiles * 4;
-        // the relu mask of the 4 columns 32 kb + 4 c .. + 3 a thread loads: MASK, words 2 (c & 1) and 2 (c & 1) + 1 of the
-        // row's mask (bits 8 kb + 2 (c >> 1) and the next of each); otherwise the 4 floats of y
-        using MaskReg = typename std::conditional<MASK, uint2, float4>::type;
-        auto fetch = [&](int64_t item, float4* g, MaskReg* m) {
-            const int64_t tile = blockIdx.x + (item >> 2) * gridDim.x;
-            const int kb = (int)(item & 3);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int64_t row = tile * BM + r16 + 16 * i;
-                const bool in = item < total && row < p.M;
-                const size_t at = (size_t)row * 128 + kb * BK;
-                g[i] = in ? __ldg(reinterpret_cast<const float4*>(p.x + at) + c) : zero;
-                if constexpr (MASK) m[i] = in ? __ldg(reinterpret_cast<const uint2*>(p.mask + (size_t)row * 4) + (c & 1)) : make_uint2(0u, 0u);
-                else m[i] = (in && p.act) ? __ldg(reinterpret_cast<const float4*>(p.act + at) + c) : zero;
+        int i_stage = 0, i_kb = 0;
+        uint32_t i_phase = 0;
+        int64_t i_tile = blockIdx.x;
+        bool issuing = true;
+        auto issue = [&]() {
+            if (!issuing) return;
+            if (!bar_wait(bar_empty + 8 * i_stage, i_phase ^ 1, p.err)) { issuing = false; return; }
+            {
+                const uint32_t dst = sbase + SMEM_A + i_stage * stage_bytes, full = bar_full + 8 * i_stage;
+                const int64_t nr = (p.M - i_tile * BM < BM) ? p.M - i_tile * BM : BM;
+                tma::mbar_expect_tx(full, boxes * KBLK_BYTES + (MASK ? (uint32_t)nr * 16 : 0u));
+                tma::tensor_load_2d(dst, tm_dy, i_kb * BK, (int)(i_tile * BM), full);
+                if (boxes == 2) tma::tensor_load_2d(dst + KBLK_BYTES, tm_y, i_kb * BK, (int)(i_tile * BM), full);
+                if (MASK) tma::bulk_load(dst + KBLK_BYTES, p.mask + (size_t)i_tile * BM * 4, (uint32_t)nr * 16, full);
             }
+            if (++i_stage == ns) { i_stage = 0; i_phase ^= 1; }
+            if (++i_kb == 4) { i_kb = 0; i_tile += gridDim.x; }
         };
-        // dpre = act ? (act > 0 ? g : 0) : g, applied when the prefetched registers are promoted: holding the mask of the
-        // current item as well would not fit beside the next item's loads.  kb: the K-block of the item in g
-        auto masked = [&](float4* g, const MaskReg* m, int kb) {
-            if constexpr (MASK) {
-                const int s = 8 * kb + 2 * (c >> 1);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    g[i].x = (m[i].x >> s) & 1u ? g[i].x : 0.f; g[i].y = (m[i].x >> (s + 1)) & 1u ? g[i].y : 0.f;
-                    g[i].z = (m[i].y >> s) & 1u ? g[i].z : 0.f; g[i].w = (m[i].y >> (s + 1)) & 1u ? g[i].w : 0.f;
-                }
-            } else {
-                if (!p.act) return;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    g[i].x = m[i].x > 0.f ? g[i].x : 0.f; g[i].y = m[i].y > 0.f ? g[i].y : 0.f;
-                    g[i].z = m[i].z > 0.f ? g[i].z : 0.f; g[i].w = m[i].w > 0.f ? g[i].w : 0.f;
-                }
-            }
-        };
+        if (tid == 0)
+            for (int64_t n = 0; n < ns - 1 && n < total; ++n) issue();
         // column sums of dpre: after each item the 4 threads of a warp that share a column group add theirs in a fixed
         // order, and lanes 8 kb .. 8 kb + 7 keep the sums of K-block kb (columns 32 kb + 4 c .. + 3)
+        const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
         float4 cs = zero;
-        float4 g[8], gn[8];
-        MaskReg mn[8];
-        fetch(0, g, mn);
-        masked(g, mn, 0);
+        int stage = 0;
+        uint32_t phase = 0;
         for (int64_t it = 0; it < total; ++it) {
             const int kb = (int)(it & 3);
-            if (tid == 0 && kb == 0 && it + 4 < total) {       // the next tile of this CTA into L2
-                const int64_t r0 = (blockIdx.x + ((it >> 2) + 1) * gridDim.x) * BM, nr = (p.M - r0 < BM) ? p.M - r0 : BM;
-                prefetch_l2(p.x + (size_t)r0 * 128, (uint32_t)(nr * 512));
-                if (!MASK && p.act) prefetch_l2(p.act + (size_t)r0 * 128, (uint32_t)(nr * 512));
-            }
-            fetch(it + 1, gn, mn);
+            if (tid == 0 && it + ns - 1 < total) issue();
+            if (!bar_wait(bar_full + 8 * stage, phase, p.err)) break;
             if (p.colsum) {
-                float4 t = zero;
+                // the thread's 4 columns of rows r16 + 16 i; dpre = act ? (act > 0 ? dy : 0) : dy, with the relu source
+                // the mask bits 8 kb + 2 (c >> 1) and the next of words 2 (c & 1) and 2 (c & 1) + 1 of the row (MASK)
+                const unsigned char* st = smem + SMEM_A + stage * stage_bytes;
+                float4 s = zero;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) { t.x += g[i].x; t.y += g[i].y; t.z += g[i].z; t.w += g[i].w; }
+                for (int i = 0; i < 8; ++i) {
+                    const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
+                    float4 g = *reinterpret_cast<const float4*>(st + off);
+                    if constexpr (MASK) {
+                        const uint2 m = *reinterpret_cast<const uint2*>(st + KBLK_BYTES + (r16 + 16 * i) * 16 + (c & 1) * 8);
+                        const int sh = 8 * kb + 2 * (c >> 1);
+                        g.x = (m.x >> sh) & 1u ? g.x : 0.f; g.y = (m.x >> (sh + 1)) & 1u ? g.y : 0.f;
+                        g.z = (m.y >> sh) & 1u ? g.z : 0.f; g.w = (m.y >> (sh + 1)) & 1u ? g.w : 0.f;
+                    } else if (boxes == 2) {
+                        const float4 m = *reinterpret_cast<const float4*>(st + KBLK_BYTES + off);
+                        g.x = m.x > 0.f ? g.x : 0.f; g.y = m.y > 0.f ? g.y : 0.f;
+                        g.z = m.z > 0.f ? g.z : 0.f; g.w = m.w > 0.f ? g.w : 0.f;
+                    }
+                    s.x += g.x; s.y += g.y; s.z += g.z; s.w += g.w;
+                }
 #pragma unroll
                 for (int o = 8; o <= 16; o <<= 1) {
-                    t.x += __shfl_xor_sync(0xffffffffu, t.x, o); t.y += __shfl_xor_sync(0xffffffffu, t.y, o);
-                    t.z += __shfl_xor_sync(0xffffffffu, t.z, o); t.w += __shfl_xor_sync(0xffffffffu, t.w, o);
+                    s.x += __shfl_xor_sync(0xffffffffu, s.x, o); s.y += __shfl_xor_sync(0xffffffffu, s.y, o);
+                    s.z += __shfl_xor_sync(0xffffffffu, s.z, o); s.w += __shfl_xor_sync(0xffffffffu, s.w, o);
                 }
-                if ((lane >> 3) == kb) { cs.x += t.x; cs.y += t.y; cs.z += t.z; cs.w += t.w; }
+                if ((lane >> 3) == kb) { cs.x += s.x; cs.y += s.y; cs.z += s.z; cs.w += s.w; }
             }
-            const int stage = (int)(it % NSTAGE);
-            if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((it / NSTAGE) & 1) ^ 1), p.err)) break;
-            unsigned char* abig = smem + SMEM_A + stage * 2 * KBLK_BYTES;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float4 b = make_float4(tf32_big(g[i].x), tf32_big(g[i].y), tf32_big(g[i].z), tf32_big(g[i].w));
-                const float4 s = tf32_small(g[i], b);
-                const int off = ((r16 >> 3) + 2 * i) * 1024 + rr * 128 + ((c ^ rr) << 4);
-                *reinterpret_cast<float4*>(abig + off) = b;
-                *reinterpret_cast<float4*>(abig + KBLK_BYTES + off) = s;
-            }
-            fence_proxy_async();
-            bar_arrive(bar_full + 8 * stage);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) g[i] = gn[i];
-            masked(g, mn, (kb + 1) & 3);
+            __syncwarp();
+            if (lane == 0) bar_arrive(bar_empty + 8 * stage);
+            if (++stage == ns) { stage = 0; phase ^= 1; }
         }
+        if (tid == 0) ring_drain(bar_full, ns, i_stage, i_phase, (i_tile - blockIdx.x) / gridDim.x * 4 + i_kb);
         if (p.colsum) reinterpret_cast<float4*>(p.colsum + ((size_t)blockIdx.x * 4 + warp) * 128 + (lane >> 3) * BK)[c] = cs;
     } else {
-        consume_tiles(p, sbase, sbias, 128 / BK, ntiles);
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+        consume_ring<false, MASK ? 1 : 2>(p, smem, reinterpret_cast<float*>(smem + SMEM_BIAS), 128 / BK, ntiles, ns, stage_bytes);
     }
 }
 
-__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params p) { bwd_dx_body<false>(p); }
-__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_mask_kernel(const Params p) { bwd_dx_body<true>(p); }
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_kernel(const Params p, const __grid_constant__ CUtensorMap tm_dy,
+                                                                   const __grid_constant__ CUtensorMap tm_y) {
+    bwd_dx_body<false>(p, &tm_dy, &tm_y);
+}
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_mask_kernel(const Params p, const __grid_constant__ CUtensorMap tm_dy,
+                                                                        const __grid_constant__ CUtensorMap tm_y) {
+    bwd_dx_body<true>(p, &tm_dy, &tm_y);
+}
 }  // namespace tc
 
 // =====================================================================================================================
 // dW = dPre^T * X  (the weight pullback of the dense layer):  dW[i][j] = sum_r dPre[r][i] * X[r][j],  r over all N rows.
-// Both operands are "MN-major" in memory (the reduction index r is the slow one); tf32 wgmma reads K-major shared memory
-// only, so the producers transpose 32 rows of each operand into the same K-major SWIZZLE_128B images the forward kernel
-// uses: A = dPre^T (128 rows i), B = X^T (Din rows j, zero up to 128).  A lane covers 8 rows r x 4 float4 columns, which
-// keeps both the global loads (64 B runs) and the transposing shared-memory stores (2-way) cheap.
+// Both operands are "MN-major" in memory (the reduction index r is the slow one) and tf32 wgmma reads K-major operands
+// only.  A block of 32 rows r is a K-block.  One thread drops its row-major tiles into a TMA ring (boxes of 32 columns x
+// 32 rows, SWIZZLE_128B): dy (or dpre) as 4 boxes, y as 4 more in linear_bwd_dw_kernel, X as Din / 32 boxes, and the
+// rows' relu mask words (32 x 16 B, 1-D bulk copy) in linear_bwd_dw_mask_kernel.
+//   A = dPre^T (128 rows i): each consumer thread reads its fragments (rows i, columns r) straight from the dy box, forms
+//       dpre, splits it into big and small in registers and issues wgmma with A from registers, as the forward kernel;
+//   B = X^T (Din rows j, zero up to 128): the four producer warps transpose the X boxes into a double-buffered K-major
+//       SWIZZLE_128B image, big and small: lane l of a warp reads column j = 32 jb + l of 4 rows (conflict-free in the
+//       swizzled box) and stores the split float4 of those 4 rows k into row j of the image (one 16 B vector per image).
+// One wgmma group stays in flight; the B slot of block n - 1 is released once its group has retired.
 // Split-K: every CTA reduces a contiguous range of rows into its own register accumulators and writes a (128 x Din)
 // partial; a second kernel adds the partials in CTA order (deterministic).
 // The accumulation chain is cut every FLUSH row blocks and each short chain is added into an fp32 register sum with
@@ -435,11 +529,14 @@ __global__ void __launch_bounds__(THREADS, 1) linear_bwd_dx_mask_kernel(const Pa
 // =====================================================================================================================
 namespace tcw {
 using namespace tc;
-constexpr int WSTAGE = 3;
 constexpr int FLUSH = 4;                      // row blocks (of 32 rows) per accumulation chain
-constexpr int STAGE_BYTES = 4 * KBLK_BYTES;   // dPre big/small, X big/small
-constexpr int SMEM_BARW = WSTAGE * STAGE_BYTES;
-constexpr int SMEM_TOTALW = SMEM_BARW + 64;
+constexpr int BOX_BYTES = 32 * 128;           // one box: 32 rows x 32 floats
+constexpr int RINGW_BYTES = 160 * 1024;       // stages: [dy 16 KB][y 16 KB, linear_bwd_dw_kernel with y][X <= 16 KB][mask 512 B]
+constexpr int MAX_WSTAGES = 4;
+constexpr int SMEM_BIMG = RINGW_BYTES;        // 2 slots x [X^T big 16 KB][X^T small 16 KB]
+constexpr int SMEM_BARW = SMEM_BIMG + 4 * KBLK_BYTES;
+constexpr int SMEM_TOTALW = SMEM_BARW + 8 * (2 * MAX_WSTAGES + 4);
+static_assert(SMEM_TOTALW <= 227 * 1024, "shared memory of the dW kernels");
 
 struct ParamsW {
     const float* __restrict__ dpre;   // [M][128] (dy in the fused pullback)
@@ -451,190 +548,184 @@ struct ParamsW {
     const float* __restrict__ act;    // linear_bwd_dw_kernel only: forward output y, dpre = y > 0 ? dy : 0; null: dpre = dy
     const uint32_t* __restrict__ mask;  // linear_bwd_dw_mask_kernel only: [M][4] relu mask of y (layout: above tc::store_tile)
 };
-constexpr int L2_AHEAD = 3;           // linear_bwd_dw_kernel: row blocks prefetched into L2 ahead of the register loads
 
 // byte offset of element (row n, k) of a K-major SWIZZLE_128B image, k < 32
 __device__ __forceinline__ int kmajor_off(int n, int k) {
     return (n >> 3) * 1024 + (n & 7) * 128 + ((((k >> 2) ^ (n & 7))) << 4) + (k & 3) * 4;
 }
+// byte offset of element (row r < 32, column c) of a row-major tile stored as 32-column SWIZZLE_128B boxes
+__device__ __forceinline__ int box_off(int r, int c) {
+    return (c >> 5) * BOX_BYTES + r * 128 + ((((c & 31) >> 2) ^ (r & 7)) << 4) + (c & 3) * 4;
+}
 
-// FUSED: the fused pullback's variant, which forms dpre from dy and the relu mask of p.act in the producers and prefetches
-// the rows L2_AHEAD blocks ahead into L2; otherwise p.dpre is read as it is.  MASK (with FUSED): the relu mask comes from
-// the bits of p.mask instead of y.
-template <bool FUSED, bool MASK = false>
-__device__ __forceinline__ void dw_body(const ParamsW& p) {
+// DPRE: 0 dpre = p.dpre as it is (dw_tf32x3_kernel); 1 dpre from dy and the mask bits (linear_bwd_dw_mask_kernel);
+// 2 dpre from dy and y when p.act, else dy (linear_bwd_dw_kernel)
+template <int DPRE>
+__device__ __forceinline__ void dw_body(const ParamsW& p, const CUtensorMap* tm_dy, const CUtensorMap* tm_y,
+                                        const CUtensorMap* tm_x) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t sbase = s_u32(smem);
-    const uint32_t bar_full = sbase + SMEM_BARW, bar_empty = bar_full + 8 * WSTAGE;
-    const int nfB = p.Din >> 2;                   // float4 per row of X
+    const uint32_t bar_full = sbase + SMEM_BARW, bar_empty = bar_full + 8 * MAX_WSTAGES;
+    const uint32_t bar_bfull = bar_empty + 8 * MAX_WSTAGES, bar_bempty = bar_bfull + 16;
+    const bool with_y = DPRE == 2 && p.act;
+    const int x_at = (with_y ? 8 : 4) * BOX_BYTES, mask_at = x_at + 4 * BOX_BYTES;
+    const int stage_bytes = mask_at + 1024, ns = RINGW_BYTES / stage_bytes < MAX_WSTAGES ? RINGW_BYTES / stage_bytes : MAX_WSTAGES;
+    const int xboxes = p.Din >> 5;
     const int64_t r_begin = (int64_t)blockIdx.x * p.rows_per_cta;
     const int64_t r_end = (r_begin + p.rows_per_cta < p.M) ? r_begin + p.rows_per_cta : p.M;
     const int64_t nblk = (r_end > r_begin) ? (r_end - r_begin + 31) / 32 : 0;
 
     if (tid == 0) {
-        for (int s = 0; s < WSTAGE; ++s) { bar_init(bar_full + 8 * s, PRODUCERS); bar_init(bar_empty + 8 * s, CONSUMER_WARPS); }
+        for (int s = 0; s < MAX_WSTAGES; ++s) { bar_init(bar_full + 8 * s, 1); bar_init(bar_empty + 8 * s, CONSUMER_WARPS + 4); }
+        for (int s = 0; s < 2; ++s) { bar_init(bar_bfull + 8 * s, 4); bar_init(bar_bempty + 8 * s, CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // rows j >= Din of the X^T images are never written: zero them once
-    for (int i = tid; i < SMEM_BARW / 16; i += THREADS) reinterpret_cast<float4*>(smem)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = tid; i < 4 * KBLK_BYTES / 16; i += THREADS)
+        reinterpret_cast<float4*>(smem + SMEM_BIMG)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     fence_proxy_async();
     __syncthreads();
 
     if (warp < PRODUCERS / 32) {
-        // ---- producers: 32 rows of dPre (128 floats) and of X (Din floats) per stage, transposed + split + swizzled
-        const int rl = lane >> 2, fl = lane & 3;
-        // the 8 float4 this thread covers in row block blk of src (row stride ld floats, nf float4 per row)
-        auto load = [&](const float* src, int ld, int nf, int64_t blk, float4* v) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const int64_t r = r_begin + blk * 32 + rl + 8 * (q & 3);
-                const int f = 4 * (warp + 4 * (q >> 2)) + fl;
-                v[q] = (blk < nblk && r < r_end && f < nf) ? __ldg(reinterpret_cast<const float4*>(src + (size_t)r * ld) + f)
-                                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+        // ---- producers: thread 0 issues the boxes ns - 1 blocks ahead; the four warps transpose X into the B slots
+        int i_stage = 0;
+        uint32_t i_phase = 0;
+        int64_t i_blk = 0;
+        bool issuing = true;
+        auto issue = [&]() {
+            if (!issuing) return;
+            if (!bar_wait(bar_empty + 8 * i_stage, i_phase ^ 1, p.err)) { issuing = false; return; }
+            {
+                const uint32_t dst = sbase + i_stage * stage_bytes, full = bar_full + 8 * i_stage;
+                const int64_t r0 = r_begin + 32 * i_blk;
+                const uint32_t nr = (uint32_t)((r_end - r0 < 32) ? r_end - r0 : 32);
+                tma::mbar_expect_tx(full, (uint32_t)(((with_y ? 8 : 4) + xboxes) * BOX_BYTES) + (DPRE == 1 ? nr * 16 : 0u));
+                for (int b = 0; b < 4; ++b) tma::tensor_load_2d(dst + b * BOX_BYTES, tm_dy, 32 * b, (int)r0, full);
+                if (with_y)
+                    for (int b = 0; b < 4; ++b) tma::tensor_load_2d(dst + (4 + b) * BOX_BYTES, tm_y, 32 * b, (int)r0, full);
+                for (int b = 0; b < xboxes; ++b) tma::tensor_load_2d(dst + x_at + b * BOX_BYTES, tm_x, 32 * b, (int)r0, full);
+                if (DPRE == 1) tma::bulk_load(dst + mask_at, p.mask + (size_t)r0 * 4, nr * 16, full);
             }
+            if (++i_stage == ns) { i_stage = 0; i_phase ^= 1; }
+            ++i_blk;
         };
-        auto put1 = [&](unsigned char* big, int n, int k, float e) {
-            const int off = kmajor_off(n, k);
-            const float b = tf32_big(e);
-            *reinterpret_cast<float*>(big + off) = b;
-            *reinterpret_cast<float*>(big + KBLK_BYTES + off) = tf32_small(e, b);
-        };
-        auto put = [&](unsigned char* big, int n0, int k, float4 v) {
-            put1(big, n0, k, v.x); put1(big, n0 + 1, k, v.y); put1(big, n0 + 2, k, v.z); put1(big, n0 + 3, k, v.w);
-        };
-        auto stage_in = [&](int64_t blk, const float4* va, const float4* vb) {
-            const int stage = (int)(blk % WSTAGE);
-            if (!bar_wait(bar_empty + 8 * stage, (uint32_t)(((blk / WSTAGE) & 1) ^ 1), p.err)) return false;
-            unsigned char* st = smem + stage * STAGE_BYTES;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const int k = rl + 8 * (q & 3);
-                const int f = 4 * (warp + 4 * (q >> 2)) + fl;
-                put(st, 4 * f, k, va[q]);
-                if (f < nfB) put(st + 2 * KBLK_BYTES, 4 * f, k, vb[q]);
+        if (tid == 0)
+            for (int64_t n = 0; n < ns - 1 && n < nblk; ++n) issue();
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int64_t blk = 0; blk < nblk; ++blk) {
+            if (tid == 0 && blk + ns - 1 < nblk) issue();
+            const int slot = (int)(blk & 1);
+            if (!bar_wait(bar_full + 8 * stage, phase, p.err)) break;
+            if (!bar_wait(bar_bempty + 8 * slot, (uint32_t)(((blk >> 1) & 1) ^ 1), p.err)) break;
+            const unsigned char* sx = smem + stage * stage_bytes + x_at;
+            unsigned char* big = smem + SMEM_BIMG + slot * 2 * KBLK_BYTES;
+            // items (jb, q) = (32-column group of X, 4 rows k = 4 q .. 4 q + 3), spread over the warps
+            for (int item = warp; item < xboxes * 8; item += 4) {
+                const int j = 32 * (item >> 3) + lane, q = item & 7;
+                float4 v;
+                v.x = *reinterpret_cast<const float*>(sx + box_off(4 * q, j));
+                v.y = *reinterpret_cast<const float*>(sx + box_off(4 * q + 1, j));
+                v.z = *reinterpret_cast<const float*>(sx + box_off(4 * q + 2, j));
+                v.w = *reinterpret_cast<const float*>(sx + box_off(4 * q + 3, j));
+                const float4 b = make_float4(tf32_big(v.x), tf32_big(v.y), tf32_big(v.z), tf32_big(v.w));
+                const int off = kmajor_off(j, 4 * q);
+                *reinterpret_cast<float4*>(big + off) = b;
+                *reinterpret_cast<float4*>(big + KBLK_BYTES + off) = tf32_small(v, b);
             }
-            fence_proxy_async();
-            bar_arrive(bar_full + 8 * stage);
-            return true;
-        };
-        if constexpr (!FUSED) {
-            float4 va[8], vb[8], na[8], nb[8];
-            load(p.dpre, 128, 32, 0, va);
-            load(p.x, p.Din, nfB, 0, vb);
-            for (int64_t blk = 0; blk < nblk; ++blk) {
-                load(p.dpre, 128, 32, blk + 1, na);
-                load(p.x, p.Din, nfB, blk + 1, nb);
-                if (!stage_in(blk, va, vb)) break;
-#pragma unroll
-                for (int q = 0; q < 8; ++q) { va[q] = na[q]; vb[q] = nb[q]; }
-            }
-        } else if constexpr (MASK) {
-            // as below with the mask bits in place of y: the 4 columns 4 f .. 4 f + 3 of a thread's float4 f are bits
-            // 2 (f >> 1) and the next of words 2 (fl & 1) and 2 (fl & 1) + 1 of the row's mask (f & 1 == fl & 1), so
-            // the two float4 of one row (q and q + 4) share one 8 B load
-            float4 va[8], vb[8], na[8];
-            uint2 nm[4];
-            auto load_mask = [&](int64_t blk) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int64_t r = r_begin + blk * 32 + rl + 8 * q;
-                    nm[q] = (blk < nblk && r < r_end) ? __ldg(reinterpret_cast<const uint2*>(p.mask + (size_t)r * 4) + (fl & 1))
-                                                      : make_uint2(0u, 0u);
-                }
-            };
-            auto promote = [&]() {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const uint2 m = nm[q & 3];
-                    const int s = 4 * (warp + 4 * (q >> 2)) + 2 * (fl >> 1);
-                    va[q].x = (m.x >> s) & 1u ? na[q].x : 0.f; va[q].y = (m.x >> (s + 1)) & 1u ? na[q].y : 0.f;
-                    va[q].z = (m.y >> s) & 1u ? na[q].z : 0.f; va[q].w = (m.y >> (s + 1)) & 1u ? na[q].w : 0.f;
-                }
-            };
-            load(p.dpre, 128, 32, 0, na);
-            load_mask(0);
-            promote();
-            for (int64_t blk = 0; blk < nblk; ++blk) {
-                if (tid == 0 && blk + L2_AHEAD < nblk) {
-                    const int64_t ra = r_begin + 32 * (blk + L2_AHEAD), nr = (r_end - ra < 32) ? r_end - ra : 32;
-                    prefetch_l2(p.dpre + (size_t)ra * 128, (uint32_t)(nr * 512));
-                    prefetch_l2(p.x + (size_t)ra * p.Din, (uint32_t)(nr * p.Din * 4));
-                }
-                load(p.dpre, 128, 32, blk + 1, na);
-                load_mask(blk + 1);
-                load(p.x, p.Din, nfB, blk, vb);
-                if (!stage_in(blk, va, vb)) break;
-                promote();
-            }
-        } else {
-            // dy and y are loaded one block ahead into registers and the mask is applied when they are promoted; x is
-            // loaded when its block is staged, from L2, where it was prefetched L2_AHEAD blocks ahead (dy, y and x all one
-            // block ahead would not fit the registers)
-            float4 va[8], vb[8], na[8], nm[8];
-            auto promote = [&]() {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    va[q] = na[q];
-                    if (p.act) {
-                        va[q].x = nm[q].x > 0.f ? va[q].x : 0.f; va[q].y = nm[q].y > 0.f ? va[q].y : 0.f;
-                        va[q].z = nm[q].z > 0.f ? va[q].z : 0.f; va[q].w = nm[q].w > 0.f ? va[q].w : 0.f;
-                    }
-                }
-            };
-            load(p.dpre, 128, 32, 0, na);
-            if (p.act) load(p.act, 128, 32, 0, nm);
-            promote();
-            for (int64_t blk = 0; blk < nblk; ++blk) {
-                if (tid == 0 && blk + L2_AHEAD < nblk) {
-                    const int64_t ra = r_begin + 32 * (blk + L2_AHEAD), nr = (r_end - ra < 32) ? r_end - ra : 32;
-                    prefetch_l2(p.dpre + (size_t)ra * 128, (uint32_t)(nr * 512));
-                    if (p.act) prefetch_l2(p.act + (size_t)ra * 128, (uint32_t)(nr * 512));
-                    prefetch_l2(p.x + (size_t)ra * p.Din, (uint32_t)(nr * p.Din * 4));
-                }
-                load(p.dpre, 128, 32, blk + 1, na);
-                if (p.act) load(p.act, 128, 32, blk + 1, nm);
-                load(p.x, p.Din, nfB, blk, vb);
-                if (!stage_in(blk, va, vb)) break;
-                promote();
-            }
+            fence_proxy_async();                               // the image is read by the tensor core (async proxy)
+            __syncwarp();
+            if (lane == 0) { bar_arrive(bar_bfull + 8 * slot); bar_arrive(bar_empty + 8 * stage); }
+            if (++stage == ns) { stage = 0; phase ^= 1; }
         }
+        if (tid == 0) ring_drain(bar_full, ns, i_stage, i_phase, i_blk);
     } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
         // ---- consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of dW (M = 128), N = Din (padded to 128)
-        const int wg = (warp - PRODUCERS / 32) >> 2;
+        const int wg = (warp - PRODUCERS / 32) >> 2, g = lane >> 2, t = lane & 3;
+        const int i0 = wg * 64 + (warp & 3) * 16 + g;          // the thread's rows i0 and i0 + 8 of dW
+        // relu mask of (r, i0 + 8 h): bit 2 (i >> 3) + (i & 1) of word (i >> 1) & 3, the same word for both rows
+        const int mword = (i0 >> 1) & 3, mbit = 2 * (i0 >> 3) + (i0 & 1);
         float acc[64] = {}, sum[64];
+        uint32_t ab0[16], as0[16], ab1[16], as1[16];
 #pragma unroll
         for (int i = 0; i < 64; ++i) sum[i] = 0.f;
-        for (int64_t blk = 0; blk < nblk; ++blk) {
-            const int stage = (int)(blk % WSTAGE);
-            if (!bar_wait(bar_full + 8 * stage, (uint32_t)((blk / WSTAGE) & 1), p.err)) break;
-            const uint32_t a_big = sbase + stage * STAGE_BYTES + wg * 64 * 128, a_small = a_big + KBLK_BYTES;
-            const uint32_t b_big = sbase + stage * STAGE_BYTES + 2 * KBLK_BYTES, b_small = b_big + KBLK_BYTES;
-            mma_kblock(acc, acc, a_big, a_small, b_big, b_small, (blk % FLUSH) == 0);
+        int stage = 0;
+        uint32_t phase = 0;
+        int64_t blk = 0;
+        bool alive = true;
+        auto step = [&](uint32_t* ab, uint32_t* as) {
+            const int slot = (int)(blk & 1);
+            if (!bar_wait(bar_full + 8 * stage, phase, p.err)) { alive = false; return; }
+            const unsigned char* st = smem + stage * stage_bytes;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int kh = 0; kh < 2; ++kh) {
+                    const int r = 8 * j + t + 4 * kh;
+                    uint32_t m = 0;
+                    if constexpr (DPRE == 1) m = *reinterpret_cast<const uint32_t*>(st + mask_at + r * 16 + mword * 4);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int e = h + 2 * kh;               // fragment element: row i0 + 8 h, column r
+                        const int off = box_off(r, i0 + 8 * h);
+                        float v = *reinterpret_cast<const float*>(st + off);
+                        if constexpr (DPRE == 1) v = (m >> (mbit + 2 * h)) & 1u ? v : 0.f;
+                        if constexpr (DPRE == 2) {
+                            if (with_y) v = *reinterpret_cast<const float*>(st + 4 * BOX_BYTES + off) > 0.f ? v : 0.f;
+                        }
+                        const float b = tf32_big(v);
+                        ab[4 * j + e] = __float_as_uint(b);
+                        as[4 * j + e] = __float_as_uint(tf32_small(v, b));
+                    }
+                }
+            }
+            __syncwarp();
             if (lane == 0) bar_arrive(bar_empty + 8 * stage);
+            if (!bar_wait(bar_bfull + 8 * slot, (uint32_t)((blk >> 1) & 1), p.err)) { alive = false; return; }
+            const uint32_t b_big = sbase + SMEM_BIMG + slot * 2 * KBLK_BYTES;
+            fence_acc(acc);
+            mma_kblock_rs(acc, acc, ab, as, b_big, b_big + KBLK_BYTES, (blk % FLUSH) == 0);
+            wgmma_wait_1();                                     // block blk - 1 has retired: its B slot is free
+            if (lane == 0 && blk > 0) bar_arrive(bar_bempty + 8 * (slot ^ 1));
             if ((blk % FLUSH) == FLUSH - 1 || blk == nblk - 1) {
+                wgmma_wait_all();
+                fence_acc(acc);
 #pragma unroll
                 for (int i = 0; i < 64; ++i) sum[i] += acc[i];
             }
+            if (++stage == ns) { stage = 0; phase ^= 1; }
+            ++blk;
+        };
+        while (alive && blk < nblk) {
+            step(ab0, as0);
+            if (alive && blk < nblk) step(ab1, as1);
         }
+        wgmma_wait_all();
+        if (!alive) return;
         const int w4 = warp & 3;
-        const int i0 = wg * 64 + w4 * 16 + (lane >> 2);
+        const int i1 = wg * 64 + w4 * 16 + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
             const int c = 8 * j + 2 * (lane & 3);
             if (c >= p.Din) continue;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                float* prow = p.partial + ((size_t)blockIdx.x * 128 + i0 + 8 * h) * p.Din;
+                float* prow = p.partial + ((size_t)blockIdx.x * 128 + i1 + 8 * h) * p.Din;
                 *reinterpret_cast<float2*>(prow + c) = make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
             }
         }
     }
 }
 
-__global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(const ParamsW p) { dw_body<false>(p); }
-__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_kernel(const ParamsW p) { dw_body<true>(p); }
-__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_mask_kernel(const ParamsW p) { dw_body<true, true>(p); }
+#define GNNB_DW_PARAMS const ParamsW p, const __grid_constant__ CUtensorMap tm_dy, const __grid_constant__ CUtensorMap tm_y, \
+                       const __grid_constant__ CUtensorMap tm_x
+__global__ void __launch_bounds__(THREADS, 1) dw_tf32x3_kernel(GNNB_DW_PARAMS) { dw_body<0>(p, &tm_dy, &tm_y, &tm_x); }
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_kernel(GNNB_DW_PARAMS) { dw_body<2>(p, &tm_dy, &tm_y, &tm_x); }
+__global__ void __launch_bounds__(THREADS, 1) linear_bwd_dw_mask_kernel(GNNB_DW_PARAMS) { dw_body<1>(p, &tm_dy, &tm_y, &tm_x); }
+#undef GNNB_DW_PARAMS
 
 // dW[i] = sum of the n-float partials; with db: threads n .. n + 127 add the 128-float column-sum partials into db
 __global__ void dw_reduce_kernel(const float* __restrict__ partial, int nparts, int n, float* __restrict__ dW,
@@ -826,6 +917,34 @@ int linear_tf32x3(const float* x, const float* W, const float* bias, int relu, i
 }
 static int linear_launch(const float* x, const float* W, int64_t ldw, const float* bias, const float* addend, int relu,
                          int64_t M, int64_t K, int64_t Nout, float* y, uint32_t* mask, cudaStream_t st);
+
+// the tensor map of a row-major fp32 matrix (rows x cols, rows ld floats apart) in the ring kernels' boxes: 32 columns
+// (one K-block) x box_rows rows (tc::BM; 32 for the dW kernels' row blocks), SWIZZLE_128B.  Encoded per call on the host; it travels as a kernel parameter.
+static int kblock_map(CUtensorMap* m, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows = tc::BM) {
+    static const PFN_cuTensorMapEncodeTiled_v12000 encode = [] {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            fn = nullptr;
+        return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+    }();
+    if (!encode) GNNB_FAIL(GNNB_ECUDA, "the driver does not provide cuTensorMapEncodeTiled");
+    // a driver call needs the device's context current in this thread (an autograd worker may not have it yet)
+    int dev = 0;
+    GNNB_CUDA(cudaGetDevice(&dev));
+    GNNB_CUDA(cudaSetDevice(dev));
+    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
+    const cuuint32_t box[2] = {(cuuint32_t)tc::BK, (cuuint32_t)box_rows}, estride[2] = {1, 1};
+    const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estride,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) GNNB_FAIL(GNNB_ECUDA, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
+    return GNNB_OK;
+}
+// the ring kernels address rows by a 32-bit box coordinate
+constexpr int64_t RING_MAX_ROWS = (int64_t)INT32_MAX - tc::BM;
 // W rows `ldw` floats apart (a column block of a wider matrix); addend (M, Nout) added before the activation
 int linear_tf32x3_ex(const float* x, const float* W, int64_t ldw, const float* bias, const float* addend, int relu, int64_t M,
                      int64_t K, int64_t Nout, float* y, cudaStream_t st) {
@@ -844,7 +963,7 @@ static int linear_launch(const float* x, const float* W, int64_t ldw, const floa
     if (wide) {
         // (a handful of row tiles cannot fill the machine: the library GEMM takes those)
         if (K % 32 != 0 || K > 2048 || Nout % 128 != 0 || Nout > tcx::MAX_NOUT || ldw % 4 != 0 || ldw < K || M < 2048) return GNNB_EUNSUPPORTED;
-    } else if (K % 32 != 0 || Nout % 16 != 0 || Nout < 16 || ldw % 4 != 0 || ldw < K) {
+    } else if (K % 32 != 0 || Nout % 16 != 0 || Nout < 16 || ldw % 4 != 0 || ldw < K || M > RING_MAX_ROWS) {
         return GNNB_EUNSUPPORTED;
     }
     if (((uintptr_t)x & 15) || ((uintptr_t)W & 15) || ((uintptr_t)y & 15) || ((uintptr_t)addend & 15)) return GNNB_EUNSUPPORTED;
@@ -864,9 +983,14 @@ static int linear_launch(const float* x, const float* W, int64_t ldw, const floa
     const int nsm = s->nsm;
     const int64_t ntiles = ceil_div(M, tc::BM);
     const unsigned grid = (unsigned)(ntiles < nsm ? ntiles : nsm);
-    if (wide) tcx::linear_wide_tf32x3_kernel<<<grid, tc::THREADS, tcx::SMEM_TOTAL_X, st>>>(p);
-    else if (mask) tc::linear_relu_mask_kernel<<<grid, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
-    else tc::linear_tf32x3_kernel<<<grid, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
+    if (wide) {
+        tcx::linear_wide_tf32x3_kernel<<<grid, tc::THREADS, tcx::SMEM_TOTAL_X, st>>>(p);
+    } else {
+        CUtensorMap tm_x;
+        GNNB_TRY(kblock_map(&tm_x, x, M, K, K));
+        if (mask) tc::linear_relu_mask_kernel<<<grid, tc::THREADS, tc::SMEM_TOTAL, st>>>(p, tm_x);
+        else tc::linear_tf32x3_kernel<<<grid, tc::THREADS, tc::SMEM_TOTAL, st>>>(p, tm_x);
+    }
     GNNB_LAUNCHED();
     return GNNB_OK;
 }
@@ -874,7 +998,7 @@ static int linear_launch(const float* x, const float* W, int64_t ldw, const floa
 // dW (Dout = 128, Din in {32, 64, 96, 128}); GNNB_EUNSUPPORTED for anything else
 int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t Dout, float* dW, cudaStream_t st) {
     if (!g_tc_enabled) return GNNB_EUNSUPPORTED;
-    if (Dout != 128 || Din % 32 != 0 || Din > 128 || Din < 32) return GNNB_EUNSUPPORTED;
+    if (Dout != 128 || Din % 32 != 0 || Din > 128 || Din < 32 || M > RING_MAX_ROWS) return GNNB_EUNSUPPORTED;
     if (((uintptr_t)dpre & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dW & 15)) return GNNB_EUNSUPPORTED;
     DeviceState* s = nullptr;
     GNNB_TRY(device_state(&s));
@@ -888,7 +1012,10 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
     rpc = ceil_div(rpc, 32) * 32;
     p.rows_per_cta = rpc;
     const int grid = (int)ceil_div(M, rpc);
-    tcw::dw_tf32x3_kernel<<<grid, tc::THREADS, tcw::SMEM_TOTALW, st>>>(p);
+    CUtensorMap tm_dy, tm_x;
+    GNNB_TRY(kblock_map(&tm_dy, dpre, M, 128, 128, 32));
+    GNNB_TRY(kblock_map(&tm_x, x, M, Din, Din, 32));
+    tcw::dw_tf32x3_kernel<<<grid, tc::THREADS, tcw::SMEM_TOTALW, st>>>(p, tm_dy, tm_dy, tm_x);
     GNNB_LAUNCHED();
     const int n = (int)(128 * Din);
     tcw::dw_reduce_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(partial, grid, n, dW);
@@ -904,7 +1031,7 @@ int dw_tf32x3(const float* dpre, const float* x, int64_t M, int64_t Din, int64_t
 int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, const float* x, const float* W, int64_t M,
                       int64_t Din, float* dx, float* dW, float* db, cudaStream_t st) {
     if (!g_tc_enabled) return GNNB_EUNSUPPORTED;
-    if (Din % 32 != 0 || Din > 128 || Din < 32 || M <= 0) return GNNB_EUNSUPPORTED;
+    if (Din % 32 != 0 || Din > 128 || Din < 32 || M <= 0 || M > RING_MAX_ROWS) return GNNB_EUNSUPPORTED;
     if (((uintptr_t)dy & 15) || ((uintptr_t)y & 15) || ((uintptr_t)x & 15) || ((uintptr_t)dx & 15) || ((uintptr_t)mask & 15))
         return GNNB_EUNSUPPORTED;
     DeviceState* s = nullptr;
@@ -920,8 +1047,11 @@ int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, con
     p.mask = const_cast<uint32_t*>(mask);
     const int64_t ntiles = ceil_div(M, tc::BM);
     const int grid_dx = (int)(ntiles < nsm ? ntiles : nsm);
-    if (mask) tc::linear_bwd_dx_mask_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
-    else tc::linear_bwd_dx_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p);
+    CUtensorMap tm_dy, tm_y;
+    GNNB_TRY(kblock_map(&tm_dy, dy, M, 128, 128));
+    GNNB_TRY(kblock_map(&tm_y, (y && !mask) ? y : dy, M, 128, 128));
+    if (mask) tc::linear_bwd_dx_mask_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p, tm_dy, tm_y);
+    else tc::linear_bwd_dx_kernel<<<grid_dx, tc::THREADS, tc::SMEM_TOTAL, st>>>(p, tm_dy, tm_y);
     GNNB_LAUNCHED();
     // dW: the split-K partition of dw_tf32x3
     tcw::ParamsW pw;
@@ -929,8 +1059,12 @@ int linear_bwd_tf32x3(const float* dy, const float* y, const uint32_t* mask, con
     const int64_t rpc = ceil_div(ceil_div(M, nsm), 32) * 32;
     pw.rows_per_cta = rpc;
     const int grid_dw = (int)ceil_div(M, rpc);
-    if (mask) tcw::linear_bwd_dw_mask_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw);
-    else tcw::linear_bwd_dw_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw);
+    CUtensorMap tw_dy, tw_y, tw_x;
+    GNNB_TRY(kblock_map(&tw_dy, dy, M, 128, 128, 32));
+    GNNB_TRY(kblock_map(&tw_y, (y && !mask) ? y : dy, M, 128, 128, 32));
+    GNNB_TRY(kblock_map(&tw_x, x, M, Din, Din, 32));
+    if (mask) tcw::linear_bwd_dw_mask_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw, tw_dy, tw_y, tw_x);
+    else tcw::linear_bwd_dw_kernel<<<grid_dw, tc::THREADS, tcw::SMEM_TOTALW, st>>>(pw, tw_dy, tw_y, tw_x);
     GNNB_LAUNCHED();
     const int n = (int)(128 * Din);
     tcw::dw_reduce_kernel<<<(unsigned)ceil_div(n + 128, 256), 256, 0, st>>>(partial, grid_dw, n, dW, colsum, grid_dx * 4, db);

@@ -1,5 +1,6 @@
-// tma.cuh — device-side wrappers of the TMA instructions this library issues: mbarrier transaction counting and the
-// 1-D bulk copy cp.async.bulk (no tensor map) from global into shared memory.
+// tma.cuh — device-side wrappers of the TMA instructions this library issues: mbarrier transaction counting, the 1-D
+// bulk copy cp.async.bulk (no tensor map) and the 2-D tiled copy cp.async.bulk.tensor (host-encoded tensor map) from
+// global into shared memory.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -36,6 +37,13 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// 2-D tiled copy (cp.async.bulk.tensor) of the box at element coordinates (x0 inner, x1 outer) of the tensor map `map`
+// (a __grid_constant__ kernel parameter) into shared `dst`, completion counted on `bar`.  Elements outside the tensor
+// arrive as zeros and the whole box counts towards the transaction bytes.
+__device__ __forceinline__ void tensor_load_2d(uint32_t dst, const void* map, int x0, int x1, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"(map), "r"(x0), "r"(x1), "r"(bar) : "memory");
 }
 
 }  // namespace tma
