@@ -48,6 +48,10 @@ struct GatParams {
     float slope;
     const int4* __restrict__ items;   // lean kernels: the plan's work items {e_begin, e_end, slot, 0} (seglean.cu)
     int32_t n_items;
+    // HALO instances (a node-partitioned shard): gathered nodes >= split read their row from x2 + (id - split)*D instead
+    // of the one base (fwd: Wx, bwd: dout).  Appended last, so the HALO = 0 instances see the fields above where they were.
+    int32_t split;
+    const float* __restrict__ x2;
 };
 
 template <int VEC> struct GV;
@@ -75,8 +79,8 @@ __device__ __forceinline__ void gst(float4* p, float4 v) { *p = v; }
 __device__ __forceinline__ void gst(float* p, float v) { *p = v; }
 
 // ------------------------------------------------------------------------------------------------ forward
-// partial slot layout (floats): [acc: D][M: H][S: H]
-template <int VEC, int K>
+// partial slot layout (floats): [acc: D][M: H][S: H].  HALO: see GatParams::x2 (er stays one array over [local | halo]).
+template <int VEC, int K, int HALO>
 __global__ void __launch_bounds__(128, (K == 1 ? 8 : 1)) gat_fwd_kernel(const GatParams p) {
     using V = typename GV<VEC>::T;
     constexpr int U = (K >= 4) ? 2 : 4;
@@ -96,6 +100,7 @@ __global__ void __launch_bounds__(128, (K == 1 ? 8 : 1)) gat_fwd_kernel(const Ga
     }
     const ChunkBounds b = chunk_bounds(p.rowptr, p.row, k, p.chunk, p.E, p.nchunks);
     const bool has_work = b.e_begin < b.e_end;
+    const float* const x2s = HALO ? p.x2 - (int64_t)p.split * p.D : nullptr;   // halo base shifted: row id indexes it
 
     V acc[K]; float M[K], S[K], eli[K];
 #pragma unroll
@@ -148,10 +153,15 @@ __global__ void __launch_bounds__(128, (K == 1 ? 8 : 1)) gat_fwd_kernel(const Ga
             for (int u = 0; u < U; ++u) {
                 const int cj = __shfl_sync(FULL, c_l, (j0 + u) & 31);
                 const bool valid = (j0 + u) < nb;
+                const bool second = HALO != 0 && cj >= p.split;
 #pragma unroll
                 for (int i = 0; i < K; ++i) {
                     const bool ok = valid && fact[i];
-                    v[u][i] = ok ? gld(reinterpret_cast<const V*>(p.Wx + (size_t)cj * p.D + foff[i])) : gzero<V>();
+                    if constexpr (HALO == 0) {
+                        v[u][i] = ok ? gld(reinterpret_cast<const V*>(p.Wx + (size_t)cj * p.D + foff[i])) : gzero<V>();
+                    } else {
+                        v[u][i] = ok ? gld(reinterpret_cast<const V*>((second ? x2s : p.Wx) + (size_t)cj * p.D + foff[i])) : gzero<V>();
+                    }
                     ev[u][i] = ok ? __ldg(p.er + (size_t)cj * p.H + head[i]) : 0.f;
                 }
             }
@@ -198,7 +208,8 @@ __global__ void __launch_bounds__(128, (K == 1 ? 8 : 1)) gat_fwd_kernel(const Ga
 // el[target] and er[source]), parked in shared memory and read back by head — the old kernel recomputed every logit on
 // every lane of the head and re-read the index arrays for each 128-float tile of the row.  One warp covers the whole
 // row of KV*128 floats.  Partial slots keep the layout [acc: D][M: H][S: H], so gat_fwd_fixup_kernel is shared.
-template <int KV>
+// HALO 1: gathered nodes >= split read x2 (seg_lean_kernel's two-base load).
+template <int KV, int HALO>
 __global__ void __launch_bounds__(256, 2) gat_fwd_lean_kernel(const GatParams p) {
     constexpr unsigned FULL = 0xffffffffu;
     constexpr int U = 8 / KV;
@@ -220,6 +231,7 @@ __global__ void __launch_bounds__(256, 2) gat_fwd_lean_kernel(const GatParams p)
         lead[i] = (f % p.C) == 0;
     }
     const float* const xl = p.Wx + lane * 4;
+    const float* const x2l = HALO ? p.x2 + lane * 4 - (int64_t)p.split * STRIDE : nullptr;
     float4 acc[KV]; float M[KV], S[KV];
 #pragma unroll
     for (int i = 0; i < KV; ++i) { acc[i] = gzero4(); M[i] = -CUDART_INF_F; S[i] = 0.f; }
@@ -259,7 +271,8 @@ __global__ void __launch_bounds__(256, 2) gat_fwd_lean_kernel(const GatParams p)
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 const int cj = __shfl_sync(FULL, c_l, j0 + u);
-                const float* xr = xl + (int64_t)cj * STRIDE;
+                const bool second = HALO != 0 && cj >= p.split;
+                const float* xr = (second ? x2l : xl) + (int64_t)cj * STRIDE;
                 if ((vmask >> (j0 + u)) & 1u) {
 #pragma unroll
                     for (int i = 0; i < KV; ++i) v[u][i] = __ldg(reinterpret_cast<const float4*>(xr + i * 128));
@@ -394,7 +407,9 @@ __global__ void __launch_bounds__(256) gat_tnode_kernel(const float* __restrict_
 
 // ----------------------------------------------------------------------------------------------- backward
 // CSR-by-source: row j = source node; col = target i.  partial slot layout: [acc: D][der: H]
-template <int VEC, int K>
+// (on a shard: the forward CSR of the backward shard, whose rows are the owned sources and whose gathered nodes are the
+// targets in [local | halo]; HALO 1 reads the dout rows of targets >= split from x2, el / M / S / T stay one array each)
+template <int VEC, int K, int HALO>
 __global__ void __launch_bounds__(128, (K == 1 ? 5 : 1)) gat_bwd_kernel(const GatParams p) {
     using V = typename GV<VEC>::T;
     constexpr int U = (K >= 4) ? 2 : 4;
@@ -415,6 +430,7 @@ __global__ void __launch_bounds__(128, (K == 1 ? 5 : 1)) gat_bwd_kernel(const Ga
     }
     const ChunkBounds b = chunk_bounds(p.rowptr, p.row, k, p.chunk, p.E, p.nchunks);
     const bool has_work = b.e_begin < b.e_end;
+    const float* const x2s = HALO ? p.x2 - (int64_t)p.split * p.D : nullptr;   // halo base shifted: row id indexes it
 
     V acc[K], wxj[K]; float dacc[K], erj[K];
 #pragma unroll
@@ -463,11 +479,16 @@ __global__ void __launch_bounds__(128, (K == 1 ? 5 : 1)) gat_bwd_kernel(const Ga
             for (int u = 0; u < U; ++u) {
                 const int ci = __shfl_sync(FULL, c_l, (j0 + u) & 31);
                 const bool valid = (j0 + u) < nb;
+                const bool second = HALO != 0 && ci >= p.split;
 #pragma unroll
                 for (int i = 0; i < K; ++i) {
                     const bool ok = valid && fact[i];
                     const size_t hq = (size_t)ci * p.H + head[i];
-                    v[u][i] = ok ? gld(reinterpret_cast<const V*>(p.dout + (size_t)ci * p.D + foff[i])) : gzero<V>();
+                    if constexpr (HALO == 0) {
+                        v[u][i] = ok ? gld(reinterpret_cast<const V*>(p.dout + (size_t)ci * p.D + foff[i])) : gzero<V>();
+                    } else {
+                        v[u][i] = ok ? gld(reinterpret_cast<const V*>((second ? x2s : p.dout) + (size_t)ci * p.D + foff[i])) : gzero<V>();
+                    }
                     eli[u][i] = ok ? __ldg(p.el + hq) : 0.f;
                     Mi[u][i] = ok ? __ldg(p.smax + hq) : 0.f;
                     Si[u][i] = ok ? __ldg(p.ssum + hq) : 1.f;
@@ -519,7 +540,8 @@ __global__ void __launch_bounds__(128, (K == 1 ? 5 : 1)) gat_bwd_kernel(const Ga
 // The source's own Wx row is read beside every gathered dout row (an L1 hit after the row's first edge) instead of being
 // loaded at the row change, where the in-order warp sat out a full memory latency every ~11 edges.
 // Partial slots keep the layout [acc: D][der: H] of gat_bwd_fixup_kernel.  C <= 128 (a head never spans two slices).
-template <int KV>
+// HALO 1: the dout rows of gathered targets >= split come from x2.
+template <int KV, int HALO>
 __global__ void __launch_bounds__(256, 2) gat_bwd_lean_kernel(const GatParams p) {
     constexpr unsigned FULL = 0xffffffffu;
     constexpr int U = (KV >= 4) ? 2 : (KV == 2 ? 2 : 4);
@@ -544,6 +566,7 @@ __global__ void __launch_bounds__(256, 2) gat_bwd_lean_kernel(const GatParams p)
         lead[i] = (f % p.C) == 0;
     }
     const float* const dl = p.dout + lane * 4;
+    const float* const d2l = HALO ? p.x2 + lane * 4 - (int64_t)p.split * STRIDE : nullptr;
     const float* const wl = p.Wx + lane * 4;
     float4 acc[KV]; float dacc[KV];
 #pragma unroll
@@ -589,7 +612,8 @@ __global__ void __launch_bounds__(256, 2) gat_bwd_lean_kernel(const GatParams p)
             for (int u = 0; u < U; ++u) {
                 const int ci = __shfl_sync(FULL, c_l, j0 + u);
                 const int rj = __shfl_sync(FULL, r_l, j0 + u);
-                const float* dr = dl + (int64_t)ci * STRIDE;
+                const bool second = HALO != 0 && ci >= p.split;
+                const float* dr = (second ? d2l : dl) + (int64_t)ci * STRIDE;
                 const float* wr = wl + (int64_t)rj * STRIDE;
                 if ((vmask >> (j0 + u)) & 1u) {
 #pragma unroll
@@ -691,27 +715,50 @@ static bool gat_shape(int64_t C, int64_t H, const void* a, const void* b, int* v
 using namespace gnnb;
 static inline unsigned nblk(int64_t n) { return (unsigned)ceil_div(n, 256); }
 
-#define GAT_DISPATCH(KERNEL, vec, kk, grid, st, p)                                            \
+#define GAT_DISPATCH(KERNEL, HALO, vec, kk, grid, st, p)                                      \
     do {                                                                                      \
-        if (vec == 4) KERNEL<4, 1><<<grid, 128, 0, st>>>(p);                                  \
-        else if (kk == 1) KERNEL<1, 1><<<grid, 128, 0, st>>>(p);                              \
-        else if (kk == 2) KERNEL<1, 2><<<grid, 128, 0, st>>>(p);                              \
-        else KERNEL<1, 4><<<grid, 128, 0, st>>>(p);                                           \
+        if (vec == 4) KERNEL<4, 1, HALO><<<grid, 128, 0, st>>>(p);                            \
+        else if (kk == 1) KERNEL<1, 1, HALO><<<grid, 128, 0, st>>>(p);                        \
+        else if (kk == 2) KERNEL<1, 2, HALO><<<grid, 128, 0, st>>>(p);                        \
+        else KERNEL<1, 4, HALO><<<grid, 128, 0, st>>>(p);                                     \
     } while (0)
 
-extern "C" {
+namespace {
 
-int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const float* er, int64_t C, int64_t H,
-                       float slope, float* out, float* alpha, float* seg_max, float* seg_sum, void* stream) {
-    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
-    if (C <= 0 || H <= 0) GNNB_FAIL(GNNB_ESIZE, "C and H must be positive");
-    if (!Wx || !el || !er || !out || !seg_max || !seg_sum) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
-    int vec, kk;
-    if (!gat_shape(C, H, Wx, out, &vec, &kk))
-        GNNB_FAIL(GNNB_EUNSUPPORTED, "fused GAT needs C/4 a power of two <= 32 with 16 B-aligned Wx / out (any number of heads), or C a "
-                                     "power of two <= 32 with C*H <= 128; use the generic apply_edges/softmax_edge_neighbors/"
-                                     "aggregate_neighbors composition");
-    cudaStream_t st = (cudaStream_t)stream;
+template <int HALO>
+int gat_fwd_lean(const GatParams& p, int64_t D, size_t smem, cudaStream_t st) {
+    const unsigned blocks = (unsigned)ceil_div(p.n_items, 8);
+    if (smem > 48 * 1024) {
+        GNNB_CUDA(cudaFuncSetAttribute(gat_fwd_lean_kernel<1, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        GNNB_CUDA(cudaFuncSetAttribute(gat_fwd_lean_kernel<2, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        GNNB_CUDA(cudaFuncSetAttribute(gat_fwd_lean_kernel<4, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    if (D == 128) gat_fwd_lean_kernel<1, HALO><<<blocks, 256, smem, st>>>(p);
+    else if (D == 256) gat_fwd_lean_kernel<2, HALO><<<blocks, 256, smem, st>>>(p);
+    else gat_fwd_lean_kernel<4, HALO><<<blocks, 256, smem, st>>>(p);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
+template <int HALO>
+int gat_bwd_lean(const GatParams& p, int64_t D, size_t smem, cudaStream_t st) {
+    const unsigned blocks = (unsigned)ceil_div(p.n_items, 8);
+    if (smem > 48 * 1024) {
+        GNNB_CUDA(cudaFuncSetAttribute(gat_bwd_lean_kernel<1, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        GNNB_CUDA(cudaFuncSetAttribute(gat_bwd_lean_kernel<2, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        GNNB_CUDA(cudaFuncSetAttribute(gat_bwd_lean_kernel<4, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    if (D == 128) gat_bwd_lean_kernel<1, HALO><<<blocks, 256, smem, st>>>(p);
+    else if (D == 256) gat_bwd_lean_kernel<2, HALO><<<blocks, 256, smem, st>>>(p);
+    else gat_bwd_lean_kernel<4, HALO><<<blocks, 256, smem, st>>>(p);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
+// The forward pass over g's by-target CSR, the one launch path of gnnb_gat_aggregate (x2 = NULL) and of
+// gnnb_gat_aggregate_halo (gathered nodes >= split read x2): out, seg_max, seg_sum over the CSR's rows.
+int gat_forward(gnnb_graph* g, const float* Wx, const float* x2, int64_t split, const float* el, const float* er, int64_t C,
+                int64_t H, float slope, float* out, float* seg_max, float* seg_sum, int vec, int kk, cudaStream_t st) {
     GNNB_TRY(ensure_csr(g, false, st));
     const Csr& c = g->by_dst;
     const int64_t D = C * H;
@@ -727,6 +774,8 @@ int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const f
     p.Wx = Wx; p.el = el; p.er = er; p.out = out; p.stat_a = seg_max; p.stat_b = seg_sum;
     p.D = D; p.C = (int32_t)C; p.H = (int32_t)H; p.E = (int32_t)g->E; p.nrows = c.nrows; p.chunk = g->chunk;
     p.nchunks = (int32_t)ceil_div(g->E, g->chunk); p.fill = 1; p.slope = slope;
+    p.x2 = x2; p.split = (int32_t)split;
+    const bool halo = x2 != nullptr;
     if (c.n_long > 0) {
         GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * p.nchunks * (D + 2 * H + 4)));
         p.ws = g->ws;
@@ -739,20 +788,12 @@ int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const f
             gat_fill_empty_kernel<<<(unsigned)ceil_div((int64_t)c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, out, D, seg_max, seg_sum, (int)H);
             GNNB_LAUNCHED();
         }
-        const unsigned blocks = (unsigned)ceil_div(c.n_items, 8);
         const size_t smem = sizeof(float) * 8 * 32 * (size_t)H;
-        if (smem > 48 * 1024) {
-            GNNB_CUDA(cudaFuncSetAttribute(gat_fwd_lean_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            GNNB_CUDA(cudaFuncSetAttribute(gat_fwd_lean_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            GNNB_CUDA(cudaFuncSetAttribute(gat_fwd_lean_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        }
-        if (D == 128) gat_fwd_lean_kernel<1><<<blocks, 256, smem, st>>>(p);
-        else if (D == 256) gat_fwd_lean_kernel<2><<<blocks, 256, smem, st>>>(p);
-        else gat_fwd_lean_kernel<4><<<blocks, 256, smem, st>>>(p);
-        GNNB_LAUNCHED();
+        GNNB_TRY(halo ? gat_fwd_lean<1>(p, D, smem, st) : gat_fwd_lean<0>(p, D, smem, st));
     } else {
         const dim3 grid((unsigned)ceil_div(p.nchunks, 4), (unsigned)ceil_div(D, (int64_t)32 * vec * kk));
-        GAT_DISPATCH(gat_fwd_kernel, vec, kk, grid, st, p);
+        if (halo) GAT_DISPATCH(gat_fwd_kernel, 1, vec, kk, grid, st, p);
+        else GAT_DISPATCH(gat_fwd_kernel, 0, vec, kk, grid, st, p);
         GNNB_LAUNCHED();
     }
     if (c.n_long > 0) {
@@ -761,12 +802,111 @@ int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const f
         else gat_fwd_fixup_kernel<1><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
         GNNB_LAUNCHED();
     }
-    if (alpha) {
+    return GNNB_OK;
+}
+
+// The pullback pass over a CSR `c` of g whose rows are the sources j and whose gathered nodes are the targets i: the
+// by-source CSR of a graph (gnnb_gat_aggregate_bwd, x2 = NULL) or the by-target CSR of a backward shard
+// (gnnb_gat_aggregate_bwd_halo).  Needs E > 0.  Writes dWx and der over c's rows, dz (E, H) in g's COO order.
+int gat_backward(gnnb_graph* g, const Csr& c, const float* Wx, const float* er, const float* dout, const float* x2,
+                 int64_t split, const float* el, const float* seg_max, const float* seg_sum, const float* T, int64_t C,
+                 int64_t H, float slope, float* dWx, float* der, float* dz, int vec, int kk, cudaStream_t st) {
+    const int64_t D = C * H;
+    GatParams p = {};
+    p.rowptr = c.rowptr; p.col = c.col; p.row = c.row; p.eid = c.eid;
+    p.Wx = Wx; p.el = el; p.er = er; p.smax = seg_max; p.ssum = seg_sum; p.tnode = T; p.dout = dout;
+    p.out = dWx; p.stat_a = der; p.dz = dz;
+    p.D = D; p.C = (int32_t)C; p.H = (int32_t)H; p.E = (int32_t)g->E; p.nrows = c.nrows; p.chunk = g->chunk;
+    p.nchunks = (int32_t)ceil_div(g->E, g->chunk); p.fill = 1; p.slope = slope;
+    p.x2 = x2; p.split = (int32_t)split;
+    const bool halo = x2 != nullptr;
+    if (c.n_long > 0) {
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * p.nchunks * (D + H + 4)));
+        p.ws = g->ws;
+    }
+    const bool lean = !g_reference_kernels && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && C <= 128 && H <= 64;
+    if (lean) {
+        GNNB_TRY(ensure_items(g, c, st));
+        p.items = reinterpret_cast<const int4*>(c.items); p.n_items = c.n_items;
+        if (c.n_empty > 0) {
+            gat_fill_empty_kernel<<<(unsigned)ceil_div((int64_t)c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, dWx, D, der, nullptr, (int)H);
+            GNNB_LAUNCHED();
+        }
+        const size_t smem = sizeof(float) * 8 * 3 * 32 * (size_t)H;
+        GNNB_TRY(halo ? gat_bwd_lean<1>(p, D, smem, st) : gat_bwd_lean<0>(p, D, smem, st));
+    } else {
+        const dim3 grid((unsigned)ceil_div(p.nchunks, 4), (unsigned)ceil_div(D, (int64_t)32 * vec * kk));
+        if (halo) GAT_DISPATCH(gat_bwd_kernel, 1, vec, kk, grid, st, p);
+        else GAT_DISPATCH(gat_bwd_kernel, 0, vec, kk, grid, st, p);
+        GNNB_LAUNCHED();
+    }
+    if (c.n_long > 0) {
+        const unsigned fb = nblk((int64_t)c.n_long * (D / vec));
+        if (vec == 4) gat_bwd_fixup_kernel<4><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
+        else gat_bwd_fixup_kernel<1><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
+        GNNB_LAUNCHED();
+    }
+    return GNNB_OK;
+}
+
+int gat_tnode(const float* dout, const float* out_fwd, int64_t n, int64_t C, int64_t H, int vec, float* T, cudaStream_t st) {
+    const unsigned tb = nblk(n * 32);
+    if (vec == 4) gat_tnode_kernel<4><<<tb, 256, 0, st>>>(dout, out_fwd, n, C * H, (int)C, (int)H, T);
+    else gat_tnode_kernel<1><<<tb, 256, 0, st>>>(dout, out_fwd, n, C * H, (int)C, (int)H, T);
+    GNNB_LAUNCHED();
+    return GNNB_OK;
+}
+
+// the two gathered bases of a halo entry: the local one, and the halo one only when some gathered node lives there
+// (a shard without halo rows takes the HALO = 0 instances); no local rows at all: the halo base alone, split 0
+void gat_bases(const float* local, const float* halo, int64_t n_local, int64_t n_src, const float** x, const float** x2) {
+    *x = local;
+    *x2 = n_local < n_src ? halo : nullptr;
+    if (!local) { *x = halo; *x2 = nullptr; }
+}
+
+}  // namespace
+
+extern "C" {
+
+int gnnb_gat_aggregate(gnnb_graph_t g, const float* Wx, const float* el, const float* er, int64_t C, int64_t H,
+                       float slope, float* out, float* alpha, float* seg_max, float* seg_sum, void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (C <= 0 || H <= 0) GNNB_FAIL(GNNB_ESIZE, "C and H must be positive");
+    if (!Wx || !el || !er || !out || !seg_max || !seg_sum) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    int vec, kk;
+    if (!gat_shape(C, H, Wx, out, &vec, &kk))
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "fused GAT needs C/4 a power of two <= 32 with 16 B-aligned Wx / out (any number of heads), or C a "
+                                     "power of two <= 32 with C*H <= 128; use the generic apply_edges/softmax_edge_neighbors/"
+                                     "aggregate_neighbors composition");
+    cudaStream_t st = (cudaStream_t)stream;
+    GNNB_TRY(gat_forward(g, Wx, nullptr, 0, el, er, C, H, slope, out, seg_max, seg_sum, vec, kk, st));
+    if (alpha && g->by_dst.nrows > 0 && g->E > 0) {
         gat_alpha_kernel<<<nblk(g->E * H), 256, 0, st>>>(g->coo_src, g->coo_dst, g->E, (int)H, el, er, seg_max, seg_sum,
                                                           slope, alpha);
         GNNB_LAUNCHED();
     }
     return GNNB_OK;
+}
+
+int gnnb_gat_aggregate_halo(gnnb_graph_t g, const float* Wx_local, const float* Wx_halo, int64_t n_local, const float* el,
+                            const float* er, int64_t C, int64_t H, float slope, float* out, float* seg_max, float* seg_sum,
+                            void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (C <= 0 || H <= 0) GNNB_FAIL(GNNB_ESIZE, "C and H must be positive");
+    if (n_local < 0 || n_local > g->n_src) GNNB_FAIL(GNNB_ESIZE, "n_local must be in [0, num_src]");
+    if (g->n_dst == 0) return GNNB_OK;   // a rank that owns no node: no row to write, the outputs may be NULL
+    if (!el || !out || !seg_max || !seg_sum || (g->E > 0 && !er)) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (n_local > 0 && !Wx_local) GNNB_FAIL(GNNB_EINVAL, "Wx_local is NULL");
+    if (n_local < g->n_src && !Wx_halo) GNNB_FAIL(GNNB_EINVAL, "Wx_halo is NULL but the shard has halo sources");
+    const float *x, *x2;
+    gat_bases(Wx_local, Wx_halo, n_local, g->n_src, &x, &x2);
+    int vec, kk;
+    const void* both = reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x2));
+    if (!gat_shape(C, H, both, out, &vec, &kk))     // `both`: the vector path needs each gathered base 16 B-aligned
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "fused GAT needs C/4 a power of two <= 32 with 16 B-aligned Wx_local / Wx_halo / out, or C a "
+                                     "power of two <= 32 with C*H <= 128");
+    return gat_forward(g, x, x2, n_local, el, er, C, H, slope, out, seg_max, seg_sum, vec, kk, (cudaStream_t)stream);
 }
 
 int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, const float* er, const float* seg_max,
@@ -781,7 +921,6 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
         GNNB_FAIL(GNNB_EUNSUPPORTED, "fused GAT pullback: unsupported (C,H) or unaligned pointers");
     cudaStream_t st = (cudaStream_t)stream;
     GNNB_TRY(ensure_csr(g, true, st));
-    const Csr& c = g->by_src;
     const int64_t D = C * H;
     const int64_t n_dst = g->n_dst, n_src = g->n_src;
     if (n_src > 0 && g->E == 0) {
@@ -796,54 +935,50 @@ int gnnb_gat_aggregate_bwd(gnnb_graph_t g, const float* Wx, const float* el, con
     GNNB_TRY(grow_buffer(&g->ws2, &g->ws2_bytes, sizeof(float) * ((size_t)n_dst * H + (size_t)g->E * H)));
     float* T = g->ws2;
     float* dz = g->ws2 + (size_t)n_dst * H;
-    {
-        const unsigned tb = nblk(n_dst * 32);
-        if (vec == 4) gat_tnode_kernel<4><<<tb, 256, 0, st>>>(dout, out_fwd, n_dst, D, (int)C, (int)H, T);
-        else gat_tnode_kernel<1><<<tb, 256, 0, st>>>(dout, out_fwd, n_dst, D, (int)C, (int)H, T);
-        GNNB_LAUNCHED();
-    }
-    GatParams p = {};
-    p.rowptr = c.rowptr; p.col = c.col; p.row = c.row; p.eid = c.eid;
-    p.Wx = Wx; p.el = el; p.er = er; p.smax = seg_max; p.ssum = seg_sum; p.tnode = T; p.dout = dout;
-    p.out = dWx; p.stat_a = der; p.dz = dz;
-    p.D = D; p.C = (int32_t)C; p.H = (int32_t)H; p.E = (int32_t)g->E; p.nrows = c.nrows; p.chunk = g->chunk;
-    p.nchunks = (int32_t)ceil_div(g->E, g->chunk); p.fill = 1; p.slope = slope;
-    if (c.n_long > 0) {
-        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * p.nchunks * (D + H + 4)));
-        p.ws = g->ws;
-    }
-    const bool lean = !g_reference_kernels && vec == 4 && (D == 128 || D == 256 || D == 512) && (C & (C - 1)) == 0 && C <= 128 && H <= 64;
-    if (lean) {
-        GNNB_TRY(ensure_items(g, c, st));
-        p.items = reinterpret_cast<const int4*>(c.items); p.n_items = c.n_items;
-        if (c.n_empty > 0) {
-            gat_fill_empty_kernel<<<(unsigned)ceil_div((int64_t)c.nrows, 256), 256, 0, st>>>(c.rowptr, c.nrows, dWx, D, der, nullptr, (int)H);
-            GNNB_LAUNCHED();
-        }
-        const unsigned blocks = (unsigned)ceil_div(c.n_items, 8);
-        const size_t smem = sizeof(float) * 8 * 3 * 32 * (size_t)H;
-        if (smem > 48 * 1024) {
-            GNNB_CUDA(cudaFuncSetAttribute(gat_bwd_lean_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            GNNB_CUDA(cudaFuncSetAttribute(gat_bwd_lean_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            GNNB_CUDA(cudaFuncSetAttribute(gat_bwd_lean_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        }
-        if (D == 128) gat_bwd_lean_kernel<1><<<blocks, 256, smem, st>>>(p);
-        else if (D == 256) gat_bwd_lean_kernel<2><<<blocks, 256, smem, st>>>(p);
-        else gat_bwd_lean_kernel<4><<<blocks, 256, smem, st>>>(p);
-        GNNB_LAUNCHED();
-    } else {
-        const dim3 grid((unsigned)ceil_div(p.nchunks, 4), (unsigned)ceil_div(D, (int64_t)32 * vec * kk));
-        GAT_DISPATCH(gat_bwd_kernel, vec, kk, grid, st, p);
-        GNNB_LAUNCHED();
-    }
-    if (c.n_long > 0) {
-        const unsigned fb = nblk((int64_t)c.n_long * (D / vec));
-        if (vec == 4) gat_bwd_fixup_kernel<4><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
-        else gat_bwd_fixup_kernel<1><<<fb, 256, 0, st>>>(p, c.long_rows, c.n_long);
-        GNNB_LAUNCHED();
-    }
+    GNNB_TRY(gat_tnode(dout, out_fwd, n_dst, C, H, vec, T, st));
+    GNNB_TRY(gat_backward(g, g->by_src, Wx, er, dout, nullptr, 0, el, seg_max, seg_sum, T, C, H, slope, dWx, der, dz, vec,
+                          kk, st));
     // del[h,i] = Σ_{k in N(i)} dz_k : the library's own deterministic segmented scatter over the (H,E) buffer
     return gnnb_scatter(g, GNNB_DST, GNNB_SUM, dz, H, del, stream);
+}
+
+int gnnb_gat_aggregate_bwd_halo(gnnb_graph_t g, const float* Wx_own, const float* er_own, const float* dout_local,
+                                const float* dout_halo, int64_t n_local, const float* el, const float* seg_max,
+                                const float* seg_sum, const float* T, int64_t C, int64_t H, float slope, float* dWx,
+                                float* der, float* dz, void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (C <= 0 || H <= 0) GNNB_FAIL(GNNB_ESIZE, "C and H must be positive");
+    if (n_local < 0 || n_local > g->n_src) GNNB_FAIL(GNNB_ESIZE, "n_local must be in [0, num_src]");
+    if (g->n_dst == 0) return GNNB_OK;   // a rank that owns no node owns no source either: nothing to write
+    if (!Wx_own || !er_own || !dWx || !der) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (g->E > 0 && (!el || !seg_max || !seg_sum || !T || !dz)) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    if (n_local > 0 && !dout_local) GNNB_FAIL(GNNB_EINVAL, "dout_local is NULL");
+    if (n_local < g->n_src && !dout_halo) GNNB_FAIL(GNNB_EINVAL, "dout_halo is NULL but the shard has halo targets");
+    const float *d, *d2;
+    gat_bases(dout_local, dout_halo, n_local, g->n_src, &d, &d2);
+    int vec, kk;
+    if (!gat_shape(C, H, Wx_own, dWx, &vec, &kk) || ((uintptr_t)d & 15) || ((uintptr_t)d2 & 15))
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "fused GAT pullback: unsupported (C,H) or unaligned pointers");
+    cudaStream_t st = (cudaStream_t)stream;
+    GNNB_TRY(ensure_csr(g, false, st));
+    const int64_t D = C * H, n_own = g->n_dst;
+    if (g->E == 0) {
+        gat_zero_kernel<<<nblk(n_own * D), 256, 0, st>>>(dWx, n_own * D); GNNB_LAUNCHED();
+        gat_zero_kernel<<<nblk(n_own * H), 256, 0, st>>>(der, n_own * H); GNNB_LAUNCHED();
+        return GNNB_OK;
+    }
+    return gat_backward(g, g->by_dst, Wx_own, er_own, d, d2, n_local, el, seg_max, seg_sum, T, C, H, slope, dWx, der, dz,
+                        vec, kk, st);
+}
+
+int gnnb_gat_tnode(const float* dout, const float* out_fwd, int64_t n, int64_t C, int64_t H, float* T, void* stream) {
+    if (C <= 0 || H <= 0 || n < 0) GNNB_FAIL(GNNB_ESIZE, "C and H must be positive, n non-negative");
+    if (n == 0) return GNNB_OK;
+    if (!dout || !out_fwd || !T) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
+    int vec, kk;
+    if (!gat_shape(C, H, dout, out_fwd, &vec, &kk))
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_tnode: unsupported (C,H) or unaligned pointers");
+    return gat_tnode(dout, out_fwd, n, C, H, vec, T, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -13,6 +13,10 @@ Both directions are "pull": the backward pass gathers dout rows of remote target
 so there is no scatter-reduce across GPUs and every result stays deterministic; inside a target row the
 edges keep their COO order, so a shard reproduces the single-GPU summation order.
 
+Layers on shards: dist_gcn_conv, dist_sage_conv (mean, +) and dist_gat_conv.  GAT's pullback has one term that
+crosses ranks, del of a target = the sum of its in-edges' dz, computed by the owners of their sources: the dz rows move
+to the targets' owners by one all-to-all in an order both shards already share (DistGraph._edge_route).
+
 `torch.distributed` is plumbing (process group, all_to_all_single); index construction below is plain torch
 ops that also run on CPU tensors with the gloo backend (tests/test_partition_gloo.py).
 """
@@ -126,6 +130,14 @@ def exchange_requests(halo_local: torch.Tensor, recv_counts: List[int], group=No
 # ---------------------------------------------------------------------------------------------------------
 # the distributed graph
 # ---------------------------------------------------------------------------------------------------------
+class _DeviceRows:
+    """(n, D) float32 rows at a device address the library owns (a push halo buffer), for torch.as_tensor (no copy)"""
+
+    def __init__(self, ptr: int, n: int, D: int):
+        self.__cuda_array_interface__ = {"shape": (n, D), "typestr": "<f4", "data": (int(ptr), False), "strides": None,
+                                         "version": 2}
+
+
 class _Shard:
     def __init__(self, n_local, n_halo, recv_counts, num_edges, send_idx, send_counts, plan):
         self.n_local = int(n_local)
@@ -135,7 +147,8 @@ class _Shard:
         self.send_counts = send_counts
         self.plan = plan
         self.num_edges = int(num_edges)
-        self.push = None           # per-D state of the peer-to-peer push path (_PushState)
+        self.push = None           # per-(D, purpose) state of the peer-to-peer push path (_push_state)
+        self.edge_route = None     # the edge-value exchange between the two shards (DistGraph._edge_route)
 
 
 def rmat_chunks(num_nodes: int, num_edges: int, seed: int, device, chunk_edges: int = 1 << 26):
@@ -178,6 +191,7 @@ class DistGraph:
         self.ownership = ownership
         self.self_loops = add_self_loops
         self._c = None
+        self._sage_cs = None
         if chunks is None:
             s = s.to(self.device)
             t = t.to(self.device)
@@ -331,14 +345,16 @@ class DistGraph:
         return recv
 
     # -- halo exchange, push path: one kernel writes the requested rows into every peer's halo buffer over NVLink
-    def _push_state(self, shard: _Shard, D: int):
-        """Peer-mapped double-buffered halo buffers for rows of D floats (built once per shard and D).  Every rank runs
-        the same collectives whatever happens locally; if any rank fails to allocate / export / map, ALL ranks fall
-        back to the NCCL exchange (returns None)."""
+    def _push_state(self, shard: _Shard, D: int, purpose: str = "x"):
+        """Peer-mapped double-buffered halo buffers for rows of D floats (built once per shard, D and purpose: two
+        exchanges of one pass that are read by the same kernel — GAT's Wx and er rows, both H wide at C = 1 — must not
+        share a buffer).  Every rank runs the same collectives whatever happens locally; if any rank fails to allocate /
+        export / map, ALL ranks fall back to the NCCL exchange (returns None)."""
         if shard.push is None:
             shard.push = {}
-        if D in shard.push:
-            return shard.push[D]
+        key = (D, purpose)
+        if key in shard.push:
+            return shard.push[key]
         dev, world, rank = self.device, self.world, self.rank
         ok = 1
         all_recv = [None] * world
@@ -380,7 +396,7 @@ class DistGraph:
         dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=self.group)
         if int(flag.item()) == 0:                               # NCCL for everyone: give back what this rank did set up
             self._release_push({"bufs": bufs, "peer_ptrs": peer_ptrs})
-            shard.push[D] = None
+            shard.push[key] = None
             return None
         seg = [0]
         for q in range(world):
@@ -390,7 +406,7 @@ class DistGraph:
               "nbuf": nbuf,
               "peer_ptrs": peer_ptrs,
               "flag": torch.zeros(1, device=dev)}
-        shard.push[D] = st
+        shard.push[key] = st
         return st
 
     def _release_push(self, st) -> None:
@@ -421,25 +437,120 @@ class DistGraph:
         except Exception:
             pass
 
-    def halo_ptr(self, shard: _Shard, x_rows: torch.Tensor) -> int:
-        """device pointer of this rank's halo rows for `x_rows` (valid until the next-but-one call for this shard)"""
+    def halo_ptr(self, shard: _Shard, x_rows: torch.Tensor, purpose: str = "x"):
+        """(device pointer of this rank's halo rows for `x_rows`, owner).  `owner` is the all-to-all receive tensor (None on
+        the push route, whose buffers the shard keeps): hold it until the kernel that reads the rows is enqueued, since a
+        pass may make several exchanges.  A push buffer stays valid until the next-but-one call for this shard and
+        purpose (the next one under GNNB_HALO_BUFFERS=1)."""
         if self.world == 1 or os.environ.get("GNNB_HALO", "push") != "push":
             t = self.halo(shard, x_rows)
-            self._keep = t                                      # keep the NCCL receive buffer alive for the kernel
-            return t.data_ptr()
+            return t.data_ptr(), t
         D = x_rows.shape[1]
-        st = self._push_state(shard, D)
+        st = self._push_state(shard, D, purpose)
         if st is None:                                          # some rank could not set up peer mapping: NCCL for everyone
             t = self.halo(shard, x_rows)
-            self._keep = t
-            return t.data_ptr()
+            return t.data_ptr(), t
         b = st["turn"]
         st["turn"] = (b + 1) % st["nbuf"]
         with torch.cuda.device(self.device):
             _lib.check(lib.gnnb_halo_push(shard.send_idx.data_ptr(), st["seg"], st["peer_c"][b], st["row0"], self.world,
                                           x_rows.data_ptr(), D, _stream(self.device)))
         dist.all_reduce(st["flag"], group=self.group)           # every rank's push kernel precedes its part of this collective
-        return st["bufs"][b]
+        return st["bufs"][b], None
+
+    def halo_rows(self, shard: _Shard, x_rows: torch.Tensor, purpose: str) -> torch.Tensor:
+        """the halo rows of `x_rows` as an (n_halo, D) tensor: the receive tensor, or a view of the push buffer (valid as
+        halo_ptr's pointer is)"""
+        ptr, t = self.halo_ptr(shard, x_rows, purpose)
+        if t is not None:
+            return t
+        D = x_rows.shape[1]
+        if shard.n_halo == 0:
+            return torch.empty((0, D), dtype=x_rows.dtype, device=x_rows.device)
+        return torch.as_tensor(_DeviceRows(ptr, shard.n_halo, D), device=self.device)
+
+    # -- the edge-value exchange (GAT's dz): backward-shard COO order -> forward-shard COO order
+    def _coo_owner(self, shard: _Shard) -> torch.Tensor:
+        """owner rank of the gathered node of every edge of the shard plan, in the plan's COO order (local: this rank;
+        halo: found from the halo segment bounds, which are grouped by owner in rank order)"""
+        E, dev = shard.num_edges, self.device
+        rowptr = torch.empty(shard.n_local + 1, dtype=torch.int32, device=dev)
+        col = torch.empty(max(E, 1), dtype=torch.int32, device=dev)
+        eid = torch.empty(max(E, 1), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.gnnb_graph_csr_device(shard.plan.h, 0, rowptr.data_ptr(), col.data_ptr(), eid.data_ptr(),
+                                                 _stream(dev)))
+        coo_col = torch.empty(E, dtype=torch.int64, device=dev)
+        coo_col[eid[:E].long()] = col[:E].long()
+        ends = torch.cumsum(torch.tensor(shard.recv_counts, dtype=torch.int64, device=dev), 0)
+        halo_owner = torch.searchsorted(ends, coo_col - shard.n_local, right=True)
+        return torch.where(coo_col < shard.n_local, torch.full_like(coo_col, self.rank), halo_owner)
+
+    def _edge_route(self):
+        """Built once.  Both shards are stable compactions of the same edge sequence with the self loops appended after the
+        originals, so the edges of rank p's forward shard whose source rank q owns and the edges of rank q's backward
+        shard whose target rank p owns are the same edges in the same order.  Send side: the backward shard's edges
+        grouped by target owner (stable); receive side: the forward shard's COO position of every received row.  The
+        pairwise counts are checked once."""
+        if self.fwd.edge_route is None:
+            W, dev = self.world, self.device
+            own_b, own_f = self._coo_owner(self.bwd), self._coo_owner(self.fwd)
+            send_perm = torch.sort(own_b, stable=True).indices
+            recv_perm = torch.sort(own_f, stable=True).indices
+            unpack = torch.empty_like(recv_perm)
+            unpack[recv_perm] = torch.arange(recv_perm.numel(), device=dev)
+            send_counts = torch.bincount(own_b, minlength=W)
+            recv_counts = torch.bincount(own_f, minlength=W)
+            peer_counts = torch.empty_like(send_counts)
+            dist.all_to_all_single(peer_counts, send_counts, group=self.group)
+            if not torch.equal(peer_counts, recv_counts):
+                raise RuntimeError(f"rank {self.rank}: the edge exchange does not pair up: the peers' backward shards send "
+                                   f"{peer_counts.tolist()} edge rows, the forward shard expects {recv_counts.tolist()}")
+            self.fwd.edge_route = {"send_idx": send_perm.to(torch.int32), "unpack_idx": unpack.to(torch.int32),
+                                   "send_counts": send_counts.tolist(), "recv_counts": recv_counts.tolist(),
+                                   # one rank: pack, exchange and unpack compose into one gather
+                                   "direct_idx": send_perm[unpack].to(torch.int32) if W == 1 else None}
+        return self.fwd.edge_route
+
+    def edge_exchange(self, v_bwd: torch.Tensor) -> torch.Tensor:
+        """(E_bwd, H) values in backward-shard COO order -> (E_fwd, H) in forward-shard COO order, every edge's row moved
+        to the rank that owns its target: one pack, one all-to-all, one unpack"""
+        r = self._edge_route()
+        H, dev = v_bwd.shape[1], self.device
+        v_bwd = v_bwd.contiguous()
+        n_send, n_recv = int(r["send_idx"].numel()), int(r["unpack_idx"].numel())
+        if r["direct_idx"] is not None:
+            out = torch.empty((n_recv, H), dtype=v_bwd.dtype, device=dev)
+            if n_recv:
+                with torch.cuda.device(dev):
+                    _lib.check(lib.gnnb_gather_rows(r["direct_idx"].data_ptr(), n_recv, v_bwd.data_ptr(), H, out.data_ptr(),
+                                                    _stream(dev)))
+            return out
+        send = torch.empty((n_send, H), dtype=v_bwd.dtype, device=dev)
+        recv = torch.empty((n_recv, H), dtype=v_bwd.dtype, device=dev)
+        out = torch.empty((n_recv, H), dtype=v_bwd.dtype, device=dev)
+        with torch.cuda.device(dev):
+            if n_send:
+                _lib.check(lib.gnnb_gather_rows(r["send_idx"].data_ptr(), n_send, v_bwd.data_ptr(), H, send.data_ptr(),
+                                                _stream(dev)))
+            dist.all_to_all_single(recv, send, output_split_sizes=r["recv_counts"], input_split_sizes=r["send_counts"],
+                                   group=self.group)
+            if n_recv:
+                _lib.check(lib.gnnb_gather_rows(r["unpack_idx"].data_ptr(), n_recv, recv.data_ptr(), H, out.data_ptr(),
+                                                _stream(dev)))
+        return out
+
+    def sage_cs(self):
+        """1 / in-degree of the targets over the backward shard's [local | halo] space (0 for a node without in-edges, which
+        no edge gathers): the scale of the mean aggregation's pullback.  Computed once."""
+        if self._sage_cs is None:
+            deg = torch.empty(self.n_local, dtype=torch.float32, device=self.device)
+            with torch.cuda.device(self.device):
+                if self.n_local:
+                    _lib.check(lib.gnnb_degree(self.fwd.plan.h, _lib.DIR_IN, None, _ptr(deg), _stream(self.device)))
+            inv = torch.where(deg > 0, 1.0 / deg, torch.zeros_like(deg))
+            self._sage_cs = torch.cat([inv, self.halo(self.bwd, inv.reshape(-1, 1)).reshape(-1)]).contiguous()
+        return self._sage_cs
 
     def gcn_c(self):
         """c = 1/sqrt(in-degree) of the owned nodes (exact: rowptr differences of the forward shard), plus the
@@ -470,12 +581,13 @@ class DistGraph:
                 self._slicing = False
             return out
         D = x_rows.shape[1]
-        hptr = self.halo_ptr(shard, x_rows)
+        hptr, recv = self.halo_ptr(shard, x_rows)
         out = torch.empty_like(x_rows)
         with torch.cuda.device(self.device):
             _lib.check(lib.gnnb_propagate_halo(shard.plan.h, _lib.COPY_XJ, aggr, x_rows.data_ptr(),
                                                hptr if shard.n_halo else None, shard.n_local, None,
                                                _ptr(cs), _ptr(ct), D, out.data_ptr(), _stream(self.device)))
+        del recv                                                # the kernel that reads it is enqueued
         return out
 
 
@@ -509,6 +621,180 @@ def dist_gcn_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
         return _linear(l, W, pr, True)            # σ.(W * x .+ b): GEMM with the bias/relu epilogue
     from .layers import _bias_act
     return _bias_act(l, pr)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# GATConv on shards: the fused attention kernels' HALO instances and the dz exchange
+# ---------------------------------------------------------------------------------------------------------
+def dist_gat_aggregate(dg: DistGraph, Wx: torch.Tensor, el: torch.Tensor, er: torch.Tensor, slope: float):
+    """gnnb_gat_aggregate on this rank's targets: Wx (n_local, H, C) and er (n_local, H) of the owned nodes, el (n_local, H).
+    One exchange of the Wx rows and one of the er rows on the forward shard, then the HALO kernel.  Returns (out, seg_max,
+    seg_sum)."""
+    N, H, Cc = Wx.shape
+    sh, dev = dg.fwd, dg.device
+    wx_ptr, wx_recv = dg.halo_ptr(sh, Wx.reshape(N, H * Cc), "gat_wx")
+    er_all = torch.cat([er, dg.halo_rows(sh, er, "gat_er")]).contiguous()
+    out = torch.empty_like(Wx)
+    smax, ssum = torch.empty_like(el), torch.empty_like(el)
+    with torch.cuda.device(dev):
+        _lib.check(lib.gnnb_gat_aggregate_halo(sh.plan.h, _ptr(Wx), wx_ptr if sh.n_halo else None, N, _ptr(el), _ptr(er_all),
+                                               Cc, H, slope, _ptr(out), _ptr(smax), _ptr(ssum), _stream(dev)))
+    del wx_recv                                                  # the kernel that reads it is enqueued
+    return out, smax, ssum
+
+
+def dist_gat_aggregate_bwd(dg: DistGraph, Wx, el, er, smax, ssum, out, dout, slope: float):
+    """gnnb_gat_aggregate_bwd on this rank's rows: T of the owned targets; one exchange of the packed [el | seg_max |
+    seg_sum | T] rows and one of the dout rows on the backward shard; the HALO pullback kernel on the backward shard (dWx
+    and der of the owned sources, dz of their out-edges); dz moved to the targets' owners (edge_exchange) and summed per
+    target there.  Returns (dWx, del, der)."""
+    N, H, Cc = Wx.shape
+    sh, dev = dg.bwd, dg.device
+    st = _stream(dev)
+    T = torch.empty_like(el)
+    with torch.cuda.device(dev):
+        _lib.check(lib.gnnb_gat_tnode(_ptr(dout), _ptr(out), N, Cc, H, _ptr(T), st))
+    packed = torch.cat([el, smax, ssum, T], dim=1)               # (n_local, 4H): one exchange for the four per-target terms
+    full = torch.cat([packed, dg.halo_rows(sh, packed, "gat_stats")])
+    el_a, smax_a, ssum_a, T_a = (full[:, k * H:(k + 1) * H].contiguous() for k in range(4))
+    d_ptr, d_recv = dg.halo_ptr(sh, dout.reshape(N, H * Cc), "gat_dout")
+    dWx, der = torch.empty_like(Wx), torch.empty_like(er)
+    dz = torch.empty((sh.num_edges, H), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.gnnb_gat_aggregate_bwd_halo(sh.plan.h, _ptr(Wx), _ptr(er), _ptr(dout), d_ptr if sh.n_halo else None, N,
+                                                   _ptr(el_a), _ptr(smax_a), _ptr(ssum_a), _ptr(T_a), Cc, H, slope, _ptr(dWx),
+                                                   _ptr(der), _ptr(dz), st))
+    del d_recv
+    dz_f = dg.edge_exchange(dz)                                  # del[h,i] = Σ_{k ∈ N(i)} dz_k, where i is owned
+    del_ = torch.empty_like(el)
+    with torch.cuda.device(dev):
+        if dz_f.shape[0]:
+            _lib.check(lib.gnnb_scatter(dg.fwd.plan.h, _lib.DST, _lib.SUM, _ptr(dz_f), H, _ptr(del_), st))
+        else:
+            del_.zero_()
+    return dWx, del_, der
+
+
+class _DistGATCoreFn(torch.autograd.Function):
+    """_GATCoreFn on shards: logit halves of the owned rows (gnnb_gat_logit_terms), dist_gat_aggregate; pullback
+    dist_gat_aggregate_bwd, then gnnb_gat_logit_terms_bwd on the owned rows (da is this rank's partial sum)."""
+
+    @staticmethod
+    def forward(ctx, Wx, a, dg: DistGraph, slope):
+        N, H, Cc = Wx.shape
+        dev = Wx.device
+        a_jl = a.detach().t().contiguous()
+        el = torch.empty((N, H), dtype=torch.float32, device=dev)
+        er = torch.empty_like(el)
+        if N:
+            with torch.cuda.device(dev):
+                _lib.check(lib.gnnb_gat_logit_terms(Wx.data_ptr(), a_jl.data_ptr(), N, Cc, H, el.data_ptr(), er.data_ptr(),
+                                                    _stream(dev)))
+        out, smax, ssum = dist_gat_aggregate(dg, Wx, el, er, slope)
+        ctx.dg, ctx.slope = dg, slope
+        ctx.save_for_backward(Wx, a_jl, el, er, smax, ssum, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        Wx, a_jl, el, er, smax, ssum, out = ctx.saved_tensors
+        N, H, Cc = Wx.shape
+        dWx, del_, der = dist_gat_aggregate_bwd(ctx.dg, Wx, el, er, smax, ssum, out, dout.contiguous(), ctx.slope)
+        da_jl = torch.zeros_like(a_jl)
+        if N:
+            with torch.cuda.device(Wx.device):
+                _lib.check(lib.gnnb_gat_logit_terms_bwd(Wx.data_ptr(), a_jl.data_ptr(), del_.data_ptr(), der.data_ptr(), N, Cc,
+                                                        H, dWx.data_ptr(), da_jl.data_ptr(), _stream(Wx.device)))
+        return dWx, da_jl.t(), None, None
+
+
+class _DistGATAggregateFn(torch.autograd.Function):
+    """_GATAggregateFn on shards, for the shapes whose logit halves torch computes (C < 4)"""
+
+    @staticmethod
+    def forward(ctx, Wx, el, er, dg: DistGraph, slope):
+        out, smax, ssum = dist_gat_aggregate(dg, Wx, el, er, slope)
+        ctx.dg, ctx.slope = dg, slope
+        ctx.save_for_backward(Wx, el, er, smax, ssum, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        Wx, el, er, smax, ssum, out = ctx.saved_tensors
+        dWx, del_, der = dist_gat_aggregate_bwd(ctx.dg, Wx, el, er, smax, ssum, out, dout.contiguous(), ctx.slope)
+        return dWx, del_, der, None, None
+
+
+def dist_gat_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
+    """gat_conv (GNNlib/src/layers/conv.jl:112-150) on the rows this rank owns; x_local is Julia-shaped (Din, n_local).
+    The graph must have been partitioned with add_self_loops = l.add_self_loops; no dropout, no edge features and a shape
+    of the fused kernels (gat_fusable).  Weight gradients (dense_x, a, bias) are per-rank partial sums: all-reduce them."""
+    from .layers import _bias_act, _jl_reshape3, gat_fusable, gat_logit_fusable
+    _, chout = l.channel
+    heads = l.heads
+    if dg.self_loops != bool(l.add_self_loops):
+        raise ValueError(f"dist_gat_conv: the graph was partitioned with add_self_loops={dg.self_loops}, the layer has "
+                         f"add_self_loops={bool(l.add_self_loops)}")
+    if getattr(l, "dense_e", None) is not None:
+        raise ValueError("dist_gat_conv: edge features are not supported on a partitioned graph")
+    if float(getattr(l, "dropout", 0.0) or 0.0) != 0.0:
+        raise ValueError("dist_gat_conv: attention dropout is not supported on a partitioned graph")
+    if not gat_fusable(chout, heads):
+        raise ValueError(f"dist_gat_conv: {chout} channels x {heads} heads is not a shape of the fused GAT kernels "
+                         "(C/4 a power of two <= 32, or C a power of two <= 32 with C*H <= 128)")
+    Wr = rows(_jl_reshape3(l.dense_x(x_local), chout, heads))   # (n_local, H, C)
+    if Wr.data_ptr() % 16 != 0:
+        Wr = Wr.clone()
+    a, slope = l.a, float(l.negative_slope)
+    if gat_logit_fusable(chout, heads) and a.dtype == torch.float32:
+        out = unrows(_DistGATCoreFn.apply(Wr, a, dg, slope))
+    else:
+        el = (Wr * a[:chout, :].t().unsqueeze(0)).sum(-1)       # rows 1..C of a pair with the target
+        er = (Wr * a[chout:, :].t().unsqueeze(0)).sum(-1)       # rows C+1..2C with the source
+        out = unrows(_DistGATAggregateFn.apply(Wr, el.contiguous(), er.contiguous(), dg, slope))
+    if not l.concat:
+        out = out.mean(dim=1, keepdim=True)
+    r = rows(out)
+    out = unrows(r.reshape(r.shape[0], r.shape[1] * r.shape[2]))   # reshape(x, :, size(x, 3)), also for zero owned rows
+    return _bias_act(l, out)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# SAGEConv on shards (mean, +): the lean reduce's HALO instance both ways
+# ---------------------------------------------------------------------------------------------------------
+class _DistSAGEPropagateFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x_rows, dg: DistGraph, aggr):
+        ctx.dg, ctx.aggr = dg, aggr
+        return dg.propagate(dg.fwd, x_rows.contiguous(), None, None, aggr)
+
+    @staticmethod
+    def backward(ctx, dout):
+        dg = ctx.dg
+        cs = dg.sage_cs() if ctx.aggr == _lib.MEAN else None    # mean: each target's row scaled by 1 / in-degree
+        return dg.propagate(dg.bwd, dout.contiguous(), cs, None, _lib.SUM), None, None
+
+
+def dist_sage_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
+    """sage_conv (GNNlib/src/layers/conv.jl:277-283) on the rows this rank owns, for aggr ∈ {mean, +}; x_local is
+    Julia-shaped (Din, n_local).  The graph must have been partitioned without self loops (the layer adds none).  Weight
+    gradients are per-rank partial sums: all-reduce them."""
+    from .layers import _Linear2Fn, _bias, _is_relu, _linear, _sigma, identity
+    from .msgpass import _aggr_code
+    aggr = _aggr_code(l.aggr)
+    if aggr not in (_lib.SUM, _lib.MEAN):
+        raise ValueError(f"dist_sage_conv: aggregation {l.aggr!r} is not supported on a partitioned graph (mean and + are)")
+    if dg.self_loops:
+        raise ValueError("dist_sage_conv: the graph was partitioned with add_self_loops=True; SAGEConv adds no self loops")
+    r1 = rows(x_local).contiguous()
+    r2 = _DistSAGEPropagateFn.apply(r1, dg, aggr)
+    W = l.weight
+    sig, b = _sigma(l), _bias(l)
+    D1, D2, Dout = r1.shape[1], r2.shape[1], W.shape[0]
+    if (r1.dtype == torch.float32 and W.dtype == torch.float32 and Dout == 128 and D1 % 32 == 0 and D2 % 32 == 0
+            and D1 <= 128 and D2 <= 128 and (sig is identity or _is_relu(sig))):
+        return unrows(_Linear2Fn.apply(r1, r2, W, None if b is None else b.contiguous(), _is_relu(sig)))
+    return _linear(l, W, unrows(torch.cat([r1, r2], dim=1)), True)
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -586,7 +872,7 @@ def bench_multi(args, world, rank, dev, seed, ClockSampler, measured_peaks, cpu_
     x.grad = None
     layer.weight.grad = None
     torch.cuda.empty_cache()
-    hp = dg.halo_ptr(dg.fwd, xr)                        # the halo rows where the step's own exchange puts them
+    hp, hp_recv = dg.halo_ptr(dg.fwd, xr)               # the halo rows where the step's own exchange puts them
     out = torch.empty_like(xr)
     st = torch.cuda.current_stream(dev).cuda_stream
 

@@ -315,6 +315,24 @@ int gnnb_gather_rows(const int32_t* idx_dev, int64_t n, const float* x, int64_t 
 int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local, const float* x_halo,
                         int64_t n_local, const float* w, const float* cs, const float* ct, int64_t D,
                         float* out, void* stream);
+/* The fused GAT core on shards (csrc/gat.cu, the HALO instances of the same kernels; same shapes as gnnb_gat_aggregate).
+ * gnnb_gat_aggregate_halo: gnnb_gat_aggregate on a forward shard plan, over its forward CSR: gathered sources < n_local
+ *   read Wx_local, the others Wx_halo + (id - n_local)*C*H.  el (H, num_dst); er (H, num_src) in [local | halo] order.
+ * gnnb_gat_aggregate_bwd_halo: the pullback kernel on the FORWARD CSR of a backward shard plan, whose rows are the owned
+ *   sources j and whose gathered nodes are the targets in [local | halo]: dout_local / dout_halo split as above;
+ *   el, seg_max, seg_sum and T (H, num_src of the shard) in [local | halo] order; Wx_own (C,H,num_dst), er_own
+ *   (H,num_dst).  Writes dWx (C,H,num_dst), der (H,num_dst) and dz (H, E) in the shard plan's COO order, unscattered:
+ *   del of a target is the sum of the dz of its in-edges, which live on the ranks that own their sources.
+ * gnnb_gat_tnode: T[h,i] = <dout[:,h,i], out[:,h,i]> over n nodes, the per-target term gnnb_gat_aggregate_bwd computes.
+ * A shard without targets (num_dst = 0) accepts NULL outputs; a shard without halo rows accepts a NULL halo pointer. */
+int gnnb_gat_aggregate_halo(gnnb_graph_t g, const float* Wx_local, const float* Wx_halo, int64_t n_local, const float* el,
+                            const float* er, int64_t C, int64_t H, float slope, float* out, float* seg_max, float* seg_sum,
+                            void* stream);
+int gnnb_gat_aggregate_bwd_halo(gnnb_graph_t g, const float* Wx_own, const float* er_own, const float* dout_local,
+                                const float* dout_halo, int64_t n_local, const float* el, const float* seg_max,
+                                const float* seg_sum, const float* T, int64_t C, int64_t H, float slope, float* dWx,
+                                float* der, float* dz, void* stream);
+int gnnb_gat_tnode(const float* dout, const float* out_fwd, int64_t n, int64_t C, int64_t H, float* T, void* stream);
 
 /* Building one rank's shards on its GPU from chunks of the global edge list (csrc/shard.cu).
  *   ownership mode 0: contiguous ranges, bounds_host[q] <= v < bounds_host[q+1] (world + 1 entries; NULL = equal ranges);

@@ -1,5 +1,6 @@
-"""torchrun --nproc-per-node N scripts/check_dist.py : the node-partitioned GCNConv (partition.dist_gcn_conv, NCCL halo
-exchange) against the single-GPU layer on the full graph: forward, dx, dW, db."""
+"""torchrun --nproc-per-node N scripts/check_dist.py : the node-partitioned GCNConv, GATConv and SAGEConv
+(partition.dist_gcn_conv / dist_gat_conv / dist_sage_conv, halo exchange over NCCL or the IPC push) against the
+single-GPU layer on the full graph: forward, dx and the all-reduced weight gradients."""
 import os
 import sys
 
@@ -53,6 +54,58 @@ for (n, E, D) in ((5000, 60000, 128), (200000, 3000000, 128), (30000, 200000, 64
         print(f"rank {rank}/{world} n={n} E={E} D={D} {how}/{ownership} n_local={dg.n_local} halo_f={dg.fwd.n_halo} "
               f"halo_b={dg.bwd.n_halo} edges_f={dg.fwd.num_edges} errs={errs} {'OK' if good else 'FAIL'}", flush=True)
         del dg
+
+
+def check_layer(name, layer, g, n, Din, Dout, loops, run_dist, params):
+    """one layer on the full graph (every rank) against its partitioned run over the ranks, two ownership modes"""
+    global ok
+    gen = torch.Generator(device=dev).manual_seed(2)
+    x_full = torch.randn(n, Din, device=dev, generator=gen)
+    dy_full = torch.randn(n, Dout, device=dev, generator=gen)
+    xr = gnn.unrows(x_full.clone()).requires_grad_(True)
+    y = layer(g, xr)
+    y.backward(gnn.unrows(dy_full))
+    y_ref, dx_ref = gnn.rows(y.detach()).clone(), gnn.rows(xr.grad).clone()
+    g_ref = [p.grad.clone() for p in params]
+    for ownership in ("contiguous", "balanced"):
+        for p in params:
+            p.grad = None
+        dg = P.DistGraph(g.s, g.t, n, add_self_loops=loops, device=dev, ownership=ownership)
+        ids = dg.local_nodes()
+        xl = gnn.unrows(x_full[ids].clone()).requires_grad_(True)
+        yl = run_dist(layer, dg, xl)
+        yl.backward(gnn.unrows(dy_full[ids].contiguous()))
+        for p in params:
+            dist.all_reduce(p.grad)
+        rel = lambda a, b: float((a - b).norm() / b.norm().clamp(min=1e-30))
+        errs = {"y": rel(gnn.rows(yl.detach()), y_ref[ids]), "dx": rel(gnn.rows(xl.grad), dx_ref[ids])}
+        errs.update({f"d{i}": rel(p.grad, r) for i, (p, r) in enumerate(zip(params, g_ref))})
+        good = all(v < 1e-5 for v in errs.values())
+        ok = ok and good
+        print(f"rank {rank}/{world} {name} n={n} {ownership} n_local={dg.n_local} halo_f={dg.fwd.n_halo} "
+              f"halo_b={dg.bwd.n_halo} errs={errs} {'OK' if good else 'FAIL'}", flush=True)
+        dg.close()
+        del dg
+    for p in params:
+        p.grad = None
+
+
+for (n, E) in ((5000, 60000), (200000, 3000000)):
+    g = gnn.rmat_graph(n, E, 17, device=dev)
+    for concat in (True, False):
+        torch.manual_seed(0)
+        gat = gnn.GATConv(128, 64, torch.relu, heads=8, concat=concat, device=dev)
+        with torch.no_grad():
+            gat.bias.normal_()
+        check_layer(f"GATConv 128->8x64 concat={concat}", gat, g, n, 128, 512 if concat else 64, True, P.dist_gat_conv,
+                    [gat.dense_x.weight, gat.a, gat.bias])
+    for aggr in (gnn.mean, "+"):
+        torch.manual_seed(0)
+        sage = gnn.SAGEConv(128, 128, torch.relu, aggr=aggr, device=dev)
+        with torch.no_grad():
+            sage.bias.normal_()
+        check_layer(f"SAGEConv 128->128 aggr={aggr if isinstance(aggr, str) else 'mean'}", sage, g, n, 128, 128, False,
+                    P.dist_sage_conv, [sage.weight, sage.bias])
 t = torch.tensor([1 if ok else 0], device=dev)
 dist.all_reduce(t, op=dist.ReduceOp.MIN)
 dist.barrier()
