@@ -21,8 +21,8 @@ from .layers_more import (CGConv, ChebConv, DConv, EdgeConv, EGNNConv, GMMConv, 
                           nn_conv, res_gated_graph_conv)
 from .readout import (Set2Set, broadcast_edges, broadcast_nodes, global_attention_pool, global_pool, reduce_edges,
                       reduce_nodes, set2set_pool, softmax_edges, softmax_nodes)
-from .transform import (add_nodes, color_refinement, csr, getgraph, random_walk_pe, remove_edges, remove_multi_edges,
-                        remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
+from .transform import (add_nodes, color_refinement, csr, getgraph, ppr_diffusion, random_walk_pe, remove_edges,
+                        remove_multi_edges, remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
 from .temporal import (DCGRU, DCGRUCell, EvolveGCNO, EvolveGCNOCell, GConvGRU, GConvGRUCell, GConvLSTM, GConvLSTMCell,
                        GNNRecurrence, TemporalSnapshotsGNNGraph, TGCN, TGCNCell, initialstates)
 from .generate import knn_graph, radius_graph

@@ -13,6 +13,7 @@
     add_nodes(g, n; ndata)           GNNGraphs/src/transform.jl:553-563
     random_walk_pe(g, walk_length)   GNNGraphs/src/transform.jl:975-990   (per-graph walks, csrc/rwpe.cu)
     color_refinement(g, x0)          GNNGraphs/src/utils.jl:340-389       (1-WL colour refinement, csrc/wl.cu)
+    ppr_diffusion(g; alpha)          GNNGraphs/src/transform.jl:1026-1051 (per-graph inverses, csrc/ppr.cu)
 
 The index work (pair encoding, stable radix sort, duplicate runs) is csrc/transform.cu; the feature aggregation of
 `remove_multi_edges` is the library's segmented scatter over the run ids it returns — the same kernels as
@@ -42,6 +43,9 @@ Deliberate differences from the reference:
 7. color_refinement refines to the fixed point, renumbers the colours from 1 in every round and groups signatures by
    a multiset hash of its own; the reference stops after at most two rounds and carries its ids over between rounds
    (see its docstring).
+8. ppr_diffusion inverts each graph of a batch on its own, by Gauss-Jordan elimination up to 240 nodes and LU above
+   (LAPACK's LU of the whole batch in the reference), so the two agree to rounding; a singular M raises
+   torch.linalg.LinAlgError where the reference throws SingularException.
 """
 from __future__ import annotations
 
@@ -490,3 +494,109 @@ def color_refinement(g: GNNGraph, x0=None, *, max_iters: Optional[int] = None):
         _lib.check(lib.gnnb_color_refinement(p.h, _ptr(x), 0 if max_iters is None else int(max_iters), out.data_ptr(),
                                              C.byref(num_colors), C.byref(niters), _stream(p.device)))
     return out, int(num_colors.value), int(niters.value)
+
+
+# ---------------------------------------------------------------------------------------------- PPR diffusion
+# Segments of at most this many nodes are inverted in shared memory (gnnb_ppr_diffusion, csrc/ppr.cu); larger ones take
+# the dense route.  Must not exceed GNNB_PPR_SMEM_MAX_NODES (include/gnnb200.h), whose larger segments the kernel skips;
+# lowering it (tests do) routes more segments to the dense route.
+_PPR_KERNEL_MAX_NODES = 240       # GNNB_PPR_SMEM_MAX_NODES
+_PPR_SMEM_MAX_NODES = _PPR_KERNEL_MAX_NODES
+_PPR_PAD = 128                    # the dense route pads a segment to a multiple of this many nodes
+_PPR_BATCH_BYTES = 1 << 30        # M and its inverse of one dense batch; a single segment may exceed it
+
+
+def _ppr_singular(what: str, step: int) -> torch.linalg.LinAlgError:
+    return torch.linalg.LinAlgError(f"ppr_diffusion: M = I + (alpha - 1) A of {what} is singular (zero pivot at step "
+                                    f"{step}); the reference's inv throws SingularException")
+
+
+def _ppr_dense(p: _Plan, w: Optional[torch.Tensor], alpha: float, segs: List[tuple], s0: torch.Tensor,
+               t0: torch.Tensor, eseg: torch.Tensor, out: torch.Tensor, fail) -> None:
+    """The segments [(i, a, b)] above the shared-memory bound, grouped by padded size P: each batch of M blocks is built
+    by gnnb_ppr_matrix into identity-padded (P, P) matrices and inverted by torch.linalg.inv_ex, and
+    out[e] = fl32(alpha) * inv[t_e - a, s_e - a] is gathered for the segments' edges (eseg[e] = segment of edge e).
+    Identity padding leaves the inverse of the real block unchanged and keeps a singular block singular (the pad rows
+    are zero in its columns)."""
+    dev = p.device
+    a32 = torch.tensor(alpha, dtype=torch.float32, device=dev)
+    groups = {}
+    for seg in segs:
+        groups.setdefault(-(-(seg[2] - seg[1]) // _PPR_PAD) * _PPR_PAD, []).append(seg)
+    slot = torch.full((segs[-1][0] + 1,), -1, dtype=torch.int64, device=dev)       # segment -> matrix of the batch
+    esafe = eseg.clamp(max=segs[-1][0])
+    for P, members in sorted(groups.items()):
+        per = max(1, _PPR_BATCH_BYTES // (2 * 4 * P * P))
+        for c0 in range(0, len(members), per):
+            chunk = members[c0:c0 + per]
+            M = torch.eye(P, dtype=torch.float32, device=dev).repeat(len(chunk), 1, 1)
+            with torch.cuda.device(dev):
+                for k, (_, a, b) in enumerate(chunk):
+                    _lib.check(lib.gnnb_ppr_matrix(p.h, _ptr(w), alpha, a, b, P, M[k].data_ptr(), _stream(dev)))
+            inv, info = torch.linalg.inv_ex(M)
+            del M
+            bad = (info > 0).nonzero().reshape(-1)
+            if bad.numel():
+                k = int(bad[0])
+                raise fail(chunk[k][0], int(info[k]))
+            ids = torch.tensor([i for i, _, _ in chunk], dtype=torch.int64, device=dev)
+            base = torch.tensor([a for _, a, _ in chunk], dtype=torch.int64, device=dev)
+            slot[ids] = torch.arange(len(chunk), device=dev)
+            e = ((eseg == esafe) & (slot[esafe] >= 0)).nonzero().reshape(-1)
+            k = slot[esafe[e]]
+            out[e] = a32 * inv[k, t0[e] - base[k], s0[e] - base[k]]
+            slot[ids] = -1
+
+
+def ppr_diffusion(g: GNNGraph, *, alpha=0.85) -> GNNGraph:
+    """Personalized-PageRank diffusion of the edge weights — transform.jl:1026-1051.  Returns a graph with g's edges,
+    node, edge and graph data, indicator and plan, whose weight of edge s -> t is fl32(alpha) * inv(M)[t, s] for
+    M = I + (fl32(alpha) - 1) A, A[t, s] the summed weight of the edges s -> t (g.w, or 1 without weights; duplicates add
+    up and all get the same new weight, self loops count).  A is not normalised: the reference's docstring mentions a
+    normalisation its code does not do, and this follows the code.  Not differentiable.
+
+    The inverse of a block-diagonal matrix is block-diagonal, so a batched graph is inverted per segment: one per run of
+    equal graph_indicator values when the indicator is non-decreasing and no edge joins two graphs, otherwise the whole
+    graph is one segment.
+      * Segments of at most _PPR_SMEM_MAX_NODES (240) nodes: gnnb_ppr_diffusion, all in one call.  M is built and
+        inverted in shared memory by Gauss-Jordan elimination with partial pivoting, one warp per segment of up to 32
+        nodes and one CTA per larger one, bit for bit the float32 statement of csrc/ppr.cu.
+      * Larger segments: the reference's dense inverse, per segment and on the device.  M is built by gnnb_ppr_matrix
+        into identity-padded batches (a multiple of 128 nodes, about 1 GB of matrices per batch) and inverted by
+        torch.linalg.inv_ex.  O(n^3) time and n^2 memory per segment: a graph too large for the card raises torch's
+        out-of-memory error, as the reference would.
+    A singular M on either route raises torch.linalg.LinAlgError naming the first singular graph (1-based) and the step
+    of its zero pivot, where the reference throws SingularException.  Non-finite weights or alpha raise nothing."""
+    g = _on_device(g)
+    dev, n, E = g.s.device, g.num_nodes, g.num_edges
+    w_out = torch.empty(E, dtype=torch.float32, device=dev)
+    if n == 0 or E == 0:
+        return _graph.set_edge_weight(g, w_out)
+    alpha = float(alpha)
+    p = g.plan()
+    w = None if g.w is None else g.w.detach().to(device=p.device, dtype=torch.float32).contiguous()
+    seg_ptr = _rwpe_segments(g, p.device)
+    bounds = [0, n] if seg_ptr is None else seg_ptr.tolist()
+    n_seg = len(bounds) - 1
+    bound = min(_PPR_SMEM_MAX_NODES, _PPR_KERNEL_MAX_NODES)
+    big = [i for i in range(n_seg) if bounds[i + 1] - bounds[i] > bound]
+
+    def fail(i: int, step: int) -> torch.linalg.LinAlgError:
+        what = "the graph" if seg_ptr is None else f"graph {int(g.graph_indicator[bounds[i]])}"
+        return _ppr_singular(what, step)
+
+    if len(big) < n_seg:
+        info = torch.empty(n_seg, dtype=torch.int32, device=p.device)
+        with torch.cuda.device(p.device):
+            _lib.check(lib.gnnb_ppr_diffusion(p.h, _ptr(w), alpha, _ptr(seg_ptr), n_seg, w_out.data_ptr(),
+                                              info.data_ptr(), _stream(p.device)))
+        bad = (info > 0).nonzero().reshape(-1)
+        if bad.numel():
+            i = int(bad[0])
+            raise fail(i, int(info[i]))
+    if big:
+        s0, t0 = g.s.to(p.device).long() - 1, g.t.to(p.device).long() - 1
+        eseg = torch.zeros(E, dtype=torch.int64, device=p.device) if seg_ptr is None else \
+            torch.searchsorted(seg_ptr, t0, right=True) - 1
+        _ppr_dense(p, w, alpha, [(i, bounds[i], bounds[i + 1]) for i in big], s0, t0, eseg, w_out, fail)
+    return _graph.set_edge_weight(g, w_out)

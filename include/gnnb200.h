@@ -475,6 +475,33 @@ int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_p
 int gnnb_random_walk_pe(gnnb_graph_t g, const float* w, const float* dinv, const int64_t* seg_ptr, int64_t n_seg,
                         int walk_length, float* out, void* stream);
 
+/* --------------------------------------------------------- personalized-PageRank diffusion (csrc/ppr.cu)
+ * replaces: ppr_diffusion(g; alpha) (GNNGraphs/src/transform.jl:1026-1051): the dense N x N matrix of the whole batch,
+ *           M = I + (alpha - 1) A with A[t, s] the summed weight of the edges s -> t, and `inv` of it; the new weight of
+ *           edge s -> t is alpha * inv(M)[t, s].  Here each segment (graph of a batch) is inverted on its own.
+ * gnnb_ppr_diffusion: per segment [base, base + n) of at most GNNB_PPR_SMEM_MAX_NODES nodes, row i of A sums its
+ *   in-edges' weights in plan order (each add rounded), am1 = alpha - 1 (rounded once), M[i][j] = am1 * A[i][j] for
+ *   j != i and M[i][i] = 1 + am1 * A[i][i]; Gauss-Jordan elimination with partial pivoting (the first largest |a[i][k]|,
+ *   i >= k, a NaN never chosen over a number) in shared memory, every product, difference and quotient rounded on its
+ *   own; w_out[e] = alpha * inv(M)[t_e - base][s_e - base] in COO order.  The bits do not depend on the launch class.
+ *   g: a square plan (GNNB_ESIZE otherwise).  w: E DEVICE floats in COO order, or NULL (every weight 1).  seg_ptr: NULL
+ *   (one segment) or n_seg + 1 non-decreasing DEVICE offsets from 0 to n, validated on the device (GNNB_EINVAL; w_out
+ *   is then untouched and info unspecified).  An edge into a segment this entry inverts whose source lies outside that
+ *   segment gives GNNB_EINVAL, and nothing is read or written outside a segment.
+ *   info: n_seg (1 without seg_ptr) DEVICE int32s: 0 = inverted, k >= 1 = zero pivot at step k (M is singular; the
+ *   segment's w_out is untouched), -1 = the segment has more than GNNB_PPR_SMEM_MAX_NODES nodes and was skipped (its
+ *   w_out is untouched: the caller inverts it with gnnb_ppr_matrix and a dense solver).  Synchronises the stream.
+ * gnnb_ppr_matrix: M of the nodes [a, b) (the same construction) into M_out, row-major with leading dimension
+ *   ld >= b - a (the caller's padding is not touched).  0 <= a <= b <= n (GNNB_EINVAL).  An edge into [a, b) whose
+ *   source lies outside it gives GNNB_EINVAL.  Synchronises the stream.
+ * GNNB_PPR_SMEM_MAX_NODES is the largest n whose matrix (odd leading dimension >= n + 1), pivot list and reduction
+ * slots fit the 227 KB of one H100 CTA; gnnb_ppr_diffusion checks the device's opt-in limit (GNNB_EUNSUPPORTED). */
+#define GNNB_PPR_SMEM_MAX_NODES 240
+int gnnb_ppr_diffusion(gnnb_graph_t g, const float* w, float alpha, const int64_t* seg_ptr, int64_t n_seg,
+                       float* w_out, int32_t* info, void* stream);
+int gnnb_ppr_matrix(gnnb_graph_t g, const float* w, float alpha, int64_t a, int64_t b, int64_t ld, float* M_out,
+                    void* stream);
+
 /* --------------------------------------------------------- 1-WL colour refinement (csrc/wl.cu)
  * replaces: color_refinement(g, x0) (GNNGraphs/src/utils.jl:340-389): a host loop hashing (x_i, sort(x[in-neighbours]))
  *           into a Dict once per node per round.

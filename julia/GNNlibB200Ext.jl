@@ -25,6 +25,7 @@ using CUDA
 using ChainRulesCore
 using Random
 using Statistics: mean
+using LinearAlgebra: I, inv, SingularException
 using GNNlib: GNNlib, propagate, copy_xj, e_mul_xj, w_mul_xj, expand_srcdst, check_num_nodes
 using GNNGraphs: GNNGraphs, GNNGraph, COO_T, edge_index, get_edge_weight
 
@@ -882,6 +883,63 @@ function GNNGraphs.random_walk_pe(g::GNNGraph{<:CuCOO}, walk_length::Int)
     return out
 end
 ChainRulesCore.@non_differentiable GNNGraphs.random_walk_pe(::Any...)
+
+## ppr_diffusion on device COO graphs — replaces GNNGraphs/src/transform.jl:1026-1051 (`inv` of the dense N x N matrix
+## I + (alpha - 1) A of the whole batch).  The inverse of a block-diagonal matrix is block-diagonal: each graph of the
+## batch of at most PPR_SMEM_MAX_NODES nodes is inverted in shared memory (gnnb_ppr_diffusion); a larger one is built by
+## gnnb_ppr_matrix into an identity-padded matrix and inverted densely.  Same routing as the Python mirror
+## (graphneuralnetworks.jl_b200/transform.py): segments = runs of a non-decreasing graph_indicator that no edge crosses,
+## otherwise the whole graph.
+const PPR_SMEM_MAX_NODES = 240                                # GNNB_PPR_SMEM_MAX_NODES
+const PPR_PAD = 128
+
+function GNNGraphs.ppr_diffusion(g::GNNGraph{<:CuCOO}; alpha = 0.85f0)
+    n, E = g.num_nodes, g.num_edges
+    s, t = edge_index(g)
+    w_out = CuVector{Float32}(undef, E)
+    (n == 0 || E == 0) && return GNNGraph((s, t, w_out), n, E, g.num_graphs, g.graph_indicator, g.ndata, g.edata, g.gdata)
+    a32 = Float32(alpha)
+    p = plan(g)
+    w = get_edge_weight(g)
+    w = w === nothing ? nothing : CuVector{Float32}(w)
+    seg = nothing
+    if g.graph_indicator !== nothing
+        order, _, sg = _knn_segments(g.graph_indicator, n)
+        gi = CuVector{Int64}(g.graph_indicator)
+        if order === nothing && sg !== nothing && all(gi[s] .== gi[t])
+            seg = sg
+        end
+    end
+    sp, ns = _knn_seg_args(seg)
+    bounds = seg === nothing ? [0, n] : Array(seg)
+    sizes = bounds[2:end] .- bounds[1:end-1]
+    big = findall(sizes .> PPR_SMEM_MAX_NODES)
+    if length(big) < ns
+        info = CuVector{Int32}(undef, ns)
+        check(ccall((:gnnb_ppr_diffusion, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Float32}, Cfloat, CuPtr{Int64}, Int64, CuPtr{Float32}, CuPtr{Int32}, Ptr{Cvoid}),
+                    p.h, cuptr(w), a32, sp, ns, w_out, info, stream()))
+        hinfo = Array(info)
+        i = findfirst(>(0), hinfo)
+        i === nothing || throw(SingularException(Int(hinfo[i])))   # the zero pivot's step, as LAPACK's info
+    end
+    for i in big
+        a, b = bounds[i], bounds[i + 1]
+        m = b - a
+        P = cld(m, PPR_PAD) * PPR_PAD
+        M = CuMatrix{Float32}(I, P, P)
+        # gnnb_ppr_matrix writes row-major rows of M; a column-major P x P buffer holds them as its transpose
+        check(ccall((:gnnb_ppr_matrix, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Float32}, Cfloat, Int64, Int64, Int64, CuPtr{Float32}, Ptr{Cvoid}),
+                    p.h, cuptr(w), a32, a, b, P, M, stream()))
+        Minv = inv(M)                                         # SingularException for a singular block
+        sel = findall((t .> a) .& (t .<= b))                  # the graph's edges (none crosses it)
+        idx = CartesianIndex.(Int.(s[sel]) .- a, Int.(t[sel]) .- a)   # (M^T)^-1 = (M^-1)^T: [s, t] of the transpose
+        w_out[sel] .= a32 .* Minv[idx]
+    end
+    return GNNGraph((s, t, w_out), n, E, g.num_graphs, g.graph_indicator, g.ndata, g.edata, g.gdata)
+end
+ChainRulesCore.@non_differentiable GNNGraphs.ppr_diffusion(::Any...)
 
 ## color_refinement on device COO graphs — replaces GNNGraphs/src/utils.jl:340-389 (a host loop that hashes
 ## (x_i, sort(x[in-neighbours])) into a Dict and indexes scalars, so it cannot run on a CuArray graph).  One pass of

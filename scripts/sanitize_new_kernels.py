@@ -1,5 +1,6 @@
 """small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans, the
-drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), colour
+drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), PPR diffusion
+(both launch classes, the dense route's matrix kernel, a seg_ptr an edge crosses), colour
 refinement (hub rows cut into long-row pieces, a path, a batch) and Set2Set (a graph with no nodes, graphs of chunk +- 1
 nodes, D = 1, 3 and 1024, the composition at D = 1025), meant to run under `compute-sanitizer --tool memcheck`
 (or racecheck / synccheck)"""
@@ -91,6 +92,29 @@ seg = torch.cat([torch.zeros(1, dtype=torch.int64, device="cuda"), torch.cumsum(
 out = torch.empty(off * 6, device="cuda")
 rc = lib.gnnb_random_walk_pe(gx.plan().h, None, dinv.data_ptr(), seg.data_ptr(), len(sizes), 6, out.data_ptr(), None)
 print("random_walk_pe crossing edge rejected", rc == gnn._lib.EINVAL)
+# ppr_diffusion: segments of 1, 5, 32 (warp class), 33 and 240 (CTA class) and 241 (dense route: gnnb_ppr_matrix),
+# weighted, then the same crossing edge, and every segment through the CTA class (variant 12)
+sizes = [1, 5, 32, 33, 240, 241]
+S, T, off = [], [], 0
+for m in sizes:
+    S.append(torch.randint(0, m, (3 * m,), device="cuda") + off); T.append(torch.randint(0, m, (3 * m,), device="cuda") + off)
+    off += m
+s_, t_ = torch.cat(S), torch.cat(T)
+gi = torch.repeat_interleave(torch.arange(1, len(sizes) + 1, device="cuda"), torch.tensor(sizes, device="cuda"))
+gw = gnn.GNNGraph(s_ + 1, t_ + 1, torch.rand(s_.numel(), device="cuda") * 0.5, num_nodes=off, num_graphs=len(sizes),
+                  graph_indicator=gi)
+print("ppr_diffusion", tuple(gnn.ppr_diffusion(gw).w.shape), "finite", bool(torch.isfinite(gnn.ppr_diffusion(gw).w).all()))
+gnn._lib.check(lib.gnnb_set_kernel_variant(12))
+print("ppr_diffusion CTA class only, finite", bool(torch.isfinite(gnn.ppr_diffusion(gw).w).all()))
+gnn._lib.check(lib.gnnb_set_kernel_variant(0))
+gx = gnn.GNNGraph(torch.cat([s_, torch.tensor([0], device="cuda")]) + 1, torch.cat([t_, torch.tensor([3], device="cuda")]) + 1,
+                  num_nodes=off)                                   # an edge from the first segment into the second
+seg = torch.cat([torch.zeros(1, dtype=torch.int64, device="cuda"), torch.cumsum(torch.tensor(sizes, device="cuda"), 0)])
+w_out = torch.empty(gx.num_edges, device="cuda"); info = torch.empty(len(sizes), dtype=torch.int32, device="cuda")
+rc = lib.gnnb_ppr_diffusion(gx.plan().h, None, 0.85, seg.data_ptr(), len(sizes), w_out.data_ptr(), info.data_ptr(), None)
+M = torch.empty(5, 7, device="cuda")
+rc2 = lib.gnnb_ppr_matrix(gx.plan().h, None, 0.85, 1, 6, 7, M.data_ptr(), None)
+print("ppr_diffusion crossing edge rejected", rc == gnn._lib.EINVAL, rc2 == gnn._lib.EINVAL)
 # color_refinement: two hubs of 3 000 in-edges (pieces of 128 and the fix-up), a path of 41 nodes, a batch of small graphs
 hs = torch.randint(0, 500, (6000,), device="cuda"); ht = torch.cat([torch.full((3000,), 7, device="cuda"),
                                                                    torch.full((3000,), 499, device="cuda")])
