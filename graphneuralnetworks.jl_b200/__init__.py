@@ -29,8 +29,9 @@ from .generate import knn_graph, radius_graph
 from .linkpred import (DotDecoder, add_edges, dot_decoder, edge_decoding, edge_encoding, intersect, negative_sample,
                        perturb_edges, rand_edge_split, rand_graph)
 from .sampling import NeighborLoader, induced_subgraph, sample_edge_ids, sample_neighbors
-from .query import (adjacency_list, adjacency_matrix, has_multi_edges, has_self_loops, inneighbors, is_bidirected,
-                    outneighbors)
+from .query import (adjacency_list, adjacency_matrix, has_isolated_nodes, has_multi_edges, has_self_loops, inneighbors,
+                    is_bidirected, laplacian_lambda_max, laplacian_matrix, normalized_laplacian, outneighbors,
+                    scaled_laplacian)
 from .hetero import (GNNHeteroGraph, HeteroGraphConv, add_edges, edge_type_subgraph, has_edge, num_edge_types,
                      num_node_types, rand_bipartite_heterograph, rand_heterograph)
 

@@ -127,6 +127,8 @@ _SIGS = {
     "gnnb_random_walk_pe": (_int, [_vp, _f32p, _f32p, _vp, _i64, _int, _f32p, _vp]),
     "gnnb_ppr_diffusion": (_int, [_vp, _f32p, C.c_float, _vp, _i64, _f32p, _vp, _vp]),
     "gnnb_ppr_matrix": (_int, [_vp, _f32p, C.c_float, _i64, _i64, _i64, _f32p, _vp]),
+    "gnnb_laplacian_lambda_max": (_int, [_vp, _f32p, _f32p, _int, _int, _vp, _i64, _vp, _vp, _vp]),
+    "gnnb_segment_dots": (_int, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _vp]),
     "gnnb_color_refinement": (_int, [_vp, _vp, _i64, _vp, C.POINTER(_i64), C.POINTER(_i64), _vp]),
     "gnnb_set2set_attend": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _vp]),
     "gnnb_set2set_attend_bwd": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _vp]),

@@ -502,6 +502,42 @@ int gnnb_ppr_diffusion(gnnb_graph_t g, const float* w, float alpha, const int64_
 int gnnb_ppr_matrix(gnnb_graph_t g, const float* w, float alpha, int64_t a, int64_t b, int64_t ld, float* M_out,
                     void* stream);
 
+/* --------------------------------------------------------- largest Laplacian eigenvalue (csrc/lmax.cu)
+ * replaces: laplacian_lambda_max(g; add_self_loops, dir) (GNNGraphs/src/query.jl:598-610): for every getgraph(g, i) a
+ *           dense normalized_laplacian and KrylovKit's eigsolve(Symmetric(L), x0, 1, :LR) on the host.  Symmetric reads
+ *           the upper triangle, so the value is the largest eigenvalue of S, S[i][j] = S[j][i] = L[i][j] for i < j.
+ * gnnb_laplacian_lambda_max: per segment [base, base + n) of at most GNNB_LMAX_SMEM_MAX_NODES nodes, with
+ *   c[i] = 1 / sqrt(deg[base + i]) in double, row i of S in shared memory (double): for dir = GNNB_DIR_OUT the weights
+ *   of the out-edges i -> t, t >= i, and of the in-edges s -> i, s < i, added at the other end's column in plan order;
+ *   for GNNB_DIR_IN and GNNB_DIR_BOTH (the reference's A' for every dir but :out) the out-edges with t <= i and the
+ *   in-edges with s > i; a self loop is read once.  S[i][j] = -(c[i] a[i][j]) c[j], S[i][i] = 1 - (c[i] (a[i][i] +
+ *   [add_self_loops])) c[i].  Householder tridiagonalisation and Sturm-count multisection to the last bit; lmax_out[s]
+ *   = the upper end of the final bracket (NaN if the tridiagonal matrix is not finite, or the segment has no nodes).
+ *   The bits do not depend on the launch class nor on the segment's position.
+ *   g: a square plan (GNNB_ESIZE otherwise).  w: E DEVICE floats in COO order, or NULL (every weight 1).  deg: n DEVICE
+ *   floats, the caller's row sums of A (dir = out) or A' (gnnb_degree with GNNB_DIR_OUT or GNNB_DIR_IN), plus 1 under
+ *   add_self_loops; the caller rejects zeros (the reference's isolated-node assertion).  seg_ptr: NULL (one segment)
+ *   or n_seg + 1 non-decreasing DEVICE offsets from 0 to n, validated on the device (GNNB_EINVAL).  An edge with one
+ *   end in a segment this entry computes and the other outside it gives GNNB_EINVAL naming the edge.
+ *   lmax_out: n_seg DEVICE doubles.  info: n_seg DEVICE int32s: 0 = computed, -1 = the segment has more than
+ *   GNNB_LMAX_SMEM_MAX_NODES nodes and was skipped (its lmax_out is untouched: the caller runs the Lanczos route).
+ *   Synchronises the stream.
+ * GNNB_LMAX_SMEM_MAX_NODES is the largest n whose n x n doubles and two working vectors fit the 227 KB of one H100
+ * CTA; the entry checks the device's opt-in limit (GNNB_EUNSUPPORTED).
+ * gnnb_segment_dots: out[s][k] = sum over the nodes i of segment s of X[k][i] * y[i] (k < K; X row-major with leading
+ *   dimension ldx >= n, y n doubles; all DEVICE).  The sum runs over chunks of GNNB_SEGDOT_CHUNK nodes counted from
+ *   the segment's start, each added in a fixed order, and the chunk sums in order: deterministic, and the same bits
+ *   wherever the segment lies.  chunk_ptr: n_seg + 1 DEVICE int64 running counts of ceil(len_s / GNNB_SEGDOT_CHUNK),
+ *   n_chunks its last entry; partial: n_chunks * K DEVICE doubles of scratch; seg_ptr as above (not validated: the
+ *   chunk ranges are clamped to [0, n)).  Does not synchronise. */
+#define GNNB_LMAX_SMEM_MAX_NODES 169
+#define GNNB_SEGDOT_CHUNK 2048
+int gnnb_laplacian_lambda_max(gnnb_graph_t g, const float* w, const float* deg, int dir, int add_self_loops,
+                              const int64_t* seg_ptr, int64_t n_seg, double* lmax_out, int32_t* info, void* stream);
+int gnnb_segment_dots(const double* X, int64_t K, int64_t ldx, const double* y, int64_t n, const int64_t* seg_ptr,
+                      const int64_t* chunk_ptr, int64_t n_seg, int64_t n_chunks, double* partial, double* out,
+                      void* stream);
+
 /* --------------------------------------------------------- 1-WL colour refinement (csrc/wl.cu)
  * replaces: color_refinement(g, x0) (GNNGraphs/src/utils.jl:340-389): a host loop hashing (x_i, sort(x[in-neighbours]))
  *           into a Dict once per node per round.

@@ -941,6 +941,57 @@ function GNNGraphs.ppr_diffusion(g::GNNGraph{<:CuCOO}; alpha = 0.85f0)
 end
 ChainRulesCore.@non_differentiable GNNGraphs.ppr_diffusion(::Any...)
 
+## laplacian_lambda_max on device COO graphs — replaces GNNGraphs/src/query.jl:598-610 (per graph a getgraph, a
+## normalized_laplacian and KrylovKit's eigsolve(Symmetric(L), ...) on the host).  A graph, or every graph of a batch,
+## of at most LMAX_SMEM_MAX_NODES nodes: gnnb_laplacian_lambda_max, in one call.  Larger ones: the reference's own method
+## through getgraph.  The degrees are the reference's row sums of A (dir = :out) or A' (every other dir), plus 1 under
+## add_self_loops.
+const LMAX_SMEM_MAX_NODES = 169                               # GNNB_LMAX_SMEM_MAX_NODES
+
+function _lmax_entry(g::GNNGraph, seg, ns, add_self_loops::Bool, dir::Symbol)
+    w = get_edge_weight(g)
+    w = w === nothing ? nothing : CuVector{Float32}(w)
+    deg = CuVector{Float32}(degree(g, Float32; dir = dir == :out ? :out : :in))
+    add_self_loops && (deg .+= 1f0)
+    @assert all(!iszero, Array(deg)) "Graph contains isolated nodes, cannot compute `normalized_adjacency`."
+    out = CuVector{Float64}(undef, ns)
+    info = CuVector{Int32}(undef, ns)
+    sp, _ = _knn_seg_args(seg)
+    d = dir == :out ? Cint(0) : (dir == :in ? Cint(1) : Cint(2))
+    check(ccall((:gnnb_laplacian_lambda_max, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Float32}, CuPtr{Float32}, Cint, Cint, CuPtr{Int64}, Int64, CuPtr{Float64},
+                 CuPtr{Int32}, Ptr{Cvoid}),
+                plan(g).h, cuptr(w), deg, d, Cint(add_self_loops), sp, ns, out, info, stream()))
+    return Array(out), Array(info)
+end
+
+function GNNGraphs.laplacian_lambda_max(g::GNNGraph{<:CuCOO}, T::DataType = Float32;
+                                        add_self_loops::Bool = false, dir::Symbol = :out)
+    if g.num_graphs == 1
+        g.num_nodes <= LMAX_SMEM_MAX_NODES || return invoke(GNNGraphs.laplacian_lambda_max, Tuple{GNNGraph, DataType},
+                                                            g, T; add_self_loops, dir)
+        return T(_lmax_entry(g, nothing, 1, add_self_loops, dir)[1][1])
+    end
+    eigenvalues = zeros(g.num_graphs)
+    gi = g.graph_indicator
+    order, _, seg = _knn_segments(gi, g.num_nodes)
+    s, t = edge_index(g)
+    giv = CuVector{Int64}(gi)
+    if order === nothing && seg !== nothing && length(seg) == g.num_graphs + 1 && all(giv[s] .== giv[t])
+        vals, info = _lmax_entry(g, seg, g.num_graphs, add_self_loops, dir)
+        for i in 1:(g.num_graphs)
+            eigenvalues[i] = info[i] == 0 ? vals[i] :
+                             GNNGraphs._eigmax(normalized_laplacian(getgraph(g, i), T; add_self_loops, dir))
+        end
+        return eigenvalues
+    end
+    for i in 1:(g.num_graphs)                                 # getgraph semantics, graph by graph
+        eigenvalues[i] = laplacian_lambda_max(getgraph(g, i), T; add_self_loops, dir)
+    end
+    return eigenvalues
+end
+ChainRulesCore.@non_differentiable GNNGraphs.laplacian_lambda_max(::Any...)
+
 ## color_refinement on device COO graphs — replaces GNNGraphs/src/utils.jl:340-389 (a host loop that hashes
 ## (x_i, sort(x[in-neighbours])) into a Dict and indexes scalars, so it cannot run on a CuArray graph).  One pass of
 ## gnnb_color_refinement's signature kernel per round and a stable radix sort of the exact (c_i, S_1, S_2) key.  Same

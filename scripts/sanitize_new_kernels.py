@@ -1,6 +1,7 @@
 """small calls of the hand-written dense-layer kernels, the closing line, the max pullback, the subgraph plans, the
 drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), PPR diffusion
-(both launch classes, the dense route's matrix kernel, a seg_ptr an edge crosses), colour
+(both launch classes, the dense route's matrix kernel, a seg_ptr an edge crosses), the largest Laplacian eigenvalue
+(both launch classes, the Lanczos route, a seg_ptr an edge crosses), colour
 refinement (hub rows cut into long-row pieces, a path, a batch) and Set2Set (a graph with no nodes, graphs of chunk +- 1
 nodes, D = 1, 3 and 1024, the composition at D = 1025), meant to run under `compute-sanitizer --tool memcheck`
 (or racecheck / synccheck)"""
@@ -115,6 +116,23 @@ rc = lib.gnnb_ppr_diffusion(gx.plan().h, None, 0.85, seg.data_ptr(), len(sizes),
 M = torch.empty(5, 7, device="cuda")
 rc2 = lib.gnnb_ppr_matrix(gx.plan().h, None, 0.85, 1, 6, 7, M.data_ptr(), None)
 print("ppr_diffusion crossing edge rejected", rc == gnn._lib.EINVAL, rc2 == gnn._lib.EINVAL)
+# laplacian_lambda_max: the same segments plus a ring in each (no isolated nodes), warp and CTA classes, the Lanczos
+# route for the 241-node one above the bound (169), every segment through the CTA class, then the crossing edge
+starts = [sum(sizes[:k]) for k in range(len(sizes))]
+ring_s = torch.cat([torch.arange(m, device="cuda") + o for m, o in zip(sizes, starts)])
+ring_t = torch.cat([(torch.arange(m, device="cuda") + 1) % m + o for m, o in zip(sizes, starts)])
+gl = gnn.GNNGraph(torch.cat([s_, ring_s]) + 1, torch.cat([t_, ring_t]) + 1, num_nodes=off, num_graphs=len(sizes),
+                  graph_indicator=gi)
+print("laplacian_lambda_max", gnn.laplacian_lambda_max(gl).tolist())
+gnn._lib.check(lib.gnnb_set_kernel_variant(12))
+print("laplacian_lambda_max CTA class only", gnn.laplacian_lambda_max(gl).tolist())
+gnn._lib.check(lib.gnnb_set_kernel_variant(0))
+deg = gnn.degree(gx).float().contiguous() + 1
+lm = torch.empty(len(sizes), dtype=torch.float64, device="cuda")
+info = torch.empty(len(sizes), dtype=torch.int32, device="cuda")
+rc = lib.gnnb_laplacian_lambda_max(gx.plan().h, None, deg.data_ptr(), 0, 1, seg.data_ptr(), len(sizes), lm.data_ptr(),
+                                   info.data_ptr(), None)
+print("laplacian_lambda_max crossing edge rejected", rc == gnn._lib.EINVAL)
 # color_refinement: two hubs of 3 000 in-edges (pieces of 128 and the fix-up), a path of 41 nodes, a batch of small graphs
 hs = torch.randint(0, 500, (6000,), device="cuda"); ht = torch.cat([torch.full((3000,), 7, device="cuda"),
                                                                    torch.full((3000,), 499, device="cuda")])
