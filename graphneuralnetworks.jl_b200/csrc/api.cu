@@ -63,7 +63,8 @@ static int check_common(gnnb_graph_t g, int msg, int aggr, int64_t D, const floa
     if (msg != GNNB_COPY_XJ && msg != GNNB_W_MUL_XJ) GNNB_FAIL(GNNB_EINVAL, "unknown message function %d", msg);
     if (aggr < GNNB_SUM || aggr > GNNB_MIN) GNNB_FAIL(GNNB_EINVAL, "unknown aggregation %d", aggr);
     if (D <= 0) GNNB_FAIL(GNNB_ESIZE, "feature dimension must be positive (got %lld)", (long long)D);
-    if (msg == GNNB_W_MUL_XJ && !w) GNNB_FAIL(GNNB_EINVAL, "w_mul_xj/e_mul_xj needs the edge weights");
+    // an edgeless plan's weight vector is empty, and an empty array's pointer may be NULL (torch, CUDA.jl)
+    if (msg == GNNB_W_MUL_XJ && !w && g->E > 0) GNNB_FAIL(GNNB_EINVAL, "w_mul_xj/e_mul_xj needs the edge weights");
     return GNNB_OK;
 }
 

@@ -156,11 +156,13 @@ int gnnb_scatter(gnnb_graph_t g, int which, int aggr, const float* m, int64_t D,
  *           its CPU SpMM specialisations (msgpass.jl:215-238) and the CUDA-ext re-routing
  *           (GNNlib/ext/GNNlibCUDAExt.jl:13-32) — fused: no (D,E) intermediate.
  *   out[:,i] = ct[i] * AGG_{k in N(i)} ( w[k] * cs[s_k] * x[:, s_k] )
- *   x  (D, num_src), out (D, num_dst); w NULL or E floats in COO order (required for W_MUL_XJ);
+ *   x  (D, num_src), out (D, num_dst); w NULL or E floats in COO order (required for W_MUL_XJ when E > 0);
  *   cs NULL or num_src floats, ct NULL or num_dst floats: optional per-node scales fused into the
  *   load / store (GCN's 1/sqrt(d), conv.jl:57-67).  MEAN divides by the in-degree (0 for isolated).
  *   transposed != 0 runs the same reduction on the reversed graph (x is (D,num_dst), out (D,num_src)):
- *   that is the pullback of the SUM/MEAN forward w.r.t. xj (SURVEY.md §9). */
+ *   that is the pullback of the SUM/MEAN forward w.r.t. xj (SURVEY.md §9).  cs still scales the
+ *   gathered node and ct the output row, so there cs has num_dst entries and ct num_src, and MEAN
+ *   divides by the out-degree. */
 int gnnb_propagate(gnnb_graph_t g, int transposed, int msg, int aggr, const float* x,
                    const float* w, const float* cs, const float* ct, int64_t D, float* out,
                    void* stream);

@@ -196,7 +196,7 @@ class FakeLib:
     def gnnb_propagate(self, h, transposed, msg, aggr, x, w, cs, ct, D, out, stream):
         self.calls.append("gnnb_propagate")
         p = self._p(h)
-        if msg == 1 and w is None:
+        if msg == 1 and w is None and p.E > 0:
             return self._fail(EINVAL, "w_mul_xj needs edge weights")
         m, dst, nd = self._messages(p, x, w if msg == 1 else None, cs, D, transposed)
         o = _segment(aggr, m, dst, nd)
