@@ -24,8 +24,9 @@ from .readout import (Set2Set, broadcast_edges, broadcast_nodes, global_attentio
 from .transform import (add_nodes, color_refinement, csr, getgraph, ppr_diffusion, random_walk_pe, remove_edges,
                         remove_multi_edges, remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
 from .temporal import (DCGRU, DCGRUCell, EvolveGCNO, EvolveGCNOCell, GConvGRU, GConvGRUCell, GConvLSTM, GConvLSTMCell,
-                       GNNRecurrence, TemporalSnapshotsGNNGraph, TGCN, TGCNCell, initialstates)
-from .generate import knn_graph, radius_graph
+                       GNNRecurrence, TemporalSnapshotsGNNGraph, TGCN, TGCNCell, add_snapshot, initialstates,
+                       remove_snapshot)
+from .generate import knn_graph, radius_graph, rand_temporal_hyperbolic_graph, rand_temporal_radius_graph
 from .linkpred import (DotDecoder, add_edges, dot_decoder, edge_decoding, edge_encoding, intersect, negative_sample,
                        perturb_edges, rand_edge_split, rand_graph)
 from .sampling import NeighborLoader, induced_subgraph, sample_edge_ids, sample_neighbors

@@ -124,6 +124,11 @@ _SIGS = {
     "gnnb_knn": (_int, [_f32p, _i64, _int, _vp, _i64, _int, _int, _vp, _vp]),
     "gnnb_radius_count": (_int, [_f32p, _i64, _int, _vp, _i64, C.c_float, _int, _vp, C.POINTER(_i64), _vp]),
     "gnnb_radius_fill": (_int, [_f32p, _i64, _int, _vp, _i64, C.c_float, _int, _vp, _vp, _i64, _vp]),
+    "gnnb_temporal_radius_points": (_int, [_i64, _i64, C.c_double, C.c_uint64, _f32p, _vp]),
+    "gnnb_temporal_hyperbolic_records": (_int, [_i64, _i64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_uint64,
+                                                _vp, _vp]),
+    "gnnb_hyperbolic_count": (_int, [_vp, _i64, _vp, _i64, C.c_double, _int, _vp, C.POINTER(_i64), _vp]),
+    "gnnb_hyperbolic_fill": (_int, [_vp, _i64, _vp, _i64, C.c_double, _int, _vp, _vp, _i64, _vp]),
     "gnnb_random_walk_pe": (_int, [_vp, _f32p, _f32p, _vp, _i64, _int, _f32p, _vp]),
     "gnnb_ppr_diffusion": (_int, [_vp, _f32p, C.c_float, _vp, _i64, _f32p, _vp, _vp]),
     "gnnb_ppr_matrix": (_int, [_vp, _f32p, C.c_float, _i64, _i64, _i64, _f32p, _vp]),

@@ -2,7 +2,9 @@
 // graph of a batch), deterministic neighbour order.
 //
 // Reference counterpart: knn_graph / radius_graph (GNNGraphs/src/generate.jl:112-145, 196-222), which build a KDTree /
-// BallTree with NearestNeighbors.jl on the CPU and separate graphs of a batch by an extra dummy coordinate.
+// BallTree with NearestNeighbors.jl on the CPU and separate graphs of a batch by an extra dummy coordinate.  The same
+// count / fill kernels, with the hyperbolic pair test as their policy, build rand_temporal_hyperbolic_graph's snapshots
+// (generate.jl:340-380, a dense n x n adjacency per snapshot there).
 //
 // Contract (the oracle restates it bit for bit):
 //   d2(i, j) = Σ_{f = 0..d-1} (p_i[f] - p_j[f])², ascending f, sub / mul / add each rounded on its own (no FMA);
@@ -10,6 +12,9 @@
 //   the fp32 bits order like the values (bits(d2) + 1 keeps 0 free as a sentinel below every real distance).
 //   knn:    the k smallest keys of the segment (j == i excluded unless self_loops), in ascending key order.
 //   radius: every j of the segment with sqrt_rn(d2) <= r (j == i excluded unless self_loops), in ascending j.
+//   hyperbolic: records (C, S, c, s) of 4 doubles; x(i, j) = C_i C_j - (S_i S_j)(c_i c_j + s_i s_j), every mul / add /
+//   sub rounded on its own (so x(i, j) == x(j, i) bit for bit); j is in the row when the two records are equal or
+//   x <= x_max (a NaN x is not), j == i excluded unless self_loops, in ascending j.
 //
 // Work decomposition: a work item is a query tile of QT consecutive points of one segment (one thread per query), so
 // one segment of 2^18 points gives 2048 items and 1024 segments of 1000 give 8192: both fill the 132 SMs.  The tile
@@ -34,6 +39,7 @@ namespace gnnb {
 namespace knn {
 
 enum { KNN = 0, COUNT = 1, FILL = 2 };
+enum { EUCLID = 0, HYPERBOLIC = 1 };                   // the pair test of the count / fill kernels
 
 constexpr int BUF_FLOATS = 4096;                       // candidate floats per tile
 constexpr int BUF_BYTES = BUF_FLOATS * 4 + 16;         // + the 16 B alignment slack of the tile's first row
@@ -53,6 +59,7 @@ struct Params {
     int* err;                // pipeline stall flag
     int* mismatch;           // FILL: a row's hits differ from offsets[i+1] - offsets[i]
     const int* bad;          // segment validation flags (the item kernel does nothing if set)
+    double xmax;             // HYPERBOLIC: the largest x of an edge
 };
 
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
@@ -63,6 +70,14 @@ __device__ __forceinline__ uint32_t dist_key(float d2) { return __float_as_uint(
 __device__ __forceinline__ float sq_term(float a, float b) {
     const float t = __fsub_rn(a, b);
     return __fmul_rn(t, t);
+}
+
+// x = C_q C_c - (S_q S_c)(c_q c_c + s_q s_c) <= xmax, or the records are equal.  Each operation is rounded on its own and
+// IEEE products and sums commute, so the test is symmetric in q and c bit for bit.
+__device__ __forceinline__ bool hyperbolic_hit(const double* q, const double* c, double xmax) {
+    const double ang = __dadd_rn(__dmul_rn(q[2], c[2]), __dmul_rn(q[3], c[3]));
+    const double x = __dsub_rn(__dmul_rn(q[0], c[0]), __dmul_rn(__dmul_rn(q[1], c[1]), ang));
+    return x <= xmax || (q[0] == c[0] && q[1] == c[1] && q[2] == c[2] && q[3] == c[3]);
 }
 
 // Stage candidates [j0, j0 + cnt) into `buf`: the bulk copy covers the 16 B aligned interior of the byte range, threads
@@ -89,8 +104,10 @@ __device__ __forceinline__ int stage_tile(const Params& p, int j0, int cnt, unsi
     return (int)((lo - a) >> 2);
 }
 
-template <int MODE, int KB, int DREG, int QT>
-__global__ void __launch_bounds__(QT) knn_kernel(const Params p) {
+// The body of the search kernels.  PAIR == HYPERBOLIC: p.pts holds records of d = 8 floats (4 doubles, 8 B aligned),
+// MODE is COUNT or FILL, DREG == 0.
+template <int MODE, int KB, int DREG, int QT, int PAIR>
+__device__ __forceinline__ void pair_search(const Params& p) {
     extern __shared__ __align__(128) unsigned char smem[];
     if (*(volatile const int*)p.bad) return;
     const int64_t item = blockIdx.x;
@@ -113,7 +130,11 @@ __global__ void __launch_bounds__(QT) knn_kernel(const Params p) {
     const int qstride = d | 1;
 
     float q[DREG > 0 ? DREG : 1];
-    if (DREG > 0) {
+    double hq[4];
+    if constexpr (PAIR == HYPERBOLIC) {
+#pragma unroll
+        for (int f = 0; f < 4; ++f) hq[f] = active ? __ldg(reinterpret_cast<const double*>(p.pts) + (size_t)i * 4 + f) : 0.0;
+    } else if (DREG > 0) {
 #pragma unroll
         for (int f = 0; f < (DREG > 0 ? DREG : 1); ++f) q[f] = (active && f < d) ? __ldg(p.pts + (size_t)i * d + f) : 0.f;
     } else {
@@ -166,6 +187,17 @@ __global__ void __launch_bounds__(QT) knn_kernel(const Params p) {
                 const int j = j0 + jl;
                 if (!p.self_loops && j == i) continue;
                 const float* c = cand + jl * d;
+                if constexpr (PAIR == HYPERBOLIC) {
+                    if (hyperbolic_hit(hq, reinterpret_cast<const double*>(c), p.xmax)) {
+                        if (MODE == FILL) {
+                            if (wpos < row_lim) p.nbr[wpos] = j;
+                            ++wpos;
+                        } else {
+                            ++cnt_out;
+                        }
+                    }
+                    continue;
+                }
                 float acc = 0.f;
                 if (DREG > 0) {
 #pragma unroll
@@ -225,6 +257,16 @@ __global__ void __launch_bounds__(QT) knn_kernel(const Params p) {
     }
 }
 
+template <int MODE, int KB, int DREG, int QT>
+__global__ void __launch_bounds__(QT) knn_kernel(const Params p) { pair_search<MODE, KB, DREG, QT, EUCLID>(p); }
+
+// A kernel of its own so that its launch bounds leave knn_kernel's register allocation alone: with __launch_bounds__(128)
+// alone ptxas fits the fill into 40 registers and spills 16 B; with a minimum of 4 CTAs it takes 78 and spills nothing.
+template <int MODE>
+__global__ void __launch_bounds__(128, 4) hyperbolic_kernel(const Params p) {
+    pair_search<MODE, 1, 0, 128, HYPERBOLIC>(p);
+}
+
 // tiles[s] = query tiles of segment s; flags bad |= 1 for a malformed seg_ptr, |= 2 for a non-empty segment with fewer
 // than `need` points
 __global__ void tiles_kernel(const int64_t* __restrict__ seg, int64_t n_seg, int64_t n, int need, int qt,
@@ -239,10 +281,12 @@ __global__ void tiles_kernel(const int64_t* __restrict__ seg, int64_t n_seg, int
     tiles[s] = flag ? 0 : (b - a + qt - 1) / qt;
 }
 
-template <int MODE, int KB, int DREG, int QT>
+template <int MODE, int KB, int DREG, int QT, int PAIR = EUCLID>
 static int launch(const Params& p, int64_t grid, cudaStream_t st) {
-    const size_t smem = 2 * BUF_BYTES + 16 + (DREG == 0 ? (size_t)QT * (p.d | 1) * 4 : 0);
-    auto kern = knn_kernel<MODE, KB, DREG, QT>;
+    const size_t smem = 2 * BUF_BYTES + 16 + (DREG == 0 && PAIR == EUCLID ? (size_t)QT * (p.d | 1) * 4 : 0);
+    void (*kern)(const Params);
+    if constexpr (PAIR == HYPERBOLIC) kern = hyperbolic_kernel<MODE>;
+    else kern = knn_kernel<MODE, KB, DREG, QT>;
     GNNB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<(unsigned)grid, QT, smem, st>>>(p);
     GNNB_LAUNCHED();
@@ -260,10 +304,11 @@ static int dispatch_d(const Params& p, int64_t n, int64_t n_seg, cudaStream_t st
 
 static int query_tile(int d) { return d <= 64 ? 128 : 64; }
 
-// One call: validate + tile the segments, run the MODE kernel, report flags.  Synchronises the stream.
+// One call: validate + tile the segments, run the MODE kernel, report flags.  Synchronises the stream.  pair ==
+// HYPERBOLIC: points are the records (d = 8 floats each) and xmax replaces r.
 static int run(int mode, const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, int k,
                int self_loops, float r, int32_t* nbr, int64_t* counts, const int64_t* offsets, int64_t capacity,
-               cudaStream_t st) {
+               cudaStream_t st, int pair = EUCLID, double xmax = 0.0) {
     DeviceScratch sc(st);
     int64_t* dseg = nullptr;
     int64_t* tiles = nullptr;   // [n_seg + 1 (+ 2 for the default segment)]: counts, then the scan into tile_ptr
@@ -294,8 +339,11 @@ static int run(int mode, const float* points, int64_t n, int d, const int64_t* s
     p.pts = points; p.seg = seg_ptr; p.tile_ptr = tile_ptr; p.n_seg = (int)n_seg; p.d = d; p.k = k;
     p.self_loops = self_loops ? 1 : 0; p.ct = BUF_FLOATS / d > 0 ? BUF_FLOATS / d : 1; p.r = r;
     p.nbr = nbr; p.counts = counts; p.offsets = offsets; p.capacity = capacity;
-    p.err = flags + 1; p.mismatch = flags + 2; p.bad = flags;
-    if (mode == KNN) {
+    p.err = flags + 1; p.mismatch = flags + 2; p.bad = flags; p.xmax = xmax;
+    if (pair == HYPERBOLIC) {
+        if (mode == COUNT) GNNB_TRY((launch<COUNT, 1, 0, 128, HYPERBOLIC>(p, ceil_div(n, 128) + n_seg, st)));
+        else GNNB_TRY((launch<FILL, 1, 0, 128, HYPERBOLIC>(p, ceil_div(n, 128) + n_seg, st)));
+    } else if (mode == KNN) {
         if (k <= 8) GNNB_TRY((dispatch_d<KNN, 8>(p, n, n_seg, st)));
         else if (k <= 16) GNNB_TRY((dispatch_d<KNN, 16>(p, n, n_seg, st)));
         else if (k <= 32) GNNB_TRY((dispatch_d<KNN, 32>(p, n, n_seg, st)));
@@ -313,6 +361,9 @@ static int run(int mode, const float* points, int64_t n, int d, const int64_t* s
     if (h[0] & 2)
         GNNB_FAIL(GNNB_ESIZE, "a segment has fewer than k%s = %d points", self_loops ? "" : " + 1", need);
     if (h[1]) GNNB_FAIL(GNNB_ECUDA, "knn: the candidate pipeline stalled (mbarrier wait timed out)");
+    if (h[2] && pair == HYPERBOLIC)
+        GNNB_FAIL(GNNB_EINVAL, "gnnb_hyperbolic_fill: offsets do not match the rows of these records, x_max, self_loop "
+                               "and segments (nothing was written outside a row's own range)");
     if (h[2])
         GNNB_FAIL(GNNB_EINVAL, "gnnb_radius_fill: offsets do not match the rows of these points, r, self_loops and "
                                "segments (nothing was written outside a row's own range)");
@@ -332,6 +383,58 @@ static int check_common(const char* who, const float* points, int64_t n, int d, 
 static int check_radius(float r) {
     if (r != r || r < 0.f) GNNB_FAIL(GNNB_EINVAL, "radius r = %g must be >= 0 and not NaN", (double)r);
     return GNNB_OK;
+}
+
+static int check_hyperbolic(const char* who, const double* records, int64_t n, const int64_t* seg_ptr, int64_t n_seg,
+                            double x_max) {
+    GNNB_TRY(check_common(who, reinterpret_cast<const float*>(records), n, 8, seg_ptr, n_seg));
+    if (x_max != x_max) GNNB_FAIL(GNNB_EINVAL, "%s: x_max is NaN", who);
+    if ((uintptr_t)records % 8) GNNB_FAIL(GNNB_EINVAL, "%s: records must be 8 B aligned", who);
+    return GNNB_OK;
+}
+
+// The count entries: offsets = running row counts, *total_host = offsets[n].  Synchronises the stream.
+static int count_rows(const char* who, const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg,
+                      float r, int self_loops, int64_t* offsets, int64_t* total_host, cudaStream_t st, int pair,
+                      double xmax) {
+    if (!offsets || !total_host) GNNB_FAIL(GNNB_EINVAL, "%s: offsets / total is NULL", who);
+    *total_host = 0;
+    GNNB_CUDA(cudaMemsetAsync(offsets, 0, sizeof(int64_t), st));
+    if (n == 0) {
+        GNNB_CUDA(cudaStreamSynchronize(st));
+        return GNNB_OK;
+    }
+    DeviceScratch sc(st);
+    int64_t* counts = nullptr;
+    void* tmp = nullptr;
+    GNNB_TRY(sc.alloc(&counts, (size_t)n));
+    GNNB_TRY(run(COUNT, points, n, d, seg_ptr, seg_ptr ? n_seg : 1, 0, self_loops, r, nullptr, counts, nullptr, 0, st,
+                 pair, xmax));
+    size_t tmp_bytes = 0;
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, counts, offsets + 1, (int)n, st));
+    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
+    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, counts, offsets + 1, (int)n, st));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    GNNB_CUDA(cudaMemcpyAsync(total_host, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    return GNNB_OK;
+}
+
+// The fill entries: row i at nbr[offsets[i] .. offsets[i+1]).  Synchronises the stream.
+static int fill_rows(const char* who, const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg,
+                     float r, int self_loops, const int64_t* offsets, int32_t* nbr, int64_t capacity, cudaStream_t st,
+                     int pair, double xmax) {
+    if (!offsets) GNNB_FAIL(GNNB_EINVAL, "%s: offsets is NULL", who);
+    if (n == 0) return GNNB_OK;
+    int64_t total = 0;
+    GNNB_CUDA(cudaMemcpyAsync(&total, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    GNNB_CUDA(cudaStreamSynchronize(st));
+    if (capacity < total)
+        GNNB_FAIL(GNNB_ESIZE, "nbr holds %lld entries, %lld needed", (long long)capacity, (long long)total);
+    if (total == 0) return GNNB_OK;
+    if (!nbr) GNNB_FAIL(GNNB_EINVAL, "%s: nbr is NULL", who);
+    return run(FILL, points, n, d, seg_ptr, seg_ptr ? n_seg : 1, 0, self_loops, r, nbr, nullptr, offsets, capacity, st,
+               pair, xmax);
 }
 
 }  // namespace knn
@@ -356,46 +459,30 @@ int gnnb_radius_count(const float* points, int64_t n, int d, const int64_t* seg_
                       int self_loops, int64_t* offsets, int64_t* total_host, void* stream) {
     GNNB_TRY(knn::check_common("gnnb_radius_count", points, n, d, seg_ptr, n_seg));
     GNNB_TRY(knn::check_radius(r));
-    if (!offsets || !total_host) GNNB_FAIL(GNNB_EINVAL, "gnnb_radius_count: offsets / total is NULL");
-    cudaStream_t st = (cudaStream_t)stream;
-    *total_host = 0;
-    GNNB_CUDA(cudaMemsetAsync(offsets, 0, sizeof(int64_t), st));
-    if (n == 0) {
-        GNNB_CUDA(cudaStreamSynchronize(st));
-        return GNNB_OK;
-    }
-    DeviceScratch sc(st);
-    int64_t* counts = nullptr;
-    void* tmp = nullptr;
-    GNNB_TRY(sc.alloc(&counts, (size_t)n));
-    GNNB_TRY(knn::run(knn::COUNT, points, n, d, seg_ptr, seg_ptr ? n_seg : 1, 0, self_loops, r, nullptr, counts,
-                      nullptr, 0, st));
-    size_t tmp_bytes = 0;
-    GNNB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, counts, offsets + 1, (int)n, st));
-    GNNB_TRY(sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 1));
-    GNNB_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, counts, offsets + 1, (int)n, st));
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    GNNB_CUDA(cudaMemcpyAsync(total_host, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    GNNB_CUDA(cudaStreamSynchronize(st));
-    return GNNB_OK;
+    return knn::count_rows("gnnb_radius_count", points, n, d, seg_ptr, n_seg, r, self_loops, offsets, total_host,
+                           (cudaStream_t)stream, knn::EUCLID, 0.0);
 }
 
 int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,
                      int self_loops, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream) {
     GNNB_TRY(knn::check_common("gnnb_radius_fill", points, n, d, seg_ptr, n_seg));
     GNNB_TRY(knn::check_radius(r));
-    if (!offsets) GNNB_FAIL(GNNB_EINVAL, "gnnb_radius_fill: offsets is NULL");
-    if (n == 0) return GNNB_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    int64_t total = 0;
-    GNNB_CUDA(cudaMemcpyAsync(&total, offsets + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    GNNB_CUDA(cudaStreamSynchronize(st));
-    if (capacity < total)
-        GNNB_FAIL(GNNB_ESIZE, "nbr holds %lld entries, %lld needed", (long long)capacity, (long long)total);
-    if (total == 0) return GNNB_OK;
-    if (!nbr) GNNB_FAIL(GNNB_EINVAL, "gnnb_radius_fill: nbr is NULL");
-    return knn::run(knn::FILL, points, n, d, seg_ptr, seg_ptr ? n_seg : 1, 0, self_loops, r, nbr, nullptr, offsets, capacity,
-                    st);
+    return knn::fill_rows("gnnb_radius_fill", points, n, d, seg_ptr, n_seg, r, self_loops, offsets, nbr, capacity,
+                          (cudaStream_t)stream, knn::EUCLID, 0.0);
+}
+
+int gnnb_hyperbolic_count(const double* records, int64_t n, const int64_t* seg_ptr, int64_t n_seg, double x_max,
+                          int self_loop, int64_t* offsets, int64_t* total_host, void* stream) {
+    GNNB_TRY(knn::check_hyperbolic("gnnb_hyperbolic_count", records, n, seg_ptr, n_seg, x_max));
+    return knn::count_rows("gnnb_hyperbolic_count", reinterpret_cast<const float*>(records), n, 8, seg_ptr, n_seg, 0.f,
+                           self_loop, offsets, total_host, (cudaStream_t)stream, knn::HYPERBOLIC, x_max);
+}
+
+int gnnb_hyperbolic_fill(const double* records, int64_t n, const int64_t* seg_ptr, int64_t n_seg, double x_max,
+                         int self_loop, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream) {
+    GNNB_TRY(knn::check_hyperbolic("gnnb_hyperbolic_fill", records, n, seg_ptr, n_seg, x_max));
+    return knn::fill_rows("gnnb_hyperbolic_fill", reinterpret_cast<const float*>(records), n, 8, seg_ptr, n_seg, 0.f,
+                          self_loop, offsets, nbr, capacity, (cudaStream_t)stream, knn::HYPERBOLIC, x_max);
 }
 
 }  // extern "C"

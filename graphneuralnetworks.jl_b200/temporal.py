@@ -1,7 +1,8 @@
 """Recurrent temporal graph layers — GraphNeuralNetworks/src/layers/temporalconv.jl:
     GNNRecurrence (:121-135), GConvGRUCell / GConvGRU (:200-293), GConvLSTMCell / GConvLSTM (:355-477),
     DCGRUCell / DCGRU (:537-613), EvolveGCNOCell / EvolveGCNO (:678-752), TGCNCell / TGCN (:809-884),
-and a minimal TemporalSnapshotsGNNGraph (GNNGraphs/src/temporalsnapshotsgnngraph.jl:56-100).
+a minimal TemporalSnapshotsGNNGraph (GNNGraphs/src/temporalsnapshotsgnngraph.jl:56-100) with add_snapshot /
+remove_snapshot (:132-145, 192-201).  The temporal graph generators are in generate.py.
 
 Holders carry the reference's field names, so a trained model copies over parameter by parameter.  Arrays are
 Julia-shaped: a static-graph sequence is x (in, T, N), one node row of T·in contiguous floats.
@@ -560,6 +561,30 @@ class TemporalSnapshotsGNNGraph:
 
     def __repr__(self):
         return f"TemporalSnapshotsGNNGraph(num_snapshots={self.num_snapshots})"
+
+
+def add_snapshot(tg: TemporalSnapshotsGNNGraph, t: int, g: GNNGraph) -> TemporalSnapshotsGNNGraph:
+    """GNNGraphs/src/temporalsnapshotsgnngraph.jl:132-145: a new temporal graph with g inserted at time index t
+    (1-based; t = num_snapshots + 1 appends).  tg is not changed."""
+    if tg.num_snapshots > 0:
+        assert g.num_nodes == tg.num_nodes[0], "number of nodes must match"
+    assert t <= tg.num_snapshots + 1, \
+        f"cannot add snapshot at time {t}, the temporal graph has only {tg.num_snapshots} snapshots"
+    if t < 1:
+        raise IndexError(f"time index {t} out of range 1:{tg.num_snapshots + 1}")   # Julia's insert! BoundsError
+    snapshots = list(tg.snapshots)
+    snapshots.insert(t - 1, g)
+    return TemporalSnapshotsGNNGraph(snapshots)
+
+
+def remove_snapshot(tg: TemporalSnapshotsGNNGraph, t: int) -> TemporalSnapshotsGNNGraph:
+    """GNNGraphs/src/temporalsnapshotsgnngraph.jl:192-201: a new temporal graph without the snapshot at time index t
+    (1-based).  tg is not changed."""
+    if not 1 <= t <= tg.num_snapshots:
+        raise IndexError(f"time index {t} out of range 1:{tg.num_snapshots}")         # Julia's deleteat! BoundsError
+    snapshots = list(tg.snapshots)
+    del snapshots[t - 1]
+    return TemporalSnapshotsGNNGraph(snapshots)
 
 
 def initialstates(layer_or_cell):

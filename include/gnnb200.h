@@ -457,6 +457,38 @@ int gnnb_radius_count(const float* points, int64_t n, int d, const int64_t* seg_
 int gnnb_radius_fill(const float* points, int64_t n, int d, const int64_t* seg_ptr, int64_t n_seg, float r,
                      int self_loops, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream);
 
+/* --------------------------------------------------------- temporal graph generators (csrc/tgen.cu, csrc/knn.cu)
+ * replaces: rand_temporal_radius_graph(n, T, speed, r) (GNNGraphs/src/generate.jl:265-284: a BallTree per snapshot)
+ *           and rand_temporal_hyperbolic_graph(n, T; α, R, speed, ζ) (generate.jl:287-297, 340-380: a dense n x n
+ *           Float64 adjacency per snapshot, acosh of every ordered pair).
+ * The random stream: every draw is u(i, τ, k) = (splitmix64(K + c) >> 11) * 2^-53, a double in [0, 1), with
+ *   K = splitmix64(seed), c = ((τ*n + i) << 1) | k; node i, k in {0, 1} its two draws at step τ; τ = 0 is the initial
+ *   placement and τ = t (1 <= t < T) the move that follows snapshot t (1-based), i.e. the one that makes row block t.
+ * Both node-dynamics entries run one thread per node with fp64 state and write snapshot t's rows at t*n .. t*n + n - 1
+ * of one (T*n)-row DEVICE array.  Every fp64 mul / add / sub below is rounded on its own (no FMA); 2π = 2 * 3.14159...
+ * gnnb_temporal_radius_points: pts (T*n, 2) fp32, the round-to-nearest of the state (x, y).  Start x = u(i,0,0),
+ *   y = u(i,0,1).  Move t: ρ = (2 speed) u(i,t,0) - speed, θ = 2π u(i,t,1), x = 1 - |1 - |x + ρ cos θ||, y likewise
+ *   with sin θ (the reference's reflection as written: with speed > 1 a point can leave [0, 1]).
+ * gnnb_temporal_hyperbolic_records: rec (T*n, 4) fp64 records (cosh ζr, sinh ζr, cos θ, sin θ).  Start p = u(i,0,0),
+ *   θ = 2π u(i,0,1).  Move t: p += (2 speed) u(i,t,0) - speed; then p > 1 -> 1 - fmod(p, 1); then p < 0 -> |p|;
+ *   θ += (2 speed) u(i,t,1) - speed (unbounded).  r = (1/α) acosh(1 + (cosh(αR) - 1) p), cosh(αR) on the host.
+ *   α > 0, R >= 0, ζ > 0 and speed finite, cosh(αR) finite, else GNNB_EINVAL.
+ * Both: n, T >= 0 (GNNB_EINVAL); T*n >= 2^31: GNNB_ESIZE before anything is allocated or launched.
+ * gnnb_hyperbolic_count / gnnb_hyperbolic_fill: the contract of gnnb_radius_count / gnnb_radius_fill (the same
+ *   segments, offsets, *total_host, rows in ascending j, recount check) on n records, with the pair test
+ *   x(i, j) = C_i C_j - (S_i S_j)(c_i c_j + s_i s_j), each operation rounded on its own in that order, so that
+ *   x(i, j) == x(j, i) bit for bit: j is in row i when (j != i or self_loop) and (the records are equal or
+ *   x <= x_max).  A NaN x is no edge.  x_max = cosh(ζR) makes this acosh(x)/ζ <= R without an acosh per pair.
+ *   records 8 B aligned, x_max not NaN (GNNB_EINVAL).
+ * All four synchronise the stream. */
+int gnnb_temporal_radius_points(int64_t n, int64_t T, double speed, uint64_t seed, float* pts, void* stream);
+int gnnb_temporal_hyperbolic_records(int64_t n, int64_t T, double alpha, double R, double speed, double zeta,
+                                     uint64_t seed, double* rec, void* stream);
+int gnnb_hyperbolic_count(const double* records, int64_t n, const int64_t* seg_ptr, int64_t n_seg, double x_max,
+                          int self_loop, int64_t* offsets, int64_t* total_host, void* stream);
+int gnnb_hyperbolic_fill(const double* records, int64_t n, const int64_t* seg_ptr, int64_t n_seg, double x_max,
+                         int self_loop, const int64_t* offsets, int32_t* nbr, int64_t capacity, void* stream);
+
 /* --------------------------------------------------------- random-walk structural encoding (csrc/rwpe.cu)
  * replaces: random_walk_pe(g, walk_length) (GNNGraphs/src/transform.jl:975-990): K products of the dense N x N matrix
  *           RW = A * Diagonal(deg_inv), whose diagonals are kept.  Here the walk of each segment runs in shared memory.

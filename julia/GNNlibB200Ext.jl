@@ -27,7 +27,7 @@ using Random
 using Statistics: mean
 using LinearAlgebra: I, inv, SingularException
 using GNNlib: GNNlib, propagate, copy_xj, e_mul_xj, w_mul_xj, expand_srcdst, check_num_nodes
-using GNNGraphs: GNNGraphs, GNNGraph, COO_T, edge_index, get_edge_weight
+using GNNGraphs: GNNGraphs, GNNGraph, COO_T, edge_index, get_edge_weight, TemporalSnapshotsGNNGraph
 
 const LIB = get(ENV, "GNNB200_LIB", "libgnnb200")
 
@@ -533,6 +533,74 @@ function GNNGraphs.radius_graph(points::CuMatrix{Float32}, r::AbstractFloat; gra
     end
     s, t = _knn_coo(centre, ids, dir)
     return GNNGraph((s, t); num_nodes = n, graph_indicator, kws...)
+end
+
+## rand_temporal_radius_graph / rand_temporal_hyperbolic_graph on the device — replace GNNGraphs/src/generate.jl:265-284
+## (a BallTree per snapshot) and :287-297,340-380 (a dense n x n Float64 adjacency per snapshot).  Own names, so that
+## GNNGraphs' array-free methods stay the CPU ones: the node dynamics of all T snapshots run in one launch from the seeded
+## stream of include/gnnb200.h, then every snapshot's edges come from one count and one fill over the T snapshots as T
+## segments.  One read-back of the T + 1 snapshot edge offsets; snapshot t is a slice of the flat rows.
+function _temporal_snapshots(offsets::CuVector{Int64}, nbr::CuVector{Int32}, n, T, dir, weighted, kws)
+    E = length(nbr)
+    counts = offsets[2:end] .- offsets[1:end-1]
+    centre = _ragged_centres(counts, E)                       # 1-based flat rows
+    eoff = Array(offsets[(0:T) .* n .+ 1])
+    snaps = Vector{GNNGraph}(undef, T)
+    for t in 1:T
+        a, b = eoff[t] + 1, eoff[t + 1]
+        sh = (t - 1) * n
+        s, d = _knn_coo(centre[a:b] .- sh, Int64.(nbr[a:b]) .+ (1 - sh), dir)
+        snaps[t] = weighted ? GNNGraph((s, d, CUDA.ones(Float32, b - a + 1)); num_nodes = n, kws...) :
+                              GNNGraph((s, d); num_nodes = n, kws...)
+    end
+    return TemporalSnapshotsGNNGraph(snaps)
+end
+
+function rand_temporal_radius_graph_cuda(n::Int, T::Int, speed::AbstractFloat, r::AbstractFloat; self_loops = false,
+                                         dir = :in, seed = nothing, rng = Random.default_rng(), kws...)
+    @assert dir ∈ (:in, :out)
+    N = n * T
+    pts = CuMatrix{Float32}(undef, 2, N)
+    check(ccall((:gnnb_temporal_radius_points, LIB), Cint, (Int64, Int64, Cdouble, UInt64, CuPtr{Float32}, Ptr{Cvoid}),
+                n, T, speed, _seed(rng, seed), pts, stream()))
+    seg = CuVector{Int64}((0:T) .* n)
+    offsets = CUDA.zeros(Int64, N + 1)
+    total = Ref{Int64}(0)
+    check(ccall((:gnnb_radius_count, LIB), Cint,
+                (CuPtr{Float32}, Int64, Cint, CuPtr{Int64}, Int64, Cfloat, Cint, CuPtr{Int64}, Ref{Int64}, Ptr{Cvoid}),
+                pts, N, 2, seg, T, r, self_loops, offsets, total, stream()))
+    nbr = CuVector{Int32}(undef, total[])
+    total[] > 0 && check(ccall((:gnnb_radius_fill, LIB), Cint,
+                               (CuPtr{Float32}, Int64, Cint, CuPtr{Int64}, Int64, Cfloat, Cint, CuPtr{Int64}, CuPtr{Int32},
+                                Int64, Ptr{Cvoid}),
+                               pts, N, 2, seg, T, r, self_loops, offsets, nbr, total[], stream()))
+    return _temporal_snapshots(offsets, nbr, n, T, dir, false, kws)
+end
+
+function rand_temporal_hyperbolic_graph_cuda(n::Int, T::Int; α::Real, R::Real, speed::Real, ζ::Real = 1,
+                                             self_loop = false, seed = nothing, rng = Random.default_rng(), kws...)
+    @assert T > 1 "The number of snapshots must be greater than 1"
+    @assert α > 0 "α must be greater than 0"
+    ζ > 0 && R >= 0 && all(isfinite, (α, R, speed, ζ)) && isfinite(cosh(α * R)) && isfinite(cosh(ζ * R)) ||
+        throw(ArgumentError("need ζ > 0, R >= 0, finite parameters and finite cosh(αR), cosh(ζR)"))
+    N = n * T
+    rec = CuMatrix{Float64}(undef, 4, N)                      # column = the record (cosh ζr, sinh ζr, cos θ, sin θ)
+    check(ccall((:gnnb_temporal_hyperbolic_records, LIB), Cint,
+                (Int64, Int64, Cdouble, Cdouble, Cdouble, Cdouble, UInt64, CuPtr{Float64}, Ptr{Cvoid}),
+                n, T, α, R, speed, ζ, _seed(rng, seed), rec, stream()))
+    seg = CuVector{Int64}((0:T) .* n)
+    offsets = CUDA.zeros(Int64, N + 1)
+    total = Ref{Int64}(0)
+    x_max = cosh(Float64(ζ) * R)                              # acosh(x)/ζ <= R without an acosh per pair
+    check(ccall((:gnnb_hyperbolic_count, LIB), Cint,
+                (CuPtr{Float64}, Int64, CuPtr{Int64}, Int64, Cdouble, Cint, CuPtr{Int64}, Ref{Int64}, Ptr{Cvoid}),
+                rec, N, seg, T, x_max, self_loop, offsets, total, stream()))
+    nbr = CuVector{Int32}(undef, total[])
+    total[] > 0 && check(ccall((:gnnb_hyperbolic_fill, LIB), Cint,
+                               (CuPtr{Float64}, Int64, CuPtr{Int64}, Int64, Cdouble, Cint, CuPtr{Int64}, CuPtr{Int32},
+                                Int64, Ptr{Cvoid}),
+                               rec, N, seg, T, x_max, self_loop, offsets, nbr, total[], stream()))
+    return _temporal_snapshots(offsets, nbr, n, T, :in, true, kws)   # GNNGraph(adj)'s order, A[nz] = 1 as weights
 end
 
 ## Link prediction on device COO graphs — replace negative_sample (GNNGraphs/src/transform.jl:890-929: a host copy,

@@ -2,8 +2,8 @@
 drop mask, the random-walk encoding (both launch classes, the propagate route, a seg_ptr an edge crosses), PPR diffusion
 (both launch classes, the dense route's matrix kernel, a seg_ptr an edge crosses), the largest Laplacian eigenvalue
 (both launch classes, the Lanczos route, a seg_ptr an edge crosses), colour
-refinement (hub rows cut into long-row pieces, a path, a batch) and Set2Set (a graph with no nodes, graphs of chunk +- 1
-nodes, D = 1, 3 and 1024, the composition at D = 1025), meant to run under `compute-sanitizer --tool memcheck`
+refinement (hub rows cut into long-row pieces, a path, a batch), Set2Set (a graph with no nodes, graphs of chunk +- 1
+nodes, D = 1, 3 and 1024, the composition at D = 1025) and the temporal graph generators, meant to run under `compute-sanitizer --tool memcheck`
 (or racecheck / synccheck)"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -206,5 +206,22 @@ for ns_, nd_ in ((300, 7), (7, 300), (40, 30)):
         xb = torch.randn(12, nd_, device="cuda").requires_grad_(True)
         lg(hg, (xa, xb)).sum().backward()
         print("gat bipartite", ns_, nd_, heads_, C_, "grad finite", bool(torch.isfinite(xa.grad).all() and torch.isfinite(xb.grad).all()))
+# temporal generators: snapshots of 1 node, n = 127 and 129 (the query tile is 128), T = 1 for the radius generator,
+# and the hyperbolic count / fill entries on records starting 8 B off the 16 B grid (head and tail of the bulk copy)
+for n_, T_ in ((1, 3), (127, 4), (129, 4), (129, 1)):
+    tg = gnn.rand_temporal_radius_graph(n_, T_, 0.3, 0.2, seed=n_)
+    print("temporal radius", n_, T_, tg.num_edges)
+    if T_ > 1:
+        th = gnn.rand_temporal_hyperbolic_graph(n_, T_, α=1.0, R=4.0, speed=0.3, self_loop=n_ == 1, seed=n_)
+        print("temporal hyperbolic", n_, T_, th.num_edges)
+import ctypes as _C  # noqa: E402
+recs = torch.empty(4 * 129 + 1, dtype=torch.float64, device="cuda")
+gnn._lib.check(L.gnnb_temporal_hyperbolic_records(129, 1, 1.0, 4.0, 0.3, 1.0, 5, recs[1:].data_ptr(), st0))
+offs = torch.empty(130, dtype=torch.int64, device="cuda"); tot = _C.c_int64(0)
+gnn._lib.check(L.gnnb_hyperbolic_count(recs[1:].data_ptr(), 129, None, 1, 27.3, 0, offs.data_ptr(), _C.byref(tot), st0))
+nb = torch.empty(max(tot.value, 1), dtype=torch.int32, device="cuda")
+gnn._lib.check(L.gnnb_hyperbolic_fill(recs[1:].data_ptr(), 129, None, 1, 27.3, 0, offs.data_ptr(), nb.data_ptr(), tot.value,
+                                      st0))
+print("hyperbolic entries, misaligned records", tot.value)
 torch.cuda.synchronize()
 print("done")
