@@ -19,8 +19,8 @@ from .layers import (AGNNConv, GATConv, GATv2Conv, GCNConv, GINConv, GatedGraphC
 from .layers_more import (CGConv, ChebConv, DConv, EdgeConv, EGNNConv, GMMConv, MEGNetConv, NNConv,
                           ResGatedGraphConv, cg_conv, cheb_conv, d_conv, edge_conv, egnn_conv, gmm_conv, megnet_conv,
                           nn_conv, res_gated_graph_conv)
-from .readout import (Set2Set, broadcast_edges, broadcast_nodes, global_attention_pool, global_pool, reduce_edges,
-                      reduce_nodes, set2set_pool, softmax_edges, softmax_nodes)
+from .readout import (Set2Set, TopKPool, broadcast_edges, broadcast_nodes, global_attention_pool, global_pool,
+                      reduce_edges, reduce_nodes, set2set_pool, softmax_edges, softmax_nodes, topk_index, topk_pool)
 from .transform import (add_nodes, color_refinement, csr, getgraph, ppr_diffusion, random_walk_pe, remove_edges,
                         remove_multi_edges, remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
 from .temporal import (DCGRU, DCGRUCell, EvolveGCNO, EvolveGCNOCell, GConvGRU, GConvGRUCell, GConvLSTM, GConvLSTMCell,

@@ -22,6 +22,7 @@ SUM, MEAN, MAX, MIN = 0, 1, 2, 3
 SRC, DST = 0, 1
 DIR_OUT, DIR_IN, DIR_BOTH = 0, 1, 2
 CODES_DIRECTED, CODES_DIRECTED_NOLOOP, CODES_UNDIRECTED, CODES_UNDIRECTED_NOLOOP, CODES_BIPARTITE = range(5)
+KEY_F32, KEY_F64, KEY_I32, KEY_I64 = range(4)
 
 
 class GNNBError(RuntimeError):
@@ -137,7 +138,12 @@ _SIGS = {
     "gnnb_color_refinement": (_int, [_vp, _vp, _i64, _vp, C.POINTER(_i64), C.POINTER(_i64), _vp]),
     "gnnb_set2set_attend": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _vp]),
     "gnnb_set2set_attend_bwd": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _vp]),
-    "gnnb_gru_rz": (_int, [_f32p, _i64, _f32p, _f32p, _i64, _i64, _f32p, _f32p, _f32p, _vp]),
+    "gnnb_topk_keep": (_int, [_vp, _int, _i64, _vp, _i64, _i64, C.c_double, _vp, _vp, _vp]),
+    "gnnb_topk_score": (_int, [_f32p, _i64, _i64, _f32p, _f32p, _vp]),
+    "gnnb_topk_gate": (_int, [_f32p, _i64, _i64, _f32p, _vp, _i64, _f32p, _vp, _vp]),
+    "gnnb_topk_gate_bwd": (_int, [_f32p, _i64, _i64, _f32p, _f32p, _vp, _i64, _f32p, _f32p, _f32p, _vp, _vp]),
+    "gnnb_topk_set_smem_max": (_int, [_i64]),
+    "gnnb_gru_rz": (_int,[_f32p, _i64, _f32p, _f32p, _i64, _i64, _f32p, _f32p, _f32p, _vp]),
     "gnnb_gru_out": (_int, [_f32p, _i64, _f32p, _f32p, _f32p, _i64, _i64, _int, _f32p, _f32p, _vp]),
     "gnnb_gru_out_bwd": (_int, [_f32p, _f32p, _f32p, _f32p, _i64, _i64, _int, _f32p, _i64, _f32p, _f32p, _vp]),
     "gnnb_gru_rz_bwd": (_int, [_f32p, _f32p, _f32p, _f32p, _f32p, _i64, _i64, _f32p, _i64, _f32p, _vp]),

@@ -121,6 +121,8 @@ struct DeviceState {
     float* bwd_part = nullptr; size_t bwd_part_bytes = 0;       // linear_bwd_tf32x3: split-K partials of dW
     float* bwd_colsum = nullptr; size_t bwd_colsum_bytes = 0;   // linear_bwd_tf32x3: column-sum partials of db
     float* gat_part = nullptr; size_t gat_part_bytes = 0;       // gnnb_gat_logit_terms_bwd: per-block partials of da
+    char* topk_ws = nullptr; size_t topk_ws_bytes = 0;          // gnnb_topk_keep: segment items, histograms, states
+    float* topk_part = nullptr; size_t topk_part_bytes = 0;     // gnnb_topk_gate_bwd: per-block partials of dp
 };
 // the current device's state, created (tensor-core kernels configured, watchdog flag allocated) on first use
 int device_state(DeviceState** out);

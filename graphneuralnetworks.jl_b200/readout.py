@@ -5,15 +5,18 @@
     broadcast_nodes / broadcast_edges  GNNlib/src/utils.jl:105-121
     global_pool, global_attention_pool GNNlib/src/layers/pool.jl:3-12
     set2set_pool, Set2Set              GNNlib/src/layers/pool.jl:29-43, GraphNeuralNetworks/src/layers/pool.jl:126-162
+    topk_index, topk_pool, TopKPool    GNNlib/src/layers/pool.jl:14-27, GraphNeuralNetworks/src/layers/pool.jl:101-123
 
 `NNlib.scatter(aggr, x, graph_indicator)` is a segmented reduce whose "edges" are the nodes and whose "targets" are the
 graphs: a bipartite plan (gnnb_graph_create with num_src = #items, num_dst = #graphs) lets the library's scatter /
 gather / neighbourhood-softmax kernels (and their pullbacks) do all of it.  Set2Set's attention runs on the same plan
-through its own fused kernel (csrc/set2set.cu).
+through its own fused kernel (csrc/set2set.cu).  Top-k pooling selects per graph by a segmented radix select and gates
+the kept rows in one pass (csrc/topk.cu).
 """
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import operator
 
 import torch
@@ -21,8 +24,8 @@ import torch
 from . import _lib
 from . import graph as _graph
 from ._lib import lib
-from .graph import GNNGraph, _Plan, _stream, graph_indicator, rows, unrows
-from .layers import _LSTMCell
+from .graph import GNNGraph, _Plan, _ptr, _stream, graph_indicator, rows, unrows
+from .layers import _LSTMCell, glorot_uniform
 from .msgpass import _EdgeSoftmaxFn, _GatherFn, _ScatterFn, _aggr_code, _f32
 
 
@@ -200,3 +203,184 @@ class Set2Set(torch.nn.Module):
 
     def forward(self, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
         return set2set_pool(self, g, x)
+
+
+# ---------------------------------------------------------------------------------------------- top-k pooling
+# Key dtypes the selection entry takes as they are, and the exact casts of the narrower ones.
+_KEY_CODES = {torch.float32: _lib.KEY_F32, torch.float64: _lib.KEY_F64, torch.int32: _lib.KEY_I32,
+              torch.int64: _lib.KEY_I64}
+_KEY_CASTS = {torch.bool: torch.int32, torch.int8: torch.int32, torch.int16: torch.int32, torch.uint8: torch.int32,
+              torch.float16: torch.float32, torch.bfloat16: torch.float32}
+
+
+def _keep_mask(y: torch.Tensor, dev, k: int, ratio: float, seg_ptr=None) -> torch.Tensor:
+    """uint8 mask of gnnb_topk_keep over the keys y (1-D) on dev: per segment of seg_ptr (None = one), the keys >= the
+    k-th largest non-NaN key (k >= 1), or the ceil(ratio * n_s)-th (k = 0)."""
+    if y.dtype in _KEY_CASTS:
+        y = y.to(_KEY_CASTS[y.dtype])
+    if y.dtype not in _KEY_CODES:
+        raise TypeError(f"top-k selection takes real or integer keys (got {y.dtype})")
+    y = y.to(dev).contiguous()
+    n = y.numel()
+    keep = torch.empty(n, dtype=torch.uint8, device=dev)
+    n_seg = 1 if seg_ptr is None else seg_ptr.numel() - 1
+    with torch.cuda.device(dev):
+        _lib.check(lib.gnnb_topk_keep(y.data_ptr() if n else None, _KEY_CODES[y.dtype], n, _ptr(seg_ptr), n_seg,
+                                      int(k), float(ratio), keep.data_ptr() if n else None, None, _stream(dev)))
+    return keep
+
+
+def topk_index(y: torch.Tensor, k: int) -> torch.Tensor:
+    """GNNlib/src/layers/pool.jl:24-27: the ascending 1-based ids i with y[i] >= the k-th largest value of y (all ties
+    kept; every id when k exceeds the length).  y is a vector or a (1, N) row.  k < 1 is an error, as the reference's
+    `v[end]` of an empty `v`.  NaN rule of this port: a NaN is never kept and does not count toward k."""
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral):
+        raise TypeError(f"topk_index takes an integer k (got {type(k).__name__})")
+    if y.dim() == 2 and y.shape[0] == 1:
+        y = y.reshape(-1)
+    if y.dim() != 1:
+        raise ValueError(f"topk_index takes a vector or a 1 x N row (got shape {tuple(y.shape)})")
+    if k < 1:
+        raise ValueError(f"topk_index needs k >= 1 (got {k}): nlargest(k, y) is empty")
+    if y.numel() == 0:
+        raise ValueError("topk_index of an empty vector: nlargest(k, y) is empty")
+    dev = _graph._compute_device(y)
+    return _keep_mask(y, dev, int(k), 0.0).nonzero().reshape(-1) + 1
+
+
+def _topk_scores(x_rows: torch.Tensor, p: torch.Tensor) -> torch.Tensor:
+    """y = p' x / norm(p) over the node rows of x (gnnb_topk_score), outside autograd: _TopKGateFn's pullback covers it"""
+    n, D = x_rows.shape
+    y = torch.empty(n, dtype=torch.float32, device=x_rows.device)
+    with torch.cuda.device(x_rows.device):
+        _lib.check(lib.gnnb_topk_score(x_rows.data_ptr(), n, D, p.detach().data_ptr(), y.data_ptr(),
+                                       _stream(x_rows.device)))
+    return y
+
+
+class _TopKGateFn(torch.autograd.Function):
+    """out_j = x_{idx_j} σ(y[idx_j]) (gnnb_topk_gate) with y = p' x / norm(p): the pullback (gnnb_topk_gate_bwd) gives
+    dx through the gather and through y, and dp through y.  idx is 0-based and ascending; the selection is not
+    differentiated."""
+
+    @staticmethod
+    def forward(ctx, x_rows, p, y, idx):
+        n, D = x_rows.shape
+        m = idx.numel()
+        out = torch.empty((m, D), dtype=torch.float32, device=x_rows.device)
+        with torch.cuda.device(x_rows.device):
+            _lib.check(lib.gnnb_topk_gate(x_rows.data_ptr(), n, D, y.data_ptr(), idx.data_ptr() if m else None, m,
+                                          out.data_ptr() if m else None, None, _stream(x_rows.device)))
+        ctx.save_for_backward(x_rows, p, y, idx)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x_rows, p, y, idx = ctx.saved_tensors
+        n, D = x_rows.shape
+        m = idx.numel()
+        dout = dout.contiguous()
+        dx = torch.empty_like(x_rows)
+        dp = torch.empty_like(p)
+        with torch.cuda.device(x_rows.device):
+            _lib.check(lib.gnnb_topk_gate_bwd(x_rows.data_ptr(), n, D, y.data_ptr(), p.data_ptr(),
+                                              idx.data_ptr() if m else None, m, dout.data_ptr() if m else None,
+                                              dx.data_ptr(), dp.data_ptr(), None, _stream(x_rows.device)))
+        return dx, dp, None, None
+
+
+def _topk_x(t, x: torch.Tensor):
+    if x.dim() != 2:
+        raise ValueError(f"topk_pool takes a (in_channel, N) matrix (got shape {tuple(x.shape)})")
+    dev = _graph._compute_device(x)
+    x_rows = _f32(rows(x), dev)
+    p = _f32(t.p, dev)
+    if p.shape != (x_rows.shape[1],):
+        raise ValueError(f"p has {tuple(p.shape)} entries; x has {x_rows.shape[1]} rows")
+    return dev, x_rows, p
+
+
+def topk_pool(t, *args):
+    """topk_pool(t, X) — GNNlib/src/layers/pool.jl:14-22: y = p' X / norm(p), idx = topk_index(y, t.k),
+    t.A_tilde .= A[idx, idx], returns X[:, idx] .* σ.(y[idx]').  Julia's broadcast of A[idx, idx] into the (k, k) A_tilde
+    needs m = length(idx) == k, or m == 1 (which fills A_tilde); any other m raises.
+
+    topk_pool(t, g, x) — the same selection applied to every graph of the batch g (t.A is not used): an int t.k keeps
+    min(k, n_i) nodes of graph i plus ties, a float t.k in (0, 1] keeps ceil(k n_i).  Returns (h, x_pooled, idx): h is
+    remove_nodes(g, <the nodes not kept>), x_pooled the gated kept columns, idx their ascending 1-based ids in g."""
+    if len(args) == 2:
+        return _topk_pool_graph(t, *args)
+    (x,) = args
+    if t.A is None:
+        raise ValueError("this TopKPool has no adjacency matrix: call it on a graph, t(g, x)")
+    if isinstance(t.k, bool) or not isinstance(t.k, numbers.Integral):
+        raise TypeError(f"the matrix form of topk_pool takes an integer k (got {t.k!r}); ratios are for graphs")
+    dev, x_rows, p = _topk_x(t, x)
+    n = x_rows.shape[0]
+    assert t.A.shape == (n, n), f"A is {tuple(t.A.shape)}; X has {n} columns"
+    if t.k < 1:
+        raise ValueError(f"topk_pool needs k >= 1 (got {t.k}): nlargest(k, y) is empty")
+    y = _topk_scores(x_rows, p)
+    idx = _keep_mask(y, dev, int(t.k), 0.0).nonzero().reshape(-1)
+    m = idx.numel()
+    if m != t.A_tilde.shape[0] and m != 1:
+        raise ValueError(f"DimensionMismatch: cannot broadcast A[idx, idx] of size ({m}, {m}) into A_tilde of size "
+                         f"{tuple(t.A_tilde.shape)}: {m} scores tie with or exceed the k-th largest, k = {t.k}")
+    with torch.no_grad():
+        ia = idx.to(t.A.device)
+        t.A_tilde[...] = t.A[ia[:, None], ia[None, :]]
+    return unrows(_TopKGateFn.apply(x_rows, p, y, idx))
+
+
+def _topk_pool_graph(t, g: GNNGraph, x: torch.Tensor):
+    from .generate import _segments
+    from .transform import _keep_nodes
+    k = t.k
+    if isinstance(k, bool) or not isinstance(k, numbers.Real):
+        raise TypeError(f"TopKPool's k must be an int or a float ratio (got {k!r})")
+    if isinstance(k, numbers.Integral):
+        if k < 1:
+            raise ValueError(f"topk_pool needs k >= 1 (got {k})")
+        kk, ratio = int(k), 0.0
+    else:
+        if not 0.0 < float(k) <= 1.0:
+            raise ValueError(f"a float k is a ratio in (0, 1] (got {k})")
+        kk, ratio = 0, float(k)
+    assert x.shape[-1] == g.num_nodes, \
+        f"Got {x.shape[-1]} as last dimension size instead of num_nodes={g.num_nodes}"
+    dev, x_rows, p = _topk_x(t, x)
+    n = x_rows.shape[0]
+    y = _topk_scores(x_rows, p)
+    order, seg_ptr = None, None
+    if g.graph_indicator is not None and n > 0:
+        order, seg_ptr, _, _ = _segments(g.graph_indicator, n, dev)
+    if order is None:
+        keep = _keep_mask(y, dev, kk, ratio, seg_ptr)
+    else:                                   # select on the stably sorted keys, scatter the mask back
+        keep = torch.empty(n, dtype=torch.uint8, device=dev)
+        keep[order] = _keep_mask(y[order], dev, kk, ratio, seg_ptr)
+    idx = keep.nonzero().reshape(-1)
+    x_pooled = unrows(_TopKGateFn.apply(x_rows, p, y, idx))
+    return _keep_nodes(g, keep), x_pooled, idx + 1
+
+
+class TopKPool(torch.nn.Module):
+    """TopKPool(adj, k, in_channel) — GraphNeuralNetworks/src/layers/pool.jl:101-123: the adjacency A, k, the float32
+    projection p = glorot_uniform(in_channel) and A_tilde, a (k, k) array of A's dtype on A's device that every
+    forward(X) overwrites with A[idx, idx].  forward(X) is topk_pool(t, X); forward(g, x) is the graph form.  adj may be
+    None for a pool used on graphs only, and there k may be a float ratio in (0, 1]."""
+
+    def __init__(self, adj, k, in_channel: int, device=None):
+        super().__init__()
+        self.A = adj
+        self.k = k
+        self.p = torch.nn.Parameter(glorot_uniform(int(in_channel), device=device).to(torch.float32))
+        if adj is not None:
+            if isinstance(k, bool) or not isinstance(k, numbers.Integral):
+                raise TypeError(f"TopKPool with an adjacency takes an integer k (got {k!r})")
+            self.A_tilde = torch.empty((int(k), int(k)), dtype=adj.dtype, device=adj.device)
+        else:
+            self.A_tilde = None
+
+    def forward(self, *args):
+        return topk_pool(self, *args)

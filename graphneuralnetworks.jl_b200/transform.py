@@ -288,6 +288,11 @@ def remove_nodes(g: GNNGraph, nodes_or_p, *, seed=None) -> GNNGraph:
         keep = _drop_mask(g.num_nodes, nodes_or_p, seed, dev)
     else:
         keep = _id_mask(nodes_or_p, g.num_nodes, dev, "node")
+    return _keep_nodes(g, keep)
+
+
+def _keep_nodes(g: GNNGraph, keep: torch.Tensor) -> GNNGraph:
+    """remove_nodes(g, <the nodes whose uint8 `keep` is 0>) for a mask on g's device."""
     s, t, n, kept, plan = _subgraph(g, keep, None)
     nodes = keep.bool().nonzero().reshape(-1)
     return _with_plan(GNNGraph(s, t, _take(g.w, kept), num_nodes=n,

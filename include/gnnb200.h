@@ -614,6 +614,50 @@ int gnnb_set2set_attend_bwd(gnnb_graph_t g, const float* x, const float* q, cons
                             const float* seg_max, const float* seg_sum, const float* dr, int64_t D,
                             float* dxe, float* dq, void* stream);
 
+/* --------------------------------------------------------- top-k pooling (csrc/topk.cu)
+ * replaces: topk_index(y, k) = collect(1:length(y))[y .>= nlargest(k, y)[end]] and the score and gate of
+ *           topk_pool(t, X) = view(X, :, idx) .* σ.(view(y, idx)'), y = t.p' * X / norm(t.p)
+ *           (GNNlib/src/layers/pool.jl:14-27), per graph of a batch.
+ * All arrays are DEVICE arrays.  No entry synchronises, and every result is run-to-run bit-identical (no float atomics).
+ * Inputs that only the device can check are reported through dev_status (a DEVICE int32, may be NULL): the entry sets it
+ * to GNNB_OK or to the status of what it found, in stream order; the host-checked errors are returned as usual.
+ *
+ * gnnb_topk_keep: keep[i] (uint8) = 1 iff keys[i] >= v_s, v_s the k_s-th largest non-NaN key of i's segment, else 0.
+ *   k_s = min(k, n_s) for k >= 1 (ratio must be 0), or ceil(ratio * n_s) in double for k = 0 and 0 < ratio <= 1; any
+ *   other (k, ratio) is GNNB_EINVAL.  n_s counts the segment's keys, NaNs included.  A NaN key is never kept and does
+ *   not count toward k_s: with fewer than k_s non-NaN keys every non-NaN key is kept, with none nothing is.  -0.0 and
+ *   +0.0 are equal (ties).  Every key equal to v_s is kept, so a segment can keep more than k_s.
+ *   key_type: GNNB_KEY_F32 | F64 | I32 | I64 (GNNB_EINVAL otherwise).  n in [0, 2^31) (GNNB_ESIZE).
+ *   seg_ptr: NULL (one segment) or n_seg + 1 non-decreasing offsets from 0 to n, n_seg in [1, 2^31) (GNNB_ESIZE),
+ *   validated on the device: a malformed seg_ptr sets dev_status to GNNB_EINVAL and keep to 0 everywhere.
+ *   Segments of up to GNNB_TOPK_SMEM_MAX keys are selected by one CTA each in shared memory, larger ones by multi-block
+ *   histogram passes; the masks are the same.  Scratch: the library's grow-only workspace of the device.
+ * gnnb_topk_score: y[j] = <p, x_j> / sqrt(Σ_d p_d²) for the n node rows x_j (x (D, n) column-major, row j at x + j*D).
+ * gnnb_topk_gate: out_j = x_{idx_j} σ(y[idx_j]) for j < m (out (D, m) column-major), idx 0-based int64;
+ *   σ(a) = 1 / (1 + t) for a >= 0, t / (1 + t) otherwise, t = exp(-|a|) (NNlib's sigmoid).  An idx_j outside [0, n)
+ *   sets dev_status to GNNB_EINDEX and out_j to NaN.
+ * gnnb_topk_gate_bwd: the pullback of y -> gate(x, y) with y = score(x, p), given dout (D, m); s_j = σ(y[idx_j]),
+ *   dy_j = s_j (1 - s_j) <dout_j, x_{idx_j}>:
+ *     dx_{idx_j} = s_j dout_j + dy_j p / ‖p‖, every other row of dx exactly 0;
+ *     dp = (Σ_j dy_j x_{idx_j}) / ‖p‖ - (Σ_j dy_j y[idx_j]) p / ‖p‖²   (per-block partials, then the blocks in order).
+ *   idx must be strictly ascending in [0, n): m > n is GNNB_EINDEX, any other violation sets dev_status to GNNB_EINDEX
+ *   and leaves that row's dx and dp terms out.  Scratch: GNNB_TOPK_DP_SLOTS(m) * (D + 1) floats of the workspace.
+ * Row loads are float4 when D % 4 == 0 and the arrays are 16 B aligned, scalar otherwise.  n, m >= 0 and D >= 1
+ * (GNNB_ESIZE), a NULL array of positive size: GNNB_ESIZE. */
+typedef enum { GNNB_KEY_F32 = 0, GNNB_KEY_F64 = 1, GNNB_KEY_I32 = 2, GNNB_KEY_I64 = 3 } gnnb_key_type;
+#define GNNB_TOPK_SMEM_MAX 8192
+#define GNNB_TOPK_DP_SLOTS(m) ((m) < 65536 ? ((m) + 63) / 64 : 1024)
+int gnnb_topk_keep(const void* keys, int key_type, int64_t n, const int64_t* seg_ptr, int64_t n_seg, int64_t k,
+                   double ratio, uint8_t* keep, int32_t* dev_status, void* stream);
+int gnnb_topk_score(const float* x, int64_t n, int64_t D, const float* p, float* y, void* stream);
+int gnnb_topk_gate(const float* x, int64_t n, int64_t D, const float* y, const int64_t* idx, int64_t m, float* out,
+                   int32_t* dev_status, void* stream);
+int gnnb_topk_gate_bwd(const float* x, int64_t n, int64_t D, const float* y, const float* p, const int64_t* idx,
+                       int64_t m, const float* dout, float* dx, float* dp, int32_t* dev_status, void* stream);
+/* tuning knob for tests and timing: segments of more than `bound` keys take the multi-block class of gnnb_topk_keep
+ * (0 <= bound <= GNNB_TOPK_SMEM_MAX, GNNB_EINVAL otherwise; default GNNB_TOPK_SMEM_MAX). */
+int gnnb_topk_set_smem_max(int64_t bound);
+
 /* --------------------------------------------------------- recurrent gates (csrc/recurrent.cu)
  * The gate arithmetic of the recurrent temporal cells (GraphNeuralNetworks/src/layers/temporalconv.jl), one pass over
  * node rows per entry instead of about ten broadcasts with their own (out, N) temporaries.  Arrays are DEVICE floats in

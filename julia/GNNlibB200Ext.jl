@@ -1146,6 +1146,72 @@ function GNNlib.set2set_pool(l, g::GNNGraph{<:CuCOO}, x::CuMatrix{Float32})
     return qstar
 end
 
+## topk_index / topk_pool on device arrays — replace GNNlib/src/layers/pool.jl:14-27.  The selection is gnnb_topk_keep
+## (one segment; NaN never kept nor counted, this library's rule), the score and gate are one pass each over X, and the
+## rrule of the gate calls gnnb_topk_gate_bwd, which gives dX through the gather and through y, and dp through y.
+const KEY_F32, KEY_F64, KEY_I32, KEY_I64 = Cint(0), Cint(1), Cint(2), Cint(3)
+_key_type(::Type{Float32}) = KEY_F32
+_key_type(::Type{Float64}) = KEY_F64
+_key_type(::Type{Int32}) = KEY_I32
+_key_type(::Type{Int64}) = KEY_I64
+
+function _topk_keep(y::CuVector{T}, k::Integer) where {T<:Union{Float32, Float64, Int32, Int64}}
+    k >= 1 || throw(ArgumentError("topk_index needs k >= 1 (got $k)"))
+    n = length(y)
+    keep = CuVector{UInt8}(undef, n)
+    check(ccall((:gnnb_topk_keep, LIB), Cint,
+                (CuPtr{Cvoid}, Cint, Int64, Ptr{Cvoid}, Int64, Int64, Cdouble, CuPtr{UInt8}, Ptr{Cvoid}, Ptr{Cvoid}),
+                y, _key_type(T), n, C_NULL, 1, k, 0.0, keep, C_NULL, stream()))
+    return keep
+end
+ChainRulesCore.@non_differentiable _topk_keep(::Any...)
+
+GNNlib.topk_index(y::CuVector{T}, k::Int) where {T<:Union{Float32, Float64, Int32, Int64}} =
+    findall(!iszero, _topk_keep(y, k))
+
+function _topk_score(X::CuMatrix{Float32}, p::CuVector{Float32})
+    D, n = size(X)
+    y = CuVector{Float32}(undef, n)
+    check(ccall((:gnnb_topk_score, LIB), Cint, (CuPtr{Float32}, Int64, Int64, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                X, n, D, p, y, stream()))
+    return y
+end
+ChainRulesCore.@non_differentiable _topk_score(::Any...)
+
+function topk_gate(X::CuMatrix{Float32}, p::CuVector{Float32}, y::CuVector{Float32}, idx::CuVector{Int64})
+    D, n = size(X)
+    m = length(idx)
+    out = CuMatrix{Float32}(undef, D, m)
+    check(ccall((:gnnb_topk_gate, LIB), Cint,
+                (CuPtr{Float32}, Int64, Int64, CuPtr{Float32}, CuPtr{Int64}, Int64, CuPtr{Float32}, Ptr{Cvoid}, Ptr{Cvoid}),
+                X, n, D, y, idx, m, out, C_NULL, stream()))
+    return out
+end
+
+function ChainRulesCore.rrule(::typeof(topk_gate), X::CuMatrix{Float32}, p::CuVector{Float32}, y::CuVector{Float32},
+                              idx::CuVector{Int64})
+    out = topk_gate(X, p, y, idx)
+    function topk_gate_pullback(Δ)
+        dout = CuMatrix{Float32}(unthunk(Δ))
+        D, n = size(X)
+        dX, dp = similar(X), similar(p)
+        check(ccall((:gnnb_topk_gate_bwd, LIB), Cint,
+                    (CuPtr{Float32}, Int64, Int64, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Int64}, Int64, CuPtr{Float32},
+                     CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}, Ptr{Cvoid}),
+                    X, n, D, y, p, idx, length(idx), dout, dX, dp, C_NULL, stream()))
+        return NoTangent(), dX, dp, NoTangent(), NoTangent()
+    end
+    return out, topk_gate_pullback
+end
+
+function GNNlib.topk_pool(t, X::CuMatrix{Float32})
+    p = CuVector{Float32}(t.p)
+    y = _topk_score(X, p)
+    idx = ChainRulesCore.ignore_derivatives(() -> CuVector{Int64}(findall(!iszero, _topk_keep(y, t.k)) .- 1))
+    ChainRulesCore.ignore_derivatives(() -> (t.Ã .= view(t.A, Array(idx) .+ 1, Array(idx) .+ 1)))
+    return topk_gate(X, p, y, idx)
+end
+
 ## The gates of the recurrent temporal cells (GraphNeuralNetworks/src/layers/temporalconv.jl) — one pass over node
 ## columns per call instead of the cells' broadcasts.  px (G·D, N): the x-side pre-activations of the G gates ([r; z; n]
 ## for the GRU cells, [i; f; c; o] for the LSTM); ah the h-side ones; every array a dense CuMatrix (node stride = rows).

@@ -223,5 +223,26 @@ nb = torch.empty(max(tot.value, 1), dtype=torch.int32, device="cuda")
 gnn._lib.check(L.gnnb_hyperbolic_fill(recs[1:].data_ptr(), 129, None, 1, 27.3, 0, offs.data_ptr(), nb.data_ptr(), tot.value,
                                       st0))
 print("hyperbolic entries, misaligned records", tot.value)
+# top-k pooling: both selection classes (a batch with empty and bound + 1 segments, the bound forced to 0), f64 keys,
+# the gate and its pullback at D = 3 and 129 from a 4 B offset, and the layer in both forms
+kv = torch.randn(9000, dtype=torch.float64, device="cuda")
+segk = torch.tensor([0, 0, 23, 500, 500, 9000], dtype=torch.int64, device="cuda")
+kp = torch.empty(9000, dtype=torch.uint8, device="cuda")
+for b_ in (None, 0):
+    if b_ is not None:
+        gnn._lib.check(L.gnnb_topk_set_smem_max(b_))
+    gnn._lib.check(L.gnnb_topk_keep(kv.data_ptr(), 1, 9000, segk.data_ptr(), 5, 0, 0.5, kp.data_ptr(), None, st0))
+    print("topk keep, bound", b_, int(kp.sum()))
+gnn._lib.lib.gnnb_topk_set_smem_max(8192)
+gk = gnn.GNNGraph(torch.arange(1, 301, device="cuda"), torch.arange(300, 0, -1, device="cuda"), num_nodes=300,
+                  num_graphs=3, graph_indicator=torch.arange(300, device="cuda") // 100 + 1)
+for D_ in (3, 129):
+    xb = torch.randn(300 * D_ + 1, device="cuda", requires_grad=True)
+    xk = xb[1:].view(300, D_).t()
+    tr = gnn.TopKPool(torch.rand(300, 300, device="cuda"), 7, D_, device="cuda")
+    tr(xk).sum().backward()
+    hk, xpk, _ = gnn.TopKPool(None, 0.3, D_, device="cuda")(gk, xk)
+    xpk.sum().backward()
+    print("topk both forms", D_, hk.num_nodes, bool(torch.isfinite(xb.grad).all()))
 torch.cuda.synchronize()
 print("done")
