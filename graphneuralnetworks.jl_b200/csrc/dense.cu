@@ -224,7 +224,7 @@ extern "C" {
 int gnnb_dense_set_tensor_core_kernel(int on) { g_tc_enabled = on ? 1 : 0; return GNNB_OK; }
 int gnnb_dense_tc_error(void) { return linear_tf32x3_error(); }
 int gnnb_dense_set_emulation(int on) { lt::want_emulation = on ? 1 : 0; if (on && lt::emulation == 0) lt::emulation = -1; return GNNB_OK; }
-int gnnb_dense_emulation_active(void) { return lt::emulation; }
+int gnnb_dense_emulation_active(void) { return lt::want_emulation ? lt::emulation : 0; }
 
 int gnnb_linear(const float* x, const float* W, const float* bias, int relu, int64_t N, int64_t Din, int64_t Dout,
                 float* y, void* stream) {
@@ -381,7 +381,7 @@ int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float
         const int rc = linear_tf32x3(dpre, s->wt, nullptr, 0, N, Dout, Din, dx, st);
         if (rc == GNNB_OK) dx = nullptr;
         else if (rc != GNNB_EUNSUPPORTED) return rc;
-    } else if (dx && g_tc_enabled && (Dout > 128 || Din > 128) && Dout % 32 == 0 && Dout <= 2048 && Din % 128 == 0 && Din <= 1024 &&
+    } else if (dx && g_tc_enabled && (Dout > 128 || Din > 128) && Dout % 32 == 0 && Dout <= 512 && Din % 128 == 0 && Din <= 1024 &&
                N >= 2048) {
         // wide shapes: the same product through the wide wgmma kernel on a transposed copy of W (<= 8 MB, kept)
         DeviceState* s = nullptr;

@@ -758,6 +758,9 @@ constexpr int XSTAGE = 3;
 constexpr int XSTAGE_BYTES = 4 * KBLK_BYTES;                    // X big, X small, W big, W small: 64 KB
 constexpr int SMEM_BIAS_X = XSTAGE * XSTAGE_BYTES;
 constexpr int MAX_NOUT = 1024;
+// the longest K: the big*big chain of K/8 accumulations on the tensor core's accumulator drifts with K, and at K = 1024 with
+// all-positive operands (2048 with any) it left the normwise 5e-6 of float64 on an H100; longer K goes to the library GEMM
+constexpr int MAX_K = 512;
 constexpr int SMEM_BAR_X = SMEM_BIAS_X + MAX_NOUT * 4;
 constexpr int SMEM_TOTAL_X = SMEM_BAR_X + 64;
 
@@ -962,7 +965,7 @@ static int linear_launch(const float* x, const float* W, int64_t ldw, const floa
     const bool wide = K > 128 || Nout > 128;
     if (wide) {
         // (a handful of row tiles cannot fill the machine: the library GEMM takes those)
-        if (K % 32 != 0 || K > 2048 || Nout % 128 != 0 || Nout > tcx::MAX_NOUT || ldw % 4 != 0 || ldw < K || M < 2048) return GNNB_EUNSUPPORTED;
+        if (K % 32 != 0 || K > tcx::MAX_K || Nout % 128 != 0 || Nout > tcx::MAX_NOUT || ldw % 4 != 0 || ldw < K || M < 2048) return GNNB_EUNSUPPORTED;
     } else if (K % 32 != 0 || Nout % 16 != 0 || Nout < 16 || ldw % 4 != 0 || ldw < K || M > RING_MAX_ROWS) {
         return GNNB_EUNSUPPORTED;
     }

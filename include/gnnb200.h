@@ -252,23 +252,27 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
 /* ------------------------------------------------------- dense layer part
  * replaces: l.σ.(weight * x .+ l.bias) of the conv layers (GNNlib/src/layers/conv.jl:39,69-71; :281) and its pullback.
  * Din, Dout <= 128: hand-written wgmma kernels (csrc/dense_tc.cu: 3xTF32 split, register accumulators, bias/relu
- * epilogue, W resident in shared memory); Din % 32 == 0 <= 2048 and Dout % 128 == 0 <= 1024 with at
+ * epilogue, W resident in shared memory); Din % 32 == 0 <= 512 and Dout % 128 == 0 <= 1024 with at
  * least 2048 nodes: the wide wgmma kernel of the same file (both operands streamed, W through cp.async.bulk; forward and
  * dx); every other shape: a library GEMM like the reference's, issued through cuBLASLt 12.9
  * with the fp32-emulated compute type where the library offers it (bf16 x9, fp32 accumulate), else the fp32 sgemm, bias (+relu) in the epilogue.  x (Din,N), W (Dout,Din) row-major as the layer stores it, bias NULL or Dout floats, y (Dout,N).
- * relu: 0 = identity, 1 = relu. */
+ * relu: 0 = identity, 1 = relu.  x, W or y off a 16 B boundary: the library GEMM; bias may sit anywhere.  The tensor-core
+ * routes keep subnormal split parts (x around 2^-115 met the same bound as normal operands on an H100): no flush floor. */
 int gnnb_linear(const float* x, const float* W, const float* bias, int relu, int64_t N, int64_t Din,
                 int64_t Dout, float* y, void* stream);
 /* pullback: dy (Dout,N); y = forward output (relu only); dpre_ws = (Dout,N) workspace (relu only);
  * outputs (each may be NULL): dx (Din,N), dW (Dout,Din), db (Dout).  The relu mask x upstream gradient and the bias
- * gradient are one hand-written pass (deterministic two-stage column sum). */
+ * gradient are one hand-written pass (deterministic two-stage column sum): with relu or db it needs Dout % 4 == 0 <= 1024
+ * and dy (relu: also y, dpre_ws) 16 B aligned, GNNB_EUNSUPPORTED otherwise; any other operand off its boundary sends its
+ * product to the library GEMM. */
 int gnnb_linear_bwd(const float* dy, const float* y, const float* x, const float* W, int relu, int64_t N,
                     int64_t Din, int64_t Dout, float* dpre_ws, float* dx, float* dW, float* db, void* stream);
 /* The relu layer with its mask kept as bits: gnnb_linear (relu = 1) that also writes mask (N x 4 words, 16 B aligned), bit
  * by bit `y > 0` of y as stored, in a layout private to the library; gnnb_linear_bwd_mask is gnnb_linear_bwd (relu = 1)
  * reading that mask instead of y, 16 B instead of 512 per node, with the same bits in dx, dW and db.  dx and dW are both
- * required there, db may be NULL.  Both serve Dout = 128, Din in {32, 64, 96, 128} with 16 B-aligned operands and the
- * tensor-core kernels on (gnnb_dense_set_tensor_core_kernel); GNNB_EUNSUPPORTED otherwise (use the y entries). */
+ * required there, db may be NULL.  Both serve Dout = 128, Din in {32, 64, 96, 128} with the tensor-core kernels on
+ * (gnnb_dense_set_tensor_core_kernel) and 16 B-aligned x, W, y, mask (forward) or dy, mask, x, dx (pullback; W, dW and db
+ * may sit anywhere); GNNB_EUNSUPPORTED otherwise (use the y entries). */
 int gnnb_linear_relu_mask(const float* x, const float* W, const float* bias, int64_t N, int64_t Din, int64_t Dout, float* y,
                           uint32_t* mask, void* stream);
 int gnnb_linear_bwd_mask(const float* dy, const uint32_t* mask, const float* x, const float* W, int64_t N, int64_t Din,
@@ -277,7 +281,9 @@ int gnnb_linear_bwd_mask(const float* dy, const uint32_t* mask, const float* x, 
  * temporary: the two column blocks of W (Dout, Din1+Din2, row-major as the layer stores it) meet x1 (Din1,N) and x2 (Din2,N)
  * in two passes of the wgmma kernel, the second adding the first's result before bias / activation.  Pullback: dx1, dx2,
  * dW (Dout, Din1+Din2), db, each may be NULL.  Shapes: Din1, Din2 multiples of 32 <= 128, Dout = 128 (forward also Dout a
- * multiple of 16 <= 128); GNNB_EUNSUPPORTED otherwise (callers concatenate and use gnnb_linear). */
+ * multiple of 16 <= 128; a second block of 128 < Din2 <= 512 with at least 2048 nodes takes the wide kernel).  16 B-aligned
+ * x1, x2, W, y (forward); dy, y, dpre_ws, and x1, x2, dx1, dx2 where requested (pullback; W, dW, db anywhere);
+ * GNNB_EUNSUPPORTED otherwise (callers concatenate and use gnnb_linear). */
 int gnnb_linear2(const float* x1, const float* x2, const float* W, const float* bias, int relu, int64_t N, int64_t Din1,
                  int64_t Din2, int64_t Dout, float* y, void* stream);
 int gnnb_linear2_bwd(const float* dy, const float* y, const float* x1, const float* x2, const float* W, int relu, int64_t N,
@@ -286,11 +292,12 @@ int gnnb_linear2_bwd(const float* dy, const float* y, const float* x1, const flo
 /* y = act(x .+ bias) on (D,N) features and its pullback, for layers whose closing `σ.(x .+ bias)` follows an aggregation
  * rather than a GEMM (GATConv: GNNlib/src/layers/conv.jl:149): one pass each instead of the broadcast-add, the
  * activation, the mask product and the column reduction.  bias NULL or D floats; relu 0/1; y may alias x.
- * bwd: dpre = dy .* (y > 0) (relu only; dpre may alias dy), db = sum over nodes of dpre (NULL to skip; deterministic). */
+ * bwd: dpre = dy .* (y > 0) (relu only; dpre may alias dy), db = sum over nodes of dpre (NULL to skip; deterministic).
+ * D % 4 == 0 (bwd: <= 1024) and x, y, bias (bwd: dy, y, dpre) 16 B aligned; GNNB_EUNSUPPORTED otherwise. */
 int gnnb_bias_act(const float* x, const float* bias, int relu, int64_t N, int64_t D, float* y, void* stream);
 int gnnb_bias_act_bwd(const float* dy, const float* y, int relu, int64_t N, int64_t D, float* dpre, float* db, void* stream);
 /* 1 (default) = try the fp32-emulated tensor-core GEMM; 0 = force the SIMT sgemm.  *_active: -1 not yet used,
- * 0 unavailable / off, 1 in use. */
+ * 0 unavailable / off, 1 in use (1 on an H100 with cuBLASLt 12.9). */
 int gnnb_dense_set_emulation(int on);
 /* The hand-written wgmma kernels (csrc/dense_tc.cu: 3xTF32 split, register accumulators, bias/relu epilogue) serve
  * Din, Dout <= 128 (Din % 32 == 0, Dout % 16 == 0) and the wide shapes named above for gnnb_linear and the dx part of

@@ -826,52 +826,6 @@ def test_halo_addressing_on_both_kernels_and_gather_rows(graph, oracle, gnn, var
 
 
 # --------------------------------------------------------------------------------------------- dense layer part
-@pytest.mark.parametrize("N,Din,Dout", [(1000, 128, 128), (777, 16, 8), (5000, 64, 256), (33, 1432, 16), (0, 8, 8),
-                                        (4096, 64, 128), (130000, 128, 64), (300, 32, 16), (129, 96, 48), (1, 128, 128),
-                                        (400000, 128, 128), (70001, 96, 128),
-                                        # the wide wgmma kernel (K or Nout above 128, N >= 2048): GATConv 512 -> 8 x 64, config 5
-                                        (40000, 512, 512), (3000, 256, 256), (20001, 512, 128), (2048, 160, 384),
-                                        (9000, 1024, 1024)])
-@pytest.mark.parametrize("relu_flag,with_bias", [(1, True), (0, True), (1, False), (0, False)])
-@pytest.mark.parametrize("emulate", [1, 0])
-def test_linear_c_abi(gnn, N, Din, Dout, relu_flag, with_bias, emulate):
-    # emulate=1: hand-written wgmma 3xTF32 kernel where the shape allows, cuBLASLt fp32-emulated GEMM elsewhere;
-    # emulate=0: cuBLASLt SIMT sgemm only (tensor-core kernel switched off)
-    """gnnb_linear / gnnb_linear_bwd (σ.(W*x .+ b), conv.jl:69-71) against fp64: the fp32-emulated tensor-core GEMM must
-    stay inside the 1e-5 bar, like the SIMT sgemm."""
-    lib = gnn._lib.lib
-    lib.gnnb_dense_set_emulation(emulate)
-    lib.gnnb_dense_set_tensor_core_kernel(emulate)
-    try:
-        gen = torch.Generator(device="cuda").manual_seed(N + Din)
-        x = torch.randn(N, Din, device="cuda", generator=gen)
-        W = torch.randn(Dout, Din, device="cuda", generator=gen) / Din ** 0.5
-        b = torch.randn(Dout, device="cuda", generator=gen) if with_bias else None
-        dy = torch.randn(N, Dout, device="cuda", generator=gen)
-        y = torch.empty(N, Dout, device="cuda")
-        gnn._lib.check(lib.gnnb_linear(x.data_ptr(), W.data_ptr(), None if b is None else b.data_ptr(), relu_flag, N, Din,
-                                       Dout, y.data_ptr(), None))
-        pre = x.double() @ W.double().t() + (0 if b is None else b.double())
-        ref = pre.clamp(min=0) if relu_flag else pre
-        if N:
-            assert rel(y.cpu(), ref.cpu()) < 5e-6
-        ws = torch.empty_like(dy); dx = torch.empty_like(x); dW = torch.empty_like(W); db = torch.empty(Dout, device="cuda")
-        gnn._lib.check(lib.gnnb_linear_bwd(dy.data_ptr(), y.data_ptr(), x.data_ptr(), W.data_ptr(), relu_flag, N, Din, Dout,
-                                           ws.data_ptr(), dx.data_ptr(), dW.data_ptr(), db.data_ptr(), None))
-        dpre = dy.double() * (y > 0) if relu_flag else dy.double()
-        if N:
-            assert rel(dx.cpu(), (dpre @ W.double()).cpu()) < 5e-6
-            assert rel(dW.cpu(), (dpre.t() @ x.double()).cpu()) < 5e-6
-            assert rel(db.cpu(), dpre.sum(0).cpu()) < 5e-6
-        else:
-            assert (db == 0).all()
-        assert lib.gnnb_dense_emulation_active() in (-1, 0, 1)
-        assert lib.gnnb_dense_tc_error() == 0          # the wgmma pipeline never timed out
-    finally:
-        lib.gnnb_dense_set_emulation(1)
-        lib.gnnb_dense_set_tensor_core_kernel(1)
-
-
 def test_linear_wide_accumulation_drift(gnn):
     """All-positive operands at K = 512: every product has the same sign, the case in which the tensor core's truncating
     accumulator drifts most.  The wide kernel keeps the full-magnitude chain at K/8 accumulations; the bar stays 5e-6."""
@@ -1094,39 +1048,6 @@ def test_gat_logit_terms_c_abi(gnn, Cc, H, n):
     da_ref = torch.cat([(dl.double()[:, :, None] * W64).sum(0), (dr.double()[:, :, None] * W64).sum(0)], dim=1)   # (H, 2C)
     assert float((outs[0][0].double() - dWx_ref).norm() / dWx_ref.norm()) < 2e-6
     assert float((outs[0][1].double() - da_ref).norm() / da_ref.norm()) < 5e-6
-
-
-@pytest.mark.parametrize("N,D1,D2", [(70001, 128, 128), (5000, 96, 32), (129, 128, 64)])
-@pytest.mark.parametrize("relu_flag,with_bias", [(1, True), (0, False)])
-def test_linear2_c_abi(gnn, N, D1, D2, relu_flag, with_bias):
-    """gnnb_linear2 / gnnb_linear2_bwd — σ.(W * vcat(x1, x2) .+ b) as two accumulating wgmma passes over the column blocks
-    of W (sage_conv, conv.jl:281) — against float64."""
-    lib = gnn._lib.lib
-    Dout = 128
-    gen = torch.Generator(device="cuda").manual_seed(N + D1)
-    x1 = torch.randn(N, D1, device="cuda", generator=gen)
-    x2 = torch.randn(N, D2, device="cuda", generator=gen)
-    W = torch.randn(Dout, D1 + D2, device="cuda", generator=gen) / (D1 + D2) ** 0.5
-    b = torch.randn(Dout, device="cuda", generator=gen) if with_bias else None
-    dy = torch.randn(N, Dout, device="cuda", generator=gen)
-    y = torch.empty(N, Dout, device="cuda")
-    gnn._lib.check(lib.gnnb_linear2(x1.data_ptr(), x2.data_ptr(), W.data_ptr(), None if b is None else b.data_ptr(), relu_flag,
-                                    N, D1, D2, Dout, y.data_ptr(), None))
-    pre = torch.cat([x1, x2], 1).double() @ W.double().t() + (0 if b is None else b.double())
-    ref = pre.clamp(min=0) if relu_flag else pre
-    assert rel(y.cpu(), ref.cpu()) < 5e-6
-    ws = torch.empty_like(dy); dx1 = torch.empty_like(x1); dx2 = torch.empty_like(x2)
-    dW = torch.empty_like(W); db = torch.empty(Dout, device="cuda")
-    gnn._lib.check(lib.gnnb_linear2_bwd(dy.data_ptr(), y.data_ptr(), x1.data_ptr(), x2.data_ptr(), W.data_ptr(), relu_flag, N, D1,
-                                        D2, Dout, ws.data_ptr(), dx1.data_ptr(), dx2.data_ptr(), dW.data_ptr(),
-                                        db.data_ptr() if with_bias else None, None))
-    dpre = dy.double() * (y > 0) if relu_flag else dy.double()
-    assert rel(dx1.cpu(), (dpre @ W.double()[:, :D1]).cpu()) < 5e-6
-    assert rel(dx2.cpu(), (dpre @ W.double()[:, D1:]).cpu()) < 5e-6
-    assert rel(dW.cpu(), (dpre.t() @ torch.cat([x1, x2], 1).double()).cpu()) < 5e-6
-    if with_bias:
-        assert rel(db.cpu(), dpre.sum(0).cpu()) < 5e-6
-    assert lib.gnnb_dense_tc_error() == 0
 
 
 @pytest.mark.parametrize("N,D", [(70001, 512), (1, 4), (4099, 36), (0, 64)])
