@@ -7,8 +7,10 @@ host-side mirror of the reference interface in this package.  Nothing here impor
 """
 from . import _lib
 from ._lib import GNNBError, device_count, launch_count, version
-from .graph import (GNNGraph, add_self_loops, batch, colmajor, degree, edge_index, get_edge_weight,
-                    graph_indicator, jl_randn, jl_zeros, rmat_graph, rows, set_edge_weight, unrows)
+from .graph import (GNNGraph, add_self_loops, batch, colmajor, degree, edge_features, edge_index, get_edge_weight,
+                    graph_features, graph_indicator, jl_randn, jl_zeros, node_features, rmat_graph, rows,
+                    set_edge_weight, unrows)
+from .basic import GNNChain, GNNLayer, Parallel, WithGraph
 from .msgpass import (Fix1, aggregate_neighbors, apply_edges, check_num_edges, check_num_nodes, copy_xi, copy_xj,
                       e_mul_xj, expand_srcdst, mean, propagate, softmax_edge_neighbors, w_mul_xj, xi_dot_xj,
                       xi_sub_xj, xj_sub_xi)
@@ -19,8 +21,9 @@ from .layers import (AGNNConv, GATConv, GATv2Conv, GCNConv, GINConv, GatedGraphC
 from .layers_more import (CGConv, ChebConv, DConv, EdgeConv, EGNNConv, GMMConv, MEGNetConv, NNConv,
                           ResGatedGraphConv, cg_conv, cheb_conv, d_conv, edge_conv, egnn_conv, gmm_conv, megnet_conv,
                           nn_conv, res_gated_graph_conv)
-from .readout import (Set2Set, TopKPool, broadcast_edges, broadcast_nodes, global_attention_pool, global_pool,
-                      reduce_edges, reduce_nodes, set2set_pool, softmax_edges, softmax_nodes, topk_index, topk_pool)
+from .readout import (GlobalAttentionPool, GlobalPool, Set2Set, TopKPool, broadcast_edges, broadcast_nodes,
+                      global_attention_pool, global_pool, reduce_edges, reduce_nodes, set2set_pool, softmax_edges,
+                      softmax_nodes, topk_index, topk_pool)
 from .transform import (add_nodes, color_refinement, csr, getgraph, ppr_diffusion, random_walk_pe, remove_edges,
                         remove_multi_edges, remove_nodes, remove_self_loops, sort_edge_index, to_bidirected, unbatch)
 from .temporal import (DCGRU, DCGRUCell, EvolveGCNO, EvolveGCNOCell, GConvGRU, GConvGRUCell, GConvLSTM, GConvLSTMCell,

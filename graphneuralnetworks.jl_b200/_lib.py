@@ -138,6 +138,8 @@ _SIGS = {
     "gnnb_color_refinement": (_int, [_vp, _vp, _i64, _vp, C.POINTER(_i64), C.POINTER(_i64), _vp]),
     "gnnb_set2set_attend": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _vp]),
     "gnnb_set2set_attend_bwd": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _vp]),
+    "gnnb_attention_pool": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _vp]),
+    "gnnb_attention_pool_bwd": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _vp]),
     "gnnb_topk_keep": (_int, [_vp, _int, _i64, _vp, _i64, _i64, C.c_double, _vp, _vp, _vp]),
     "gnnb_topk_score": (_int, [_f32p, _i64, _i64, _f32p, _f32p, _vp]),
     "gnnb_topk_gate": (_int, [_f32p, _i64, _i64, _f32p, _vp, _i64, _f32p, _vp, _vp]),

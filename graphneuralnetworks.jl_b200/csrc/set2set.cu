@@ -12,6 +12,12 @@
 // rows go to partial slots: [acc: D][M][S] in the layout of gat.cu's forward fix-up with one head, and plain D-float
 // sums in the layout of segreduce.cu's fix-up for dq.  Both fix-ups combine the slots in chunk order, so every output is
 // run-to-run bit-identical.  No atomics.
+//
+// Attention pooling (global_attention_pool, GNNlib/src/layers/pool.jl:7-12) is the same attention with a given score per
+// source, s_k = gate[s_k], instead of <q_i, x_{s_k}>: the kernels take the score as a policy (GATE), so the forward
+// shares the loop, the online softmax, the lanes and gat.cu's fix-up.  Its pullback has no per-target sum (dgate_e and
+// dfe are per edge), so the pieces of a long row need no slots there:
+//   backward: α_k = exp(gate[s_k] − M_i) / S_i;  T_i = <du_i, u_i>;  dgate_e_k = α_k (<du_i, f_{s_k}> − T_i);  dfe_k = α_k du_i
 #include "common.cuh"
 #include <math_constants.h>
 
@@ -29,12 +35,12 @@ struct S2SParams {
     const int32_t* __restrict__ row;  // target of each edge
     const int32_t* __restrict__ eid;  // COO position of each edge
     const float* __restrict__ x;      // [num_src][D]
-    const float* __restrict__ q;      // [num_dst][D]
+    const float* __restrict__ q;      // [num_dst][D]; attention pooling: the gate [num_src]
     const float* __restrict__ r;      // bwd: the forward's r      [num_dst][D]
     const float* __restrict__ smax;   // bwd: the forward's seg_max, seg_sum
     const float* __restrict__ ssum;
     const float* __restrict__ dr;     // bwd                        [num_dst][D]
-    float* __restrict__ out;          // fwd: r; bwd: dq            [num_dst][D]
+    float* __restrict__ out;          // fwd: r; bwd: dq            [num_dst][D]; attention pooling bwd: dgate_e [E]
     float* __restrict__ out_max;      // fwd: seg_max, seg_sum      [num_dst]
     float* __restrict__ out_sum;
     float* __restrict__ dxe;          // bwd                        [E][D]
@@ -73,6 +79,8 @@ __device__ __forceinline__ float4 s2s_axpy(float4 acc, float4 a, float s) {
     return make_float4(fmaf(a.x, s, acc.x), fmaf(a.y, s, acc.y), fmaf(a.z, s, acc.z), fmaf(a.w, s, acc.w));
 }
 __device__ __forceinline__ float s2s_axpy(float acc, float a, float s) { return fmaf(a, s, acc); }
+__device__ __forceinline__ float4 s2s_scale(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
+__device__ __forceinline__ float s2s_scale(float a, float s) { return a * s; }
 __device__ __forceinline__ float4 s2s_div(float4 a, float s) {
     return make_float4(__fdiv_rn(a.x, s), __fdiv_rn(a.y, s), __fdiv_rn(a.z, s), __fdiv_rn(a.w, s));
 }
@@ -99,8 +107,10 @@ __device__ __forceinline__ void load_edge(const S2SParams& p, int my, int e_end,
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-template <int VEC, int K>
-__global__ void __launch_bounds__(256) set2set_fwd_kernel(const S2SParams p) {
+// GATE = false: s_k = <q_i, x_{s_k}> (Set2Set).  GATE = true: s_k = gate[s_k], a given score per source in p.q
+// (attention pooling); q is not read.
+template <bool GATE, int VEC, int K>
+__device__ __forceinline__ void attend_fwd(const S2SParams& p) {
     using V = typename SV<VEC>::T;
     constexpr int U = InFlight<VEC * K>::U;
     const int lane = threadIdx.x & 31;
@@ -121,6 +131,8 @@ __global__ void __launch_bounds__(256) set2set_fwd_kernel(const S2SParams p) {
     for (int e = it.x; e < e_end; e += 32) {
         int c_l, r_l, id_l; bool last_l;
         load_edge(p, e + lane, e_end, c_l, r_l, id_l, last_l);
+        float g_l = 0.f;
+        if constexpr (GATE) { if (e + lane < e_end) g_l = __ldg(p.q + c_l); }
         const int nb = min(32, e_end - e);
         const unsigned bmask = partial ? 0u : __ballot_sync(FULL, last_l);
 #pragma unroll 1
@@ -144,17 +156,23 @@ __global__ void __launch_bounds__(256) set2set_fwd_kernel(const S2SParams p) {
                         const int rj = __shfl_sync(FULL, r_l, j);
 #pragma unroll
                         for (int i = 0; i < K; ++i) {
-                            qv[i] = s2s_zero<V>();
-                            if (act[i]) s2s_ld(p.q + (int64_t)rj * p.D + f[i], qv[i]);
+                            if constexpr (!GATE) {
+                                qv[i] = s2s_zero<V>();
+                                if (act[i]) s2s_ld(p.q + (int64_t)rj * p.D + f[i], qv[i]);
+                            }
                             acc[i] = s2s_zero<V>();
                         }
                         M = -CUDART_INF_F; S = 0.f;
                         fresh = false;
                     }
                     float s = 0.f;
+                    if constexpr (GATE) {
+                        s = __shfl_sync(FULL, g_l, j);
+                    } else {
 #pragma unroll
-                    for (int i = 0; i < K; ++i) s = s2s_dot(qv[i], v[u][i], s);
-                    s = warp_sum(s);
+                        for (int i = 0; i < K; ++i) s = s2s_dot(qv[i], v[u][i], s);
+                        s = warp_sum(s);
+                    }
                     const float Mn = fmaxf(M, s);
                     const float Ms = softmax_shift(Mn);
                     const float sc = expf(M - Ms);     // exp(-inf) = 0 on the first edge of a row
@@ -185,8 +203,10 @@ __global__ void __launch_bounds__(256) set2set_fwd_kernel(const S2SParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-template <int VEC, int K>
-__global__ void __launch_bounds__(256) set2set_bwd_kernel(const S2SParams p) {
+// GATE = true: the score is the given gate (p.q), so there is no dq; out receives dgate_e[k] = ds_k per edge (COO
+// order), dxe the per-edge α_k dr_i, and a long row's pieces are independent: no partial slots.
+template <bool GATE, int VEC, int K>
+__device__ __forceinline__ void attend_bwd(const S2SParams& p) {
     using V = typename SV<VEC>::T;
     constexpr int U = InFlight<VEC * K>::U;
     const int lane = threadIdx.x & 31;
@@ -207,6 +227,8 @@ __global__ void __launch_bounds__(256) set2set_bwd_kernel(const S2SParams p) {
     for (int e = it.x; e < e_end; e += 32) {
         int c_l, r_l, id_l; bool last_l;
         load_edge(p, e + lane, e_end, c_l, r_l, id_l, last_l);
+        float g_l = 0.f;
+        if constexpr (GATE) { if (e + lane < e_end) g_l = __ldg(p.q + c_l); }
         const int nb = min(32, e_end - e);
         const unsigned bmask = partial ? 0u : __ballot_sync(FULL, last_l);
 #pragma unroll 1
@@ -232,49 +254,78 @@ __global__ void __launch_bounds__(256) set2set_bwd_kernel(const S2SParams p) {
 #pragma unroll
                         for (int i = 0; i < K; ++i) {
                             V rv = s2s_zero<V>();
-                            qv[i] = s2s_zero<V>(); dv[i] = s2s_zero<V>();
+                            if constexpr (!GATE) qv[i] = s2s_zero<V>();
+                            dv[i] = s2s_zero<V>();
                             if (act[i]) {
                                 const int64_t o = (int64_t)rj * p.D + f[i];
-                                s2s_ld(p.q + o, qv[i]); s2s_ld(p.dr + o, dv[i]); s2s_ld(p.r + o, rv);
+                                if constexpr (!GATE) s2s_ld(p.q + o, qv[i]);
+                                s2s_ld(p.dr + o, dv[i]); s2s_ld(p.r + o, rv);
                             }
                             t = s2s_dot(dv[i], rv, t);
-                            acc[i] = s2s_zero<V>();
+                            if constexpr (!GATE) acc[i] = s2s_zero<V>();
                         }
                         T = warp_sum(t);
                         M = __ldg(p.smax + rj); S = __ldg(p.ssum + rj);
                         fresh = false;
                     }
                     float s = 0.f, gd = 0.f;
+                    if constexpr (GATE) {
+                        s = __shfl_sync(FULL, g_l, j);
 #pragma unroll
-                    for (int i = 0; i < K; ++i) { s = s2s_dot(qv[i], v[u][i], s); gd = s2s_dot(dv[i], v[u][i], gd); }
-                    s = warp_sum(s);
+                        for (int i = 0; i < K; ++i) gd = s2s_dot(dv[i], v[u][i], gd);
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < K; ++i) {
+                            s = s2s_dot(qv[i], v[u][i], s); gd = s2s_dot(dv[i], v[u][i], gd);
+                        }
+                        s = warp_sum(s);
+                    }
                     gd = warp_sum(gd);
                     const float al = __fdiv_rn(expf(s - M), S);
                     const float ds = al * (gd - T);
                     const int ek = __shfl_sync(FULL, id_l, j);
-#pragma unroll
-                    for (int i = 0; i < K; ++i) {
-                        if (act[i]) s2s_st(p.dxe + (int64_t)ek * p.D + f[i], s2s_lin(dv[i], al, qv[i], ds));
-                        acc[i] = s2s_axpy(acc[i], v[u][i], ds);
-                    }
-                    if ((bmask >> j) & 1u) {           // row end: dq, exactly once
-                        const int rj = __shfl_sync(FULL, r_l, j);
+                    if constexpr (GATE) {
 #pragma unroll
                         for (int i = 0; i < K; ++i)
-                            if (act[i]) s2s_st(p.out + (int64_t)rj * p.D + f[i], acc[i]);
+                            if (act[i]) s2s_st(p.dxe + (int64_t)ek * p.D + f[i], s2s_scale(dv[i], al));
+                        if (lane == 0) p.out[ek] = ds;
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < K; ++i) {
+                            if (act[i]) s2s_st(p.dxe + (int64_t)ek * p.D + f[i], s2s_lin(dv[i], al, qv[i], ds));
+                            acc[i] = s2s_axpy(acc[i], v[u][i], ds);
+                        }
+                    }
+                    if ((bmask >> j) & 1u) {           // row end: dq, exactly once
+                        if constexpr (!GATE) {
+                            const int rj = __shfl_sync(FULL, r_l, j);
+#pragma unroll
+                            for (int i = 0; i < K; ++i)
+                                if (act[i]) s2s_st(p.out + (int64_t)rj * p.D + f[i], acc[i]);
+                        }
                         fresh = true;
                     }
                 }
             }
         }
     }
-    if (partial) {
+    if (!GATE && partial) {
         float* base = p.ws + (int64_t)it.z * p.D;
 #pragma unroll
         for (int i = 0; i < K; ++i)
             if (act[i]) s2s_st(base + f[i], acc[i]);
     }
 }
+
+template <int VEC, int K>
+__global__ void __launch_bounds__(256) set2set_fwd_kernel(const S2SParams p) { attend_fwd<false, VEC, K>(p); }
+template <int VEC, int K>
+__global__ void __launch_bounds__(256) set2set_bwd_kernel(const S2SParams p) { attend_bwd<false, VEC, K>(p); }
+template <int VEC, int K>
+__global__ void __launch_bounds__(256) attention_pool_fwd_kernel(const S2SParams p) { attend_fwd<true, VEC, K>(p); }
+// min blocks 1: without it ptxas trades a few spills (K = 2 and 32) for occupancy the gather-bound loop does not need
+template <int VEC, int K>
+__global__ void __launch_bounds__(256, 1) attention_pool_bwd_kernel(const S2SParams p) { attend_bwd<true, VEC, K>(p); }
 
 // targets without edges (every target when rowptr is NULL): out = 0 and, when smax is given, seg_max = -Inf and
 // seg_sum = 0.  One warp per target.
@@ -295,30 +346,36 @@ int fill_empty(const int32_t* rowptr, int32_t nrows, float* out, int64_t D, floa
     return GNNB_OK;
 }
 
-template <int VEC, int K>
+template <bool GATE, int VEC, int K>
 int launch2(bool bwd, const S2SParams& p, cudaStream_t st) {
     const unsigned blocks = (unsigned)ceil_div(p.n_items, 8);
-    if (bwd) set2set_bwd_kernel<VEC, K><<<blocks, 256, 0, st>>>(p);
-    else set2set_fwd_kernel<VEC, K><<<blocks, 256, 0, st>>>(p);
+    if constexpr (GATE) {
+        if (bwd) attention_pool_bwd_kernel<VEC, K><<<blocks, 256, 0, st>>>(p);
+        else attention_pool_fwd_kernel<VEC, K><<<blocks, 256, 0, st>>>(p);
+    } else {
+        if (bwd) set2set_bwd_kernel<VEC, K><<<blocks, 256, 0, st>>>(p);
+        else set2set_fwd_kernel<VEC, K><<<blocks, 256, 0, st>>>(p);
+    }
     GNNB_LAUNCHED();
     return GNNB_OK;
 }
 // K = slices per lane, the power of two that covers D (D <= GNNB_SET2SET_MAX_D = 32 floats per lane)
+template <bool GATE>
 int launch(bool bwd, bool vec4, const S2SParams& p, cudaStream_t st) {
     if (p.n_items == 0) return GNNB_OK;
     const int64_t k = ceil_div(p.D, vec4 ? 128 : 32);
     if (vec4) {
-        if (k <= 1) return launch2<4, 1>(bwd, p, st);
-        if (k <= 2) return launch2<4, 2>(bwd, p, st);
-        if (k <= 4) return launch2<4, 4>(bwd, p, st);
-        return launch2<4, 8>(bwd, p, st);
+        if (k <= 1) return launch2<GATE, 4, 1>(bwd, p, st);
+        if (k <= 2) return launch2<GATE, 4, 2>(bwd, p, st);
+        if (k <= 4) return launch2<GATE, 4, 4>(bwd, p, st);
+        return launch2<GATE, 4, 8>(bwd, p, st);
     }
-    if (k <= 1) return launch2<1, 1>(bwd, p, st);
-    if (k <= 2) return launch2<1, 2>(bwd, p, st);
-    if (k <= 4) return launch2<1, 4>(bwd, p, st);
-    if (k <= 8) return launch2<1, 8>(bwd, p, st);
-    if (k <= 16) return launch2<1, 16>(bwd, p, st);
-    return launch2<1, 32>(bwd, p, st);
+    if (k <= 1) return launch2<GATE, 1, 1>(bwd, p, st);
+    if (k <= 2) return launch2<GATE, 1, 2>(bwd, p, st);
+    if (k <= 4) return launch2<GATE, 1, 4>(bwd, p, st);
+    if (k <= 8) return launch2<GATE, 1, 8>(bwd, p, st);
+    if (k <= 16) return launch2<GATE, 1, 16>(bwd, p, st);
+    return launch2<GATE, 1, 32>(bwd, p, st);
 }
 
 bool aligned16(const void* a) { return (reinterpret_cast<uintptr_t>(a) & 15) == 0; }
@@ -357,7 +414,7 @@ int gnnb_set2set_attend(gnnb_graph_t g, const float* x, const float* q, int64_t 
         GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * p.slot));
         p.ws = g->ws;
     }
-    GNNB_TRY(launch(false, vec4, p, st));
+    GNNB_TRY(launch<false>(false, vec4, p, st));
     return gat_fwd_fixup_one_head(c, g->E, g->chunk, D, vec4, p.ws, r, seg_max, seg_sum, st);
 }
 
@@ -389,8 +446,62 @@ int gnnb_set2set_attend_bwd(gnnb_graph_t g, const float* x, const float* q, cons
         GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * D));
         p.ws = g->ws;
     }
-    GNNB_TRY(launch(true, vec4, p, st));
+    GNNB_TRY(launch<false>(true, vec4, p, st));
     return seg_fixup_sum(c, g->E, g->chunk, D, p.ws, dq, st);
+}
+
+int gnnb_attention_pool(gnnb_graph_t g, const float* f, const float* gate, int64_t D, float* u, float* seg_max,
+                        float* seg_sum, void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (D < 1) GNNB_FAIL(GNNB_ESIZE, "attention_pool: D must be >= 1 (got %lld)", (long long)D);
+    if (D > GNNB_SET2SET_MAX_D)
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "attention_pool: D = %lld is above GNNB_SET2SET_MAX_D = %d; compose "
+                  "softmax_nodes / reduce_nodes", (long long)D, GNNB_SET2SET_MAX_D);
+    const int32_t nd = g->n_dst;
+    if ((nd > 0 && (!u || !seg_max || !seg_sum)) || (g->E > 0 && (!f || !gate)))
+        GNNB_FAIL(GNNB_ESIZE, "attention_pool: NULL array of positive size");
+    if (nd == 0) return GNNB_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    GNNB_TRY(ensure_csr(g, false, st));
+    const Csr& c = g->by_dst;
+    if (g->E == 0) return fill_empty(nullptr, nd, u, D, seg_max, seg_sum, st);
+    GNNB_TRY(ensure_items(g, c, st));
+    if (c.n_empty > 0) GNNB_TRY(fill_empty(c.rowptr, nd, u, D, seg_max, seg_sum, st));
+    const bool vec4 = D % 4 == 0 && aligned16(f) && aligned16(u);
+    S2SParams p = {};
+    p.items = reinterpret_cast<const int4*>(c.items); p.n_items = c.n_items;
+    p.col = c.col; p.row = c.row; p.eid = c.eid;
+    p.x = f; p.q = gate; p.out = u; p.out_max = seg_max; p.out_sum = seg_sum;
+    p.D = D; p.slot = (D + 2 + 3) & ~(int64_t)3;       // gat_fwd_fixup_kernel's slot with H = 1
+    if (c.n_long > 0) {
+        GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, sizeof(float) * (size_t)2 * ceil_div(g->E, g->chunk) * p.slot));
+        p.ws = g->ws;
+    }
+    GNNB_TRY(launch<true>(false, vec4, p, st));
+    return gat_fwd_fixup_one_head(c, g->E, g->chunk, D, vec4, p.ws, u, seg_max, seg_sum, st);
+}
+
+int gnnb_attention_pool_bwd(gnnb_graph_t g, const float* f, const float* gate, const float* u, const float* seg_max,
+                            const float* seg_sum, const float* du, int64_t D, float* dfe, float* dgate_e, void* stream) {
+    if (!g) GNNB_FAIL(GNNB_EINVAL, "graph handle is NULL");
+    if (D < 1) GNNB_FAIL(GNNB_ESIZE, "attention_pool_bwd: D must be >= 1 (got %lld)", (long long)D);
+    if (D > GNNB_SET2SET_MAX_D)
+        GNNB_FAIL(GNNB_EUNSUPPORTED, "attention_pool_bwd: D = %lld is above GNNB_SET2SET_MAX_D = %d", (long long)D,
+                  GNNB_SET2SET_MAX_D);
+    if (g->E > 0 && (!f || !gate || !u || !seg_max || !seg_sum || !du || !dfe || !dgate_e))
+        GNNB_FAIL(GNNB_ESIZE, "attention_pool_bwd: NULL array of positive size");
+    if (g->E == 0) return GNNB_OK;                     // every output is per edge
+    cudaStream_t st = (cudaStream_t)stream;
+    GNNB_TRY(ensure_csr(g, false, st));
+    const Csr& c = g->by_dst;
+    GNNB_TRY(ensure_items(g, c, st));
+    const bool vec4 = D % 4 == 0 && aligned16(f) && aligned16(u) && aligned16(du) && aligned16(dfe);
+    S2SParams p = {};
+    p.items = reinterpret_cast<const int4*>(c.items); p.n_items = c.n_items;
+    p.col = c.col; p.row = c.row; p.eid = c.eid;
+    p.x = f; p.q = gate; p.r = u; p.smax = seg_max; p.ssum = seg_sum; p.dr = du; p.out = dgate_e; p.dxe = dfe;
+    p.D = D;
+    return launch<true>(true, vec4, p, st);
 }
 
 }  // extern "C"

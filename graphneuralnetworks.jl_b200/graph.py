@@ -7,6 +7,8 @@ GNNGraphs functions that sit on the hot path (SURVEY.md §8 a9-a11, a17):
     set_edge_weight     GNNGraphs/src/transform.jl:568-577
     batch (COO)         GNNGraphs/src/transform.jl:682-709
     graph_indicator     GNNGraphs/src/query.jl:500-512
+    GNNGraph(g; ndata, edata, gdata)                     GNNGraphs/src/gnngraph.jl:187-210
+    node_features / edge_features / graph_features      GNNGraphs/src/query.jl:516-544
 
 Conventions follow the reference: node ids are 1-based Int64 (or Int32) vectors ``s`` (source) and ``t``
 (target); feature arrays are Julia-shaped ``(D, num_nodes)`` / ``(K, num_edges)`` whose *memory* is
@@ -112,6 +114,20 @@ def _as_index(v, device=None) -> torch.Tensor:
     return t.contiguous()
 
 
+# caches a graph keeps that depend on its topology alone (never on its features): a copy with replaced data shares them
+_TOPOLOGY_CACHES = ("_plan", "_gi_plan_n", "_gi_plan_e", "_lmax_cache", "_gcn_c_cache", "_cheb_op_cache", "_dconv_gt")
+_KEEP = object()
+
+
+def _graphdata(d, default_name: str, n: int, what: str) -> dict:
+    """normalize_graphdata (GNNGraphs/src/datastore.jl): None -> empty, a bare tensor -> {default_name: it}; every array's
+    last dimension must be n"""
+    d = {} if d is None else ({default_name: d} if isinstance(d, torch.Tensor) else dict(d))
+    for k, v in d.items():
+        assert v.shape[-1] == n, f"{k} has last dimension {v.shape[-1]}; the graph has {what} = {n}"
+    return d
+
+
 class GNNGraph:
     """COO graph ``(s, t[, w])`` with 1-based node ids — GNNGraph{<:COO_T} (GNNGraphs/src/gnngraph.jl:108-117).
 
@@ -119,10 +135,21 @@ class GNNGraph:
     accepted (gnngraph.jl:120-199); ``num_nodes`` defaults to ``max(maximum(s), maximum(t))``
     (convert.jl:33-36).  Indices are validated once, on the device, when the plan is built
     (``1 <= idx <= num_nodes``, convert.jl:49-54 -> AssertionError).
+
+    ``GNNGraph(g, ndata=..., edata=..., gdata=...)`` (gnngraph.jl:187-210) is ``g`` with the given stores replaced (the
+    others kept): a bare tensor is named ``x`` / ``e`` / ``u`` and its last dimension must be num_nodes / num_edges /
+    num_graphs.  The copy shares ``g``'s topology and the caches built from it alone (the plan, the graph-indicator
+    plans, λmax), and no cache that holds features.
     """
 
-    def __init__(self, s, t=None, w=None, *, num_nodes: Optional[int] = None, ndata=None, edata=None,
-                 gdata=None, num_graphs: int = 1, graph_indicator=None, device=None):
+    def __init__(self, s, t=None, w=None, *, num_nodes: Optional[int] = None, ndata=_KEEP, edata=_KEEP,
+                 gdata=_KEEP, num_graphs: int = 1, graph_indicator=None, device=None):
+        if isinstance(s, GNNGraph):
+            assert t is None and w is None and num_nodes is None and device is None, \
+                "GNNGraph(g; ndata, edata, gdata) takes the graph and the data stores only"
+            self._copy(s, ndata, edata, gdata)
+            return
+        ndata, edata, gdata = (None if d is _KEEP else d for d in (ndata, edata, gdata))
         if t is None:
             as_edges = isinstance(s, tuple) and len(s) in (2, 3)           # (s, t) / (s, t, w): tuples
             if not as_edges and isinstance(s, list) and len(s) in (2, 3) and all(hasattr(v, "__len__") for v in s):
@@ -163,6 +190,20 @@ class GNNGraph:
             assert v.shape[-1] == self.num_edges, f"edata[{k}] last dim must be num_edges"
         self._plan: Optional[_Plan] = None
         self._loops: Optional["GNNGraph"] = None
+
+    def _copy(self, g: "GNNGraph", ndata, edata, gdata) -> None:
+        self.s, self.t, self.w = g.s, g.t, g.w
+        self.num_edges, self.num_nodes, self.num_graphs = g.num_edges, g.num_nodes, g.num_graphs
+        self.graph_indicator = g.graph_indicator
+        self.ndata = _graphdata(g.ndata if ndata is _KEEP else ndata, "x", g.num_nodes, "num_nodes")
+        self.edata = _graphdata(g.edata if edata is _KEEP else edata, "e", g.num_edges, "num_edges")
+        self.gdata = _graphdata(g.gdata if gdata is _KEEP else gdata, "u", g.num_graphs, "num_graphs")
+        self._plan = None
+        self._loops = None                 # add_self_loops' result carries the features: never shared
+        for k in _TOPOLOGY_CACHES:
+            v = getattr(g, k, None)
+            if v is not None:
+                setattr(self, k, v)
 
     # -- conveniences mirroring g.x / g.e property access (datastore.jl getproperty)
     @property
@@ -363,6 +404,29 @@ def degree(g: GNNGraph, T=None, *args, dir: str = "out", edge_weight=True) -> to
     if T is None:
         T = torch.float32 if w is not None else g.s.dtype
     return out.to(T)
+
+
+def _only(store: dict, name: str):
+    if not store:
+        return None
+    if len(store) > 1:
+        raise ValueError(f"multiple feature arrays ({', '.join(store)}): access them through g.{name}")
+    return next(iter(store.values()))
+
+
+def node_features(g: GNNGraph):
+    """GNNGraphs/src/query.jl:516-524: None when ndata is empty, its only array otherwise (ValueError for several)."""
+    return _only(g.ndata, "ndata")
+
+
+def edge_features(g: GNNGraph):
+    """GNNGraphs/src/query.jl:526-534."""
+    return _only(g.edata, "edata")
+
+
+def graph_features(g: GNNGraph):
+    """GNNGraphs/src/query.jl:536-544."""
+    return _only(g.gdata, "gdata")
 
 
 def graph_indicator(g: GNNGraph, edges=False) -> torch.Tensor:

@@ -27,6 +27,7 @@ import torch
 
 from . import _lib
 from ._lib import lib
+from .basic import _EdgeFeatureLayer, GNNLayer
 from .graph import GNNGraph, _is_hetero, _stream, add_self_loops, degree, homogeneous_only, num_src_dst, relation, rows, unrows
 from .msgpass import (Fix1, _GCNPropagateFn, _f32, aggregate_neighbors, apply_edges, check_num_nodes, copy_xj,
                       e_mul_xj, expand_srcdst, mean, propagate, softmax_edge_neighbors, w_mul_xj)
@@ -330,7 +331,7 @@ def glorot_uniform(*shape, device=None) -> torch.Tensor:
     return (torch.rand(*shape, device=device) * 2 - 1) * s
 
 
-class GCNConv(torch.nn.Module):
+class GCNConv(GNNLayer):
     """GCNConv(in => out, σ=identity; bias=true, add_self_loops=true, use_edge_weight=false)
     — GraphNeuralNetworks/src/layers/conv.jl:77-104."""
 
@@ -585,7 +586,7 @@ class _Dense(torch.nn.Module):
         return _linear(self, self.weight, x, True)     # W * x .+ b (σ = identity)
 
 
-class GATConv(torch.nn.Module):
+class GATConv(_EdgeFeatureLayer):
     """GATConv(in => out, σ=identity; heads=1, concat=true, negative_slope=0.2, add_self_loops=true, dropout=0)
     — GraphNeuralNetworks/src/layers/conv.jl:309-346 (ein = 0: no edge features)."""
 
@@ -665,7 +666,7 @@ def sage_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     return _linear(l, W, xm, True)                            # σ.(W * vcat(xi, m) .+ b): one GEMM, bias/σ in the epilogue
 
 
-class SAGEConv(torch.nn.Module):
+class SAGEConv(GNNLayer):
     """SAGEConv(in => out, σ=identity; aggr=mean, bias=true) — GraphNeuralNetworks/src/layers/conv.jl:770-787."""
 
     def __init__(self, ch_in: int, ch_out: int, sigma: Callable = identity, *, aggr=mean, bias: bool = True,
@@ -1014,7 +1015,7 @@ class _BatchNorm(torch.nn.Module):
         return unrows(self.bn(rows(x)))
 
 
-class GraphConv(torch.nn.Module):
+class GraphConv(GNNLayer):
     """GraphConv(in => out, σ=identity; aggr=+, bias=true) — GraphNeuralNetworks/src/layers/conv.jl:226-251."""
 
     def __init__(self, ch_in, ch_out, sigma: Callable = identity, *, aggr=operator.add, bias=True, device=None):
@@ -1028,7 +1029,7 @@ class GraphConv(torch.nn.Module):
         return graph_conv(self, g, x)
 
 
-class GINConv(torch.nn.Module):
+class GINConv(GNNLayer):
     """GINConv(nn, ϵ; aggr=+) — GraphNeuralNetworks/src/layers/conv.jl:628-640 (ϵ is not trainable there either)."""
 
     def __init__(self, nn: Callable, eps: float = 0.0, *, aggr=operator.add):
@@ -1039,7 +1040,7 @@ class GINConv(torch.nn.Module):
         return gin_conv(self, g, x)
 
 
-class AGNNConv(torch.nn.Module):
+class AGNNConv(GNNLayer):
     """AGNNConv(; init_beta=1, trainable=true, add_self_loops=true) — GraphNeuralNetworks/src/layers/conv.jl:988-1003."""
 
     def __init__(self, *, init_beta: float = 1.0, trainable: bool = True, add_self_loops: bool = True, device=None):
@@ -1053,7 +1054,7 @@ class AGNNConv(torch.nn.Module):
         return agnn_conv(self, g, x)
 
 
-class SGConv(torch.nn.Module):
+class SGConv(GNNLayer):
     """SGConv(in => out, k=1; bias=true, add_self_loops=true, use_edge_weight=false) — conv.jl:1197-1222."""
 
     def __init__(self, ch_in, ch_out, k: int = 1, *, bias=True, add_self_loops=True, use_edge_weight=False,
@@ -1077,7 +1078,7 @@ class TAGConv(SGConv):
         return tag_conv(self, g, x, edge_weight)
 
 
-class GatedGraphConv(torch.nn.Module):
+class GatedGraphConv(GNNLayer):
     """GatedGraphConv(out, num_layers; aggr=+) — GraphNeuralNetworks/src/layers/conv.jl:515-530."""
 
     def __init__(self, dims: int, num_layers: int, *, aggr=operator.add, device=None):
@@ -1091,7 +1092,7 @@ class GatedGraphConv(torch.nn.Module):
         return gated_graph_conv(self, g, x)
 
 
-class GATv2Conv(torch.nn.Module):
+class GATv2Conv(_EdgeFeatureLayer):
     """GATv2Conv(in => out, σ=identity; heads=1, concat=true, negative_slope=0.2, bias=true, add_self_loops=true,
     dropout=0) and the (in, ein) => out form — GraphNeuralNetworks/src/layers/conv.jl:413-462."""
 
@@ -1116,7 +1117,7 @@ class GATv2Conv(torch.nn.Module):
         return gatv2_conv(self, g, x, e)
 
 
-class TransformerConv(torch.nn.Module):
+class TransformerConv(_EdgeFeatureLayer):
     """TransformerConv((in, ein) => out; heads=1, concat=true, add_self_loops=false, bias_qkv=true, bias_root=true,
     root_weight=true, gating=false, skip_connection=false, batch_norm=false, ff_channels=0)
     — GraphNeuralNetworks/src/layers/conv.jl:1473-1539."""

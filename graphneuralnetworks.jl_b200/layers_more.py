@@ -24,7 +24,8 @@ from typing import Callable, Optional
 import numpy as np
 import torch
 
-from .graph import GNNGraph, degree, homogeneous_only, rows, unrows
+from .basic import _EdgeFeatureLayer, GNNLayer
+from .graph import GNNGraph, degree, edge_features, homogeneous_only, node_features, rows, unrows
 from .layers import (_add_bias, _bias, _Dense, _DenseAct, _jl_reshape3, _matmul, _sigma, glorot_uniform, identity,
                      relu)
 from .msgpass import (Fix1, aggregate_neighbors, apply_edges, check_num_edges, check_num_nodes, e_mul_xj,
@@ -290,7 +291,7 @@ class Chain(torch.nn.Sequential):
     """Flux.Chain of callables on Julia-shaped arrays"""
 
 
-class ChebConv(torch.nn.Module):
+class ChebConv(GNNLayer):
     """ChebConv(in => out, k; bias=true) — GraphNeuralNetworks/src/layers/conv.jl:162-175"""
 
     def __init__(self, ch_in, ch_out, k: int, *, bias=True, device=None):
@@ -303,7 +304,7 @@ class ChebConv(torch.nn.Module):
         return cheb_conv(self, g, x)
 
 
-class EdgeConv(torch.nn.Module):
+class EdgeConv(GNNLayer):
     """EdgeConv(nn; aggr=max) — conv.jl:575-585"""
 
     def __init__(self, nn: Callable, *, aggr=max):
@@ -314,7 +315,7 @@ class EdgeConv(torch.nn.Module):
         return edge_conv(self, g, x)
 
 
-class NNConv(torch.nn.Module):
+class NNConv(_EdgeFeatureLayer):
     """NNConv(in => out, nn, σ=identity; aggr=+, bias=true) — conv.jl:701-717"""
 
     def __init__(self, ch_in, ch_out, nn: Callable, sigma: Callable = identity, *, aggr=operator.add, bias=True,
@@ -328,7 +329,7 @@ class NNConv(torch.nn.Module):
         return nn_conv(self, g, x, e)
 
 
-class ResGatedGraphConv(torch.nn.Module):
+class ResGatedGraphConv(GNNLayer):
     """ResGatedGraphConv(in => out, σ=identity; bias=true) — conv.jl:838-859"""
 
     def __init__(self, ch_in, ch_out, sigma: Callable = identity, *, bias=True, device=None):
@@ -342,7 +343,7 @@ class ResGatedGraphConv(torch.nn.Module):
         return res_gated_graph_conv(self, g, x)
 
 
-class CGConv(torch.nn.Module):
+class CGConv(_EdgeFeatureLayer):
     """CGConv((in, ein) => out, act=identity; bias=true, residual=false) — conv.jl:914-932"""
 
     def __init__(self, ch_in, ch_out, act: Callable = identity, *, residual=False, bias=True, device=None):
@@ -357,7 +358,7 @@ class CGConv(torch.nn.Module):
         return cg_conv(self, g, x, e)
 
 
-class MEGNetConv(torch.nn.Module):
+class MEGNetConv(GNNLayer):
     """MEGNetConv(ϕe, ϕv; aggr=mean) / MEGNetConv(in => out; aggr=mean) — conv.jl:1035-1055"""
 
     def __init__(self, a, b, *, aggr=mean, device=None):
@@ -371,8 +372,13 @@ class MEGNetConv(torch.nn.Module):
     def forward(self, g, x, e):
         return megnet_conv(self, g, x, e)
 
+    def graph_forward(self, g):
+        """conv.jl:1056-1059: both the node and the edge features are replaced"""
+        x, e = self(g, node_features(g), edge_features(g))
+        return GNNGraph(g, ndata=x, edata=e)
 
-class GMMConv(torch.nn.Module):
+
+class GMMConv(_EdgeFeatureLayer):
     """GMMConv((in, ein) => out, σ=identity; K=1, bias=true, residual=false) — conv.jl:1111-1137"""
 
     def __init__(self, ch_in, ch_out, sigma: Callable = identity, *, K: int = 1, bias=True, residual=False, device=None):
@@ -388,7 +394,7 @@ class GMMConv(torch.nn.Module):
         return gmm_conv(self, g, x, e)
 
 
-class EGNNConv(torch.nn.Module):
+class EGNNConv(GNNLayer):
     """EGNNConv((in, ein) => out; hidden_size=2in, residual=false) — conv.jl:1349-1386"""
 
     def __init__(self, ch_in, ch_out, *, hidden_size: Optional[int] = None, residual=False, device=None):
@@ -407,7 +413,7 @@ class EGNNConv(torch.nn.Module):
         return egnn_conv(self, g, h, x, e)
 
 
-class DConv(torch.nn.Module):
+class DConv(GNNLayer):
     """DConv(in => out, k; bias=true) — conv.jl:1574-1589.  weights is (2, k, out, in)."""
 
     def __init__(self, ch_in, ch_out, k: int, *, bias=True, device=None):

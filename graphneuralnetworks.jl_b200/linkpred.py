@@ -40,6 +40,7 @@ import torch
 from . import _lib
 from . import graph as _graph
 from ._lib import lib
+from .basic import GNNLayer
 from .graph import GNNGraph, _as_index, _stream
 from .msgpass import apply_edges, xi_dot_xj
 from .query import has_multi_edges, has_self_loops, is_bidirected
@@ -317,7 +318,7 @@ def dot_decoder(g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     return apply_edges(xi_dot_xj, g, xi=x, xj=x)
 
 
-class DotDecoder(torch.nn.Module):
+class DotDecoder(GNNLayer):
     """DotDecoder() — GraphNeuralNetworks/src/layers/basic.jl:187-212; no parameters."""
 
     def forward(self, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:

@@ -4,13 +4,15 @@
     softmax_nodes / softmax_edges      GNNlib/src/utils.jl:44-72
     broadcast_nodes / broadcast_edges  GNNlib/src/utils.jl:105-121
     global_pool, global_attention_pool GNNlib/src/layers/pool.jl:3-12
+    GlobalPool, GlobalAttentionPool    GraphNeuralNetworks/src/layers/pool.jl:1-99
     set2set_pool, Set2Set              GNNlib/src/layers/pool.jl:29-43, GraphNeuralNetworks/src/layers/pool.jl:126-162
     topk_index, topk_pool, TopKPool    GNNlib/src/layers/pool.jl:14-27, GraphNeuralNetworks/src/layers/pool.jl:101-123
 
 `NNlib.scatter(aggr, x, graph_indicator)` is a segmented reduce whose "edges" are the nodes and whose "targets" are the
 graphs: a bipartite plan (gnnb_graph_create with num_src = #items, num_dst = #graphs) lets the library's scatter /
 gather / neighbourhood-softmax kernels (and their pullbacks) do all of it.  Set2Set's attention runs on the same plan
-through its own fused kernel (csrc/set2set.cu).  Top-k pooling selects per graph by a segmented radix select and gates
+through its own fused kernel (csrc/set2set.cu), and so does global_attention_pool with a gate of one row (the same
+kernel with the gate as the score).  Top-k pooling selects per graph by a segmented radix select and gates
 the kept rows in one pass (csrc/topk.cu).
 """
 from __future__ import annotations
@@ -24,8 +26,9 @@ import torch
 from . import _lib
 from . import graph as _graph
 from ._lib import lib
-from .graph import GNNGraph, _Plan, _ptr, _stream, graph_indicator, rows, unrows
-from .layers import _LSTMCell, glorot_uniform
+from .basic import GNNLayer
+from .graph import GNNGraph, _Plan, _ptr, _stream, graph_indicator, node_features, rows, unrows
+from .layers import _LSTMCell, glorot_uniform, identity
 from .msgpass import _EdgeSoftmaxFn, _GatherFn, _ScatterFn, _aggr_code, _f32
 
 
@@ -117,16 +120,92 @@ def global_pool(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     return reduce_nodes(l.aggr, g, x)
 
 
-def global_attention_pool(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
-    """GNNlib/src/layers/pool.jl:7-12."""
-    alpha = softmax_nodes(g, l.fgate(x))
-    feats = alpha * l.ffeat(x)
-    return reduce_nodes(operator.add, g, feats)
-
-
 # Feature sizes up to this go through the fused attention (gnnb_set2set_attend, csrc/set2set.cu); larger ones through
 # broadcast_nodes / softmax_nodes / reduce_nodes.  Must not exceed GNNB_SET2SET_MAX_D (include/gnnb200.h).
 _SET2SET_MAX_D = 1024      # GNNB_SET2SET_MAX_D
+# The same bound for global_attention_pool's fused route (gnnb_attention_pool); wider ffeat outputs compose.
+_ATTENTION_POOL_MAX_D = 1024      # GNNB_SET2SET_MAX_D
+
+
+class _AttentionPoolFn(torch.autograd.Function):
+    """u = Σ_k softmax(gate)_k f_k per graph (gnnb_attention_pool) on the graph-indicator plan, where edge k is node k:
+    the per-edge dfe and dgate_e of the pullback are df and dgate.  Keeps f, gate, u and the G-sized softmax
+    statistics."""
+
+    @staticmethod
+    def forward(ctx, f_rows, gate, plan, G):
+        D = f_rows.shape[1]
+        u = torch.empty((G, D), dtype=torch.float32, device=f_rows.device)
+        smax = torch.empty(G, dtype=torch.float32, device=f_rows.device)
+        ssum = torch.empty(G, dtype=torch.float32, device=f_rows.device)
+        with torch.cuda.device(plan.device):
+            _lib.check(lib.gnnb_attention_pool(plan.h, f_rows.data_ptr(), gate.data_ptr(), D, u.data_ptr(),
+                                               smax.data_ptr(), ssum.data_ptr(), _stream(plan.device)))
+        ctx.plan = plan
+        ctx.save_for_backward(f_rows, gate, u, smax, ssum)
+        return u
+
+    @staticmethod
+    def backward(ctx, du):
+        f_rows, gate, u, smax, ssum = ctx.saved_tensors
+        du = du.contiguous()
+        df = torch.empty_like(f_rows)
+        dgate = torch.empty_like(gate)
+        with torch.cuda.device(ctx.plan.device):
+            _lib.check(lib.gnnb_attention_pool_bwd(ctx.plan.h, f_rows.data_ptr(), gate.data_ptr(), u.data_ptr(),
+                                                   smax.data_ptr(), ssum.data_ptr(), du.data_ptr(), f_rows.shape[1],
+                                                   df.data_ptr(), dgate.data_ptr(), _stream(ctx.plan.device)))
+        return df, dgate, None, None
+
+
+def global_attention_pool(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
+    """GNNlib/src/layers/pool.jl:7-12: u = reduce_nodes(+, g, softmax_nodes(g, fgate(x)) .* ffeat(x)).
+    A gate of one row and a 2-D ffeat(x) of 1 to _ATTENTION_POOL_MAX_D rows take one fused pass over ffeat(x), forward
+    and pullback (a graph with no nodes gets u = 0); any other shapes (a gate per channel, wider features) compose
+    softmax_nodes and reduce_nodes."""
+    gate = l.fgate(x)
+    feats = l.ffeat(x)
+    if gate.dim() == 2 and gate.shape[0] == 1 and feats.dim() == 2 and 1 <= feats.shape[0] <= _ATTENTION_POOL_MAX_D:
+        assert gate.shape[-1] == feats.shape[-1] == g.num_nodes, \
+            f"fgate(x) has {gate.shape[-1]} and ffeat(x) {feats.shape[-1]} columns; the graph has {g.num_nodes} nodes"
+        ip = _indicator_plan(g, False)
+        dev = ip.plan.device
+        u = _AttentionPoolFn.apply(_f32(rows(feats), dev), _f32(gate.reshape(-1), dev), ip.plan, ip.n_segments)
+        return unrows(u)
+    alpha = softmax_nodes(g, gate)
+    return reduce_nodes(operator.add, g, alpha * feats)
+
+
+class GlobalPool(GNNLayer):
+    """GlobalPool(aggr) — GraphNeuralNetworks/src/layers/pool.jl:1-41: l(g, x) = reduce_nodes(aggr, g, x);
+    l(g) = GNNGraph(g, gdata=l(g, node_features(g)))."""
+
+    def __init__(self, aggr):
+        super().__init__()
+        self.aggr = aggr
+
+    def forward(self, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
+        return global_pool(self, g, x)
+
+    def graph_forward(self, g: GNNGraph) -> GNNGraph:
+        return GNNGraph(g, gdata=self(g, node_features(g)))
+
+
+class GlobalAttentionPool(GNNLayer):
+    """GlobalAttentionPool(fgate, ffeat=identity) — GraphNeuralNetworks/src/layers/pool.jl:43-99: l(g, x) =
+    global_attention_pool; l(g) = GNNGraph(g, gdata=l(g, node_features(g))).  fgate and ffeat are registered when they
+    are Modules.  Unlike the reference's struct, this is a GNNLayer, so a GNNChain passes it the graph."""
+
+    def __init__(self, fgate, ffeat=identity):
+        super().__init__()
+        self.fgate = fgate
+        self.ffeat = ffeat
+
+    def forward(self, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
+        return global_attention_pool(self, g, x)
+
+    def graph_forward(self, g: GNNGraph) -> GNNGraph:
+        return GNNGraph(g, gdata=self(g, node_features(g)))
 
 
 class _Set2SetAttendFn(torch.autograd.Function):
@@ -190,9 +269,9 @@ def set2set_pool(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     return qstar
 
 
-class Set2Set(torch.nn.Module):
+class Set2Set(GNNLayer):
     """Set2Set(n_in, n_iters, n_layers = 1) — GraphNeuralNetworks/src/layers/pool.jl:126-162: an LSTMCell(2·n_in => n_in)
-    and num_iters; forward(g, x) returns the (2·n_in, num_graphs) readout (set2set_pool)."""
+    and num_iters; forward(g, x) returns the (2·n_in, num_graphs) readout (set2set_pool); l(g) puts it in gdata."""
 
     def __init__(self, n_in: int, n_iters: int, n_layers: int = 1, device=None):
         super().__init__()
@@ -203,6 +282,9 @@ class Set2Set(torch.nn.Module):
 
     def forward(self, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
         return set2set_pool(self, g, x)
+
+    def graph_forward(self, g: GNNGraph) -> GNNGraph:
+        return GNNGraph(g, gdata=self(g, node_features(g)))
 
 
 # ---------------------------------------------------------------------------------------------- top-k pooling

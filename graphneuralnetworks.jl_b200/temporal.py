@@ -30,6 +30,7 @@ import torch
 
 from . import _lib
 from ._lib import lib
+from .basic import GNNLayer
 from .graph import GNNGraph, _stream, add_self_loops, rows, unrows
 from .layers import GCNConv, _bias_act, _DenseAct, _linear, _LSTMCell, gcn_conv, glorot_uniform, relu
 from .layers_more import ChebConv, Chain, DConv, cheb_basis, cheb_operator, diffusion_basis, transposed_graph
@@ -290,7 +291,7 @@ class _GRUCellBase(torch.nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ GConvGRU
-class GConvGRUCell(_GRUCellBase):
+class GConvGRUCell(_GRUCellBase, GNNLayer):
     """GConvGRUCell(in => out, k; bias=true) — temporalconv.jl:200-254: six ChebConvs, fields conv_x_r … conv_h_h."""
 
     def __init__(self, ch_in: int, ch_out: int, k: int, *, bias: bool = True, device=None):
@@ -369,7 +370,7 @@ class DCGRUCell(_GRUCellBase):
 
 
 # ------------------------------------------------------------------------------------------------ TGCN
-class TGCNCell(_GRUCellBase):
+class TGCNCell(_GRUCellBase, GNNLayer):
     """TGCNCell(in => out) — temporalconv.jl:809-849: conv_z / conv_r / conv_h are GNNChain(GCNConv(in => out, relu),
     GCNConv(out => out)), dense_z / dense_r Dense(2out => out, sigmoid), dense_h Dense(2out => out, tanh).  All the
     graph work is on the x side: two propagates per layer call."""
@@ -419,7 +420,7 @@ class TGCNCell(_GRUCellBase):
 
 
 # ------------------------------------------------------------------------------------------------ GConvLSTM
-class GConvLSTMCell(torch.nn.Module):
+class GConvLSTMCell(GNNLayer):
     """GConvLSTMCell(in => out, k; bias=true) — temporalconv.jl:355-437: conv_x_* / conv_h_* ChebConvs, peepholes w_*
     (out, 1) and biases b_* (out,) for the gates i, f, c, o."""
 
@@ -471,7 +472,7 @@ class GConvLSTMCell(torch.nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ EvolveGCNO
-class EvolveGCNOCell(torch.nn.Module):
+class EvolveGCNOCell(GNNLayer):
     """EvolveGCNOCell(in => out; bias=true) — temporalconv.jl:678-705: conv = GCNConv(in => out), lstm =
     LSTMCell(in·out => in·out).  The LSTM evolves the GCN weight and does not read x: per step one gate pass on a
     single row (the LSTM entry without peepholes), then the GCN with that weight."""
@@ -592,7 +593,7 @@ def initialstates(layer_or_cell):
     return layer_or_cell.initialstates()
 
 
-class GNNRecurrence(torch.nn.Module):
+class GNNRecurrence(GNNLayer):
     """GNNRecurrence(cell) — temporalconv.jl:121-135.  layer(g, x[, state]):
       GNNGraph: x (in, T, N) -> y (out, T, N);  TemporalSnapshotsGNNGraph: x a list of (in, N_t) -> a list."""
 

@@ -621,6 +621,29 @@ int gnnb_set2set_attend_bwd(gnnb_graph_t g, const float* x, const float* q, cons
                             const float* seg_max, const float* seg_sum, const float* dr, int64_t D,
                             float* dxe, float* dq, void* stream);
 
+/* --------------------------------------------------------- attention pooling (csrc/set2set.cu)
+ * replaces the composition of global_attention_pool (GNNlib/src/layers/pool.jl:7-12) for a gate of one row:
+ *           softmax_nodes(g, gate), the D x N product α .* f and reduce_nodes(+, g, ·), in one pass over f.  The Set2Set
+ *           attention with a given score per source instead of <q, x>:
+ *   M_i = max_k gate[s_k];  S_i = Σ_k exp(gate[s_k] − M_i)
+ *   u[:, i] = Σ_k exp(gate[s_k] − M_i) f[:, s_k] / S_i    (k over the in-edges of target i, in plan order)
+ * f (D, num_src), u (D, num_dst): DEVICE floats, column i contiguous; gate (num_src): DEVICE floats.  seg_max, seg_sum
+ * (num_dst) are kept for the pullback.  A target with no edges: u = 0, seg_max = −Inf, seg_sum = 0.  On the
+ * graph-indicator plan (edge k = node k -> its graph) the targets are the graphs of a batch.
+ * Bounds, errors and determinism as gnnb_set2set_attend: 1 <= D (GNNB_ESIZE) <= GNNB_SET2SET_MAX_D
+ * (GNNB_EUNSUPPORTED), a NULL array of positive size is GNNB_ESIZE, no atomics, results run-to-run bit-identical.
+ * Does not synchronise. */
+int gnnb_attention_pool(gnnb_graph_t g, const float* f, const float* gate, int64_t D,
+                        float* u, float* seg_max, float* seg_sum, void* stream);
+/* pullback given du (D, num_dst): α_k = exp(gate[s_k] − M_i) / S_i from seg_max / seg_sum (the forward's bits),
+ * T_i = <du_i, u_i>,
+ *   dgate_e[k] = α_k (<du[:, t_k], f[:, s_k]> − T_i)
+ *   dfe[:, k]  = α_k du[:, t_k]                     per edge, in COO order: every entry written exactly once
+ * On the graph-indicator plan dfe is df and dgate_e is dgate.  Same bounds and errors as the forward. */
+int gnnb_attention_pool_bwd(gnnb_graph_t g, const float* f, const float* gate, const float* u,
+                            const float* seg_max, const float* seg_sum, const float* du, int64_t D,
+                            float* dfe, float* dgate_e, void* stream);
+
 /* --------------------------------------------------------- top-k pooling (csrc/topk.cu)
  * replaces: topk_index(y, k) = collect(1:length(y))[y .>= nlargest(k, y)[end]] and the score and gate of
  *           topk_pool(t, X) = view(X, :, idx) .* σ.(view(y, idx)'), y = t.p' * X / norm(t.p)

@@ -1146,6 +1146,49 @@ function GNNlib.set2set_pool(l, g::GNNGraph{<:CuCOO}, x::CuMatrix{Float32})
     return qstar
 end
 
+## global_attention_pool on device COO graphs — replaces GNNlib/src/layers/pool.jl:7-12 for a gate of one row:
+## softmax_nodes, the D x N product α .* ffeat(x) and reduce_nodes(+) are one pass of gnnb_attention_pool over the
+## graph-indicator plan; its rrule calls gnnb_attention_pool_bwd, whose per-edge dfe and dgate_e are df and dgate on that
+## plan, and keeps only graph-sized state besides f and the gate.  Other shapes (a gate per channel, D above
+## SET2SET_MAX_D) take the reference's composition, as in the Python mirror.
+function _attention_pool(p::Plan, f::CuMatrix{Float32}, gate::CuVector{Float32}, G::Integer)
+    D = size(f, 1)
+    u = CuMatrix{Float32}(undef, D, G)
+    smax, ssum = CuVector{Float32}(undef, G), CuVector{Float32}(undef, G)
+    check(ccall((:gnnb_attention_pool, LIB), Cint,
+                (Ptr{Cvoid}, CuPtr{Float32}, CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32},
+                 Ptr{Cvoid}),
+                p.h, f, gate, D, u, smax, ssum, stream()))
+    return u, smax, ssum
+end
+
+attention_pool(p::Plan, f::CuMatrix{Float32}, gate::CuVector{Float32}, G::Integer) = _attention_pool(p, f, gate, G)[1]
+
+function ChainRulesCore.rrule(::typeof(attention_pool), p::Plan, f::CuMatrix{Float32}, gate::CuVector{Float32},
+                              G::Integer)
+    u, smax, ssum = _attention_pool(p, f, gate, G)
+    function attention_pool_pullback(Δ)
+        du = CuMatrix{Float32}(unthunk(Δ))
+        df, dgate = similar(f), similar(gate)
+        check(ccall((:gnnb_attention_pool_bwd, LIB), Cint,
+                    (Ptr{Cvoid}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32}, CuPtr{Float32},
+                     CuPtr{Float32}, Int64, CuPtr{Float32}, CuPtr{Float32}, Ptr{Cvoid}),
+                    p.h, f, gate, u, smax, ssum, du, size(f, 1), df, dgate, stream()))
+        return NoTangent(), NoTangent(), df, dgate, NoTangent()
+    end
+    return u, attention_pool_pullback
+end
+
+function GNNlib.global_attention_pool(l, g::GNNGraph{<:CuCOO}, x::AbstractMatrix)
+    gate, feats = l.fgate(x), l.ffeat(x)
+    if !(gate isa CuMatrix{Float32} && size(gate, 1) == 1 && feats isa CuMatrix{Float32} &&
+         1 <= size(feats, 1) <= SET2SET_MAX_D)
+        return invoke(GNNlib.global_attention_pool, Tuple{Any, GNNGraph, AbstractArray}, l, g, x)
+    end
+    @assert size(gate, 2) == size(feats, 2) == g.num_nodes "fgate(x) and ffeat(x) need num_nodes = $(g.num_nodes) columns"
+    return attention_pool(_indicator_plan(g), feats, vec(gate), g.num_graphs)
+end
+
 ## topk_index / topk_pool on device arrays — replace GNNlib/src/layers/pool.jl:14-27.  The selection is gnnb_topk_keep
 ## (one segment; NaN never kept nor counted, this library's rule), the score and gate are one pass each over X, and the
 ## rrule of the gate calls gnnb_topk_gate_bwd, which gives dX through the gather and through y, and dp through y.

@@ -156,6 +156,15 @@ for Ds in (1, 3, 1024, 1025):
     ys = l(gs, xs)
     ys.sum().backward()
     print("set2set D", Ds, "empty graph r == 0", bool((ys[Ds:, 2] == 0).all()), "grad finite", bool(torch.isfinite(xs.grad).all()))
+# attention pooling: the same graphs (127, 128, 129 nodes at chunk 128, one without nodes), forward and backward at
+# D = 1, 3, 1024 (the fused entries) and 1025 (the composition)
+for Da in (1, 3, 1024, 1025):
+    fa = torch.randn(Da, gi.numel(), device="cuda").requires_grad_(True)
+    ga = torch.randn(1, gi.numel(), device="cuda").requires_grad_(True)
+    ua = gnn.GlobalAttentionPool(lambda v: ga, lambda v: fa)(gs, fa)
+    ua.sum().backward()
+    print("attention_pool D", Da, "empty graph u == 0", bool((ua[:, 2] == 0).all()), "grads finite",
+          bool(torch.isfinite(fa.grad).all() and torch.isfinite(ga.grad).all()))
 # recurrent gates: every entry at D = 1, 3, 64, 129 on a strided PX and with a 4-byte offset (the scalar path), then
 # every temporal layer forward and backward on a small graph
 from gnnb200._lib import lib as L, check as chk  # noqa: E402
