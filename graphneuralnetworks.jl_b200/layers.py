@@ -28,7 +28,7 @@ import torch
 from . import _lib
 from ._lib import lib
 from .basic import _EdgeFeatureLayer, GNNLayer
-from .graph import GNNGraph, _is_hetero, _stream, add_self_loops, degree, homogeneous_only, num_src_dst, relation, rows, unrows
+from .graph import GNNGraph, _is_hetero, _ptr, _stream, add_self_loops, degree, homogeneous_only, num_src_dst, relation, rows, unrows
 from .msgpass import (Fix1, _GCNPropagateFn, _f32, aggregate_neighbors, apply_edges, check_num_nodes, copy_xj,
                       e_mul_xj, expand_srcdst, mean, propagate, softmax_edge_neighbors, w_mul_xj)
 
@@ -229,33 +229,40 @@ def gcn_conv(l, g: GNNGraph, x: torch.Tensor, edge_weight: Optional[torch.Tensor
             edge_weight = torch.cat([edge_weight, torch.ones(g.num_nodes, dtype=edge_weight.dtype,
                                                              device=edge_weight.device)])
             assert edge_weight.numel() == g.num_edges
-    Dout, Din = weight.shape
+    return _gcn_dense(l, weight, x, lambda h: _gcn_propagate(l, g, h, edge_weight, norm_fn))
+
+
+def _gcn_dense(l, W: torch.Tensor, x: torch.Tensor, propagate_fn: Callable) -> torch.Tensor:
+    """σ.(W * P(x) .+ b) for the normalised propagation P of gcn_conv and dist_gcn_conv: W multiplies before P when
+    Dout < Din (P moves fewer columns), after it otherwise, where one GEMM also takes the bias/relu epilogue."""
+    Dout, Din = W.shape
     if Dout < Din:
-        x = _linear(l, weight, x, False)  # multiply before convolution if it is more convenient
+        return _bias_act(l, propagate_fn(_linear(l, W, x, False)))
+    return _linear(l, W, propagate_fn(x), True)
+
+
+def _gcn_propagate(l, g: GNNGraph, x: torch.Tensor, edge_weight, norm_fn) -> torch.Tensor:
+    """c .* propagate(c .* x) with c = norm_fn(in-degree) (conv.jl:44-67)."""
     xj, xi = expand_srcdst(g, x)
     check_num_nodes(g, xj)
     use_w = bool(getattr(l, "use_edge_weight", False)) and g.w is not None
     if edge_weight is None and not use_w and norm_fn is None:
         plan = g.plan()
-        out = unrows(_GCNPropagateFn.apply(_f32(rows(xj), plan.device), plan, None))   # c: the plan's own
+        return unrows(_GCNPropagateFn.apply(_f32(rows(xj), plan.device), plan, None))   # c: the plan's own
+    nf = norm_fn or default_norm_fn
+    if edge_weight is not None:
+        d = degree(g, torch.float32, dir="in", edge_weight=edge_weight)
     else:
-        nf = norm_fn or default_norm_fn
-        if edge_weight is not None:
-            d = degree(g, torch.float32, dir="in", edge_weight=edge_weight)
-        else:
-            d = degree(g, torch.float32, dir="in", edge_weight=bool(getattr(l, "use_edge_weight", False)))
-        c = nf(d)
-        xs = xj * c.reshape(1, -1)
-        if edge_weight is not None:
-            out = propagate(e_mul_xj, g, operator.add, xj=xs, e=edge_weight)
-        elif use_w:
-            out = propagate(w_mul_xj, g, operator.add, xj=xs)
-        else:
-            out = propagate(copy_xj, g, operator.add, xj=xs)
-        out = out * c.reshape(1, -1)
-    if Dout >= Din:
-        return _linear(l, weight, out, True)      # σ.(W * x .+ b): one GEMM with the bias/relu epilogue
-    return _bias_act(l, out)
+        d = degree(g, torch.float32, dir="in", edge_weight=bool(getattr(l, "use_edge_weight", False)))
+    c = nf(d)
+    xs = xj * c.reshape(1, -1)
+    if edge_weight is not None:
+        out = propagate(e_mul_xj, g, operator.add, xj=xs, e=edge_weight)
+    elif use_w:
+        out = propagate(w_mul_xj, g, operator.add, xj=xs)
+    else:
+        out = propagate(copy_xj, g, operator.add, xj=xs)
+    return out * c.reshape(1, -1)
 
 
 class _GCNBipartiteFn(torch.autograd.Function):
@@ -349,129 +356,116 @@ class GCNConv(GNNLayer):
 
 
 # ------------------------------------------------------------------------------------------- GATConv
-class _GATAggregateFn(torch.autograd.Function):
-    """Fused logits -> leakyrelu -> neighbourhood softmax -> α-weighted sum: gnnb_gat_aggregate(+_bwd)."""
+def _gat_aggregate(plan, Wx, el, er, slope):
+    """gnnb_gat_aggregate over a plan: the fused logits -> leakyrelu -> neighbourhood softmax -> α-weighted sum.  Wx
+    (N_src, H, C) and er (N_src, H) have a row per source, el (N_dst, H) one per target.  Returns (out, seg_max, seg_sum),
+    like partition.dist_gat_aggregate on a partitioned graph."""
+    _, H, Cc = Wx.shape
+    N = el.shape[0]
+    out = torch.empty((N, H, Cc), dtype=torch.float32, device=Wx.device)
+    smax = torch.empty((N, H), dtype=torch.float32, device=Wx.device)
+    ssum = torch.empty((N, H), dtype=torch.float32, device=Wx.device)
+    with torch.cuda.device(plan.device):
+        _lib.check(lib.gnnb_gat_aggregate(plan.h, Wx.data_ptr(), el.data_ptr(), er.data_ptr(), Cc, H, slope,
+                                          out.data_ptr(), None, smax.data_ptr(), ssum.data_ptr(), _stream(plan.device)))
+    return out, smax, ssum
+
+
+def _gat_aggregate_bwd(plan, Wx, el, er, smax, ssum, out, dout, slope):
+    """gnnb_gat_aggregate_bwd over a plan.  Returns (dWx, del, der)."""
+    _, H, Cc = Wx.shape
+    dWx, del_, der = torch.empty_like(Wx), torch.empty_like(el), torch.empty_like(er)
+    with torch.cuda.device(plan.device):
+        _lib.check(lib.gnnb_gat_aggregate_bwd(plan.h, Wx.data_ptr(), el.data_ptr(), er.data_ptr(), smax.data_ptr(),
+                                              ssum.data_ptr(), out.data_ptr(), dout.data_ptr(), Cc, H, slope,
+                                              dWx.data_ptr(), del_.data_ptr(), der.data_ptr(), _stream(plan.device)))
+    return dWx, del_, der
+
+
+def _gat_logit_terms(Wx, a_jl, el, er) -> None:
+    """gnnb_gat_logit_terms over the rows of Wx (N, H, C) into el and er (N, H); a None half is not computed.  No rows
+    (a rank that owns none): no pass."""
+    N, H, Cc = Wx.shape
+    if N:
+        with torch.cuda.device(Wx.device):
+            _lib.check(lib.gnnb_gat_logit_terms(Wx.data_ptr(), a_jl.data_ptr(), N, Cc, H, _ptr(el), _ptr(er),
+                                                _stream(Wx.device)))
+
+
+def _gat_logit_terms_bwd(Wx, a_jl, del_, der, dWx) -> torch.Tensor:
+    """gnnb_gat_logit_terms_bwd: adds the el / er chain of the rows of Wx into dWx in place (a None del or der adds
+    nothing) and returns da, (H, 2C) like a_jl, with a zero half for a None one."""
+    N, H, Cc = Wx.shape
+    if not N:
+        return torch.zeros_like(a_jl)
+    da = torch.empty_like(a_jl)
+    with torch.cuda.device(Wx.device):
+        _lib.check(lib.gnnb_gat_logit_terms_bwd(Wx.data_ptr(), a_jl.data_ptr(), _ptr(del_), _ptr(der), N, Cc, H,
+                                                dWx.data_ptr(), da.data_ptr(), _stream(Wx.device)))
+    return da
+
+
+class _GATFn(torch.autograd.Function):
+    """gat_conv's fused edge part.  Wxj (N_src, H, C) projects the sources, Wxi (N_dst, H, C) the targets (None: the
+    same tensor as Wxj).  Given the attention vector a (2C, H), gnnb_gat_logit_terms computes the per-node logit halves,
+    el from Wxi and er from Wxj: one pass for one projection, one pass per half for two.  Otherwise el and er are inputs
+    that torch computed.  Then `aggregate(target, Wxj, el, er, slope) -> (out, seg_max, seg_sum)`, over a plan
+    (_gat_aggregate) or a partitioned graph (partition.dist_gat_aggregate).
+    Backward: `aggregate_bwd(target, Wxj, el, er, seg_max, seg_sum, out, dout, slope) -> (dWxj, del, der)`, then
+    gnnb_gat_logit_terms_bwd adds the er chain into dWxj and the el chain into dWxi (zero-filled first), each with its
+    half of da; for two projections da is the sum of the two."""
 
     @staticmethod
-    def forward(ctx, Wx_rows, el_rows, er_rows, plan, slope):
-        _, H, Cc = Wx_rows.shape
-        N = el_rows.shape[0]                   # targets (num_dst); Wx and er have a row per source
-        out = torch.empty((N, H, Cc), dtype=torch.float32, device=Wx_rows.device)
-        smax = torch.empty((N, H), dtype=torch.float32, device=Wx_rows.device)
-        ssum = torch.empty((N, H), dtype=torch.float32, device=Wx_rows.device)
-        with torch.cuda.device(plan.device):
-            _lib.check(lib.gnnb_gat_aggregate(plan.h, Wx_rows.data_ptr(), el_rows.data_ptr(), er_rows.data_ptr(),
-                                              Cc, H, slope, out.data_ptr(), None, smax.data_ptr(),
-                                              ssum.data_ptr(), _stream(plan.device)))
-        ctx.plan, ctx.slope, ctx.dims = plan, slope, (Cc, H)
-        ctx.save_for_backward(Wx_rows, el_rows, er_rows, smax, ssum, out)
+    def forward(ctx, Wxj, Wxi, a, el, er, target, aggregate, aggregate_bwd, slope):
+        a_jl = None
+        if a is not None:
+            a_jl = a.detach().t().contiguous()             # Julia (2C, H) column-major memory = rows (H, 2C)
+            Wt = Wxj if Wxi is None else Wxi
+            el = torch.empty(Wt.shape[:2], dtype=torch.float32, device=Wt.device)
+            er = torch.empty(Wxj.shape[:2], dtype=torch.float32, device=Wxj.device)
+            if Wxi is None:
+                _gat_logit_terms(Wxj, a_jl, el, er)
+            else:
+                _gat_logit_terms(Wxi, a_jl, el, None)
+                _gat_logit_terms(Wxj, a_jl, None, er)
+        out, smax, ssum = aggregate(target, Wxj, el, er, slope)
+        ctx.target, ctx.aggregate_bwd, ctx.slope = target, aggregate_bwd, slope
+        ctx.save_for_backward(Wxj, Wxi, a_jl, el, er, smax, ssum, out)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        Wx_rows, el_rows, er_rows, smax, ssum, out = ctx.saved_tensors
-        Cc, H = ctx.dims
-        dout = dout.contiguous()
-        dWx = torch.empty_like(Wx_rows)
-        del_ = torch.empty_like(el_rows)
-        der = torch.empty_like(er_rows)
-        with torch.cuda.device(ctx.plan.device):
-            _lib.check(lib.gnnb_gat_aggregate_bwd(ctx.plan.h, Wx_rows.data_ptr(), el_rows.data_ptr(),
-                                                  er_rows.data_ptr(), smax.data_ptr(), ssum.data_ptr(),
-                                                  out.data_ptr(), dout.data_ptr(), Cc, H, ctx.slope, dWx.data_ptr(),
-                                                  del_.data_ptr(), der.data_ptr(), _stream(ctx.plan.device)))
-        return dWx, del_, der, None, None
+        Wxj, Wxi, a_jl, el, er, smax, ssum, out = ctx.saved_tensors
+        dWxj, del_, der = ctx.aggregate_bwd(ctx.target, Wxj, el, er, smax, ssum, out, dout.contiguous(), ctx.slope)
+        if a_jl is None:                                   # torch's el and er: torch carries their chain
+            return dWxj, None, None, del_, der, None, None, None, None
+        if Wxi is None:
+            dWxi, da = None, _gat_logit_terms_bwd(Wxj, a_jl, del_, der, dWxj)
+        else:
+            dWxi = torch.zeros_like(Wxi)
+            da = _gat_logit_terms_bwd(Wxj, a_jl, None, der, dWxj) + _gat_logit_terms_bwd(Wxi, a_jl, del_, None, dWxi)
+        return dWxj, dWxi, da.t(), None, None, None, None, None, None
 
 
-class _GATCoreFn(torch.autograd.Function):
-    """The whole edge part of gat_conv for one projection Wx (N, H, C) and attention vector a (2C, H): per-node logit
-    halves (gnnb_gat_logit_terms, one pass over Wx), then the fused logits -> leakyrelu -> neighbourhood softmax ->
-    α-weighted sum (gnnb_gat_aggregate).  Backward: gnnb_gat_aggregate_bwd, then gnnb_gat_logit_terms_bwd adds the el / er
-    chain into dWx in place and reduces da — no (C,H,N) temporaries, no eager broadcast-multiply-reduce."""
-
-    @staticmethod
-    def forward(ctx, Wx_rows, a, plan, slope):
-        N, H, Cc = Wx_rows.shape
-        dev = Wx_rows.device
-        a_jl = a.detach().t().contiguous()                 # Julia (2C, H) column-major memory = rows (H, 2C)
-        el = torch.empty((N, H), dtype=torch.float32, device=dev)
-        er = torch.empty_like(el)
-        out = torch.empty_like(Wx_rows)
-        smax, ssum = torch.empty_like(el), torch.empty_like(el)
-        with torch.cuda.device(plan.device):
-            st = _stream(plan.device)
-            _lib.check(lib.gnnb_gat_logit_terms(Wx_rows.data_ptr(), a_jl.data_ptr(), N, Cc, H, el.data_ptr(), er.data_ptr(), st))
-            _lib.check(lib.gnnb_gat_aggregate(plan.h, Wx_rows.data_ptr(), el.data_ptr(), er.data_ptr(), Cc, H, slope,
-                                              out.data_ptr(), None, smax.data_ptr(), ssum.data_ptr(), st))
-        ctx.plan, ctx.slope, ctx.dims = plan, slope, (Cc, H)
-        ctx.save_for_backward(Wx_rows, a_jl, el, er, smax, ssum, out)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        Wx_rows, a_jl, el, er, smax, ssum, out = ctx.saved_tensors
-        Cc, H = ctx.dims
-        N = Wx_rows.shape[0]
-        dout = dout.contiguous()
-        dWx = torch.empty_like(Wx_rows)
-        del_, der = torch.empty_like(el), torch.empty_like(er)
-        da_jl = torch.empty_like(a_jl)
-        with torch.cuda.device(ctx.plan.device):
-            st = _stream(ctx.plan.device)
-            _lib.check(lib.gnnb_gat_aggregate_bwd(ctx.plan.h, Wx_rows.data_ptr(), el.data_ptr(), er.data_ptr(), smax.data_ptr(),
-                                                  ssum.data_ptr(), out.data_ptr(), dout.data_ptr(), Cc, H, ctx.slope,
-                                                  dWx.data_ptr(), del_.data_ptr(), der.data_ptr(), st))
-            _lib.check(lib.gnnb_gat_logit_terms_bwd(Wx_rows.data_ptr(), a_jl.data_ptr(), del_.data_ptr(), der.data_ptr(), N, Cc,
-                                                    H, dWx.data_ptr(), da_jl.data_ptr(), st))
-        return dWx, da_jl.t(), None, None
+def _gat_edge_part(l, Wxj, Wxi, target, aggregate, aggregate_bwd) -> torch.Tensor:
+    """The fused edge part of gat_conv and dist_gat_conv on Julia-shaped projections (C, H, N); Wxi None when the targets'
+    projection is Wxj.  The projections go to the kernels as 16 B-aligned rows; gnnb_gat_logit_terms computes the logit
+    halves for its shapes and a float32 `a`, torch otherwise.  Returns (C, H, N_dst)."""
+    _, chout = l.channel
+    a, slope = l.a, float(l.negative_slope)
+    Wr = _aligned_rows(Wxj, target.device)                  # (N_src, H, C)
+    Wi = None if Wxi is None else _aligned_rows(Wxi, target.device)
+    if gat_logit_fusable(chout, l.heads) and a.dtype == torch.float32:
+        return unrows(_GATFn.apply(Wr, Wi, a, None, None, target, aggregate, aggregate_bwd, slope))
+    Wt = Wr if Wi is None else Wi
+    el = (Wt * a[:chout, :].t().unsqueeze(0)).sum(-1)       # rows 1..C of a pair with the target
+    er = (Wr * a[chout:, :].t().unsqueeze(0)).sum(-1)       # rows C+1..2C with the source
+    return unrows(_GATFn.apply(Wr, None, None, el.contiguous(), er.contiguous(), target, aggregate, aggregate_bwd, slope))
 
 
-class _GATPairFn(torch.autograd.Function):
-    """gat_conv's edge part for two projections: Wxj (N_src, H, C) over the sources, Wxi (N_dst, H, C) over the targets.
-    el from Wxi and er from Wxj, one half per gnnb_gat_logit_terms pass, then gnnb_gat_aggregate over the plan.
-    Backward: gnnb_gat_aggregate_bwd gives dWxj, del, der; gnnb_gat_logit_terms_bwd adds the er chain into dWxj and the
-    el chain into dWxi, each with its half of da (the other half zero), and da is their sum."""
-
-    @staticmethod
-    def forward(ctx, Wxj_rows, Wxi_rows, a, plan, slope):
-        Ns, H, Cc = Wxj_rows.shape
-        Nd = Wxi_rows.shape[0]
-        dev = Wxj_rows.device
-        a_jl = a.detach().t().contiguous()                 # Julia (2C, H) column-major memory = rows (H, 2C)
-        el = torch.empty((Nd, H), dtype=torch.float32, device=dev)
-        er = torch.empty((Ns, H), dtype=torch.float32, device=dev)
-        out = torch.empty((Nd, H, Cc), dtype=torch.float32, device=dev)
-        smax, ssum = torch.empty_like(el), torch.empty_like(el)
-        with torch.cuda.device(plan.device):
-            st = _stream(plan.device)
-            _lib.check(lib.gnnb_gat_logit_terms(Wxi_rows.data_ptr(), a_jl.data_ptr(), Nd, Cc, H, el.data_ptr(), None, st))
-            _lib.check(lib.gnnb_gat_logit_terms(Wxj_rows.data_ptr(), a_jl.data_ptr(), Ns, Cc, H, None, er.data_ptr(), st))
-            _lib.check(lib.gnnb_gat_aggregate(plan.h, Wxj_rows.data_ptr(), el.data_ptr(), er.data_ptr(), Cc, H, slope,
-                                              out.data_ptr(), None, smax.data_ptr(), ssum.data_ptr(), st))
-        ctx.plan, ctx.slope, ctx.dims = plan, slope, (Cc, H)
-        ctx.save_for_backward(Wxj_rows, Wxi_rows, a_jl, el, er, smax, ssum, out)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        Wxj_rows, Wxi_rows, a_jl, el, er, smax, ssum, out = ctx.saved_tensors
-        Cc, H = ctx.dims
-        Ns, Nd = Wxj_rows.shape[0], Wxi_rows.shape[0]
-        dout = dout.contiguous()
-        dWxj = torch.empty_like(Wxj_rows)
-        dWxi = torch.zeros_like(Wxi_rows)
-        del_, der = torch.empty_like(el), torch.empty_like(er)
-        da_r, da_l = torch.empty_like(a_jl), torch.empty_like(a_jl)
-        with torch.cuda.device(ctx.plan.device):
-            st = _stream(ctx.plan.device)
-            _lib.check(lib.gnnb_gat_aggregate_bwd(ctx.plan.h, Wxj_rows.data_ptr(), el.data_ptr(), er.data_ptr(),
-                                                  smax.data_ptr(), ssum.data_ptr(), out.data_ptr(), dout.data_ptr(), Cc, H,
-                                                  ctx.slope, dWxj.data_ptr(), del_.data_ptr(), der.data_ptr(), st))
-            _lib.check(lib.gnnb_gat_logit_terms_bwd(Wxj_rows.data_ptr(), a_jl.data_ptr(), None, der.data_ptr(), Ns, Cc, H,
-                                                    dWxj.data_ptr(), da_r.data_ptr(), st))
-            _lib.check(lib.gnnb_gat_logit_terms_bwd(Wxi_rows.data_ptr(), a_jl.data_ptr(), del_.data_ptr(), None, Nd, Cc, H,
-                                                    dWxi.data_ptr(), da_l.data_ptr(), st))
-        return dWxj, dWxi, (da_l + da_r).t(), None, None
+def _aligned_rows(W: torch.Tensor, device) -> torch.Tensor:
+    r = _f32(rows(W), device)
+    return r if r.data_ptr() % 16 == 0 else r.clone()       # a misaligned view: the fused kernels take 16 B-aligned rows
 
 
 def gat_logit_fusable(chout: int, heads: int) -> bool:
@@ -530,36 +524,10 @@ def gat_conv(l, g: GNNGraph, x: torch.Tensor, e: Optional[torch.Tensor] = None, 
     if xi is not xj:
         Wxi = _jl_reshape3(l.dense_x(xi), chout, heads)
     nodrop = float(getattr(l, "dropout", 0.0) or 0.0) == 0.0
-    if fused and e is None and xi is not xj and gat_fusable(chout, heads) and nodrop:
-        # two projections (the (xj, xi) form; a relation between two node types): el from W xi over the num_dst
-        # targets, er from W xj over the num_src sources, then the fused logits -> leakyrelu -> neighbourhood softmax
-        # -> α-weighted sum over the relation's plan
-        plan = relation(g).plan()
-        Wr = _f32(rows(Wxj), plan.device)                       # (N_src, H, C)
-        if Wr.data_ptr() % 16 != 0:
-            Wr = Wr.clone()
-        Wi = _f32(rows(Wxi), plan.device)                       # (N_dst, H, C)
-        if Wi.data_ptr() % 16 != 0:
-            Wi = Wi.clone()
-        a = l.a
-        if gat_logit_fusable(chout, heads) and a.dtype == torch.float32:
-            out = unrows(_GATPairFn.apply(Wr, Wi, a, plan, float(l.negative_slope)))
-        else:
-            el = (Wi * a[:chout, :].t().unsqueeze(0)).sum(-1)   # rows 1..C of a pair with the target
-            er = (Wr * a[chout:, :].t().unsqueeze(0)).sum(-1)   # rows C+1..2C with the source
-            out = unrows(_GATAggregateFn.apply(Wr, el.contiguous(), er.contiguous(), plan, float(l.negative_slope)))
-    elif fused and e is None and xi is xj and gat_fusable(chout, heads) and nodrop:
-        plan = g.plan()
-        Wr = _f32(rows(Wxj), plan.device)                       # (N, H, C)
-        if Wr.data_ptr() % 16 != 0:                             # a misaligned view: the fused kernels take 16 B-aligned rows
-            Wr = Wr.clone()
-        a = l.a                                                 # (2C, H)
-        if gat_logit_fusable(chout, heads) and a.dtype == torch.float32:
-            out = unrows(_GATCoreFn.apply(Wr, a, plan, float(l.negative_slope)))
-        else:
-            el = (Wr * a[:chout, :].t().unsqueeze(0)).sum(-1)   # (N, H): rows 1..C pair with the target
-            er = (Wr * a[chout:, :].t().unsqueeze(0)).sum(-1)   # rows C+1..2C pair with the source
-            out = unrows(_GATAggregateFn.apply(Wr, el.contiguous(), er.contiguous(), plan, float(l.negative_slope)))
+    if fused and e is None and gat_fusable(chout, heads) and nodrop:
+        # a second projection in the (xj, xi) form (a relation between two node types): el from W xi over the num_dst
+        # targets, er from W xj over the num_src sources
+        out = _gat_edge_part(l, Wxj, None if xi is xj else Wxi, g.plan(), _gat_aggregate, _gat_aggregate_bwd)
     else:
         m = apply_edges(Fix1(gat_message, l), g, Wxi, Wxj, e)
         α = softmax_edge_neighbors(g, m["logα"])
@@ -568,10 +536,7 @@ def gat_conv(l, g: GNNGraph, x: torch.Tensor, e: Optional[torch.Tensor] = None, 
             α = torch.nn.functional.dropout(α, p, training=getattr(l, "training", True))
         β = α * m["Wxj"]
         out = aggregate_neighbors(g, operator.add, β)
-    if not l.concat:
-        out = out.mean(dim=1, keepdim=True)
-    out = unrows(rows(out).reshape(out.shape[-1], -1))  # reshape(x, :, size(x, 3))
-    return _bias_act(l, out)
+    return _attention_tail(l, out)
 
 
 class _Dense(torch.nn.Module):
@@ -654,16 +619,20 @@ def sage_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     check_num_nodes(g, x)
     xj, xi = expand_srcdst(g, x)
     m = propagate(copy_xj, g, l.aggr, xj=xj)
+    return _sage_linear(l, rows(xi), rows(m))
+
+
+def _sage_linear(l, r1: torch.Tensor, r2: torch.Tensor) -> torch.Tensor:
+    """σ.(W * vcat(x1, x2) .+ b) on rows r1 (N, D1) and r2 (N, D2), the dense part of sage_conv and dist_sage_conv."""
     W = l.weight
     sig, b = _sigma(l), _bias(l)
-    r1, r2 = rows(xi), rows(m)
     D1, D2, Dout = r1.shape[1], r2.shape[1], W.shape[0]
     if (r1.is_cuda and r1.dtype == torch.float32 and W.dtype == torch.float32 and Dout == 128 and D1 % 32 == 0 and D2 % 32 == 0
             and D1 <= 128 and D2 <= 128 and (sig is identity or _is_relu(sig))):
         # the two column blocks of W in two accumulating wgmma passes: no vcat temporary
         return unrows(_Linear2Fn.apply(r1.contiguous(), r2.contiguous(), W, None if b is None else b.contiguous(), _is_relu(sig)))
-    xm = unrows(torch.cat([r1, r2], dim=1))                   # vcat(xi, m): (2·in, N)
-    return _linear(l, W, xm, True)                            # σ.(W * vcat(xi, m) .+ b): one GEMM, bias/σ in the epilogue
+    xm = unrows(torch.cat([r1, r2], dim=1))                   # vcat(x1, x2): (D1 + D2, N)
+    return _linear(l, W, xm, True)                            # one GEMM, bias/σ in the epilogue
 
 
 class SAGEConv(GNNLayer):
@@ -906,10 +875,12 @@ def gatv2_message(l, Wxi, Wxj, e):
 
 
 def _attention_tail(l, out: torch.Tensor) -> torch.Tensor:
-    """`!concat -> mean over heads; reshape(x, :, N); σ.(x .+ bias)` shared by gat_conv and gatv2_conv."""
+    """`!concat -> mean over heads; reshape(x, :, N); σ.(x .+ bias)` on (C, H, N) shared by gat_conv, gatv2_conv and
+    dist_gat_conv."""
     if not l.concat:
         out = out.mean(dim=1, keepdim=True)
-    out = unrows(rows(out).reshape(out.shape[-1], -1))
+    r = rows(out)
+    out = unrows(r.reshape(r.shape[0], r.shape[1] * r.shape[2]))   # reshape(x, :, size(x, 3)), also for N = 0
     return _bias_act(l, out)
 
 

@@ -610,17 +610,8 @@ def dist_gcn_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
     The graph must have been partitioned with add_self_loops = l.add_self_loops.  Weight gradients are per-rank
     partial sums: all-reduce them like any data-parallel layer."""
     assert dg.self_loops == bool(l.add_self_loops)
-    from .layers import _linear
-    W = l.weight
-    Dout, Din = W.shape
-    x = x_local
-    if Dout < Din:
-        x = _linear(l, W, x, False)
-    pr = unrows(_DistGCNPropagateFn.apply(rows(x), dg))
-    if Dout >= Din:
-        return _linear(l, W, pr, True)            # σ.(W * x .+ b): GEMM with the bias/relu epilogue
-    from .layers import _bias_act
-    return _bias_act(l, pr)
+    from .layers import _gcn_dense
+    return _gcn_dense(l, l.weight, x_local, lambda h: unrows(_DistGCNPropagateFn.apply(rows(h), dg)))
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -675,61 +666,11 @@ def dist_gat_aggregate_bwd(dg: DistGraph, Wx, el, er, smax, ssum, out, dout, slo
     return dWx, del_, der
 
 
-class _DistGATCoreFn(torch.autograd.Function):
-    """_GATCoreFn on shards: logit halves of the owned rows (gnnb_gat_logit_terms), dist_gat_aggregate; pullback
-    dist_gat_aggregate_bwd, then gnnb_gat_logit_terms_bwd on the owned rows (da is this rank's partial sum)."""
-
-    @staticmethod
-    def forward(ctx, Wx, a, dg: DistGraph, slope):
-        N, H, Cc = Wx.shape
-        dev = Wx.device
-        a_jl = a.detach().t().contiguous()
-        el = torch.empty((N, H), dtype=torch.float32, device=dev)
-        er = torch.empty_like(el)
-        if N:
-            with torch.cuda.device(dev):
-                _lib.check(lib.gnnb_gat_logit_terms(Wx.data_ptr(), a_jl.data_ptr(), N, Cc, H, el.data_ptr(), er.data_ptr(),
-                                                    _stream(dev)))
-        out, smax, ssum = dist_gat_aggregate(dg, Wx, el, er, slope)
-        ctx.dg, ctx.slope = dg, slope
-        ctx.save_for_backward(Wx, a_jl, el, er, smax, ssum, out)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        Wx, a_jl, el, er, smax, ssum, out = ctx.saved_tensors
-        N, H, Cc = Wx.shape
-        dWx, del_, der = dist_gat_aggregate_bwd(ctx.dg, Wx, el, er, smax, ssum, out, dout.contiguous(), ctx.slope)
-        da_jl = torch.zeros_like(a_jl)
-        if N:
-            with torch.cuda.device(Wx.device):
-                _lib.check(lib.gnnb_gat_logit_terms_bwd(Wx.data_ptr(), a_jl.data_ptr(), del_.data_ptr(), der.data_ptr(), N, Cc,
-                                                        H, dWx.data_ptr(), da_jl.data_ptr(), _stream(Wx.device)))
-        return dWx, da_jl.t(), None, None
-
-
-class _DistGATAggregateFn(torch.autograd.Function):
-    """_GATAggregateFn on shards, for the shapes whose logit halves torch computes (C < 4)"""
-
-    @staticmethod
-    def forward(ctx, Wx, el, er, dg: DistGraph, slope):
-        out, smax, ssum = dist_gat_aggregate(dg, Wx, el, er, slope)
-        ctx.dg, ctx.slope = dg, slope
-        ctx.save_for_backward(Wx, el, er, smax, ssum, out)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        Wx, el, er, smax, ssum, out = ctx.saved_tensors
-        dWx, del_, der = dist_gat_aggregate_bwd(ctx.dg, Wx, el, er, smax, ssum, out, dout.contiguous(), ctx.slope)
-        return dWx, del_, der, None, None
-
-
 def dist_gat_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
     """gat_conv (GNNlib/src/layers/conv.jl:112-150) on the rows this rank owns; x_local is Julia-shaped (Din, n_local).
     The graph must have been partitioned with add_self_loops = l.add_self_loops; no dropout, no edge features and a shape
     of the fused kernels (gat_fusable).  Weight gradients (dense_x, a, bias) are per-rank partial sums: all-reduce them."""
-    from .layers import _bias_act, _jl_reshape3, gat_fusable, gat_logit_fusable
+    from .layers import _attention_tail, _gat_edge_part, _jl_reshape3, gat_fusable
     _, chout = l.channel
     heads = l.heads
     if dg.self_loops != bool(l.add_self_loops):
@@ -742,21 +683,8 @@ def dist_gat_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
     if not gat_fusable(chout, heads):
         raise ValueError(f"dist_gat_conv: {chout} channels x {heads} heads is not a shape of the fused GAT kernels "
                          "(C/4 a power of two <= 32, or C a power of two <= 32 with C*H <= 128)")
-    Wr = rows(_jl_reshape3(l.dense_x(x_local), chout, heads))   # (n_local, H, C)
-    if Wr.data_ptr() % 16 != 0:
-        Wr = Wr.clone()
-    a, slope = l.a, float(l.negative_slope)
-    if gat_logit_fusable(chout, heads) and a.dtype == torch.float32:
-        out = unrows(_DistGATCoreFn.apply(Wr, a, dg, slope))
-    else:
-        el = (Wr * a[:chout, :].t().unsqueeze(0)).sum(-1)       # rows 1..C of a pair with the target
-        er = (Wr * a[chout:, :].t().unsqueeze(0)).sum(-1)       # rows C+1..2C with the source
-        out = unrows(_DistGATAggregateFn.apply(Wr, el.contiguous(), er.contiguous(), dg, slope))
-    if not l.concat:
-        out = out.mean(dim=1, keepdim=True)
-    r = rows(out)
-    out = unrows(r.reshape(r.shape[0], r.shape[1] * r.shape[2]))   # reshape(x, :, size(x, 3)), also for zero owned rows
-    return _bias_act(l, out)
+    Wx = _jl_reshape3(l.dense_x(x_local), chout, heads)         # (C, H, n_local)
+    return _attention_tail(l, _gat_edge_part(l, Wx, None, dg, dist_gat_aggregate, dist_gat_aggregate_bwd))
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -779,7 +707,7 @@ def dist_sage_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
     """sage_conv (GNNlib/src/layers/conv.jl:277-283) on the rows this rank owns, for aggr ∈ {mean, +}; x_local is
     Julia-shaped (Din, n_local).  The graph must have been partitioned without self loops (the layer adds none).  Weight
     gradients are per-rank partial sums: all-reduce them."""
-    from .layers import _Linear2Fn, _bias, _is_relu, _linear, _sigma, identity
+    from .layers import _sage_linear
     from .msgpass import _aggr_code
     aggr = _aggr_code(l.aggr)
     if aggr not in (_lib.SUM, _lib.MEAN):
@@ -787,14 +715,7 @@ def dist_sage_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
     if dg.self_loops:
         raise ValueError("dist_sage_conv: the graph was partitioned with add_self_loops=True; SAGEConv adds no self loops")
     r1 = rows(x_local).contiguous()
-    r2 = _DistSAGEPropagateFn.apply(r1, dg, aggr)
-    W = l.weight
-    sig, b = _sigma(l), _bias(l)
-    D1, D2, Dout = r1.shape[1], r2.shape[1], W.shape[0]
-    if (r1.dtype == torch.float32 and W.dtype == torch.float32 and Dout == 128 and D1 % 32 == 0 and D2 % 32 == 0
-            and D1 <= 128 and D2 <= 128 and (sig is identity or _is_relu(sig))):
-        return unrows(_Linear2Fn.apply(r1, r2, W, None if b is None else b.contiguous(), _is_relu(sig)))
-    return _linear(l, W, unrows(torch.cat([r1, r2], dim=1)), True)
+    return _sage_linear(l, r1, _DistSAGEPropagateFn.apply(r1, dg, aggr))
 
 
 # ---------------------------------------------------------------------------------------------------------
