@@ -111,6 +111,7 @@ _SIGS = {
     "gnnb_gat_aggregate_bwd_halo": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _f32p, _i64, _i64,
                                            C.c_float, _f32p, _f32p, _f32p, _vp]),
     "gnnb_gat_tnode": (_int, [_f32p, _f32p, _i64, _i64, _i64, _f32p, _vp]),
+    "gnnb_gcn_edge_weight_grad_halo": (_int, [_vp, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _i64, _f32p, _vp]),
     "gnnb_dev_alloc": (_int, [C.POINTER(_vp), _i64]),
     "gnnb_dev_free": (_int, [_vp]),
     "gnnb_ipc_get_handle": (_int, [_vp, _vp]),

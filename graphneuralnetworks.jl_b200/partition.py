@@ -15,7 +15,9 @@ edges keep their COO order, so a shard reproduces the single-GPU summation order
 
 Layers on shards: dist_gcn_conv, dist_sage_conv (mean, +) and dist_gat_conv.  GAT's pullback has one term that
 crosses ranks, del of a target = the sum of its in-edges' dz, computed by the owners of their sources: the dz rows move
-to the targets' owners by one all-to-all in an order both shards already share (DistGraph._edge_route).
+to the targets' owners by one all-to-all in an order both shards already share (DistGraph._edge_route).  Weighted
+GCNConv keeps each shard's edge weights (an ownership mask over the global order) and moves an explicit per-rank
+edge_weight to the backward shard over the same route reversed; its gradient is gnnb_gcn_edge_weight_grad_halo.
 
 `torch.distributed` is plumbing (process group, all_to_all_single); index construction below is plain torch
 ops that also run on CPU tensors with the gloo backend (tests/test_partition_gloo.py).
@@ -81,7 +83,7 @@ def degree_order(chunks, num_nodes: int, device) -> torch.Tensor:
     """nodes by decreasing in+out degree (stable: ties keep id order) — the order in which 'balanced' ownership deals
     them to the ranks; the torch restatement of gnnb_degree_accumulate + the sort of gnnb_balanced_relabel."""
     cost = torch.zeros(num_nodes, dtype=torch.int64, device=device)
-    for sc, tc in chunks:
+    for sc, tc, *_ in chunks:
         cost += torch.bincount(sc.to(device).to(torch.int64) - 1, minlength=num_nodes)
         cost += torch.bincount(tc.to(device).to(torch.int64) - 1, minlength=num_nodes)
     return torch.sort(cost, descending=True, stable=True).indices
@@ -177,11 +179,16 @@ class DistGraph:
     v % world) or 'balanced' (nodes sorted by decreasing degree and dealt to the ranks in turn: edges, nodes and served
     halo rows all balanced whatever the id space looks like — RMAT probabilities are products over id bits, so neither
     ranges nor v % world balance it; needs `chunks` to be iterable twice).  `local_nodes()` lists the owned node ids in
-    local-row order."""
+    local-row order.
 
-    def __init__(self, s: Optional[torch.Tensor], t: Optional[torch.Tensor], num_nodes: int, *, add_self_loops: bool = False,
-                 group=None, device=None, bounds: Optional[List[int]] = None, ownership: str = "contiguous",
-                 chunks=None, chunk_edges: int = 1 << 26):
+    Edge weights: `w` aligned with the global (s, t), or (s, t, w) chunks.  Each rank keeps the weights of its forward
+    shard's edges (`w_fwd`) and of its backward shard's (`w_bwd`), in shard COO order with weight 1 for every appended
+    self loop; both shards are stable compactions of the global order, so each is an ownership mask over the chunk
+    (`owned_by_target`), and no weight crosses ranks."""
+
+    def __init__(self, s: Optional[torch.Tensor], t: Optional[torch.Tensor], num_nodes: int, *, w=None,
+                 add_self_loops: bool = False, group=None, device=None, bounds: Optional[List[int]] = None,
+                 ownership: str = "contiguous", chunks=None, chunk_edges: int = 1 << 26):
         self.group = group
         self.world = dist.get_world_size(group)
         self.rank = dist.get_rank(group)
@@ -191,17 +198,27 @@ class DistGraph:
         self.ownership = ownership
         self.self_loops = add_self_loops
         self._c = None
+        self._cw = None
         self._sage_cs = None
+        self._weighted = None                                # decided by the first chunk unless `w` says it
         if chunks is None:
             s = s.to(self.device)
             t = t.to(self.device)
+            if w is not None:
+                w = torch.as_tensor(w, device=self.device).reshape(-1)
+                if w.numel() != s.numel():
+                    raise ValueError(f"DistGraph: {s.numel()} edges but {w.numel()} edge weights")
+                self._weighted = True
             if ownership == "contiguous" and bounds is None:
                 s0, t0 = s.to(torch.int64) - 1, t.to(torch.int64) - 1
                 cost = (torch.bincount(t0, minlength=num_nodes) + torch.bincount(s0, minlength=num_nodes) + NODE_COST)
                 bounds = balanced_bounds(cost, self.world)
                 del s0, t0, cost
             E = int(s.numel())
-            chunks = [(s[i:i + chunk_edges], t[i:i + chunk_edges]) for i in range(0, max(E, 1), chunk_edges)] if E else []
+            chunks = [(s[i:i + chunk_edges], t[i:i + chunk_edges]) + (() if w is None else (w[i:i + chunk_edges],))
+                      for i in range(0, max(E, 1), chunk_edges)] if E else []
+        elif w is not None:
+            raise ValueError("DistGraph: with `chunks`, pass the weights as (s, t, w) chunks")
         self._order = self._relabel = None
         if ownership == "balanced":
             if not isinstance(chunks, (list, tuple)) and not callable(chunks):
@@ -214,7 +231,7 @@ class DistGraph:
                 self._relabel = torch.empty(N, dtype=torch.int32, device=self.device)
                 order = torch.empty(N, dtype=torch.int32, device=self.device)
                 with torch.cuda.device(self.device):
-                    for sc, tc in it:
+                    for sc, tc, *_ in it:
                         sc, tc = sc.to(self.device).contiguous(), tc.to(self.device).contiguous()
                         _lib.check(lib.gnnb_degree_accumulate(sc.data_ptr(), tc.data_ptr(), sc.numel(), sc.element_size(), 1, N,
                                                               cost.data_ptr(), _stream(self.device)))
@@ -246,10 +263,49 @@ class DistGraph:
             torch.cuda.synchronize(self.device)
         else:
             self.fwd, self.bwd = self._build_torch(chunks)
+        # the edges of the global list whose target this rank owns: the forward shard without its self loops
+        self.num_owned_edges = self.fwd.num_edges - (self.n_local if self.self_loops else 0)
 
     @classmethod
     def from_chunks(cls, chunks, num_nodes: int, **kw):
+        """chunks: (s, t) or, with edge weights, (s, t, w) tuples — every chunk the one or every chunk the other"""
         return cls(None, None, num_nodes, chunks=chunks, **kw)
+
+    # -- ownership of edges, and the weights each shard keeps
+    def _owned(self, v: torch.Tensor) -> torch.Tensor:
+        """True where this rank owns node v (1-based global ids): the builder's rule (to_pid with the relabel table)"""
+        pid = to_pid(v.to(self.device).to(torch.int64) - 1, self.world, self.first, self.ownership, self._relabel)
+        return (pid >= self.lo) & (pid < self.hi)
+
+    def owned_by_target(self, t: torch.Tensor) -> torch.Tensor:
+        """Mask over the edges of a global list or chunk (1-based targets t): True for the edges whose target this rank
+        owns, i.e. its forward shard's edges in their shard order.  `edge_weight[dg.owned_by_target(t)]` is the per-rank
+        `edge_weight` of dist_gcn_conv, and the same mask places its gradient back in the global list."""
+        return self._owned(t)
+
+    def _chunk_weights(self, sc: torch.Tensor, wc) -> Optional[torch.Tensor]:
+        """the float32 weights of one (s, t[, w]) chunk on the device, or None; every chunk must agree on having them"""
+        w = wc[0] if wc else None
+        if self._weighted is None:
+            self._weighted = w is not None
+        if (w is not None) != self._weighted:
+            raise ValueError("DistGraph: either every chunk carries edge weights or none does")
+        if w is None:
+            return None
+        w = torch.as_tensor(w, device=self.device).reshape(-1)
+        if w.numel() != sc.numel():
+            raise ValueError(f"DistGraph: a chunk of {sc.numel()} edges carries {w.numel()} edge weights")
+        return w.to(torch.float32)
+
+    def _keep_weights(self, wf: List[torch.Tensor], wb: List[torch.Tensor]) -> None:
+        """w_fwd / w_bwd from the masked chunk weights, weight 1 appended for every self loop (gcn_conv's rule)"""
+        self.w_fwd = self.w_bwd = None
+        if not self._weighted:
+            return
+        loops = [torch.ones(self.n_local, dtype=torch.float32, device=self.device)] if self.self_loops else []
+        empty = [torch.zeros(0, dtype=torch.float32, device=self.device)]
+        self.w_fwd = torch.cat(empty + wf + loops).contiguous()
+        self.w_bwd = torch.cat(empty + wb + loops).contiguous()
 
     @classmethod
     def from_rmat(cls, num_nodes: int, num_edges: int, seed: int = 17, *, device, chunk_edges: int = 1 << 26, **kw):
@@ -269,7 +325,7 @@ class DistGraph:
         dev, world = self.device, self.world
         b = C.c_void_p()
         bounds_arr = (C.c_int64 * (world + 1))(*self.first) if self.ownership == "contiguous" else None
-        shards = []
+        shards, wf, wb = [], [], []
         t_sh = time.perf_counter()
         with torch.cuda.device(dev):
             st = _stream(dev)
@@ -277,10 +333,14 @@ class DistGraph:
                                                      0 if self.ownership == "contiguous" else 1, bounds_arr,
                                                      None if self._relabel is None else self._relabel.data_ptr()))
             try:
-                for sc, tc in chunks:
+                for sc, tc, *wc in chunks:
                     sc, tc = sc.to(dev).contiguous(), tc.to(dev).contiguous()
                     assert sc.dtype == tc.dtype and sc.dtype in (torch.int32, torch.int64)
+                    w = self._chunk_weights(sc, wc)
                     _lib.check(lib.gnnb_shard_builder_add(b, sc.data_ptr(), tc.data_ptr(), sc.numel(), sc.element_size(), 1, st))
+                    if w is not None:                        # the builder keeps each shard's edges stably: same masks
+                        wf.append(w[self._owned(tc)])
+                        wb.append(w[self._owned(sc)])
                 for direction in (0, 1):
                     h = C.c_void_p()
                     nl, nh, ne = C.c_int64(), C.c_int64(), C.c_int64()
@@ -292,6 +352,7 @@ class DistGraph:
                     shards.append((h, nl.value, nh.value, ne.value, list(rc), halo_local))
             finally:
                 lib.gnnb_shard_builder_destroy(b)
+        self._keep_weights(wf, wb)
         torch.cuda.synchronize(dev)
         self.timing["shards_ms"] = (time.perf_counter() - t_sh) * 1e3
         t_ex = time.perf_counter()
@@ -320,6 +381,12 @@ class DistGraph:
         t0 = torch.cat([c[1] for c in chunks]).to(self.device).to(torch.int64) - 1 if chunks else torch.zeros(0, dtype=torch.int64)
         ps = to_pid(s0, self.world, self.first, self.ownership, self._relabel)
         pt = to_pid(t0, self.world, self.first, self.ownership, self._relabel)
+        ws = [self._chunk_weights(c[0], c[2:]) for c in chunks]
+        if self._weighted:
+            w = torch.cat([torch.zeros(0, dtype=torch.float32, device=self.device)] + ws)
+            self._keep_weights([w[self._owned(t0 + 1)]], [w[self._owned(s0 + 1)]])
+        else:
+            self._keep_weights([], [])
         out = []
         for key0, other0 in ((pt, ps), (ps, pt)):
             d = build_shard(key0, other0, self.lo, self.hi, self.first, self.self_loops)
@@ -506,37 +573,51 @@ class DistGraph:
             if not torch.equal(peer_counts, recv_counts):
                 raise RuntimeError(f"rank {self.rank}: the edge exchange does not pair up: the peers' backward shards send "
                                    f"{peer_counts.tolist()} edge rows, the forward shard expects {recv_counts.tolist()}")
+            unpack_b = torch.empty_like(send_perm)                 # the reverse route: backward-shard position of
+            unpack_b[send_perm] = torch.arange(send_perm.numel(), device=dev)   # every row received from a target's owner
             self.fwd.edge_route = {"send_idx": send_perm.to(torch.int32), "unpack_idx": unpack.to(torch.int32),
                                    "send_counts": send_counts.tolist(), "recv_counts": recv_counts.tolist(),
                                    # one rank: pack, exchange and unpack compose into one gather
-                                   "direct_idx": send_perm[unpack].to(torch.int32) if W == 1 else None}
+                                   "direct_idx": send_perm[unpack].to(torch.int32) if W == 1 else None,
+                                   "rev_send_idx": recv_perm.to(torch.int32), "rev_unpack_idx": unpack_b.to(torch.int32),
+                                   "rev_direct_idx": recv_perm[unpack_b].to(torch.int32) if W == 1 else None}
         return self.fwd.edge_route
 
     def edge_exchange(self, v_bwd: torch.Tensor) -> torch.Tensor:
         """(E_bwd, H) values in backward-shard COO order -> (E_fwd, H) in forward-shard COO order, every edge's row moved
         to the rank that owns its target: one pack, one all-to-all, one unpack"""
         r = self._edge_route()
-        H, dev = v_bwd.shape[1], self.device
-        v_bwd = v_bwd.contiguous()
-        n_send, n_recv = int(r["send_idx"].numel()), int(r["unpack_idx"].numel())
-        if r["direct_idx"] is not None:
-            out = torch.empty((n_recv, H), dtype=v_bwd.dtype, device=dev)
+        return self._move_edge_rows(v_bwd, r["send_idx"], r["send_counts"], r["recv_counts"], r["unpack_idx"], r["direct_idx"])
+
+    def edge_exchange_reverse(self, v_fwd: torch.Tensor) -> torch.Tensor:
+        """(E_fwd, H) values in forward-shard COO order -> (E_bwd, H) in backward-shard COO order, every edge's row moved
+        to the rank that owns its source: edge_exchange run backwards over the same route"""
+        r = self._edge_route()
+        return self._move_edge_rows(v_fwd, r["rev_send_idx"], r["recv_counts"], r["send_counts"], r["rev_unpack_idx"],
+                                    r["rev_direct_idx"])
+
+    def _move_edge_rows(self, v, send_idx, send_counts, recv_counts, unpack_idx, direct_idx) -> torch.Tensor:
+        H, dev = v.shape[1], self.device
+        v = v.contiguous()
+        n_send, n_recv = int(send_idx.numel()), int(unpack_idx.numel())
+        if direct_idx is not None:
+            out = torch.empty((n_recv, H), dtype=v.dtype, device=dev)
             if n_recv:
                 with torch.cuda.device(dev):
-                    _lib.check(lib.gnnb_gather_rows(r["direct_idx"].data_ptr(), n_recv, v_bwd.data_ptr(), H, out.data_ptr(),
+                    _lib.check(lib.gnnb_gather_rows(direct_idx.data_ptr(), n_recv, v.data_ptr(), H, out.data_ptr(),
                                                     _stream(dev)))
             return out
-        send = torch.empty((n_send, H), dtype=v_bwd.dtype, device=dev)
-        recv = torch.empty((n_recv, H), dtype=v_bwd.dtype, device=dev)
-        out = torch.empty((n_recv, H), dtype=v_bwd.dtype, device=dev)
+        send = torch.empty((n_send, H), dtype=v.dtype, device=dev)
+        recv = torch.empty((n_recv, H), dtype=v.dtype, device=dev)
+        out = torch.empty((n_recv, H), dtype=v.dtype, device=dev)
         with torch.cuda.device(dev):
             if n_send:
-                _lib.check(lib.gnnb_gather_rows(r["send_idx"].data_ptr(), n_send, v_bwd.data_ptr(), H, send.data_ptr(),
+                _lib.check(lib.gnnb_gather_rows(send_idx.data_ptr(), n_send, v.data_ptr(), H, send.data_ptr(),
                                                 _stream(dev)))
-            dist.all_to_all_single(recv, send, output_split_sizes=r["recv_counts"], input_split_sizes=r["send_counts"],
+            dist.all_to_all_single(recv, send, output_split_sizes=recv_counts, input_split_sizes=send_counts,
                                    group=self.group)
             if n_recv:
-                _lib.check(lib.gnnb_gather_rows(r["unpack_idx"].data_ptr(), n_recv, recv.data_ptr(), H, out.data_ptr(),
+                _lib.check(lib.gnnb_gather_rows(unpack_idx.data_ptr(), n_recv, recv.data_ptr(), H, out.data_ptr(),
                                                 _stream(dev)))
         return out
 
@@ -565,18 +646,39 @@ class DistGraph:
             self._c = (c, cf.contiguous(), cb.contiguous())
         return self._c
 
-    def propagate(self, shard: _Shard, x_rows: torch.Tensor, cs, ct, aggr=_lib.SUM) -> torch.Tensor:
+    def gcn_scales(self, w_fwd: torch.Tensor):
+        """(d, c, cf, cb) of the weighted normalisation: d = weighted in-degree of the owned nodes from the forward shard's
+        weights `w_fwd` (gnnb_degree, local), c = 1/sqrt(d) as gcn_conv's default norm_fn, and c's halo copies on both
+        shards"""
+        from .layers import default_norm_fn
+        d = torch.empty(self.n_local, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            if self.n_local:
+                _lib.check(lib.gnnb_degree(self.fwd.plan.h, _lib.DIR_IN, _ptr(w_fwd), _ptr(d), _stream(self.device)))
+        c = default_norm_fn(d)
+        cf = torch.cat([c, self.halo(self.fwd, c.reshape(-1, 1)).reshape(-1)])
+        cb = torch.cat([c, self.halo(self.bwd, c.reshape(-1, 1)).reshape(-1)])
+        return d, c, cf.contiguous(), cb.contiguous()
+
+    def gcn_c_weighted(self):
+        """gcn_scales of the graph's own weights (w_fwd), computed once"""
+        if self._cw is None:
+            self._cw = self.gcn_scales(self.w_fwd)
+        return self._cw
+
+    def propagate(self, shard: _Shard, x_rows: torch.Tensor, cs, ct, aggr=_lib.SUM, w=None) -> torch.Tensor:
+        """one pass over `shard`: copy_xj, or w_mul_xj with the shard's edge weights `w` (COO order)"""
         slices = int(os.environ.get("GNNB_HALO_SLICES", "1"))
         if slices > 1 and x_rows.shape[1] % slices == 0 and not getattr(self, "_slicing", False):
             # column-sliced pass: exchange and reduce `D / slices` feature columns at a time, so that the halo buffers
             # shrink by `slices` (config 5: 62 GB of halo rows per pass at D = 256 do not fit beside the features);
             # costs two strided copies of the local rows and re-reads the index arrays once per slice
-            w = x_rows.shape[1] // slices
+            k = x_rows.shape[1] // slices
             out = torch.empty_like(x_rows)
             self._slicing = True
             try:
                 for i in range(slices):
-                    out[:, i * w:(i + 1) * w] = self.propagate(shard, x_rows[:, i * w:(i + 1) * w].contiguous(), cs, ct, aggr)
+                    out[:, i * k:(i + 1) * k] = self.propagate(shard, x_rows[:, i * k:(i + 1) * k].contiguous(), cs, ct, aggr, w)
             finally:
                 self._slicing = False
             return out
@@ -584,8 +686,8 @@ class DistGraph:
         hptr, recv = self.halo_ptr(shard, x_rows)
         out = torch.empty_like(x_rows)
         with torch.cuda.device(self.device):
-            _lib.check(lib.gnnb_propagate_halo(shard.plan.h, _lib.COPY_XJ, aggr, x_rows.data_ptr(),
-                                               hptr if shard.n_halo else None, shard.n_local, None,
+            _lib.check(lib.gnnb_propagate_halo(shard.plan.h, _lib.COPY_XJ if w is None else _lib.W_MUL_XJ, aggr,
+                                               x_rows.data_ptr(), hptr if shard.n_halo else None, shard.n_local, _ptr(w),
                                                _ptr(cs), _ptr(ct), D, out.data_ptr(), _stream(self.device)))
         del recv                                                # the kernel that reads it is enqueued
         return out
@@ -605,13 +707,80 @@ class _DistGCNPropagateFn(torch.autograd.Function):
         return dg.propagate(dg.bwd, dout.contiguous(), cb, c), None
 
 
-def dist_gcn_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
+class _DistGCNWeightedFn(torch.autograd.Function):
+    """y = c .* propagate(w_mul_xj, c .* h) on the forward shard, c = 1/sqrt(weighted in-degree), for the graph's weights
+    (w None) or an explicit per-rank edge_weight (w: one value per original forward-shard edge).
+
+    Pullback for h: the same pass on the backward shard with w_bwd (the graph's, or w moved there by
+    edge_exchange_reverse).  Pullback for w, when it requires grad: the forward keeps the unscaled sums u (y = u .* c)
+    and the backward the unscaled pullback sums dhs (dh = dhs .* c), as the single-GPU composition does; then
+        dc = <dy, u> + <dhs, h>  per owned node (its target and its source role),  dd = dc through c = 1/sqrt(d),
+        dw_e = <c_t dy_t, c_s h_s> + dd_t                                  (gnnb_gcn_edge_weight_grad_halo)
+    over the forward shard, whose halo rows of h are exchanged again here rather than kept from the forward."""
+
+    @staticmethod
+    def forward(ctx, h_rows, w, dg: DistGraph):
+        h_rows = h_rows.contiguous()
+        if w is None:
+            w_f = dg.w_fwd
+            d, c, cf, cb = dg.gcn_c_weighted()
+        else:
+            w_f = w.to(dg.device, torch.float32).contiguous()
+            if dg.self_loops:                                   # weight 1 for every appended loop (gcn_conv's rule)
+                w_f = torch.cat([w_f, torch.ones(dg.n_local, dtype=torch.float32, device=dg.device)])
+            d, c, cf, cb = dg.gcn_scales(w_f)
+        ctx.dg, ctx.explicit, ctx.w_f, ctx.c, ctx.cb = dg, w is not None, w_f, c, cb
+        ctx.want_w = w is not None and ctx.needs_input_grad[1]
+        u = dg.propagate(dg.fwd, h_rows, cf, None, w=w_f)      # c_t applied outside, as gcn_conv: 0 * Inf = NaN for a
+        if ctx.want_w:                                          # target without in-edges and d = 0
+            ctx.h, ctx.u, ctx.d, ctx.cf = h_rows, u, d, cf
+        return u * c[:, None]
+
+    @staticmethod
+    def backward(ctx, dy):
+        dg, c, cb = ctx.dg, ctx.c, ctx.cb
+        dy = dy.contiguous()
+        w_b = dg.edge_exchange_reverse(ctx.w_f.reshape(-1, 1)).reshape(-1) if ctx.explicit else dg.w_bwd
+        dhs = dg.propagate(dg.bwd, dy, cb, None, w=w_b)
+        if not ctx.want_w:
+            return dhs * c[:, None], None, None
+        from .layers import default_norm_fn
+        h, D = ctx.h, ctx.h.shape[1]
+        dc = (dy * ctx.u).sum(1) + (dhs * h).sum(1)
+        with torch.enable_grad():
+            d = ctx.d.detach().requires_grad_(True)
+            dd, = torch.autograd.grad(default_norm_fn(d), d, dc)
+        h_halo = dg.halo_rows(dg.fwd, h, "x")
+        dw = torch.empty(dg.fwd.num_edges, dtype=torch.float32, device=dg.device)
+        with torch.cuda.device(dg.device):
+            _lib.check(lib.gnnb_gcn_edge_weight_grad_halo(dg.fwd.plan.h, _ptr(dy), _ptr(h), _ptr(h_halo) if dg.fwd.n_halo else None,
+                                                          dg.n_local, _ptr(ctx.cf), _ptr(c), _ptr(dd.contiguous()), D, _ptr(dw),
+                                                          _stream(dg.device)))
+        del h_halo                                              # the kernel that reads it is enqueued
+        return dhs * c[:, None], dw[:dg.num_owned_edges], None  # the loops' weights are constants
+
+
+def dist_gcn_conv(l, dg: DistGraph, x_local: torch.Tensor, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """gcn_conv (GNNlib/src/layers/conv.jl:14-72) on the rows this rank owns; x_local is Julia-shaped (Din, n_local).
     The graph must have been partitioned with add_self_loops = l.add_self_loops.  Weight gradients are per-rank
-    partial sums: all-reduce them like any data-parallel layer."""
+    partial sums: all-reduce them like any data-parallel layer.
+
+    Edge weights follow the reference's rule: an explicit `edge_weight` is used (l.use_edge_weight is then ignored);
+    otherwise the graph's weights when l.use_edge_weight is true and `dg` has them; otherwise the unweighted
+    normalisation.  `edge_weight` is this rank's: one value per edge whose target it owns, in global order
+    (`w[dg.owned_by_target(t)]` of a global list), and may require grad; its gradient comes back in the same order."""
     assert dg.self_loops == bool(l.add_self_loops)
     from .layers import _gcn_dense
-    return _gcn_dense(l, l.weight, x_local, lambda h: unrows(_DistGCNPropagateFn.apply(rows(h), dg)))
+    if edge_weight is not None:
+        if edge_weight.numel() != dg.num_owned_edges:
+            raise ValueError(f"Wrong number of edge weights (expected {dg.num_owned_edges}, the edges whose target rank "
+                             f"{dg.rank} owns, but given {edge_weight.numel()})")
+        w = edge_weight.reshape(-1)
+    elif getattr(l, "use_edge_weight", False) and dg.w_fwd is not None:
+        w = None
+    else:
+        return _gcn_dense(l, l.weight, x_local, lambda h: unrows(_DistGCNPropagateFn.apply(rows(h), dg)))
+    return _gcn_dense(l, l.weight, x_local, lambda h: unrows(_DistGCNWeightedFn.apply(rows(h), w, dg)))
 
 
 # ---------------------------------------------------------------------------------------------------------

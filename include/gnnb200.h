@@ -342,6 +342,17 @@ int gnnb_gat_aggregate_bwd_halo(gnnb_graph_t g, const float* Wx_own, const float
                                 const float* seg_sum, const float* T, int64_t C, int64_t H, float slope, float* dWx,
                                 float* der, float* dz, void* stream);
 int gnnb_gat_tnode(const float* dout, const float* out_fwd, int64_t n, int64_t C, int64_t H, float* T, void* stream);
+/* gnnb_gcn_edge_weight_grad_halo: the edge-weight gradient of the weighted GCN propagate y_t = ct[t] Σ_{e: s→t} w_e cs[s]
+ * h_s on the forward CSR of a (shard) plan:
+ *     dw[e] = Σ_f (dout[t,f] * ct[t]) * (h[s,f] * cs[s]) + dd[t]        for every edge e = (s → t), COO order,
+ * each product rounded as written (an infinite scale gives the IEEE results of the scaled rows).  dout (num_dst, D);
+ * gathered sources < n_local read h_local, the others h_halo + (id - n_local)*D; cs (num_src, [local | halo] order), ct
+ * and dd (num_dst) are optional (NULL: 1, 1, 0).  dd is the caller's degree term -½ d^{-3/2} dc of c = d^{-1/2}.  One warp
+ * per work item of the plan, every value written once without atomics (deterministic).  h_halo NULL with n_local =
+ * num_src is the one-base pass over an ordinary plan.  A plan without edges accepts NULL pointers. */
+int gnnb_gcn_edge_weight_grad_halo(gnnb_graph_t g, const float* dout, const float* h_local, const float* h_halo,
+                                   int64_t n_local, const float* cs, const float* ct, const float* dd, int64_t D,
+                                   float* dw, void* stream);
 
 /* Building one rank's shards on its GPU from chunks of the global edge list (csrc/shard.cu).
  *   ownership mode 0: contiguous ranges, bounds_host[q] <= v < bounds_host[q+1] (world + 1 entries; NULL = equal ranges);
