@@ -47,11 +47,13 @@ __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_fwd_kernel(const f
     }
 }
 
-// persistent: warp w of the grid owns nodes w, w + W, ...; per-lane da partials stay in registers across its nodes
+// persistent: warp w of the grid owns nodes w, w + W, ...; per-lane da partials stay in registers across its nodes.
+// One slice of H heads: Wx, a, del, der and dWx point at the slice's first head, ldh is the heads per node of the whole
+// arrays (row strides ldh * C and ldh), partial holds the slice's [h][2C] block.
 template <int G, int PASSES>
 __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_bwd_kernel(const float* __restrict__ Wx, const float* __restrict__ a,
                                                                          const float* __restrict__ del, const float* __restrict__ der,
-                                                                         int64_t N, int C, int H, float* __restrict__ dWx,
+                                                                         int64_t N, int C, int H, int ldh, float* __restrict__ dWx,
                                                                          float* __restrict__ partial) {
     constexpr int HPP = 32 / G;
     extern __shared__ float sm[];              // [LOGIT_WARPS][2 * H * C]
@@ -71,13 +73,13 @@ __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_bwd_kernel(const f
         }
     }
     for (int64_t n = (int64_t)blockIdx.x * LOGIT_WARPS + warp; n < N; n += W) {
-        const float* row = Wx + n * (int64_t)H * C;
-        float* drow = dWx + n * (int64_t)H * C;
+        const float* row = Wx + n * (int64_t)ldh * C;
+        float* drow = dWx + n * (int64_t)ldh * C;
 #pragma unroll
         for (int p = 0; p < PASSES; ++p) {
             const int h = p * HPP + sub;
             if (h < H) {
-                const float dl = __ldg(del + n * H + h), dr = __ldg(der + n * H + h);
+                const float dl = __ldg(del + n * ldh + h), dr = __ldg(der + n * ldh + h);
                 const float4 w = __ldg(reinterpret_cast<const float4*>(row + h * C + c4));
                 float4 d = *reinterpret_cast<const float4*>(drow + h * C + c4);
                 d.x += dl * ai[p].x + dr * aj[p].x; d.y += dl * ai[p].y + dr * aj[p].y;
@@ -132,11 +134,12 @@ __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_half_fwd_kernel(co
     }
 }
 
-// pullback of one half: dWx[c,h,n] += d[h,n] a[off+c,h]; the da partial holds sum_n d Wx in its half and 0 in the other
+// pullback of one half: dWx[c,h,n] += d[h,n] a[off+c,h]; the da partial holds sum_n d Wx in its half and 0 in the other.
+// One slice of H heads with row stride ldh, as gat_logit_bwd_kernel.
 template <int G, int PASSES>
 __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_half_bwd_kernel(const float* __restrict__ Wx, const float* __restrict__ a,
-                                                                              const float* __restrict__ dh, int64_t N, int C, int H, int off,
-                                                                              float* __restrict__ dWx, float* __restrict__ partial) {
+                                                                              const float* __restrict__ dh, int64_t N, int C, int H, int ldh,
+                                                                              int off, float* __restrict__ dWx, float* __restrict__ partial) {
     constexpr int HPP = 32 / G;
     extern __shared__ float sm[];              // [LOGIT_WARPS][2 * H * C]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -151,13 +154,13 @@ __global__ void __launch_bounds__(LOGIT_WARPS * 32) gat_logit_half_bwd_kernel(co
         if (h < H) ah[p] = __ldg(reinterpret_cast<const float4*>(a + (int64_t)h * 2 * C + off + c4));
     }
     for (int64_t n = (int64_t)blockIdx.x * LOGIT_WARPS + warp; n < N; n += W) {
-        const float* row = Wx + n * (int64_t)H * C;
-        float* drow = dWx + n * (int64_t)H * C;
+        const float* row = Wx + n * (int64_t)ldh * C;
+        float* drow = dWx + n * (int64_t)ldh * C;
 #pragma unroll
         for (int p = 0; p < PASSES; ++p) {
             const int h = p * HPP + sub;
             if (h < H) {
-                const float d = __ldg(dh + n * H + h);
+                const float d = __ldg(dh + n * ldh + h);
                 const float4 w = __ldg(reinterpret_cast<const float4*>(row + h * C + c4));
                 float4 v = *reinterpret_cast<const float4*>(drow + h * C + c4);
                 v.x += d * ah[p].x; v.y += d * ah[p].y; v.z += d * ah[p].z; v.w += d * ah[p].w;
@@ -238,54 +241,61 @@ int gnnb_gat_logit_terms_bwd(const float* Wx, const float* a, const float* del, 
     if (N < 0 || C <= 0 || H <= 0) GNNB_FAIL(GNNB_ESIZE, "bad sizes");
     if (!da) GNNB_FAIL(GNNB_EINVAL, "da is NULL");
     cudaStream_t st = (cudaStream_t)stream;
-    const int A = (int)(2 * H * C);
-    if (N == 0) { GNNB_CUDA(cudaMemsetAsync(da, 0, sizeof(float) * (size_t)A, st)); return GNNB_OK; }
+    if (N == 0) { GNNB_CUDA(cudaMemsetAsync(da, 0, sizeof(float) * (size_t)(2 * H * C), st)); return GNNB_OK; }
     if (!Wx || !a || (!del && !der) || !dWx_accum) GNNB_FAIL(GNNB_EINVAL, "NULL argument");
     int G = 0;
     if (!logit_shape(C, H, &G) || ((uintptr_t)Wx & 15) || ((uintptr_t)a & 15) || ((uintptr_t)dWx_accum & 15))
         GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms_bwd: C/4 must be a power of two <= 32, C*H <= 4096, 16 B-aligned operands");
+    // heads in slices of 8 passes of 32/G heads (C * heads <= 1024 per slice): a slice's block stage needs at most
+    // 8 warps x 2 x 1024 floats = 64 KB of shared memory.  nblocks depends on N alone, so each head's da is summed in the
+    // same order whatever H and the slice; the slices run in order on one stream and reuse one partial buffer.
     const int hpp = 32 / G;
-    const int passes = (int)ceil_div(H, hpp);
-    if (passes > 8) GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms_bwd: more than 8 passes of heads per warp");
-    const size_t smem = sizeof(float) * (size_t)LOGIT_WARPS * A;
-    if (smem > 200 * 1024) GNNB_FAIL(GNNB_EUNSUPPORTED, "gat_logit_terms_bwd: 2*H*C too large for the block stage");
-    int64_t want = ceil_div(N, LOGIT_WARPS);
+    const int64_t slice = 8 * hpp;
+    const int64_t want = ceil_div(N, LOGIT_WARPS);
     const int nblocks = (int)(want < kNumSMs * 4 ? want : kNumSMs * 4);
     DeviceState* s = nullptr;
     GNNB_TRY(device_state(&s));
-    GNNB_TRY(grow_buffer(&s->gat_part, &s->gat_part_bytes, sizeof(float) * (size_t)nblocks * A));
+    GNNB_TRY(grow_buffer(&s->gat_part, &s->gat_part_bytes, sizeof(float) * (size_t)nblocks * 2 * (H < slice ? H : slice) * C));
     float* part_buf = s->gat_part;
-    if (!del || !der) {                        // one half: del (target half of da) or der (source half)
-        const float* dh = del ? del : der;
-        const int off = del ? 0 : (int)C;
+    const int ldh = (int)H;
+    for (int64_t h0 = 0; h0 < H; h0 += slice) {
+        const int hs = (int)(H - h0 < slice ? H - h0 : slice);
+        const int passes = (int)ceil_div(hs, hpp);
+        const int A = 2 * hs * (int)C;
+        const size_t smem = sizeof(float) * (size_t)LOGIT_WARPS * A;
+        const float* Wxs = Wx + h0 * C;
+        const float* as = a + h0 * 2 * C;
+        float* dWxs = dWx_accum + h0 * C;
+        if (!del || !der) {                    // one half: del (target half of da) or der (source half)
+            const float* dh = (del ? del : der) + h0;
+            const int off = del ? 0 : (int)C;
 #define GNNB_LHB(GG, PP) { auto k = gat_logit_half_bwd_kernel<GG, PP>; \
-        if (smem > 48 * 1024) GNNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k<<<nblocks, LOGIT_WARPS * 32, smem, st>>>(Wx, a, dh, N, (int)C, (int)H, off, dWx_accum, part_buf); }
+            if (smem > 48 * 1024) GNNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            k<<<nblocks, LOGIT_WARPS * 32, smem, st>>>(Wxs, as, dh, N, (int)C, hs, ldh, off, dWxs, part_buf); }
 #define GNNB_LHBP(GG) switch (passes) { case 1: GNNB_LHB(GG, 1) break; case 2: GNNB_LHB(GG, 2) break; case 3: case 4: GNNB_LHB(GG, 4) break; default: GNNB_LHB(GG, 8) break; }
-        switch (G) {
-            case 1: GNNB_LHBP(1) break; case 2: GNNB_LHBP(2) break; case 4: GNNB_LHBP(4) break;
-            case 8: GNNB_LHBP(8) break; case 16: GNNB_LHBP(16) break; default: GNNB_LHBP(32) break;
-        }
+            switch (G) {
+                case 1: GNNB_LHBP(1) break; case 2: GNNB_LHBP(2) break; case 4: GNNB_LHBP(4) break;
+                case 8: GNNB_LHBP(8) break; case 16: GNNB_LHBP(16) break; default: GNNB_LHBP(32) break;
+            }
 #undef GNNB_LHBP
 #undef GNNB_LHB
-        GNNB_LAUNCHED();
-        gat_logit_final_kernel<<<(unsigned)ceil_div((int64_t)A, 128), 128, 0, st>>>(part_buf, nblocks, A, da);
-        GNNB_LAUNCHED();
-        return GNNB_OK;
-    }
+        } else {
+            const float *dl = del + h0, *dr = der + h0;
 #define GNNB_LB(GG, PP) { auto k = gat_logit_bwd_kernel<GG, PP>; \
-        if (smem > 48 * 1024) GNNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k<<<nblocks, LOGIT_WARPS * 32, smem, st>>>(Wx, a, del, der, N, (int)C, (int)H, dWx_accum, part_buf); }
+            if (smem > 48 * 1024) GNNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            k<<<nblocks, LOGIT_WARPS * 32, smem, st>>>(Wxs, as, dl, dr, N, (int)C, hs, ldh, dWxs, part_buf); }
 #define GNNB_LBP(GG) switch (passes) { case 1: GNNB_LB(GG, 1) break; case 2: GNNB_LB(GG, 2) break; case 3: case 4: GNNB_LB(GG, 4) break; default: GNNB_LB(GG, 8) break; }
-    switch (G) {
-        case 1: GNNB_LBP(1) break; case 2: GNNB_LBP(2) break; case 4: GNNB_LBP(4) break;
-        case 8: GNNB_LBP(8) break; case 16: GNNB_LBP(16) break; default: GNNB_LBP(32) break;
-    }
+            switch (G) {
+                case 1: GNNB_LBP(1) break; case 2: GNNB_LBP(2) break; case 4: GNNB_LBP(4) break;
+                case 8: GNNB_LBP(8) break; case 16: GNNB_LBP(16) break; default: GNNB_LBP(32) break;
+            }
 #undef GNNB_LBP
 #undef GNNB_LB
-    GNNB_LAUNCHED();
-    gat_logit_final_kernel<<<(unsigned)ceil_div((int64_t)A, 128), 128, 0, st>>>(part_buf, nblocks, A, da);
-    GNNB_LAUNCHED();
+        }
+        GNNB_LAUNCHED();
+        gat_logit_final_kernel<<<(unsigned)ceil_div((int64_t)A, 128), 128, 0, st>>>(part_buf, nblocks, A, da + h0 * 2 * C);
+        GNNB_LAUNCHED();
+    }
     return GNNB_OK;
 }
 

@@ -471,7 +471,7 @@ def _aligned_rows(W: torch.Tensor, device) -> torch.Tensor:
 def gat_logit_fusable(chout: int, heads: int) -> bool:
     """shapes csrc/gatlogit.cu covers: C/4 a power of two <= 32, C*H <= 4096 (config 3: 64 x 8)"""
     g = chout // 4
-    return chout % 4 == 0 and g > 0 and (g & (g - 1)) == 0 and g <= 32 and chout * heads <= 4096 and (heads * 4 + chout // 4 - 1) // (chout // 4) <= 64
+    return chout % 4 == 0 and g > 0 and (g & (g - 1)) == 0 and g <= 32 and chout * heads <= 4096
 
 
 def gat_fusable(chout: int, heads: int) -> bool:

@@ -8,8 +8,9 @@ Checked per rank against the one-GPU library on the same graph and against float
   normwise against float64 elsewhere; everything bit for bit at W = 1 in node order (balanced ownership reorders the
   rows, and with them the chunks of the long ones);
 - the dz exchange: every edge value, tagged with the edge's global (source, target), lands on the same edge;
-- dist_gat_conv (concat true and false, a lean shape and C = 1) and dist_sage_conv (mean, +): y, dx and the all-reduced
-  weight gradients against float64 autograd of the dense formula;
+- dist_gat_conv (concat true and false, a lean shape, C = 1 and 128 x 16, whose logit pullback runs in two slices of
+  heads) and dist_sage_conv (mean, +): y, dx and the all-reduced weight gradients against float64 autograd of the dense
+  formula;
 - three steps on one DistGraph equal fresh one-step runs bit for bit;
 - the argument errors."""
 import datetime
@@ -223,7 +224,7 @@ def check_layers(R, tag, dg, full, loops):
     n = N_NODES
     ids = dg.local_nodes()
     R.set_route()
-    for Cc, H in ((32, 4), (1, 8)):
+    for Cc, H in ((32, 4), (1, 8), (128, 16)):           # (128, 16): the logit pullback in two slices of heads
         for concat in (True, False):
             layer = gat_layer(R, Cc, H, concat, loops)
             gen = torch.Generator(device=R.dev).manual_seed(Cc + H)
