@@ -106,6 +106,8 @@ _SIGS = {
     "gnnb_dense_emulation_active": (_int, []),
     "gnnb_gather_rows": (_int, [_vp, _i64, _f32p, _i64, _f32p, _vp]),
     "gnnb_propagate_halo": (_int, [_vp, _int, _int, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _i64, _f32p, _vp]),
+    "gnnb_propagate_maxmin_bwd_halo": (_int, [_vp, _int, _int, _f32p, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _i64, _f32p,
+                                              _vp]),
     "gnnb_gat_aggregate_halo": (_int, [_vp, _f32p, _f32p, _i64, _f32p, _f32p, _i64, _i64, C.c_float, _f32p, _f32p, _f32p,
                                        _vp]),
     "gnnb_gat_aggregate_bwd_halo": (_int, [_vp, _f32p, _f32p, _f32p, _f32p, _i64, _f32p, _f32p, _f32p, _f32p, _i64, _i64,

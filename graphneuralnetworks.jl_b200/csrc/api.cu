@@ -21,6 +21,9 @@ int edge_dot(gnnb_graph* g, const float* dout, const float* x, const float* cs, 
              float* dw_coo, cudaStream_t st);
 int maxmin_bwd(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
                int64_t D, float* dx, cudaStream_t st);
+int maxmin_bwd_halo(gnnb_graph* g, const float* w_plan_dst, const float* x_own, const float* dout_local,
+                    const float* dout_halo, const float* out_local, const float* out_halo, int32_t n_local, int64_t D,
+                    float* dx, cudaStream_t st);
 
 __global__ void mul_vec_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, float* __restrict__ o) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -225,6 +228,25 @@ int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local,
     a.cs = cs; a.ct = ct; a.out = out; a.D = D; a.aggr = aggr;
     GNNB_TRY(plan_weights(g, c, msg, w, 0, &a.w, st));
     return seg_reduce(g, c, a, st);
+}
+
+int gnnb_propagate_maxmin_bwd_halo(gnnb_graph_t g, int msg, int aggr, const float* x_own, const float* dout_local,
+                                   const float* dout_halo, const float* out_local, const float* out_halo, int64_t n_local,
+                                   const float* w, int64_t D, float* dx, void* stream) {
+    GNNB_TRY(check_common(g, msg, aggr, D, w));
+    if (aggr != GNNB_MAX && aggr != GNNB_MIN)
+        GNNB_FAIL(GNNB_EINVAL, "maxmin_bwd_halo serves max and min (sum and mean pull back through gnnb_propagate_halo)");
+    if (n_local < 0 || n_local > g->n_src) GNNB_FAIL(GNNB_ESIZE, "n_local must be in [0, num_src]");
+    if (g->n_dst == 0) return GNNB_OK;   // a rank that owns no node: no source row to write, dx may be NULL
+    if (!x_own || !dx) GNNB_FAIL(GNNB_EINVAL, "x_own/dx is NULL");
+    if (n_local > 0 && (!dout_local || !out_local)) GNNB_FAIL(GNNB_EINVAL, "dout_local/out_local is NULL");
+    if (n_local < g->n_src && (!dout_halo || !out_halo))
+        GNNB_FAIL(GNNB_EINVAL, "dout_halo/out_halo is NULL but the shard has halo targets");
+    cudaStream_t st = (cudaStream_t)stream;
+    GNNB_TRY(ensure_csr(g, false, st));
+    const float* wp = nullptr;
+    GNNB_TRY(plan_weights(g, g->by_dst, msg, w, 0, &wp, st));
+    return maxmin_bwd_halo(g, wp, x_own, dout_local, dout_halo, out_local, out_halo, (int32_t)n_local, D, dx, st);
 }
 
 // ---- host-buffer entries ------------------------------------------------------------------------

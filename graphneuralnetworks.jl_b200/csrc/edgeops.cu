@@ -101,10 +101,13 @@ __global__ void edge_dot_kernel(const int32_t* __restrict__ row, const int32_t* 
 
 // pullback of MAX/MIN aggregation w.r.t. x (every tied extremum receives the gradient: NNlib rule)
 //   dx[j,:] = sum_{e in out-edges of j} w_e * dout[t_e,:] .* ( x[j,:]*w_e == out_fwd[t_e,:] )
+// HALO 1 (the forward CSR of a backward shard plan): targets >= split read dout2 / of2 + (t - split)*D
+template <int HALO>
 __global__ void maxmin_bwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ col,
                                   const float* __restrict__ w_plan, int32_t nrows, const float* __restrict__ x,
                                   const float* __restrict__ dout, const float* __restrict__ out_fwd,
-                                  int64_t D, float* __restrict__ dx) {
+                                  int64_t D, float* __restrict__ dx, const float* __restrict__ dout2,
+                                  const float* __restrict__ of2, int32_t split) {
     const int lane = threadIdx.x & 31;
     const int64_t j = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (j >= nrows) return;
@@ -114,9 +117,11 @@ __global__ void maxmin_bwd_kernel(const int32_t* __restrict__ rowptr, const int3
         float acc = 0.f;
         for (int e = rs; e < re; ++e) {
             const int64_t t = col[e];
+            const bool second = HALO != 0 && t >= split;
+            const int64_t tr = second ? t - split : t;
             const float w = w_plan ? w_plan[e] : 1.f;
             const float m = __fmul_rn(xv, w);
-            if (m == __ldg(out_fwd + t * D + f)) acc += w * __ldg(dout + t * D + f);
+            if (m == __ldg((second ? of2 : out_fwd) + tr * D + f)) acc += w * __ldg((second ? dout2 : dout) + tr * D + f);
         }
         dx[j * D + f] = acc;
     }
@@ -257,20 +262,38 @@ int edge_dot(gnnb_graph* g, const float* dout, const float* x, const float* cs, 
     return GNNB_OK;
 }
 
-int maxmin_bwd_lean(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
-                    int64_t D, float* dx, cudaStream_t st);   // seglean.cu
-int maxmin_bwd(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
-               int64_t D, float* dx, cudaStream_t st) {
-    const Csr& c = g->by_src;
+int maxmin_bwd_lean(gnnb_graph* g, const Csr& c, const float* w_plan, const float* x, const float* dout,
+                    const float* out_fwd, bool halo, const float* dout2, const float* of2, int32_t split, int64_t D,
+                    float* dx, cudaStream_t st);   // seglean.cu
+// the max / min pullback over `c`, whose rows are the sources j and whose gathered nodes the targets t (weights in c's
+// plan order): the by-source plan of a graph (halo = false), or the forward CSR of a backward shard plan whose targets
+// >= split read dout2 / of2 (halo = true)
+static int maxmin_bwd_rows(gnnb_graph* g, const Csr& c, const float* w_plan, const float* x, const float* dout,
+                           const float* out_fwd, bool halo, const float* dout2, const float* of2, int32_t split,
+                           int64_t D, float* dx, cudaStream_t st) {
     if (c.nrows == 0) return GNNB_OK;
     {   // rows of 128 / 256 / 512 floats: the work-item kernel (seglean.cu); other widths: one warp per source row
-        const int rc = maxmin_bwd_lean(g, w_plan_src, x, dout, out_fwd, D, dx, st);
+        const int rc = maxmin_bwd_lean(g, c, w_plan, x, dout, out_fwd, halo, dout2, of2, split, D, dx, st);
         if (rc != GNNB_EUNSUPPORTED) return rc;
     }
-    maxmin_bwd_kernel<<<nblk((int64_t)c.nrows * 32), 256, 0, st>>>(c.rowptr, c.col, w_plan_src, c.nrows, x, dout,
-                                                                   out_fwd, D, dx);
+    if (halo)
+        maxmin_bwd_kernel<1><<<nblk((int64_t)c.nrows * 32), 256, 0, st>>>(c.rowptr, c.col, w_plan, c.nrows, x, dout,
+                                                                          out_fwd, D, dx, dout2, of2, split);
+    else
+        maxmin_bwd_kernel<0><<<nblk((int64_t)c.nrows * 32), 256, 0, st>>>(c.rowptr, c.col, w_plan, c.nrows, x, dout,
+                                                                          out_fwd, D, dx, nullptr, nullptr, 0);
     GNNB_LAUNCHED();
     return GNNB_OK;
+}
+int maxmin_bwd(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
+               int64_t D, float* dx, cudaStream_t st) {
+    return maxmin_bwd_rows(g, g->by_src, w_plan_src, x, dout, out_fwd, false, nullptr, nullptr, 0, D, dx, st);
+}
+int maxmin_bwd_halo(gnnb_graph* g, const float* w_plan_dst, const float* x_own, const float* dout_local,
+                    const float* dout_halo, const float* out_local, const float* out_halo, int32_t n_local, int64_t D,
+                    float* dx, cudaStream_t st) {
+    return maxmin_bwd_rows(g, g->by_dst, w_plan_dst, x_own, dout_local, out_local, true, dout_halo, out_halo, n_local, D,
+                           dx, st);
 }
 
 }  // namespace gnnb

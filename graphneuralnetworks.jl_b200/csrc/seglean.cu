@@ -211,8 +211,10 @@ __device__ __forceinline__ float4 lcomb(float4 a, float4 v, float s1, float s2, 
 // GCN propagate took 19.3 / 35.8 / 28.3 ms against 16.5 / 35.4 / 27.9 ms here at D = 128 / 256 / 512; DESIGN.md §4.)
 // Everything that steers control flow is made warp-uniform through a vote (ballot / any), so that the
 // compiler keeps the loop free of divergence handling; shuffles are never executed under a lane-dependent condition.
+// The halo instances of MEAN and MAX/MIN (shards: dist_propagate, dist_sage_conv) are built for 2 CTAs per SM, which lets
+// them keep their registers (for 4 they spill up to 168 bytes per thread at 512 floats, for 3 up to 60).
 template <int KV, int SMODE, bool HAS_W, int HALO, int AGG>
-__global__ void __launch_bounds__(256, 4) seg_lean_kernel(const LeanParams p) {
+__global__ void __launch_bounds__(256, (HALO != 0 && AGG != AG_SUM) ? 2 : 4) seg_lean_kernel(const LeanParams p) {
     constexpr unsigned FULL = 0xffffffffu;
     constexpr int U = 8 / KV;                 // row loads a warp keeps in flight (4 KB)
     constexpr int64_t STRIDE = (int64_t)KV * 128;
@@ -346,9 +348,13 @@ struct MaxBwdParams {
     float* __restrict__ dx;
     float* __restrict__ ws;
     int32_t n_items;
+    // HALO 1 (the forward CSR of a backward shard plan): targets >= split read dout2 / of2 + (t - split)*D
+    int32_t split;
+    const float* __restrict__ dout2;
+    const float* __restrict__ of2;
 };
 
-template <int KV, bool HAS_W>
+template <int KV, bool HAS_W, int HALO>
 __global__ void __launch_bounds__(256, 2) maxmin_bwd_lean_kernel(const MaxBwdParams p) {
     constexpr unsigned FULL = 0xffffffffu;
     constexpr int U = KV == 1 ? 4 : (KV == 2 ? 2 : 1);      // edges in flight per warp (three rows each)
@@ -394,11 +400,15 @@ __global__ void __launch_bounds__(256, 2) maxmin_bwd_lean_kernel(const MaxBwdPar
                 const int cj = __shfl_sync(FULL, c_l, j0 + u);
                 const int rj = __shfl_sync(FULL, r_l, j0 + u);
                 if ((vmask >> (j0 + u)) & 1u) {
-                    const int64_t to = (int64_t)cj * STRIDE + lane * 4, xo = (int64_t)rj * STRIDE + lane * 4;
+                    const bool second = HALO != 0 && cj >= p.split;
+                    const int64_t to = (int64_t)(second ? cj - p.split : cj) * STRIDE + lane * 4,
+                                  xo = (int64_t)rj * STRIDE + lane * 4;
+                    const float* const of = second ? p.of2 : p.of;
+                    const float* const dout = second ? p.dout2 : p.dout;
 #pragma unroll
                     for (int i = 0; i < KV; ++i) {
-                        vo[u][i] = __ldg(reinterpret_cast<const float4*>(p.of + to + i * 128));
-                        vd[u][i] = __ldg(reinterpret_cast<const float4*>(p.dout + to + i * 128));
+                        vo[u][i] = __ldg(reinterpret_cast<const float4*>(of + to + i * 128));
+                        vd[u][i] = __ldg(reinterpret_cast<const float4*>(dout + to + i * 128));
                         vx[u][i] = __ldg(reinterpret_cast<const float4*>(p.x + xo + i * 128));
                     }
                 }
@@ -443,7 +453,8 @@ int launch_lean3(const LeanParams& p, cudaStream_t st) {
     return GNNB_OK;
 }
 // instances: SUM with every scale source, with and without a halo base; MEAN and MAX/MIN for the plain messages
-// (copy_xj, w_mul_xj) — the shapes the layers use; anything else stays with seg_reduce_kernel
+// (copy_xj, w_mul_xj), with and without a halo base — the shapes the layers use; anything else stays with
+// seg_reduce_kernel
 template <int KV>
 int launch_lean1(const LeanParams& p, int smode, bool has_w, int halo, int agg, cudaStream_t st) {
 #define GNNB_LEAN(S, W, H, A) if (smode == S && has_w == W && halo == H && agg == A) return launch_lean3<KV, S, W, H, A>(p, st);
@@ -453,6 +464,8 @@ int launch_lean1(const LeanParams& p, int smode, bool has_w, int halo, int agg, 
     GNNB_LEAN(1, true, 1, AG_SUM) GNNB_LEAN(2, false, 1, AG_SUM) GNNB_LEAN(2, true, 1, AG_SUM)
     GNNB_LEAN(0, false, 0, AG_MEAN) GNNB_LEAN(0, true, 0, AG_MEAN)
     GNNB_LEAN(0, false, 0, AG_MAX) GNNB_LEAN(0, true, 0, AG_MAX)
+    GNNB_LEAN(0, false, 1, AG_MEAN) GNNB_LEAN(0, true, 1, AG_MEAN)
+    GNNB_LEAN(0, false, 1, AG_MAX) GNNB_LEAN(0, true, 1, AG_MAX)
 #undef GNNB_LEAN
     return GNNB_EUNSUPPORTED;
 }
@@ -642,7 +655,7 @@ int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, cu
     const int agg = ismax ? AG_MAX : (a.aggr == GNNB_MEAN ? AG_MEAN : AG_SUM);
     const int smode = (a.cs == nullptr) ? 0 : (a.es != nullptr ? 1 : 2);
     const bool halo = a.x2 != nullptr;
-    if (agg != AG_SUM && (smode != 0 || halo)) return GNNB_EUNSUPPORTED;
+    if (agg != AG_SUM && smode != 0) return GNNB_EUNSUPPORTED;
     GNNB_TRY(ensure_items(g, c, st));
     if (c.n_empty > 0) {
         const float v = a.aggr == GNNB_MAX ? -HUGE_VALF : (a.aggr == GNNB_MIN ? HUGE_VALF : 0.f);
@@ -676,15 +689,18 @@ int seg_reduce_lean(gnnb_graph* g, const Csr& c, const SegArgs& a, float* ws, cu
     return rc;
 }
 
-// max / min pullback through the work items of the by-source plan; GNNB_EUNSUPPORTED = not this kernel's shape
+// max / min pullback through the work items of `c`, whose rows are the sources j and whose gathered nodes the targets t:
+// the by-source plan of a graph, or the forward CSR of a backward shard plan with the targets >= split read from dout2 /
+// of2 (halo = true); GNNB_EUNSUPPORTED = not this kernel's shape
 int seg_fixup_sum(const Csr& c, int64_t E, int chunk, int64_t D, float* ws, float* out, cudaStream_t st);   // segreduce.cu
-int maxmin_bwd_lean(gnnb_graph* g, const float* w_plan_src, const float* x, const float* dout, const float* out_fwd,
-                    int64_t D, float* dx, cudaStream_t st) {
+int maxmin_bwd_lean(gnnb_graph* g, const Csr& c, const float* w_plan, const float* x, const float* dout,
+                    const float* out_fwd, bool halo, const float* dout2, const float* of2, int32_t split, int64_t D,
+                    float* dx, cudaStream_t st) {
     if (D != 128 && D != 256 && D != 512) return GNNB_EUNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(dout) & 15) ||
-        (reinterpret_cast<uintptr_t>(out_fwd) & 15) || (reinterpret_cast<uintptr_t>(dx) & 15))
+        (reinterpret_cast<uintptr_t>(out_fwd) & 15) || (reinterpret_cast<uintptr_t>(dx) & 15) ||
+        (reinterpret_cast<uintptr_t>(dout2) & 15) || (reinterpret_cast<uintptr_t>(of2) & 15))
         return GNNB_EUNSUPPORTED;
-    const Csr& c = g->by_src;
     if (g->E == 0) return GNNB_EUNSUPPORTED;
     GNNB_TRY(ensure_items(g, c, st));
     if (c.n_empty > 0) {
@@ -694,17 +710,23 @@ int maxmin_bwd_lean(gnnb_graph* g, const float* w_plan_src, const float* x, cons
     MaxBwdParams p;
     p.items = reinterpret_cast<const int4*>(c.items);
     p.n_items = c.n_items;
-    p.col = c.col; p.row = c.row; p.w = w_plan_src; p.x = x; p.dout = dout; p.of = out_fwd; p.dx = dx; p.ws = nullptr;
+    p.col = c.col; p.row = c.row; p.w = w_plan; p.x = x; p.dout = dout; p.of = out_fwd; p.dx = dx; p.ws = nullptr;
+    p.split = split; p.dout2 = dout2; p.of2 = of2;
     if (c.n_long > 0) {
         GNNB_TRY(grow_buffer(&g->ws, &g->ws_bytes, (size_t)2 * ceil_div(g->E, g->chunk) * D * sizeof(float)));
         p.ws = g->ws;
     }
     if (p.n_items > 0) {
         const unsigned blocks = (unsigned)ceil_div(p.n_items, 8);
-        const bool hw = w_plan_src != nullptr;
-        if (D == 128) { if (hw) maxmin_bwd_lean_kernel<1, true><<<blocks, 256, 0, st>>>(p); else maxmin_bwd_lean_kernel<1, false><<<blocks, 256, 0, st>>>(p); }
-        else if (D == 256) { if (hw) maxmin_bwd_lean_kernel<2, true><<<blocks, 256, 0, st>>>(p); else maxmin_bwd_lean_kernel<2, false><<<blocks, 256, 0, st>>>(p); }
-        else { if (hw) maxmin_bwd_lean_kernel<4, true><<<blocks, 256, 0, st>>>(p); else maxmin_bwd_lean_kernel<4, false><<<blocks, 256, 0, st>>>(p); }
+        const bool hw = w_plan != nullptr;
+#define GNNB_MAXBWD(KV, H) \
+        { if (hw) maxmin_bwd_lean_kernel<KV, true, H><<<blocks, 256, 0, st>>>(p); else maxmin_bwd_lean_kernel<KV, false, H><<<blocks, 256, 0, st>>>(p); }
+        if (halo) {
+            if (D == 128) GNNB_MAXBWD(1, 1) else if (D == 256) GNNB_MAXBWD(2, 1) else GNNB_MAXBWD(4, 1)
+        } else {
+            if (D == 128) GNNB_MAXBWD(1, 0) else if (D == 256) GNNB_MAXBWD(2, 0) else GNNB_MAXBWD(4, 0)
+        }
+#undef GNNB_MAXBWD
         GNNB_LAUNCHED();
     }
     if (c.n_long > 0) GNNB_TRY(seg_fixup_sum(c, g->E, g->chunk, D, p.ws, dx, st));

@@ -655,7 +655,11 @@ def graph_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:102-108: σ.(W1*xi .+ W2*propagate(copy_xj, g, aggr, xj) .+ b)."""
     check_num_nodes(g, x)
     xj, xi = expand_srcdst(g, x)
-    m = propagate(copy_xj, g, l.aggr, xj=xj)
+    return _graph_conv_dense(l, xi, propagate(copy_xj, g, l.aggr, xj=xj))
+
+
+def _graph_conv_dense(l, xi: torch.Tensor, m: torch.Tensor) -> torch.Tensor:
+    """σ.(W1*xi .+ W2*m .+ b) on Julia-shaped xi and m, the dense part of graph_conv and dist_graph_conv."""
     out = unrows(torch.addmm(rows(xi) @ l.weight1.t(), rows(m), l.weight2.t()))
     return _bias_act(l, out)
 
@@ -664,7 +668,11 @@ def gin_conv(l, g: GNNGraph, x: torch.Tensor) -> torch.Tensor:
     """GNNlib/src/layers/conv.jl:250-256: nn((1 + ϵ) .* xi .+ propagate(copy_xj, g, aggr, xj))."""
     check_num_nodes(g, x)
     xj, xi = expand_srcdst(g, x)
-    m = propagate(copy_xj, g, l.aggr, xj=xj)
+    return _gin_dense(l, xi, propagate(copy_xj, g, l.aggr, xj=xj))
+
+
+def _gin_dense(l, xi: torch.Tensor, m: torch.Tensor) -> torch.Tensor:
+    """nn((1 + ϵ) .* xi .+ m) on Julia-shaped xi and m, the node-local part of gin_conv and dist_gin_conv."""
     eps = 0.0
     for name in ("\u03f5", "\u03b5", "eps"):     # ϵ (the reference's field; Python NFKC-normalises it to ε in identifiers)
         if hasattr(l, name):

@@ -13,7 +13,9 @@ Both directions are "pull": the backward pass gathers dout rows of remote target
 so there is no scatter-reduce across GPUs and every result stays deterministic; inside a target row the
 edges keep their COO order, so a shard reproduces the single-GPU summation order.
 
-Layers on shards: dist_gcn_conv, dist_sage_conv (mean, +) and dist_gat_conv.  GAT's pullback has one term that
+Message passing on shards: dist_propagate (copy_xj / w_mul_xj with +, mean, max or min; max and min pull back through
+gnnb_propagate_maxmin_bwd_halo, which reads the halo rows of dout and of the forward result).  Layers on shards:
+dist_gcn_conv, dist_sage_conv (mean, +), dist_graph_conv, dist_gin_conv and dist_gat_conv.  GAT's pullback has one term that
 crosses ranks, del of a target = the sum of its in-edges' dz, computed by the owners of their sources: the dz rows move
 to the targets' owners by one all-to-all in an order both shards already share (DistGraph._edge_route).  Weighted
 GCNConv keeps each shard's edge weights (an ownership mask over the global order) and moves an explicit per-rank
@@ -666,21 +668,29 @@ class DistGraph:
             self._cw = self.gcn_scales(self.w_fwd)
         return self._cw
 
+    def _column_sliced(self, f, *cols) -> Optional[torch.Tensor]:
+        """f(*cols) one block of `D / GNNB_HALO_SLICES` feature columns at a time, or None when the pass is not sliced.
+        Column-sliced passes exchange and reduce a slice at a time, so that the halo buffers shrink by the slice count
+        (config 5: 62 GB of halo rows per pass at D = 256 do not fit beside the features); they cost strided copies of
+        the local rows and re-read the index arrays once per slice.  Every aggregation is column-wise, so the slices are
+        independent."""
+        slices = int(os.environ.get("GNNB_HALO_SLICES", "1"))
+        if slices <= 1 or cols[0].shape[1] % slices or getattr(self, "_slicing", False):
+            return None
+        k = cols[0].shape[1] // slices
+        out = torch.empty_like(cols[0])
+        self._slicing = True
+        try:
+            for i in range(slices):
+                out[:, i * k:(i + 1) * k] = f(*(c[:, i * k:(i + 1) * k].contiguous() for c in cols))
+        finally:
+            self._slicing = False
+        return out
+
     def propagate(self, shard: _Shard, x_rows: torch.Tensor, cs, ct, aggr=_lib.SUM, w=None) -> torch.Tensor:
         """one pass over `shard`: copy_xj, or w_mul_xj with the shard's edge weights `w` (COO order)"""
-        slices = int(os.environ.get("GNNB_HALO_SLICES", "1"))
-        if slices > 1 and x_rows.shape[1] % slices == 0 and not getattr(self, "_slicing", False):
-            # column-sliced pass: exchange and reduce `D / slices` feature columns at a time, so that the halo buffers
-            # shrink by `slices` (config 5: 62 GB of halo rows per pass at D = 256 do not fit beside the features);
-            # costs two strided copies of the local rows and re-reads the index arrays once per slice
-            k = x_rows.shape[1] // slices
-            out = torch.empty_like(x_rows)
-            self._slicing = True
-            try:
-                for i in range(slices):
-                    out[:, i * k:(i + 1) * k] = self.propagate(shard, x_rows[:, i * k:(i + 1) * k].contiguous(), cs, ct, aggr, w)
-            finally:
-                self._slicing = False
+        out = self._column_sliced(lambda xs: self.propagate(shard, xs, cs, ct, aggr, w), x_rows)
+        if out is not None:
             return out
         D = x_rows.shape[1]
         hptr, recv = self.halo_ptr(shard, x_rows)
@@ -691,6 +701,25 @@ class DistGraph:
                                                _ptr(cs), _ptr(ct), D, out.data_ptr(), _stream(self.device)))
         del recv                                                # the kernel that reads it is enqueued
         return out
+
+    def maxmin_pullback(self, dout: torch.Tensor, x_rows: torch.Tensor, out: torch.Tensor, aggr, w=None) -> torch.Tensor:
+        """dx of the owned rows for max / min aggregation over the forward shard (out its result), by the backward shard:
+        the halo rows of dout and of out are pulled (two purposes: one kernel reads both), then
+        gnnb_propagate_maxmin_bwd_halo with the backward shard's edge weights `w` (COO order) or none"""
+        dx = self._column_sliced(lambda d, x, o: self.maxmin_pullback(d, x, o, aggr, w), dout, x_rows, out)
+        if dx is not None:
+            return dx
+        sh, D = self.bwd, x_rows.shape[1]
+        d_ptr, d_recv = self.halo_ptr(sh, dout, "maxmin_dout")
+        o_ptr, o_recv = self.halo_ptr(sh, out, "maxmin_out")
+        dx = torch.empty_like(x_rows)
+        with torch.cuda.device(self.device):
+            _lib.check(lib.gnnb_propagate_maxmin_bwd_halo(sh.plan.h, _lib.COPY_XJ if w is None else _lib.W_MUL_XJ, aggr,
+                                                          _ptr(x_rows), _ptr(dout), d_ptr if sh.n_halo else None,
+                                                          _ptr(out), o_ptr if sh.n_halo else None, sh.n_local, _ptr(w),
+                                                          D, _ptr(dx), _stream(self.device)))
+        del d_recv, o_recv                                      # the kernel that reads them is enqueued
+        return dx
 
 
 class _DistGCNPropagateFn(torch.autograd.Function):
@@ -857,19 +886,115 @@ def dist_gat_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
 
 
 # ---------------------------------------------------------------------------------------------------------
-# SAGEConv on shards (mean, +): the lean reduce's HALO instance both ways
+# message passing on shards: propagate(copy_xj | w_mul_xj, g, +|mean|max|min), and the layers built on it
 # ---------------------------------------------------------------------------------------------------------
-class _DistSAGEPropagateFn(torch.autograd.Function):
+class _DistPropagateFn(torch.autograd.Function):
+    """propagate(copy_xj | w_mul_xj, g, aggr) on the owned rows: gnnb_propagate_halo over the forward shard.  w: None
+    (copy_xj), the graph's own dg.w_fwd, or explicit weights of every forward-shard edge (loops included).
+
+    Pullback for x: + and mean run gnnb_propagate_halo over the backward shard (mean: each target's row scaled by
+    1 / in-degree, sage_cs); max and min pull the halo rows of dout and of the forward result over the backward shard and
+    run gnnb_propagate_maxmin_bwd_halo.  The backward shard's weights are dg.w_bwd for the graph's, or the explicit ones
+    moved there by edge_exchange_reverse.  Pullback for explicit weights (+ and mean only): dw_e = <dout_t, x_s> ct[t]
+    by gnnb_gcn_edge_weight_grad_halo over the forward shard (ct = 1 / in-degree for mean), whose halo rows of x are
+    exchanged again here rather than kept from the forward.  The edge-weight gradient of max / min is refused by
+    dist_propagate before any exchange.
+
+    Tensors are kept with save_for_backward: the forward result kept as a ctx attribute would form the cycle
+    out -> grad_fn -> ctx -> out, which only the cyclic collector frees."""
+
     @staticmethod
-    def forward(ctx, x_rows, dg: DistGraph, aggr):
+    def forward(ctx, x_rows, w, dg: DistGraph, aggr):
+        ismax = aggr in (_lib.MAX, _lib.MIN)
+        ctx.want_w = w is not None and ctx.needs_input_grad[1]
+        x_rows = x_rows.contiguous()
+        out = dg.propagate(dg.fwd, x_rows, None, None, aggr, w=w)
         ctx.dg, ctx.aggr = dg, aggr
-        return dg.propagate(dg.fwd, x_rows.contiguous(), None, None, aggr)
+        ctx.graph_w = w is not None and w is dg.w_fwd           # the backward shard keeps the graph's own weights
+        ctx.save_for_backward(x_rows if (ismax or ctx.want_w) else None, out if ismax else None,
+                              None if ctx.graph_w else w)
+        return out
 
     @staticmethod
     def backward(ctx, dout):
-        dg = ctx.dg
-        cs = dg.sage_cs() if ctx.aggr == _lib.MEAN else None    # mean: each target's row scaled by 1 / in-degree
-        return dg.propagate(dg.bwd, dout.contiguous(), cs, None, _lib.SUM), None, None
+        dg, aggr = ctx.dg, ctx.aggr
+        x, out, w = ctx.saved_tensors
+        dout = dout.contiguous()
+        w_b = dg.w_bwd if ctx.graph_w else None
+        if w is not None:
+            w_b = dg.edge_exchange_reverse(w.detach().reshape(-1, 1)).reshape(-1)
+        if aggr in (_lib.MAX, _lib.MIN):
+            return dg.maxmin_pullback(dout, x, out, aggr, w_b), None, None, None
+        cs = dg.sage_cs() if aggr == _lib.MEAN else None        # mean: each target's row scaled by 1 / in-degree
+        dx = dg.propagate(dg.bwd, dout, cs, None, _lib.SUM, w=w_b)
+        if not ctx.want_w:
+            return dx, None, None, None
+        D = x.shape[1]
+        ct = dg.sage_cs()[:dg.n_local].contiguous() if aggr == _lib.MEAN else None
+        x_halo = dg.halo_rows(dg.fwd, x, "x")
+        dw = torch.empty(dg.fwd.num_edges, dtype=torch.float32, device=dg.device)
+        with torch.cuda.device(dg.device):
+            _lib.check(lib.gnnb_gcn_edge_weight_grad_halo(dg.fwd.plan.h, _ptr(dout), _ptr(x), _ptr(x_halo) if dg.fwd.n_halo else None,
+                                                          dg.n_local, None, _ptr(ct), None, D, _ptr(dw), _stream(dg.device)))
+        del x_halo                                              # the kernel that reads it is enqueued
+        return dx, dw, None, None
+
+
+def dist_propagate(f, dg: DistGraph, aggr, x_local: torch.Tensor, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """propagate(f, g, aggr; xj = x) (GNNlib/src/msgpass.jl:71-79) on the rows this rank owns, over the graph as
+    partitioned (its self loops included); x_local and the result are Julia-shaped (D, n_local).  Differentiable in
+    x_local and, for + and mean, in edge_weight.
+
+    f is copy_xj or w_mul_xj; aggr +, mean, max or min.  w_mul_xj multiplies each message by the explicit `edge_weight`
+    when given (this rank's: one value per edge whose target it owns, in global order, `w[dg.owned_by_target(t)]` of a
+    global list; each self loop of the partition gets weight 1), otherwise by the graph's own weights, otherwise by
+    nothing (copy_xj), as the single-GPU w_mul_xj.  The edge-weight gradient of max / min is not implemented (nor is
+    it on one GPU): a weight that requires grad is refused there."""
+    from .msgpass import _aggr_code, copy_xj, w_mul_xj
+    if f is not copy_xj and f is not w_mul_xj:
+        raise ValueError(f"dist_propagate: message function {getattr(f, '__name__', f)!r} is not supported on a "
+                         "partitioned graph (copy_xj and w_mul_xj are)")
+    code = _aggr_code(aggr)
+    w = None
+    if edge_weight is not None:
+        if f is not w_mul_xj:
+            raise ValueError("dist_propagate: copy_xj takes no edge weights (w_mul_xj does)")
+        if edge_weight.numel() != dg.num_owned_edges:
+            raise ValueError(f"Wrong number of edge weights (expected {dg.num_owned_edges}, the edges whose target rank "
+                             f"{dg.rank} owns, but given {edge_weight.numel()})")
+        w = edge_weight.reshape(-1).to(dg.device, torch.float32).contiguous()
+        if dg.self_loops:
+            w = torch.cat([w, torch.ones(dg.n_local, dtype=torch.float32, device=dg.device)])
+    elif f is w_mul_xj:
+        w = dg.w_fwd
+    if (code in (_lib.MAX, _lib.MIN) and w is not None and w.requires_grad and torch.is_grad_enabled()):
+        raise ValueError("dist_propagate: the edge-weight gradient of max / min aggregation is not implemented")
+    return unrows(_DistPropagateFn.apply(rows(x_local), w, dg, code))
+
+
+def _no_loops(dg: DistGraph, name: str) -> None:
+    if dg.self_loops:
+        raise ValueError(f"{name}: the graph was partitioned with add_self_loops=True; the layer adds no self loops")
+
+
+def dist_graph_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
+    """graph_conv (GNNlib/src/layers/conv.jl:102-108), σ.(W1·x .+ W2·propagate(copy_xj, g, aggr, x) .+ b), on the rows
+    this rank owns, for every aggregation; x_local is Julia-shaped (Din, n_local).  The graph must have been partitioned
+    without self loops.  Weight gradients are per-rank partial sums: all-reduce them."""
+    from .layers import _graph_conv_dense
+    from .msgpass import copy_xj
+    _no_loops(dg, "dist_graph_conv")
+    return _graph_conv_dense(l, x_local, dist_propagate(copy_xj, dg, l.aggr, x_local))
+
+
+def dist_gin_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
+    """gin_conv (GNNlib/src/layers/conv.jl:250-256), nn((1 + ϵ)·x .+ propagate(copy_xj, g, aggr, x)), on the rows this
+    rank owns; x_local is Julia-shaped (Din, n_local).  The graph must have been partitioned without self loops.
+    Gradients of nn's parameters are per-rank partial sums: all-reduce them."""
+    from .layers import _gin_dense
+    from .msgpass import copy_xj
+    _no_loops(dg, "dist_gin_conv")
+    return _gin_dense(l, x_local, dist_propagate(copy_xj, dg, l.aggr, x_local))
 
 
 def dist_sage_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
@@ -884,7 +1009,7 @@ def dist_sage_conv(l, dg: DistGraph, x_local: torch.Tensor) -> torch.Tensor:
     if dg.self_loops:
         raise ValueError("dist_sage_conv: the graph was partitioned with add_self_loops=True; SAGEConv adds no self loops")
     r1 = rows(x_local).contiguous()
-    return _sage_linear(l, r1, _DistSAGEPropagateFn.apply(r1, dg, aggr))
+    return _sage_linear(l, r1, _DistPropagateFn.apply(r1, None, dg, aggr))
 
 
 # ---------------------------------------------------------------------------------------------------------

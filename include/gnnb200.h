@@ -324,6 +324,17 @@ int gnnb_gather_rows(const int32_t* idx_dev, int64_t n, const float* x, int64_t 
 int gnnb_propagate_halo(gnnb_graph_t g, int msg, int aggr, const float* x_local, const float* x_halo,
                         int64_t n_local, const float* w, const float* cs, const float* ct, int64_t D,
                         float* out, void* stream);
+/* gnnb_propagate_maxmin_bwd_halo: the MAX/MIN pullback of gnnb_propagate_halo, on the FORWARD CSR of a backward shard
+ * plan (rows = owned sources j, num_dst of the plan; gathered = targets in [local | halo] order, num_src):
+ *     dx[j,:] = Σ_{e: j→t, shard COO order} w_e · dout[t,:] .* (x_own[j,:]·w_e == out_fwd[t,:])     (NNlib's every-tie rule)
+ * dout / out_fwd of targets < n_local read *_local, the others *_halo + (t - n_local)*D.  w: the backward shard's edge
+ * weights in its COO order, or NULL (copy_xj).  A plan without rows accepts NULL outputs; a shard without halo rows
+ * accepts NULL halo pointers.  SUM and MEAN are refused (GNNB_EINVAL): they pull back through gnnb_propagate_halo on the
+ * backward shard.  Rows of 128 / 256 / 512 floats with 16 B-aligned operands run the work-item kernel, long rows in
+ * pieces added in chunk order; other widths one warp per row.  No atomics: deterministic. */
+int gnnb_propagate_maxmin_bwd_halo(gnnb_graph_t g, int msg, int aggr, const float* x_own, const float* dout_local,
+                                   const float* dout_halo, const float* out_local, const float* out_halo, int64_t n_local,
+                                   const float* w, int64_t D, float* dx, void* stream);
 /* The fused GAT core on shards (csrc/gat.cu, the HALO instances of the same kernels; same shapes as gnnb_gat_aggregate).
  * gnnb_gat_aggregate_halo: gnnb_gat_aggregate on a forward shard plan, over its forward CSR: gathered sources < n_local
  *   read Wx_local, the others Wx_halo + (id - n_local)*C*H.  el (H, num_dst); er (H, num_src) in [local | halo] order.

@@ -1,6 +1,7 @@
-"""torchrun --nproc-per-node N scripts/check_dist.py : the node-partitioned GCNConv, GATConv and SAGEConv
-(partition.dist_gcn_conv / dist_gat_conv / dist_sage_conv, halo exchange over NCCL or the IPC push) against the
-single-GPU layer on the full graph: forward, dx and the all-reduced weight gradients."""
+"""torchrun --nproc-per-node N scripts/check_dist.py : the node-partitioned GCNConv, GATConv, SAGEConv, GraphConv and
+GINConv (partition.dist_gcn_conv / dist_gat_conv / dist_sage_conv / dist_graph_conv / dist_gin_conv, halo exchange over
+NCCL or the IPC push) against the single-GPU layer on the full graph: forward, dx and the all-reduced weight
+gradients."""
 import os
 import sys
 
@@ -106,6 +107,21 @@ for (n, E) in ((5000, 60000), (200000, 3000000)):
             sage.bias.normal_()
         check_layer(f"SAGEConv 128->128 aggr={aggr if isinstance(aggr, str) else 'mean'}", sage, g, n, 128, 128, False,
                     P.dist_sage_conv, [sage.weight, sage.bias])
+    # GraphConv and GINConv on the graph plus a ring, so that every node has an in-edge (max / min without -Inf rows)
+    ring = torch.arange(1, n + 1, device=dev, dtype=g.s.dtype)
+    gr = gnn.GNNGraph(torch.cat([g.s, ring % n + 1]), torch.cat([g.t, ring]), num_nodes=n)
+    for aggr in ("+", gnn.mean, "max", "min"):
+        torch.manual_seed(0)
+        gc = gnn.GraphConv(128, 64, torch.tanh, aggr=aggr, device=dev)
+        with torch.no_grad():
+            gc.bias.normal_()
+        check_layer(f"GraphConv 128->64 aggr={aggr if isinstance(aggr, str) else 'mean'}", gc, gr, n, 128, 64, False,
+                    P.dist_graph_conv, [gc.weight1, gc.weight2, gc.bias])
+    for aggr in ("+", "max"):
+        torch.manual_seed(0)
+        lin = torch.nn.Linear(128, 64, device=dev)
+        gin = gnn.GINConv(lambda h, lin=lin: gnn.unrows(torch.tanh(lin(gnn.rows(h)))), 0.5, aggr=aggr)
+        check_layer(f"GINConv 128->64 aggr={aggr}", gin, gr, n, 128, 64, False, P.dist_gin_conv, [lin.weight, lin.bias])
 t = torch.tensor([1 if ok else 0], device=dev)
 dist.all_reduce(t, op=dist.ReduceOp.MIN)
 dist.barrier()
